@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- atoms/s for one CHGNet energy+forces(+stress) evaluation on perturbed diamond Si.
 
-  python bench.py --gpus N --steps K --warmup W            # our arm (libb200mlip, sm_100a)
+  python bench.py --gpus N --steps K --warmup W            # our arm (libb200mlip, sm_90a)
   python bench.py --impl reference --steps K --warmup W    # reference arm: CPU restatement of the
                                                            # reference's path on the host cores
 
@@ -12,12 +12,14 @@ Contract (see the task statement): one JSON line on stdout from rank 0.
             pinned host positions -> GPU graph build -> forward -> backward -> forces back to host
   roofline= edge-gather (atom conv forward) kernel, algorithmic bytes / event time / measured HBM peak
 Workload (default, every N): the metric's own cell -- 50 x 50 x 50 conventional Si cells = 1 000 000 atoms, sliced
-into N slabs ("scaling": "strong"; one B200 holds it).  `--cells 23` runs BASELINE config[1] (97 336 atoms) the same
+into N slabs ("scaling": "strong"; one 80 GB H100 holds it).  `--cells 23` runs BASELINE config[1] (97 336 atoms) the same
 way; `--weak-cells n` grows an n x n x (n*N) cell with N instead ("scaling": "weak").  Activations per pass are GBs,
-far larger than the 126 MB L2, so no explicit flush is needed between timed steps.
+far larger than the 50 MB L2, so no explicit flush is needed between timed steps.
 Every line carries a `parity` object computed in the run: net-force and virial-symmetry residuals, energy per atom,
 a checksum of the forces of 4096 seeded atoms and -- at N > 1 -- the difference of E and of ALL forces against a
 single-partition evaluation of the same cell done on rank 0's GPU outside the timed region.
+`--dump-outputs DIR` writes, after the timed steps, what the last timed step computed (energy, forces, stress) as
+DIR/<name>.npy; the inputs (structure, seeded weights) are the same in every run with the same arguments.
 """
 from __future__ import annotations
 
@@ -44,27 +46,7 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def ncu_traffic(natoms, world):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the edge-gather kernel, per launch.  NOT measured in this run
-    (ncu cannot run inside a timed bench): it is read from the committed `ncu --set full` capture of the same
-    workload and kernel (profiles/*_ncu_edge_gather.json, newest first) and labelled as such; (None, reason) when no
-    capture matches the workload."""
-    import glob
-
-    for p in sorted(glob.glob(os.path.join(ROOT, "profiles", "*_ncu_edge_gather.json")), reverse=True):
-        try:
-            with open(p) as f:
-                d = json.load(f)
-            if d.get("atoms") == natoms and world == 1:
-                return (d["dram_bytes_read"] + d["dram_bytes_write"],
-                        f"static: {os.path.relpath(p, ROOT)} (ncu --set full, kernel {d.get('kernel', '?')}, "
-                        f"commit {d.get('commit', '?')})")
-        except Exception:  # noqa: BLE001
-            pass
-    return None, "no committed ncu capture for this workload"
+    return 3350.0, "NVIDIA H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
@@ -145,7 +127,9 @@ def cpu_reference_step(n_cells, threads):
     t0 = time.perf_counter()
     kind = "port"
     t_graph = None
+    builder = "numpy restatement of the reference's graph builder (oracle/graph_ref.py; oracle/_ref not built)"
     if G.load_ref_extension() is not None and n_cells >= 6:
+        builder = "reference C graph builder (oracle/_ref, P=2)"
         frac = atoms.get_scaled_positions(wrap=True)
         ref = G.ref_get_subgraphs(cart, frac, lat, pbc, 2, 5.0, 3.0, True, num_threads=threads)
         t_graph = time.perf_counter() - t0
@@ -169,7 +153,7 @@ def cpu_reference_step(n_cells, threads):
     e, _ = model.forward_graph(pos, vec, t(i1), t(i2), t(bond_edges), t(la), t(lb), t(ce), types)
     e.backward()
     t_model = time.perf_counter() - t1
-    return len(atoms), t_graph + t_model, {"graph_s": t_graph, "model_s": t_model, "kind": kind}
+    return len(atoms), t_graph + t_model, {"graph_s": t_graph, "model_s": t_model, "kind": kind, "graph_builder": builder}
 
 
 def best_thread_count(n_cells=8):
@@ -177,8 +161,8 @@ def best_thread_count(n_cells=8):
     (up to every host core) on the SAME sample size the baseline is then timed on, so the CPU arm is not handicapped
     on many-core hosts.  Returns (threads, {threads: seconds})."""
     cores = os.cpu_count() or 1
-    # (beyond 64 threads these small tensors get dramatically slower -- 36-52 s per step at 128 threads on the bench host,
-    #  profiles/r02j, r02r -- so the probe stops there instead of spending a minute to confirm it)
+    # (beyond 64 threads these small tensors get dramatically slower, so the probe stops there instead of spending a
+    #  minute to confirm it)
     cands = sorted({c for c in (8, 16, 32, 64) if c <= cores}) or [cores]
     best, best_t, seen = cands[0], 1e30, {}
     cpu_reference_step(n_cells, cands[0])  # first call pays imports / allocator warm-up
@@ -204,8 +188,8 @@ def run_reference(args):
         ts.append(sec)
     sec = float(np.mean(ts))
     val = atoms / sec
-    sample = (f"{atoms}-atom perturbed diamond Si ({n_cells}x{n_cells}x{n_cells} cells), reference C graph build (oracle/_ref, P=2, "
-              f"{det['graph_s']:.2f}s) + PyTorch-CPU restatement fwd+autograd bwd ({det['model_s']:.2f}s); {cores} threads = "
+    sample = (f"{atoms}-atom perturbed diamond Si ({n_cells}x{n_cells}x{n_cells} cells), {det['graph_builder']} "
+              f"({det['graph_s']:.2f}s) + PyTorch-CPU restatement fwd+autograd bwd ({det['model_s']:.2f}s); {cores} threads = "
               f"fastest of {probe} s/step on this sample (host has {os.cpu_count()} cores)")
     line = {
         "impl": "reference", "metric": METRIC, "value": val, "unit": "atoms/s", "n_gpus": args.gpus,
@@ -214,7 +198,8 @@ def run_reference(args):
         "config": {"workload": "CHGNet energy+forces+stress, perturbed diamond Si, r_cut=5A r_bond=3A",
                    "note": "bounded CPU sample (8000 atoms) of the same workload family; atoms/s of this path is size "
                            "independent above a few thousand atoms"},
-        "cpu_baseline": {"value": val, "unit": "atoms/s", "cores": cores, "kind": "port", "sample": sample},
+        "cpu_baseline": {"value": val, "unit": "atoms/s", "cores": cores, "kind": "port", "graph_builder": det["graph_builder"],
+                         "sample": sample},
         "e2e": {"value": val, "unit": "atoms/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
     print(json.dumps(line), flush=True)
@@ -257,6 +242,15 @@ def parity_block(atoms, out, pot_factory, rank, world, local, release=None):
     return blk
 
 
+def dump_outputs(out_dir, eng):
+    """energy, forces and stress of the engine's last evaluation, as a caller of the timed path receives them"""
+    e, f, s = eng.results()
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "energy.npy"), np.array([e], dtype=np.float64))
+    np.save(os.path.join(out_dir, "forces.npy"), np.ascontiguousarray(f, dtype=np.float32))
+    np.save(os.path.join(out_dir, "stress.npy"), np.ascontiguousarray(s, dtype=np.float32))
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -289,7 +283,8 @@ def run_ours(args):
         atoms = SimpleAtoms(base.get_chemical_symbols() * len(shifts), (pos[None] + shifts[:, None]).reshape(-1, 3),
                             lat * np.array(reps)[:, None])
     elif strong:  # default: fixed total cell (50 -> the metric's 1 000 000-atom cell), sliced across the ranks
-        n = args.cells
+        # TensorNet keeps ~5.9 KB per edge (DESIGN.md 8): the 1 M-atom cell does not fit an 80 GB H100, 30^3 cells do
+        n = args.cells if args.cells is not None else (30 if tn else 50)
         atoms = si_diamond(n)
     else:       # fixed work per GPU, the cell grows along z with the number of ranks
         n = args.weak_cells
@@ -331,6 +326,8 @@ def run_ours(args):
     barrier()
     t1 = time.perf_counter()
     wall_ms = (t1 - t0) * 1e3
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng)
     tmax = torch.tensor([dev_ms], dtype=torch.float64, device="cuda")
     if world > 1:
         dist.all_reduce(tmax, op=dist.ReduceOp.MAX)
@@ -379,10 +376,10 @@ def run_ours(args):
         g_ms = float(np.mean(gather_ms))
         alg_bytes = SURVEY_BYTES_PER_EDGE * c["n_edges"]
         n_loc, n_own = c["n_own"] + c["n_halo"], c["n_own"]
-        # own layout: indices+vec4 28 B, be 48 B, saved u|v 512 B per edge; A rows, C rows, agg, Q rows per node/bond
-        own_bytes = (28.0 + 48.0 + 512.0) * c["n_edges"] + 512.0 * n_loc + 512.0 * n_own + 256.0 * n_own + 0.75 * 512.0 * c["n_bond_own"]
+        # own layout: indices+vec4 28 B per edge (the radial basis is recomputed in the kernel, nothing is saved for the
+        # backward); A rows, C rows, agg, Q rows per node/bond
+        own_bytes = 28.0 * c["n_edges"] + 512.0 * n_loc + 512.0 * n_own + 256.0 * n_own + 0.75 * 512.0 * c["n_bond_own"]
         achieved = alg_bytes / (g_ms * 1e-3) / 1e9
-        traffic, traffic_src = ncu_traffic(natoms, world)
         line = {
             "metric": METRIC, "value": value, "unit": "atoms/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong" if strong else "weak",
@@ -395,7 +392,7 @@ def run_ours(args):
                         f"(min distance 2.2 A, 0.05 atoms/A^3; 10-40 edges and 0-12 bonds per atom), r_cut=5A r_bond=3A"),
                        "atoms": natoms, "atoms_per_gpu": natoms // world, "edges_per_gpu": c["n_edges"],
                        "angles_per_gpu": c["n_angles"], "parallelism": f"slab{world}",
-                       "cache": "activations per pass >> 126 MB L2 (no explicit flush needed)"},
+                       "cache": "activations per pass >> 50 MB L2 (no explicit flush needed)"},
             "value_note": "device time of forward+backward on the resident graph; `e2e` (host positions in, graph rebuilt every "
                           "step, forces out) is the figure comparable with the reference arm, whose steps include its graph build",
             "wall_ms_per_step": wall_ms / args.steps,
@@ -405,19 +402,18 @@ def run_ours(args):
             "parity": parity,
             "e2e": {"value": e2e_val, "unit": "atoms/s", "ms_per_step": e2e_ms,
                     "h2d_bytes_per_step": natoms * (24 + 4) + 72 + 12, "d2h_bytes_per_step": natoms * 12 + 8 + 36 + natoms * 4},
-            "roofline": {"bound": "hbm", "kernel": "k_atomconv_fwd_v3 (edge gather: cp.async-staged A[src] rows, tcgen05 3xTF32)", "achieved": achieved,
+            "roofline": {"bound": "hbm", "kernel": "k_atomconv_fwd (edge gather: bulk-copy-staged A[src] rows, FP32 FFMA)", "achieved": achieved,
                          "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "bytes_per_launch": alg_bytes, "bytes_convention": "SURVEY 8(d): 314 B/edge",
-                         "kernel_ms": g_ms, "achieved_own_layout": own_bytes / (g_ms * 1e-3) / 1e9,
-                         "traffic": traffic, "traffic_source": traffic_src},
+                         "kernel_ms": g_ms, "achieved_own_layout": own_bytes / (g_ms * 1e-3) / 1e9},
         }
         if world == 1 and not args.no_cpu_baseline:
             cores, probe = best_thread_count(8)
             a, sec, det = cpu_reference_step(8, cores)
             line["cpu_baseline"] = {
-                "value": a / sec, "unit": "atoms/s", "cores": cores, "kind": "port",
+                "value": a / sec, "unit": "atoms/s", "cores": cores, "kind": "port", "graph_builder": det["graph_builder"],
                 "sample": f"{a}-atom Si (8x8x8), {cores} threads = fastest of {probe} s/step on this sample (host has "
-                          f"{os.cpu_count()} cores), reference C graph build {det['graph_s']:.2f}s + PyTorch-CPU "
+                          f"{os.cpu_count()} cores), {det['graph_builder']} {det['graph_s']:.2f}s + PyTorch-CPU "
                           f"restatement fwd+bwd {det['model_s']:.2f}s"}
         print(json.dumps(line), flush=True)
     if world > 1:
@@ -430,9 +426,9 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    ap.add_argument("--cells", type=int, default=50,
+    ap.add_argument("--cells", type=int, default=None,
                     help="strong scaling (default): a fixed C x C x C cell for every N (50 -> the metric's 1 000 000 atoms; "
-                         "23 -> 97 336 = BASELINE config[1])")
+                         "23 -> 97 336 = BASELINE config[1]); default 50 for CHGNet, 30 (216 000 atoms) for TensorNet")
     ap.add_argument("--weak-cells", type=int, default=0,
                     help="weak scaling instead: n x n x (n*N) cells, i.e. fixed work per GPU (0 = off)")
     ap.add_argument("--rough-atoms", type=int, default=0,
@@ -440,6 +436,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--model", default="chgnet", choices=["chgnet", "tensornet"],
                     help="tensornet: the SURVEY 8(f).2 path (reduced JSON line; the metric and the default are CHGNet)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the energy, forces and stress of the last one as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

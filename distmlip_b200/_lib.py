@@ -1,6 +1,6 @@
 """ctypes binding of libb200mlip.so (the C-ABI in include/b200mlip.h).
 
-There is NO CPU fallback: if the shared library is missing, or no sm_100 device is visible,
+There is NO CPU fallback: if the shared library is missing, or no sm_90 (H100) device is visible,
 every entry point raises.  Nothing under oracle/ is ever imported from here.
 """
 from __future__ import annotations
@@ -16,7 +16,7 @@ LIB_PATH = os.path.join(_HERE, "libb200mlip.so")
 SYMBOLS = [
     "b2m_create", "b2m_destroy", "b2m_last_error", "b2m_load_weights", "b2m_set_element_refs",
     "b2m_finalize_weights", "b2m_set_scaling", "b2m_comm_unique_id", "b2m_comm_init", "b2m_set_partition", "b2m_set_structure", "b2m_compute",
-    "b2m_compute_resident", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
+    "b2m_compute_resident", "b2m_get_results", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
     "b2m_debug_tensor", "b2m_last_timings", "b2m_release_workspace", "b2m_set_view", "b2m_create_tensornet",
 ]
 
@@ -74,6 +74,7 @@ def load_library():
     lib.b2m_set_structure.argtypes = [vp, i64, P(dbl), P(dbl), P(C.c_int32), P(C.c_int), dbl]
     lib.b2m_compute.argtypes = [vp, i32, i32, P(dbl), P(C.c_float), P(C.c_float)]
     lib.b2m_compute_resident.argtypes = [vp, i32, i32, i32, P(dbl), P(C.c_float)]
+    lib.b2m_get_results.argtypes = [vp, P(dbl), P(C.c_float), P(C.c_float)]
     lib.b2m_get_sitewise.argtypes = [vp, P(C.c_float)]
     lib.b2m_get_counts.argtypes = [vp, P(i64), i32]
     lib.b2m_get_partition_info.argtypes = [vp, i32, P(i64), i64]
@@ -203,6 +204,15 @@ class Engine:
         self._ck(self.lib.b2m_compute_resident(self.h, int(bool(forces)), int(bool(stress)), int(reps), C.byref(e),
                                                C.byref(ms)))
         return e.value, ms.value
+
+    def results(self):
+        """energy, forces [natoms, 3] and stress [3, 3] of the last evaluation (no new evaluation)"""
+        e = C.c_double()
+        f = np.empty((self.natoms, 3), dtype=np.float32)
+        s = np.empty(9, dtype=np.float32)
+        self._ck(self.lib.b2m_get_results(self.h, C.byref(e), f.ctypes.data_as(C.POINTER(C.c_float)),
+                                          s.ctypes.data_as(C.POINTER(C.c_float))))
+        return e.value, f, s.reshape(3, 3)
 
     def sitewise(self):
         out = np.empty(self.natoms, dtype=np.float32)

@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libb200mlip (sm_100a only).
+// common.cuh -- shared host/device helpers for libb200mlip (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -73,13 +73,11 @@ static Nccl g_nccl;
 
 // ------------------------------------------------------------------------------------------
 struct AtomLayerW {
-  float *W1s_k, *W1e_k, *W1t_k, *b1, *W1s_raw, *W1e_raw, *W1t_raw, *M, *W2k, *W2raw, *b2, *Wout_k, *Wout_raw;
-  float *W2can, *Mcan, *W2Tcan;  // tcgen05 operands (canonical UMMA layout, tf32 hi/lo planes)
+  float *W1s_k, *W1e_k, *W1t_k, *b1, *W1s_raw, *W1e_raw, *W1t_raw, *M, *W2can, *W2Tcan, *b2, *Wout_k, *Wout_raw;
 };
 struct BondLayerW {
-  float *W1a_k, *W1b_k, *W1c_k, *Wg_k, *b1, *W1a_raw, *W1b_raw, *W1c_raw, *Wg_raw, *W2k, *W2raw, *b2, *Wout_k, *Wout_raw;
-  float *WAa_k, *WAb_k, *WAc_k, *WAg_k, *bA, *WAa_raw, *WAb_raw, *WAc_raw, *WAg_raw;
-  float *Wgcan, *W2can, *W2Tcan, *WgTcan, *WAgcan, *WAgTcan;  // tcgen05 operands
+  float *W1a_k, *W1b_k, *W1c_k, *Wgcan, *b1, *W1a_raw, *W1b_raw, *W1c_raw, *WgTcan, *W2can, *W2Tcan, *b2, *Wout_k, *Wout_raw;
+  float *WAa_k, *WAb_k, *WAc_k, *WAgcan, *bA, *WAa_raw, *WAb_raw, *WAc_raw, *WAgTcan;
 };
 
 }  // namespace b2m
@@ -152,6 +150,7 @@ struct b2m_engine {
   int hpoint = 0;
   DBuf<float> precv[2];            // adjoint rows pushed by my neighbours (backward), double-buffered by point parity
   DBuf<float> ftmp;                // leader: staging of a peer's force array
+  DBuf<float> fsum;                // leader: the group's summed forces (the partitions' own arrays stay untouched)
   int view = 0;                    // leader: partition addressed by the inspection calls (b2m_set_view)
   // page-locked staging owned by the library: host arrays go through it with a few copy threads (a single-threaded
   // memcpy of 24 MB of positions was the largest host item of an end-to-end step at 1 M atoms)
@@ -162,8 +161,7 @@ struct b2m_engine {
   // graph + workspace
   Graph g;
   bool have_graph = false;
-  std::vector<DBuf<float>> x, h, ang, upd, uv, uvB, dsB, uvA;
-  DBuf<float> be_e, dbe_e;  // [E,12] radial basis and derivative, once per step
+  std::vector<DBuf<float>> x, h, ang, upd;
   bool want_grads = true;
   // first-layer projections of every atom-conv layer (A = x W1s^T, C = x W1t^T + b1, Q = h W1e^T), one buffer per
   // layer: the backward gathers the rows the forward wrote instead of re-running three GEMMs per layer
@@ -180,13 +178,11 @@ struct b2m_engine {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> gather_ev;
   long long launches_last = 0;
   double last_energy = 0;
-  std::map<const float*, const float*> canon_of;  // FFMA-layout GEMM operand -> canonical tcgen05 copy
-  int num_sms = 148;
-  bool use_tc = true;  // tcgen05 kernels; B2M_LEGACY_FFMA=1 selects the FP32-FFMA tile kernels (A/B checks)
+  std::map<const float*, const float*> canon_of;  // FFMA-layout GEMM operand -> canonical wgmma copy
+  int num_sms = 132;
+  bool use_tc = true;  // row GEMMs on the wgmma kernels; B2M_LEGACY_FFMA=1 selects the FP32-FFMA GEMM tiles (A/B checks)
   bool debug_no_halo = false;  // B2M_DEBUG_NO_HALO=1: a b2m_set_partition view may run with its exchanges skipped (wrong
                                // numbers, right amount of per-partition work: timing one slab of an N-way split on one GPU)
-  int ac_gen = 3;      // atom-conv kernel generation on the tcgen05 path: 3 (default, kernels_ac3.cu), 1 = first generation,
-                       // 4 = third-generation forward with the first-generation backward (B2M_ATOMCONV, A/B checks)
 };
 
 namespace b2m {
@@ -231,15 +227,6 @@ static std::vector<float> vcat(const std::vector<float>& a, const std::vector<fl
   o.insert(o.end(), b.begin(), b.end());
   return o;
 }
-// [2][64][64] k-major from a stacked [128][64] raw block: out[br][k][n] = raw[br*64+n][k]
-static std::vector<float> branch_kmajor(const std::vector<float>& raw128x64) {
-  std::vector<float> o(2 * 64 * 64);
-  for (int br = 0; br < 2; br++)
-    for (int k = 0; k < 64; k++)
-      for (int n = 0; n < 64; n++) o[((size_t)br * 64 + k) * 64 + n] = raw128x64[((size_t)br * 64 + n) * 64 + k];
-  return o;
-}
-
 // tf32 "hi" part: round-to-nearest (ties away) on the 13 dropped mantissa bits == cvt.rna.tf32.f32
 static float tf32_hi_host(float x) {
   uint32_t u;
@@ -266,6 +253,18 @@ static std::vector<float> canon_split(const std::vector<float>& raw, int N, int 
   return o;
 }
 
+// both 64-row branches (L then G) of a stacked [128][64] block as wgmma B operands of the fused kernels:
+// per branch canon_split of B[n][k] = raw[br*64 + n][k] (transposed = false) or raw[br*64 + k][n] (true)
+static std::vector<float> second_layer_can(const std::vector<float>& raw128x64, bool transposed) {
+  std::vector<float> out;
+  for (int br = 0; br < 2; br++) {
+    std::vector<float> blk(raw128x64.begin() + (size_t)br * 4096, raw128x64.begin() + (size_t)(br + 1) * 4096);
+    const auto c = canon_split(transposed ? transpose(blk, 64, 64) : blk, 64, 64, 64);
+    out.insert(out.end(), c.begin(), c.end());
+  }
+  return out;
+}
+
 static void finalize_weights(b2m_engine* e) {
   const int nb = e->desc.n_blocks;
   for (auto& kv : e->host_w) {
@@ -281,13 +280,13 @@ static void finalize_weights(b2m_engine* e) {
   Packer P;
   std::map<std::string, size_t> off;
   std::vector<std::string> gemm_names;
-  // every [K][N] row-major GEMM operand also gets a tcgen05 copy: canonical hi/lo planes of its [N][K] view
+  // every [K][N] row-major GEMM operand also gets a wgmma copy: canonical hi/lo planes of its [N][K] view
   auto put = [&](const std::string& name, const std::vector<float>& v) {
     off[name] = P.add(v);
     const bool is_k = name.size() > 2 && name.substr(name.size() - 2) == "_k";
     const bool is_raw = name.size() > 4 && name.substr(name.size() - 4) == "_raw";
     const bool is_f = name == "F0k" || name == "F1k" || name == "F0raw" || name == "F1raw";
-    if ((is_k || is_raw || is_f) && name.find("Wg_k") == std::string::npos && name.find("WAg_k") == std::string::npos) {
+    if (is_k || is_raw || is_f) {
       int K = 0, N = 0;
       if (v.size() == 64 * 64) K = 64, N = 64;
       else if (v.size() == 64 * 128) {
@@ -349,17 +348,11 @@ static void finalize_weights(b2m_engine* e) {
     put(q + "W1e_raw", W1e);
     put(q + "W1t_raw", W1t);
     put(q + "M", M);
-    put(q + "W2k", branch_kmajor(W2));
-    put(q + "W2raw", W2);
+    put(q + "W2can", second_layer_can(W2, false));
+    put(q + "W2Tcan", second_layer_can(W2, true));
     put(q + "b2", b2);
     put(q + "Wout_k", transpose(Wout, 64, 64));
     put(q + "Wout_raw", Wout);
-    {
-      const std::vector<float> W2L(W2.begin(), W2.begin() + 4096), W2G(W2.begin() + 4096, W2.end());
-      put(q + "W2can", vcat(canon_split(W2L, 64, 64, 64), canon_split(W2G, 64, 64, 64)));
-      put(q + "Mcan", canon_split(M, 128, 9, 16));
-      put(q + "W2Tcan", vcat(canon_split(transpose(W2L, 64, 64), 64, 64, 64), canon_split(transpose(W2G, 64, 64), 64, 64, 64)));
-    }
   }
   for (int l = 0; l < nb - 1; l++) {
     const std::string p = "bond_graph_layers." + std::to_string(l) + ".conv_layer.";
@@ -384,40 +377,26 @@ static void finalize_weights(b2m_engine* e) {
     put(q + "W1a_k", transpose(W1a, 128, 64));
     put(q + "W1b_k", transpose(W1b, 128, 64));
     put(q + "W1c_k", transpose(W1c, 128, 64));
-    put(q + "Wg_k", branch_kmajor(W1g));
+    put(q + "Wgcan", second_layer_can(W1g, false));
     put(q + "b1", b1);
     put(q + "W1a_raw", W1a);
     put(q + "W1b_raw", W1b);
     put(q + "W1c_raw", W1c);
-    put(q + "Wg_raw", W1g);
-    put(q + "W2k", branch_kmajor(W2));
-    put(q + "W2raw", W2);
+    put(q + "WgTcan", canon_split(transpose(W1g, 128, 64), 64, 128, 128));
+    put(q + "W2can", second_layer_can(W2, false));
+    put(q + "W2Tcan", second_layer_can(W2, true));
     put(q + "b2", b2);
     put(q + "Wout_k", transpose(Wout, 64, 64));
     put(q + "Wout_raw", Wout);
     put(q + "WAa_k", transpose(WAa, 128, 64));
     put(q + "WAb_k", transpose(WAb, 128, 64));
     put(q + "WAc_k", transpose(WAc, 128, 64));
-    put(q + "WAg_k", branch_kmajor(WAg));
+    put(q + "WAgcan", second_layer_can(WAg, false));
     put(q + "bA", bA);
     put(q + "WAa_raw", WAa);
     put(q + "WAb_raw", WAb);
     put(q + "WAc_raw", WAc);
-    put(q + "WAg_raw", WAg);
-    {
-      auto rows64 = [](const std::vector<float>& m, int br) {
-        return std::vector<float>(m.begin() + (size_t)br * 4096, m.begin() + (size_t)(br + 1) * 4096);
-      };
-      const std::vector<float> W2L(W2.begin(), W2.begin() + 4096), W2G(W2.begin() + 4096, W2.end());
-      put(q + "Wgcan", canon_split(W1g, 128, 64, 64));
-      put(q + "W2can", vcat(canon_split(W2L, 64, 64, 64), canon_split(W2G, 64, 64, 64)));
-      put(q + "W2Tcan", vcat(canon_split(transpose(W2L, 64, 64), 64, 64, 64), canon_split(transpose(W2G, 64, 64), 64, 64, 64)));
-      put(q + "WgTcan", vcat(canon_split(transpose(rows64(W1g, 0), 64, 64), 64, 64, 64),
-                             canon_split(transpose(rows64(W1g, 1), 64, 64), 64, 64, 64)));
-      put(q + "WAgcan", canon_split(WAg, 128, 64, 64));
-      put(q + "WAgTcan", vcat(canon_split(transpose(rows64(WAg, 0), 64, 64), 64, 64, 64),
-                              canon_split(transpose(rows64(WAg, 1), 64, 64), 64, 64, 64)));
-    }
+    put(q + "WAgTcan", canon_split(transpose(WAg, 128, 64), 64, 128, 128));
   }
   const auto& F0 = W(e, "final_layer.layers.0.weight", {D, D});
   const auto& F1 = W(e, "final_layer.layers.1.weight", {D, D});
@@ -466,28 +445,25 @@ static void finalize_weights(b2m_engine* e) {
     AtomLayerW& w = e->aw[l];
     w.W1s_k = dp(q + "W1s_k"), w.W1e_k = dp(q + "W1e_k"), w.W1t_k = dp(q + "W1t_k"), w.b1 = dp(q + "b1");
     w.W1s_raw = dp(q + "W1s_raw"), w.W1e_raw = dp(q + "W1e_raw"), w.W1t_raw = dp(q + "W1t_raw");
-    w.M = dp(q + "M"), w.W2k = dp(q + "W2k"), w.W2raw = dp(q + "W2raw"), w.b2 = dp(q + "b2");
+    w.M = dp(q + "M"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
     w.Wout_k = dp(q + "Wout_k"), w.Wout_raw = dp(q + "Wout_raw");
-    w.W2can = dp(q + "W2can"), w.Mcan = dp(q + "Mcan"), w.W2Tcan = dp(q + "W2Tcan");
   }
   e->bw.resize(nb - 1);
   for (int l = 0; l < nb - 1; l++) {
     const std::string q = "b" + std::to_string(l) + ".";
     BondLayerW& w = e->bw[l];
-    w.W1a_k = dp(q + "W1a_k"), w.W1b_k = dp(q + "W1b_k"), w.W1c_k = dp(q + "W1c_k"), w.Wg_k = dp(q + "Wg_k");
+    w.W1a_k = dp(q + "W1a_k"), w.W1b_k = dp(q + "W1b_k"), w.W1c_k = dp(q + "W1c_k"), w.Wgcan = dp(q + "Wgcan");
     w.b1 = dp(q + "b1"), w.W1a_raw = dp(q + "W1a_raw"), w.W1b_raw = dp(q + "W1b_raw"), w.W1c_raw = dp(q + "W1c_raw");
-    w.Wg_raw = dp(q + "Wg_raw"), w.W2k = dp(q + "W2k"), w.W2raw = dp(q + "W2raw"), w.b2 = dp(q + "b2");
+    w.WgTcan = dp(q + "WgTcan"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
     w.Wout_k = dp(q + "Wout_k"), w.Wout_raw = dp(q + "Wout_raw");
-    w.WAa_k = dp(q + "WAa_k"), w.WAb_k = dp(q + "WAb_k"), w.WAc_k = dp(q + "WAc_k"), w.WAg_k = dp(q + "WAg_k");
+    w.WAa_k = dp(q + "WAa_k"), w.WAb_k = dp(q + "WAb_k"), w.WAc_k = dp(q + "WAc_k"), w.WAgcan = dp(q + "WAgcan");
     w.bA = dp(q + "bA"), w.WAa_raw = dp(q + "WAa_raw"), w.WAb_raw = dp(q + "WAb_raw"), w.WAc_raw = dp(q + "WAc_raw");
-    w.WAg_raw = dp(q + "WAg_raw");
-    w.Wgcan = dp(q + "Wgcan"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.WgTcan = dp(q + "WgTcan");
-    w.WAgcan = dp(q + "WAgcan"), w.WAgTcan = dp(q + "WAgTcan");
+    w.WAgTcan = dp(q + "WAgTcan");
   }
   e->finalized = true;
 }
 
-// node-level GEMM dispatch: tcgen05 when a canonical copy of B exists, FFMA tile kernel otherwise
+// node-level GEMM dispatch: wgmma when a canonical copy of B exists, FFMA tile kernel otherwise
 static void gemm(b2m_engine* e, const float* A, int lda, const float* B, float* C, int ldc, int M, int N, int K,
                  const float* bias, const float* R, int ldr, bool accum) {
   if (e->use_tc) {
@@ -497,7 +473,7 @@ static void gemm(b2m_engine* e, const float* A, int lda, const float* B, float* 
       return;
     }
   }
-  B2M_REQUIRE(!e->use_tc, B2M_ERR_STATE, "tcgen05 path: GEMM operand without a canonical copy");
+  B2M_REQUIRE(!e->use_tc, B2M_ERR_STATE, "wgmma path: GEMM operand without a canonical copy");
   launch_gemm(e->st, A, lda, B, C, ldc, M, N, K, bias, R, ldr, accum);  // FP32-FFMA tile kernel (legacy path only)
 }
 
@@ -513,20 +489,9 @@ static void alloc_workspace(b2m_engine* e) {
   e->upd.resize(nb - 1);
   for (auto& b : e->x) b.ensure(nl * D + 64);
   for (auto& b : e->h) b.ensure(bl * D + 64);
-  const size_t Apad = (A + 127) / 128 * 128;  // tile-interleaved on the tcgen05 path: whole tiles
+  const size_t Apad = (A + 127) / 128 * 128;  // whole 128-row tiles
   for (auto& b : e->ang) b.ensure(Apad * D + 64);
   for (auto& b : e->upd) b.ensure(bo * D + 64);
-  e->uv.resize(nb);
-  if (e->use_tc)
-    for (auto& b : e->uv) b.ensure(((E + 127) / 128 * 128) * D2 + 64);  // u|v kept for the backward (tile-interleaved)
-  e->uvB.resize(nb - 1), e->dsB.resize(nb - 1), e->uvA.resize(nb - 1);
-  if (e->use_tc) {
-    e->be_e.ensure(((E + 127) / 128 * 128) * 12 + 64), e->dbe_e.ensure(((E + 127) / 128 * 128) * 12 + 64);
-    const size_t Ap = (A + 127) / 128 * 128;
-    for (auto& b : e->uvB) b.ensure(Ap * D2 + 64);
-    for (auto& b : e->dsB) b.ensure(Ap * D2 + 64);
-    for (int l = 0; l < nb - 2; l++) e->uvA[l].ensure(Ap * D2 + 64);
-  }
   e->ApL.resize(nb), e->CpL.resize(nb), e->QpL.resize(nb);
   for (int l = 0; l < nb; l++) {
     e->ApL[l].ensure(nl * D2 + 64), e->CpL[l].ensure(no * D2 + 64);
@@ -696,9 +661,8 @@ static AtomConvArgs atom_args(b2m_engine* e, int l) {
   a.e_src = g.e_src.p, a.e_dst = g.e_dst.p, a.e_bond = g.e_bond.p, a.e_vec = g.e_vec.p;
   const int ps = e->proj_slot(l);
   a.Aproj = e->ApL[ps].p, a.Cproj = e->CpL[ps].p, a.Qproj = l > 0 ? e->QpL[ps].p : nullptr;
-  a.M = w.M, a.W2k = w.W2k, a.W2raw = w.W2raw, a.b2 = w.b2, a.Wabw = e->d_Wabw;
+  a.M = w.M, a.W2can = w.W2can, a.W2Tcan = w.W2Tcan, a.b2 = w.b2, a.Wabw = e->d_Wabw;
   a.rp = e->rp2;
-  a.be = e->be_e.p, a.dbe = e->dbe_e.p;
   return a;
 }
 static void atom_projections(b2m_engine* e, int l) {
@@ -720,16 +684,7 @@ static void atom_layer_fwd(b2m_engine* e, int l) {
   B2M_CK(cudaEventCreate(&e0));
   B2M_CK(cudaEventCreate(&e1));
   B2M_CK(cudaEventRecord(e0, e->st));
-  if (e->use_tc) {
-    AtomConvTcW tw{w.W2can, w.Mcan, w.W2Tcan};
-    a.uv_save = e->want_grads ? e->uv[l].p : nullptr;
-    if (e->ac_gen >= 3)
-      launch_atomconv_fwd_v3(e->st, a, tw, e->num_sms);
-    else
-      launch_atomconv_fwd_tc(e->st, a, tw, e->num_sms);
-  } else {
-    launch_atomconv_fwd(e->st, a);
-  }
+  launch_atomconv_fwd(e->st, a);
   B2M_CK(cudaEventRecord(e1, e->st));
   e->gather_ev.push_back({e0, e1});
   gemm(e, e->agg.p, D, w.Wout_k, e->x[l + 1].p, D, g.n_own, D, D, nullptr, e->x[l].p, D, false);
@@ -749,16 +704,7 @@ static void atom_layer_bwd(b2m_engine* e, int l) {
     launch_zero_rows(e->st, e->gC.p, (int64_t)g.n_own * D2);
     a.gA = e->gA.p, a.gC = e->gC.p, a.gQ = e->gQ.p;
   }
-  if (e->use_tc) {
-    AtomConvTcW tw{w.W2can, w.Mcan, w.W2Tcan};
-    a.uv = e->uv[l].p;
-    if (e->ac_gen >= 3 && e->ac_gen != 4)  // B2M_ATOMCONV=4: third-generation forward with the first-generation backward
-      launch_atomconv_bwd_v3(e->st, a, tw, e->num_sms);
-    else
-      launch_atomconv_bwd_tc(e->st, a, tw, e->num_sms);
-  } else {
-    launch_atomconv_bwd(e->st, a);
-  }
+  launch_atomconv_bwd(e->st, a);
   if (need_gx) {
     gemm(e, e->gA.p, D2, w.W1s_raw, e->gx.p, D, g.n_loc, D, D2, nullptr, nullptr, 0, true);
     gemm(e, e->gC.p, D2, w.W1t_raw, e->gx.p, D, g.n_own, D, D2, nullptr, nullptr, 0, true);
@@ -776,32 +722,11 @@ static LineArgs line_args(b2m_engine* e, int l, bool hidden) {
   a.ang = e->ang[l].p;
   a.Ha = e->Ha.p, a.Hb = e->Hb.p, a.Xc = e->Xc.p;
   if (hidden) {
-    a.Wgk = w.Wg_k, a.Wgraw = w.Wg_raw, a.W2k = w.W2k, a.W2raw = w.W2raw, a.b2 = w.b2;
+    a.Wgcan = w.Wgcan, a.WgTcan = w.WgTcan, a.W2can = w.W2can, a.W2Tcan = w.W2Tcan, a.b2 = w.b2;
   } else {
-    a.Wgk = w.WAg_k, a.Wgraw = w.WAg_raw;
-  }
-  if (e->use_tc) {
-    float* uvp = hidden ? e->uvB[l].p : e->uvA[l].p;
-    a.uv = uvp, a.ds = hidden ? e->dsB[l].p : nullptr;
-    if (e->want_grads) a.uv_save = uvp, a.ds_save = hidden ? e->dsB[l].p : nullptr;
+    a.Wgcan = w.WAgcan, a.WgTcan = w.WAgTcan;
   }
   return a;
-}
-static LineTcW line_tcw(b2m_engine* e, int l, bool hidden) {
-  const BondLayerW& w = e->bw[l];
-  LineTcW t;
-  if (hidden) {
-    t.Wgcan = w.Wgcan, t.W2can = w.W2can, t.W2Tcan = w.W2Tcan, t.WgTcan = w.WgTcan;
-  } else {
-    t.Wgcan = w.WAgcan, t.W2can = nullptr, t.W2Tcan = nullptr, t.WgTcan = w.WAgTcan;
-  }
-  return t;
-}
-static void line_fwd_dispatch(b2m_engine* e, int l, bool hidden, const LineArgs& a) {
-  if (e->use_tc)
-    launch_line_fwd_tc(e->st, a, line_tcw(e, l, hidden), hidden, e->num_sms);
-  else
-    launch_line_fwd(e->st, a, hidden);
 }
 // first-layer projections of the line-graph MLPs: Ha / Hb from the bond features, Xc from the atom features
 static void line_proj_Ha(b2m_engine* e, int l, bool hidden) {
@@ -828,10 +753,7 @@ static void line_bwd_common(b2m_engine* e, int l, bool hidden, LineArgs& a) {
   launch_zero_rows(e->st, e->gHb.p, (int64_t)g.B_own * D2);
   launch_zero_rows(e->st, e->gXc.p, (int64_t)g.n_loc * D2);
   a.gang = e->gang.p, a.gHa = e->gHa.p, a.gHb = e->gHb.p, a.gXc = e->gXc.p;
-  if (e->use_tc)
-    launch_line_bwd_tc(e->st, a, line_tcw(e, l, hidden), hidden, e->num_sms);
-  else
-    launch_line_bwd(e->st, a, hidden);
+  launch_line_bwd(e->st, a, hidden);
   gemm(e, e->gHa.p, D2, hidden ? w.W1a_raw : w.WAa_raw, e->gh.p, D, g.B_loc, D, D2, nullptr, nullptr, 0, true);
   gemm(e, e->gHb.p, D2, hidden ? w.W1b_raw : w.WAb_raw, e->gh.p, D, g.B_own, D, D2, nullptr, nullptr, 0, true);
   gemm(e, e->gXc.p, D2, hidden ? w.W1c_raw : w.WAc_raw, e->gx.p, D, g.n_loc, D, D2, nullptr, nullptr, 0, true);
@@ -840,10 +762,9 @@ static void line_bwd_common(b2m_engine* e, int l, bool hidden, LineArgs& a) {
 static void forward(b2m_engine* e) {
   Graph& g = e->g;
   const int nb = e->desc.n_blocks;
-  if (e->use_tc) launch_edge_basis(e->st, g.E, g.e_vec.p, e->rp2, e->be_e.p, e->dbe_e.p);
   launch_embed(e->st, g.n_loc, g.type.p, e->d_emb, e->x[0].p);
   launch_bond_init(e->st, g.B_loc, g.b_vec.p, e->rp2, e->d_Wbe, e->h[0].p);
-  launch_angle_init(e->st, g.A, g.a_in.p, g.a_out.p, g.b_vec.p, e->d_fa, e->d_Wae, e->ang[0].p, e->use_tc);
+  launch_angle_init(e->st, g.A, g.a_in.p, g.a_out.p, g.b_vec.p, e->d_fa, e->d_Wae, e->ang[0].p);
   for (int l = 0; l < nb - 1; l++) {
     atom_layer_fwd(e, l);
     const BondLayerW& w = e->bw[l];
@@ -855,7 +776,7 @@ static void forward(b2m_engine* e) {
     launch_zero_rows(e->st, e->aggB.p, (int64_t)g.B_own * D);
     LineArgs a = line_args(e, l, true);
     a.aggB = e->aggB.p;
-    line_fwd_dispatch(e, l, true, a);
+    launch_line_fwd(e->st, a, true);
     gemm(e, e->aggB.p, D, w.Wout_k, e->upd[l].p, D, g.B_own, D, D, nullptr, nullptr, 0, false);
     launch_bond_update_fwd(e->st, g.B_own, g.b_vec.p, e->rp3, e->d_W3bw, e->h[l].p, e->upd[l].p, e->h[l + 1].p);
     if (l < nb - 2) {
@@ -868,7 +789,7 @@ static void forward(b2m_engine* e) {
       line_proj_Ha(e, l, false);
       LineArgs b = line_args(e, l, false);
       b.ang_out = e->ang[l + 1].p;
-      line_fwd_dispatch(e, l, false, b);
+      launch_line_fwd(e->st, b, false);
     }
   }
   // site-wise readout after block n-2 (chgnet.py:392-398)
@@ -903,16 +824,15 @@ static void backward(b2m_engine* e) {
   for (int l = nb - 2; l >= 0; l--) {
     const BondLayerW& w = e->bw[l];
     if (l < nb - 2) {
-      // the tcgen05 backward works from the tensors saved by the forward; only the FFMA generation recomputes
-      // the first-layer projections
-      if (!e->use_tc) line_projections(e, l, false);
+      // the first-layer projections of the angle update are recomputed (the buffers hold the next layer's)
+      line_projections(e, l, false);
       LineArgs a = line_args(e, l, false);
       line_bwd_common(e, l, false, a);
       halo_backward(e, e->gh.p, true);
     }
     launch_bond_update_bwd(e->st, g.B_own, g.b_vec.p, e->rp3, e->d_W3bw, e->gh.p, e->upd[l].p, e->gupd.p, e->gdb.p);
     gemm(e, e->gupd.p, D, w.Wout_raw, e->gaggB.p, D, g.B_own, D, D, nullptr, nullptr, 0, false);
-    if (!e->use_tc) line_projections(e, l, true);
+    line_projections(e, l, true);
     LineArgs a = line_args(e, l, true);
     a.gaggB = e->gaggB.p;
     line_bwd_common(e, l, true, a);
@@ -921,7 +841,7 @@ static void backward(b2m_engine* e) {
   }
   // geometry: h0 = W_be be(d_b), theta/Fourier, then edges -> forces and virial
   launch_h0_bwd(e->st, g.B_loc, g.b_vec.p, e->rp2, e->d_Wbe, e->gh.p, e->gdb.p);
-  launch_angle_init_bwd(e->st, g.A, g.a_in.p, g.a_out.p, g.b_vec.p, e->d_fa, e->d_Wae, e->gang.p, e->gbvec.p, e->use_tc);
+  launch_angle_init_bwd(e->st, g.A, g.a_in.p, g.a_out.p, g.b_vec.p, e->d_fa, e->d_Wae, e->gang.p, e->gbvec.p);
   launch_edge_final(e->st, g.E, g.e_src.p, g.e_dst.p, g.e_bond.p, g.e_vec.p, g.gid.p, e->gd.p, e->gdb.p, e->gbvec.p,
                     e->forces.p, e->scal.p + 1);
   launch_halo_bond_final(e->st, g.B_own, g.B_loc, g.b_src_gid.p, g.b_dst.p, g.b_vec.p, g.gid.p, e->gdb.p, e->gbvec.p,
@@ -1050,19 +970,23 @@ static void run_any(b2m_engine* e, bool grads) {
 static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) {
   double hs[10];
   B2M_CK(cudaMemcpyAsync(hs, e->scal.p, 10 * sizeof(double), cudaMemcpyDeviceToHost, e->st));
+  const float* fsrc = e->forces.p;
   if (!e->parts.empty() && forces) {  // group: sum the partitions' force arrays on the leader's device
     const size_t n = (size_t)e->g.N * 3;
     e->ftmp.ensure(n + 64);
+    e->fsum.ensure(n + 64);
+    B2M_CK(cudaMemcpyAsync(e->fsum.p, e->forces.p, n * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
     for (size_t p = 1; p < e->parts.size(); p++) {
       B2M_CK(cudaMemcpyAsync(e->ftmp.p, e->parts[p]->forces.p, n * sizeof(float), cudaMemcpyDefault, e->st));
-      k_add_inplace<<<cdiv((int64_t)n, 256), 256, 0, e->st>>>((int64_t)n, e->ftmp.p, e->forces.p);
+      k_add_inplace<<<cdiv((int64_t)n, 256), 256, 0, e->st>>>((int64_t)n, e->ftmp.p, e->fsum.p);
       B2M_CK(cudaGetLastError());
     }
+    fsrc = e->fsum.p;
   }
   const size_t fbytes = (size_t)e->g.N * 3 * sizeof(float);
   if (forces) {
     ensure_pinned(e->pin_out, e->pin_out_cap, fbytes);
-    B2M_CK(cudaMemcpyAsync(e->pin_out, e->forces.p, fbytes, cudaMemcpyDeviceToHost, e->st));
+    B2M_CK(cudaMemcpyAsync(e->pin_out, fsrc, fbytes, cudaMemcpyDeviceToHost, e->st));
   }
   B2M_CK(cudaStreamSynchronize(e->st));
   if (forces) par_memcpy(forces, e->pin_out, fbytes);
@@ -1132,12 +1056,10 @@ static b2m_engine* create_one(const b2m_model_desc* desc, int device, int count)
     B2M_CK(cudaSetDevice(e->device));
     cudaDeviceProp prop;
     B2M_CK(cudaGetDeviceProperties(&prop, e->device));
-    if (prop.major != 10) throw Error(B2M_ERR_CUDA, "libb200mlip is built for sm_100a (B200) only");
+    if (prop.major != 9 || prop.minor != 0) throw Error(B2M_ERR_CUDA, "libb200mlip is built for sm_90a (H100) only");
     e->num_sms = prop.multiProcessorCount;
     const char* leg = getenv("B2M_LEGACY_FFMA");
     e->use_tc = !(leg && leg[0] == '1');
-    const char* gen = getenv("B2M_ATOMCONV");
-    e->ac_gen = gen ? atoi(gen) : 3;
     const char* nh = getenv("B2M_DEBUG_NO_HALO");
     e->debug_no_halo = nh && nh[0] == '1';
     B2M_CK(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
@@ -1408,6 +1330,13 @@ int b2m_compute_resident(b2m_handle h, int want_forces, int want_stress, int rep
   API_END
 }
 
+int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9) {
+  API_BEGIN
+  B2M_REQUIRE(h->have_graph, B2M_ERR_STATE, "no structure");
+  fetch(h, energy, forces, stress9);
+  API_END
+}
+
 int b2m_get_sitewise(b2m_handle h, float* out) {
   API_BEGIN
   B2M_REQUIRE(h->have_graph && out, B2M_ERR_STATE, "no structure");
@@ -1509,18 +1438,8 @@ int b2m_debug_tensor(b2m_handle h, const char* name, float* out, int64_t cap, in
     throw Error(B2M_ERR_INVALID, "unknown debug tensor: " + n);
   }
   B2M_REQUIRE(r * c <= cap, B2M_ERR_INVALID, "debug buffer too small");
-  const bool angle_tensor = n.rfind("ang", 0) == 0 || n == "gang";
-  if (angle_tensor && h->use_tc) {  // tile-interleaved on the device: hand the caller the logical [A][64] rows
-    const size_t padded = (size_t)(r + 127) / 128 * 128 * 64;
-    std::vector<float> tmp(padded);
-    B2M_CK(cudaMemcpyAsync(tmp.data(), src, padded * sizeof(float), cudaMemcpyDeviceToHost, h->st));
-    B2M_CK(cudaStreamSynchronize(h->st));
-    for (int64_t i = 0; i < r; i++)
-      for (int k = 0; k < 64; k++) out[i * 64 + k] = tmp[ang_index(i, k, 1)];
-  } else {
-    B2M_CK(cudaMemcpyAsync(out, src, r * c * sizeof(float), cudaMemcpyDeviceToHost, h->st));
-    B2M_CK(cudaStreamSynchronize(h->st));
-  }
+  B2M_CK(cudaMemcpyAsync(out, src, r * c * sizeof(float), cudaMemcpyDeviceToHost, h->st));
+  B2M_CK(cudaStreamSynchronize(h->st));
   *rows = r, *cols = c;
   API_END
 }
@@ -1534,12 +1453,12 @@ int b2m_release_workspace(b2m_handle h) {
       if (b.p) cudaFree(b.p);
       b.p = nullptr, b.cap = 0;
     };
-    for (auto* v : {&e->x, &e->h, &e->ang, &e->upd, &e->uv, &e->uvB, &e->dsB, &e->uvA, &e->ApL, &e->CpL, &e->QpL})
+    for (auto* v : {&e->x, &e->h, &e->ang, &e->upd, &e->ApL, &e->CpL, &e->QpL})
       for (auto& b : *v) drop(b);
-    for (auto* b : {&e->be_e, &e->dbe_e, &e->Ha, &e->Hb, &e->Xc, &e->agg, &e->aggB, &e->y1p, &e->y1, &e->y2p, &e->y2,
+    for (auto* b : {&e->Ha, &e->Hb, &e->Xc, &e->agg, &e->aggB, &e->y1p, &e->y1, &e->y2p, &e->y2,
                     &e->e_atom, &e->site, &e->gx, &e->gh, &e->gang, &e->gA, &e->gC, &e->gQ, &e->gHa, &e->gHb, &e->gXc,
                     &e->gagg, &e->gupd, &e->gaggB, &e->gd, &e->gdb, &e->gbvec, &e->gy1, &e->gy2, &e->forces,
-                    &e->sendbuf, &e->recvbuf, &e->site_full, &e->precv[0], &e->precv[1], &e->ftmp})
+                    &e->sendbuf, &e->recvbuf, &e->site_full, &e->precv[0], &e->precv[1], &e->ftmp, &e->fsum})
       drop(*b);
     tn_release(e);
     e->g.~Graph();  // the resident graph goes too

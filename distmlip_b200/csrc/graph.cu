@@ -1,7 +1,7 @@
 // graph.cu -- GPU graph build: wrap, slab partition, global cell list, CSR neighbour list,
 // halo sections, bond graph, centre-grouped angle list.  Integer/f64 work, HBM-bound.
 //
-// Reference behaviour reproduced (file:line in /root/reference/DistMLIP/distributed):
+// Reference behaviour reproduced (file:line in the reference's DistMLIP/distributed):
 //   * wrap to the cell, unwrap correction ....................... fpis.c:492-506
 //   * edge rule  tol < d^2 < r^2 + tol, i != j (no self images) . fpis.c:760, 827
 //   * bond rule  d^2 < r_bond^2 + tol ........................... fpis.c:763, 844

@@ -1,7 +1,8 @@
-// kernels.cu -- hand-written sm_100a kernels of the CHGNet hot path (fp32 FFMA math,
+// kernels.cu -- hand-written sm_90a kernels of the CHGNet hot path (fp32 FFMA math,
 // cp.async.bulk (TMA) row gathers into shared memory, segmented scatter-adds).
 // See kernels.cuh for the formulation; oracle/manual_ref.py is the CPU mirror of every stage.
 #include "kernels.cuh"
+#include "wgmma.cuh"
 
 namespace b2m {
 
@@ -78,47 +79,76 @@ __device__ __forceinline__ void rbf_env_k(float d, float freq, const RadialParam
   dbe = ok ? (env + rbf * denv) * drbf : 0.f;
 }
 
-// thread -> micro-tile mapping of the 256-thread fused kernels:
-//   branch = tid>>7 (0: "layers", 1: "gates"), rows r_i = rg + 16 i, cols c_j = cg*4 + (j&3) + 32 (j>>2)
+// thread -> accumulator mapping of the 256-thread fused kernels: branch = warpgroup = tid>>7 (0: "layers", 1: "gates");
+// a warpgroup's 128 x 64 product is two m64n64 wgmma fragments, so thread (warp w, lane l) owns rows
+// r_i = 64 (i>>1) + 16 w + l/4 + 8 (i&1), i < 4, and columns c_j = 8 (j>>1) + 2 (l%4) + (j&1), j < 16
+constexpr int AR = 4, AC = 16;
 struct Map {
-  int branch, rg, cg;
+  int branch, rb, cb;
   __device__ __forceinline__ Map() {
     const int tid = threadIdx.x;
     branch = tid >> 7;
-    const int t128 = tid & 127, lane = tid & 31;
-    rg = (t128 >> 5) * 4 + (lane >> 3);
-    cg = lane & 7;
+    const int lane = tid & 31;
+    rb = ((tid & 127) >> 5) * 16 + (lane >> 2);
+    cb = 2 * (lane & 3);
   }
-  __device__ __forceinline__ int row(int i) const { return rg + 16 * i; }
-  __device__ __forceinline__ int col(int j) const { return cg * 4 + (j & 3) + 32 * (j >> 2); }
+  __device__ __forceinline__ int row(int i) const { return 64 * (i >> 1) + rb + 8 * (i & 1); }
+  __device__ __forceinline__ int col(int j) const { return 8 * (j >> 1) + cb + (j & 1); }
 };
 
-// acc[8][8] += At[r_i][kofs + k] * Wk[k][c_j], k < 64.  At: smem row-major pitch lda; Wk: smem [64][64].
-__device__ __forceinline__ void gemm64(const float* __restrict__ At, int lda, int kofs, const float* __restrict__ Wk,
-                                       float (&acc)[8][8], const Map& m) {
-  const float* a0 = At + m.rg * lda + kofs;
-  const float* w0p = Wk + m.cg * 4;
-#pragma unroll 4
-  for (int k = 0; k < 64; k++) {
-    const float4 w0 = *reinterpret_cast<const float4*>(w0p + k * 64);
-    const float4 w1 = *reinterpret_cast<const float4*>(w0p + k * 64 + 32);
+// d = (accumulate ? d : 0) + At[row0 .. row0+63][acol .. acol+64) . B[0..63][bk .. bk+64)^T on the tensor cores
+// (warpgroup-collective), 3xTF32 (hi.hi + lo.hi + hi.lo, fp32 accumulate).  At: fp32 in shared memory, row pitch lda
+// (A fragments are read into registers: lda % 32 == 4 keeps the 32 lanes on 32 banks); B: canonical K-major
+// [64 n][K k] image in shared memory, tf32 hi plane at b_hi and lo plane at b_lo.
+__device__ __forceinline__ void wg_mm64(const float* At, int lda, int row0, int acol, uint32_t b_hi, uint32_t b_lo,
+                                        int bk, bool accumulate, float (&d)[32]) {
+  constexpr uint32_t LBO = 8 * 128;  // byte step between core matrices along K (N = 64)
+  const int lane = threadIdx.x & 31;
+  const float* p0 = At + (row0 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2)) * lda + acol + (lane & 3);
+  const float* p1 = p0 + 8 * lda;
+  uint32_t ah[8][4], al[8][4];
 #pragma unroll
-    for (int i = 0; i < 8; i++) {
-      const float av = a0[i * 16 * lda + k];
-      acc[i][0] = fmaf(av, w0.x, acc[i][0]);
-      acc[i][1] = fmaf(av, w0.y, acc[i][1]);
-      acc[i][2] = fmaf(av, w0.z, acc[i][2]);
-      acc[i][3] = fmaf(av, w0.w, acc[i][3]);
-      acc[i][4] = fmaf(av, w1.x, acc[i][4]);
-      acc[i][5] = fmaf(av, w1.y, acc[i][5]);
-      acc[i][6] = fmaf(av, w1.z, acc[i][6]);
-      acc[i][7] = fmaf(av, w1.w, acc[i][7]);
+  for (int ks = 0; ks < 8; ks++) {
+    const float x[4] = {p0[8 * ks], p1[8 * ks], p0[8 * ks + 4], p1[8 * ks + 4]};
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      ah[ks][q] = tf32_hi_bits(x[q]);
+      al[ks][q] = __float_as_uint(x[q] - __uint_as_float(ah[ks][q]));
     }
+  }
+  const uint32_t koff = (uint32_t)(bk / 4) * LBO;
+  acc_fence(d);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 8; ks++) {
+#pragma unroll
+    for (int term = 0; term < 3; term++) {
+      const uint64_t bd = gmma_desc((term == 2 ? b_lo : b_hi) + koff + ks * 2 * LBO, LBO, 128u);
+      wgmma_tf32_n64_rA(d, term == 1 ? al[ks] : ah[ks], bd, (accumulate || ks > 0 || term > 0) ? 1 : 0);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+  acc_fence(d);
+}
+
+// acc (Map layout) = At[0..127][kofs .. kofs+64) . B^T for this thread's branch; Bcan: the branch's canonical image
+// (hi plane of 4096 floats, then lo plane)
+__device__ __forceinline__ void gemm64(const float* At, int lda, int kofs, const float* Bcan, float (&acc)[AR][AC]) {
+  const uint32_t bh = s_u32(Bcan), bl = bh + 4096u * 4u;
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    float d[32];
+    wg_mm64(At, lda, 64 * h, kofs, bh, bl, 0, false, d);
+#pragma unroll
+    for (int q = 0; q < 32; q++) acc[2 * h + ((q >> 1) & 1)][2 * (q >> 2) + (q & 1)] = d[q];
   }
 }
 
+// weights -> shared memory; the fence makes the generic-proxy stores visible to wgmma after the next barrier
 __device__ __forceinline__ void stage_w(float* Wsm, const float* __restrict__ g, int nfloat4) {
   for (int i = threadIdx.x; i < nfloat4; i += NT) reinterpret_cast<float4*>(Wsm)[i] = reinterpret_cast<const float4*>(g)[i];
+  fence_proxy_async_smem();
 }
 
 // running segmented sum over rows [r0, r1) of a smem tile column, flushed with atomics when the key changes
@@ -281,11 +311,11 @@ __device__ __forceinline__ AngleGeom angle_geom(const float4 a, const float4 b) 
   return g;
 }
 
-// ang0[r][c] = sum_k fourier_k(theta_r) Wae[c][k]      (128 angles per block = one tile of the interleaved layout)
+// ang0[r][c] = sum_k fourier_k(theta_r) Wae[c][k]      (128 angles per block)
 __global__ void __launch_bounds__(256) k_angle_init(int64_t na, const int* __restrict__ a_in,
                                                     const int* __restrict__ a_out, const float4* __restrict__ b_vec,
                                                     const float* __restrict__ fa, const float* __restrict__ Wae,
-                                                    float* __restrict__ ang0, int il) {
+                                                    float* __restrict__ ang0) {
   __shared__ float f_s[128][12];
   __shared__ float Ws[64 * 9];
   const int64_t r0 = (int64_t)blockIdx.x * 128;
@@ -318,16 +348,13 @@ __global__ void __launch_bounds__(256) k_angle_init(int64_t na, const int* __res
 #pragma unroll
       for (int j = 0; j < 4; j++) v[j] = fmaf(f, Ws[(4 * cq + j) * 9 + k], v[j]);
     }
-    if (il)
-      reinterpret_cast<float4*>(ang0)[(size_t)blockIdx.x * 16 * 128 + i] = make_float4(v[0], v[1], v[2], v[3]);
-    else
-      *reinterpret_cast<float4*>(ang0 + (size_t)(r0 + r) * 64 + 4 * cq) = make_float4(v[0], v[1], v[2], v[3]);
+    *reinterpret_cast<float4*>(ang0 + (size_t)(r0 + r) * 64 + 4 * cq) = make_float4(v[0], v[1], v[2], v[3]);
   }
 }
 void launch_angle_init(cudaStream_t st, int64_t na, const int* a_in, const int* a_out, const float4* b_vec,
-                       const float* fa, const float* Wae, float* ang0, bool interleaved) {
+                       const float* fa, const float* Wae, float* ang0) {
   if (na <= 0) return;
-  k_angle_init<<<cdiv(na, 128), 256, 0, st>>>(na, a_in, a_out, b_vec, fa, Wae, ang0, interleaved ? 1 : 0);
+  k_angle_init<<<cdiv(na, 128), 256, 0, st>>>(na, a_in, a_out, b_vec, fa, Wae, ang0);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }
@@ -361,8 +388,8 @@ void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats) {
 // ============================================================================================
 struct AtomSmemFwd {
   static constexpr int kTile = 32;  // float offset of tile (128 B for the mbarrier)
-  static constexpr int kW = kTile + TM * LD;
-  static constexpr int kBe = kW + 8192;
+  static constexpr int kW = kTile + TM * LD;      // wgmma images of W2 (2 branches x hi | lo)
+  static constexpr int kBe = kW + 16384;
   static constexpr int kWab = kBe + TM * 12;
   static constexpr int kB2 = kWab + 576;
   static constexpr int kD = kB2 + 128;
@@ -371,7 +398,7 @@ struct AtomSmemFwd {
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
 
-__global__ void __launch_bounds__(NT, 2) k_atomconv_fwd(const AtomConvArgs a) {
+__global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
   uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);
   float* tile = smem + AtomSmemFwd::kTile;
@@ -411,7 +438,7 @@ __global__ void __launch_bounds__(NT, 2) k_atomconv_fwd(const AtomConvArgs a) {
   // TMA row gather: A[src] (512 B per edge) straight into the tile
   if (tid == 0) mbar_expect_tx(mbar, (uint32_t)nvalid * 512u);
   if (tid < nvalid) bulk_g2s(tile + tid * LD, a.Aproj + (size_t)s_src[tid] * D2, 512u, mbar);
-  stage_w(Wsm, a.W2k, 2048);
+  stage_w(Wsm, a.W2can, 4096);
   for (int i = tid; i < 576; i += NT) wabW[i] = a.Wabw[i];
   if (tid < 128) b2s[tid] = a.b2[tid];
   {
@@ -452,32 +479,32 @@ __global__ void __launch_bounds__(NT, 2) k_atomconv_fwd(const AtomConvArgs a) {
   }
   __syncthreads();
   const Map m;
-  float acc[8][8];
+  float acc[AR][AC];
 #pragma unroll
-  for (int i = 0; i < 8; i++)
-    for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-  gemm64(tile, LD, m.branch * 64, Wsm + m.branch * 4096, acc, m);
+  for (int i = 0; i < AR; i++)
+    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+  gemm64(tile, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
 #pragma unroll
-  for (int i = 0; i < 8; i++)
+  for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
       acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
     }
   __syncthreads();
   if (m.branch == 1) {
 #pragma unroll
-    for (int i = 0; i < 8; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++) tile[m.row(i) * LD + m.col(j)] = acc[i][j];
+      for (int j = 0; j < AC; j++) tile[m.row(i) * LD + m.col(j)] = acc[i][j];
   }
   __syncthreads();
   if (m.branch == 0) {
 #pragma unroll
-    for (int i = 0; i < 8; i++) {
+    for (int i = 0; i < AR; i++) {
       const int r = m.row(i);
 #pragma unroll
-      for (int j = 0; j < 8; j++) {
+      for (int j = 0; j < AC; j++) {
         const int c = m.col(j);
         float wab = 0.f;
 #pragma unroll
@@ -510,9 +537,9 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a) {
 struct AtomSmemBwd {
   static constexpr int kP = 32;
   static constexpr int kH = kP + TM * LD;
-  static constexpr int kWt = kH + TM * LD;     // gwab tile [TM][LDA]
-  static constexpr int kW = kWt + TM * LDA;
-  static constexpr int kBe = kW + 8192;
+  static constexpr int kGw = kH + TM * LD;     // dE/dw_ab . W_ab per (row, radial k) [TM][12]
+  static constexpr int kW = kGw + TM * 12;     // wgmma images of W2 / W2^T (2 branches x hi | lo)
+  static constexpr int kBe = kW + 16384;
   static constexpr int kDbe = kBe + TM * 12;
   static constexpr int kWab = kDbe + TM * 12;
   static constexpr int kM = kWab + 576;
@@ -528,7 +555,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);
   float* tileP = smem + AtomSmemBwd::kP;
   float* tileH = smem + AtomSmemBwd::kH;
-  float* tileW = smem + AtomSmemBwd::kWt;
+  float* gws = smem + AtomSmemBwd::kGw;
   float* Wsm = smem + AtomSmemBwd::kW;
   float* be_s = smem + AtomSmemBwd::kBe;
   float* dbe_s = smem + AtomSmemBwd::kDbe;
@@ -567,7 +594,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   __syncthreads();
   if (tid == 0) mbar_expect_tx(mbar, (uint32_t)nvalid * 512u);
   if (tid < nvalid) bulk_g2s(tileP + tid * LD, a.Aproj + (size_t)s_src[tid] * D2, 512u, mbar);
-  stage_w(Wsm, a.W2k, 2048);
+  stage_w(Wsm, a.W2can, 4096);
   for (int i = tid; i < 576; i += NT) wabW[i] = a.Wabw[i];
   for (int i = tid; i < 1152; i += NT) Msm[i] = a.M[i];
   if (tid < 128) b2s[tid] = a.b2[tid];
@@ -607,32 +634,37 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   }
   __syncthreads();
   const Map m;
-  float acc[8][8];
+  float acc[AR][AC];
 #pragma unroll
-  for (int i = 0; i < 8; i++)
-    for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-  gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 4096, acc, m);
+  for (int i = 0; i < AR; i++)
+    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+  gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
 #pragma unroll
-  for (int i = 0; i < 8; i++)
+  for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int j = 0; j < 8; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];  // u (L) / v (G)
+    for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];  // u (L) / v (G)
   __syncthreads();  // hid + W2k no longer needed
   // exchange activations between the two branches through tileH
 #pragma unroll
-  for (int i = 0; i < 8; i++)
+  for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const float u = acc[i][j];
       tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
     }
-  stage_w(Wsm, a.W2raw, 2048);
+  stage_w(Wsm, a.W2Tcan, 4096);
   __syncthreads();
+  float gw[AR][9];  // branch 0: this thread's columns of sum_c dE/dw_ab[r][c] W_ab[c][k]
 #pragma unroll
-  for (int i = 0; i < 8; i++) {
+  for (int i = 0; i < AR; i++)
+#pragma unroll
+    for (int k = 0; k < 9; k++) gw[i][k] = 0.f;
+#pragma unroll
+  for (int i = 0; i < AR; i++) {
     const int r = m.row(i);
     const int dst = s_dst[r];
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const int c = m.col(j);
       const float u = acc[i][j];
       const float po = tileH[r * LD + (1 - m.branch) * 64 + c];  // partner activation
@@ -645,33 +677,44 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
         if (m.branch == 0) {
           const float s = sigm(u);
           const float oL = u * s;
-          tileW[r * LDA + c] = gm * oL * po;                 // d/d w_ab
+          const float gwv = gm * oL * po;                    // d/d w_ab
+#pragma unroll
+          for (int k = 0; k < 9; k++) gw[i][k] = fmaf(gwv, wabW[c * 9 + k], gw[i][k]);
           g = gm * po * wab * (s * (1.f + u * (1.f - s)));    // d/du
         } else {
           const float oG = sigm(u);
           g = gm * po * wab * oG * (1.f - oG);               // d/dv
         }
-      } else if (m.branch == 0) {
-        tileW[r * LDA + c] = 0.f;
       }
       acc[i][j] = g;
     }
   }
+  if (m.branch == 0) {  // the four lanes l/4 = const of a warp own one row's 64 columns
+#pragma unroll
+    for (int i = 0; i < AR; i++)
+#pragma unroll
+      for (int k = 0; k < 9; k++) {
+        float v = gw[i][k];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        if ((threadIdx.x & 3) == 0) gws[m.row(i) * 12 + k] = v;
+      }
+  }
   __syncthreads();
 #pragma unroll
-  for (int i = 0; i < 8; i++)
+  for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int j = 0; j < 8; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+    for (int j = 0; j < AC; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
   __syncthreads();
   // ghid = [gu @ W2L, gv @ W2G];  gpre = ghid * dsilu(pre)
 #pragma unroll
-  for (int i = 0; i < 8; i++)
-    for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-  gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 4096, acc, m);
+  for (int i = 0; i < AR; i++)
+    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+  gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
 #pragma unroll
-  for (int i = 0; i < 8; i++)
+  for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
       tileP[idx] = acc[i][j] * dsilu_f(tileP[idx]);
     }
@@ -684,8 +727,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
       const int k0 = kh ? 5 : 0, k1 = kh ? 9 : 5;
       const bool viaM = !(useQ && s_bond[r] >= 0);
       for (int k = k0; k < k1; k++) {
-        float s = 0.f;
-        for (int c = 0; c < 64; c++) s = fmaf(tileW[r * LDA + c], wabW[c * 9 + k], s);
+        float s = gws[r * 12 + k];
         if (viaM)
           for (int j = 0; j < 128; j++) s = fmaf(tileP[r * LD + j], Msm[j * 9 + k], s);
         part = fmaf(s, dbe_s[r * 12 + k], part);
@@ -728,13 +770,13 @@ void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a) {
 // ============================================================================================
 struct LineSmem {
   static constexpr int kP = 32;
-  static constexpr int kAng = kP + TM * LD;
-  static constexpr int kW = kAng + TM * LDA;
-  static constexpr int kB2 = kW + 8192;
+  static constexpr int kAng = kP + TM * LD;   // [TM][LDA] angle rows; the backward's tileH [TM][LD] aliases them
+  static constexpr int kH = kAng;             // (backward only, first written after the angle rows have been read)
+  static constexpr int kW = kAng + TM * LD;   // wgmma images of the weights (2 branches x hi | lo, or Wg^T hi | lo)
+  static constexpr int kB2 = kW + 16384;
   static constexpr int kIdx = kB2 + 128;
   static constexpr int kFwdTotal = kIdx + 3 * TM;
-  static constexpr int kH = kFwdTotal;  // backward only
-  static constexpr int kBwdTotal = kH + TM * LD;
+  static constexpr int kBwdTotal = kFwdTotal;
   static constexpr size_t fwd_bytes = (size_t)kFwdTotal * 4;
   static constexpr size_t bwd_bytes = (size_t)kBwdTotal * 4;
 };
@@ -775,7 +817,7 @@ __device__ __forceinline__ int line_prologue(const LineArgs& a, float* smem, int
     for (int k = 0; k < 64; k++) angT[tid * LDA + k] = 0.f;
     for (int k = 0; k < 128; k++) tileP[tid * LD + k] = 0.f;
   }
-  stage_w(Wsm, a.Wgk, 2048);
+  stage_w(Wsm, a.Wgcan, 4096);
   if (tid < 128) b2s[tid] = a.b2 ? a.b2[tid] : 0.f;
   mbar_wait(mbar, 0);
   __syncthreads();
@@ -796,17 +838,17 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
   const int nvalid = line_prologue(a, smem, r0);
   (void)s_a;
   const Map m;
-  float acc[8][8];
+  float acc[AR][AC];
 #pragma unroll
-  for (int i = 0; i < 8; i++)
-    for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-  gemm64(angT, LDA, 0, Wsm + m.branch * 4096, acc, m);
+  for (int i = 0; i < AR; i++)
+    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+  gemm64(angT, LDA, 0, Wsm + m.branch * 8192, acc);
 #pragma unroll
-  for (int i = 0; i < 8; i++) {
+  for (int i = 0; i < AR; i++) {
     const int r = m.row(i);
     const int ib = s_b[r], ic = s_c[r];
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const int col = m.branch * 64 + m.col(j);
       float p = 0.f;
       if (r < nvalid) p = tileP[r * LD + col] + acc[i][j] + a.Hb[(size_t)ib * D2 + col] + a.Xc[(size_t)ic * D2 + col];
@@ -819,16 +861,16 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
   }
   __syncthreads();
   if (HIDDEN) {
-    stage_w(Wsm, a.W2k, 2048);
+    stage_w(Wsm, a.W2can, 4096);
     __syncthreads();
 #pragma unroll
-    for (int i = 0; i < 8; i++)
-      for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-    gemm64(tileP, LD, m.branch * 64, Wsm + m.branch * 4096, acc, m);
+    for (int i = 0; i < AR; i++)
+      for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+    gemm64(tileP, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
 #pragma unroll
-    for (int i = 0; i < 8; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++) {
+      for (int j = 0; j < AC; j++) {
         const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
         acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
       }
@@ -836,18 +878,18 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
   }
   if (m.branch == 1) {
 #pragma unroll
-    for (int i = 0; i < 8; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++)
+      for (int j = 0; j < AC; j++)
         tileP[m.row(i) * LD + m.col(j)] = acc[i][j];
   }
   __syncthreads();
   if (m.branch == 0) {
 #pragma unroll
-    for (int i = 0; i < 8; i++) {
+    for (int i = 0; i < AR; i++) {
       const int r = m.row(i);
 #pragma unroll
-      for (int j = 0; j < 8; j++) {
+      for (int j = 0; j < AC; j++) {
         const int c = m.col(j);
         const float mv = acc[i][j] * tileP[r * LD + c];
         if (HIDDEN) {
@@ -880,17 +922,18 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
   const int64_t r0 = (int64_t)blockIdx.x * TM;
   const int nvalid = line_prologue(a, smem, r0);
   const Map m;
-  float acc[8][8];
+  float acc[AR][AC];
 #pragma unroll
-  for (int i = 0; i < 8; i++)
-    for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-  gemm64(angT, LDA, 0, Wsm + m.branch * 4096, acc, m);
+  for (int i = 0; i < AR; i++)
+    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+  gemm64(angT, LDA, 0, Wsm + m.branch * 8192, acc);
+  __syncthreads();  // both warpgroups have read the angle rows: tileH (aliasing them) may be written
 #pragma unroll
-  for (int i = 0; i < 8; i++) {
+  for (int i = 0; i < AR; i++) {
     const int r = m.row(i);
     const int ib = s_b[r], ic = s_c[r];
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const int col = m.branch * 64 + m.col(j);
       float p = 0.f;
       if (r < nvalid) p = tileP[r * LD + col] + acc[i][j] + a.Hb[(size_t)ib * D2 + col] + a.Xc[(size_t)ic * D2 + col];
@@ -904,34 +947,34 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
   }
   __syncthreads();
   if (HIDDEN) {
-    stage_w(Wsm, a.W2k, 2048);
+    stage_w(Wsm, a.W2can, 4096);
     __syncthreads();
 #pragma unroll
-    for (int i = 0; i < 8; i++)
-      for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 4096, acc, m);
+    for (int i = 0; i < AR; i++)
+      for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
 #pragma unroll
-    for (int i = 0; i < 8; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
+      for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
     __syncthreads();
   }
   // acc = pre-activation of the last layer of this GatedMLP (u | v).  Exchange activations.
 #pragma unroll
-  for (int i = 0; i < 8; i++)
+  for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const float u = acc[i][j];
       tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
     }
-  if (HIDDEN) stage_w(Wsm, a.W2raw, 2048);
+  if (HIDDEN) stage_w(Wsm, a.W2Tcan, 4096);
   __syncthreads();
 #pragma unroll
-  for (int i = 0; i < 8; i++) {
+  for (int i = 0; i < AR; i++) {
     const int r = m.row(i);
     const int ib = s_b[r];
 #pragma unroll
-    for (int j = 0; j < 8; j++) {
+    for (int j = 0; j < AC; j++) {
       const int c = m.col(j);
       const float u = acc[i][j];
       const float po = tileH[r * LD + (1 - m.branch) * 64 + c];
@@ -952,56 +995,43 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
   __syncthreads();
   if (HIDDEN) {
 #pragma unroll
-    for (int i = 0; i < 8; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+      for (int j = 0; j < AC; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
     __syncthreads();
 #pragma unroll
-    for (int i = 0; i < 8; i++)
-      for (int j = 0; j < 8; j++) acc[i][j] = 0.f;
-    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 4096, acc, m);
+    for (int i = 0; i < AR; i++)
+      for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
+    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
 #pragma unroll
-    for (int i = 0; i < 8; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++) {
+      for (int j = 0; j < AC; j++) {
         const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
         tileP[idx] = acc[i][j] * dsilu_f(tileP[idx]);
       }
   } else {
 #pragma unroll
-    for (int i = 0; i < 8; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < 8; j++) tileP[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+      for (int j = 0; j < AC; j++) tileP[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
   }
   __syncthreads();
-  // gang += gpre @ Wg_raw   (K = 128, N = 64)
-  stage_w(Wsm, a.Wgraw, 2048);
+  // gang += gpre @ Wg   (K = 128, N = 64) on the tensor cores: warpgroup w takes rows 64 w .. 64 w + 63
+  stage_w(Wsm, a.WgTcan, 4096);
   __syncthreads();
   {
-    const int rg16 = tid >> 4, cg16 = tid & 15;
-    float a3[8][4];
+    float d[32];
+    const uint32_t bh = s_u32(Wsm), bl = bh + 64u * 128u * 4u;
+    wg_mm64(tileP, LD, 64 * m.branch, 0, bh, bl, 0, false, d);
+    wg_mm64(tileP, LD, 64 * m.branch, 64, bh, bl, 64, true, d);
 #pragma unroll
-    for (int i = 0; i < 8; i++)
-      for (int j = 0; j < 4; j++) a3[i][j] = 0.f;
-#pragma unroll 4
-    for (int k = 0; k < 128; k++) {
-      const float4 w = *reinterpret_cast<const float4*>(&Wsm[k * 64 + cg16 * 4]);
-#pragma unroll
-      for (int i = 0; i < 8; i++) {
-        const float av = tileP[(rg16 + 16 * i) * LD + k];
-        a3[i][0] = fmaf(av, w.x, a3[i][0]);
-        a3[i][1] = fmaf(av, w.y, a3[i][1]);
-        a3[i][2] = fmaf(av, w.z, a3[i][2]);
-        a3[i][3] = fmaf(av, w.w, a3[i][3]);
-      }
-    }
-#pragma unroll
-    for (int i = 0; i < 8; i++) {
-      const int r = rg16 + 16 * i;
+    for (int q = 0; q < 32; q += 2) {
+      const int r = 64 * m.branch + m.rb + 8 * ((q >> 1) & 1), c = 8 * (q >> 2) + m.cb;
       if (r < nvalid) {
-        float4* gp = reinterpret_cast<float4*>(&a.gang[(size_t)(r0 + r) * D + cg16 * 4]);
-        float4 v = *gp;
-        v.x += a3[i][0], v.y += a3[i][1], v.z += a3[i][2], v.w += a3[i][3];
+        float2* gp = reinterpret_cast<float2*>(&a.gang[(size_t)(r0 + r) * D + c]);
+        float2 v = *gp;
+        v.x += d[q], v.y += d[q + 1];
         *gp = v;
       }
     }
@@ -1050,7 +1080,7 @@ void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden) {
 // bond update (node-level, after the W_out GEMM):  h' = h + upd * w3b(d_b)
 // ============================================================================================
 // 128 bonds per block, 16-byte accesses: these are pure streaming kernels (300 MB per launch at 97 k atoms) and ran at a
-// third of the HBM rate with 32 bonds per block and 4-byte accesses (profiles/r02k_kernel_shares_97k.txt)
+// third of the HBM rate with 32 bonds per block and 4-byte accesses
 constexpr int BNR = 128;  // bonds per block
 template <int MODE>  // 0: fwd, 1: bwd (gupd, gdb), 2: h0 backward (gdb only)
 __global__ void __launch_bounds__(256) k_bond_node(int nb, const float4* __restrict__ b_vec, RadialParams rp,
@@ -1144,13 +1174,13 @@ void launch_h0_bwd(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp
   launch_bond_node<2>(st, nb, b_vec, rp, Wbe, gh0, nullptr, nullptr, gdb);
 }
 
-// theta / Fourier backward (128 angles per block = one tile of the interleaved layout)
+// theta / Fourier backward (128 angles per block)
 constexpr int ANR = 128;
 __global__ void __launch_bounds__(256) k_angle_init_bwd(int64_t na, const int* __restrict__ a_in,
                                                         const int* __restrict__ a_out,
                                                         const float4* __restrict__ b_vec, const float* __restrict__ fa,
                                                         const float* __restrict__ Wae, const float* __restrict__ gang0,
-                                                        float* __restrict__ gbvec, int il) {
+                                                        float* __restrict__ gbvec) {
   extern __shared__ float ab_smem[];
   float(*G)[65] = reinterpret_cast<float(*)[65]>(ab_smem);                  // [ANR][65]
   float(*gf_s)[12] = reinterpret_cast<float(*)[12]>(ab_smem + ANR * 65);    // [ANR][12]
@@ -1158,19 +1188,9 @@ __global__ void __launch_bounds__(256) k_angle_init_bwd(int64_t na, const int* _
   const int64_t r0 = (int64_t)blockIdx.x * ANR;
   const int tid = threadIdx.x;
   for (int i = tid; i < 576; i += 256) Ws[i] = Wae[i];
-  if (il) {  // tile-interleaved: float4 (c/4, row) -> consecutive lanes read consecutive rows of one column group
-    const float4* g4 = reinterpret_cast<const float4*>(gang0) + (size_t)blockIdx.x * 16 * 128;
-    for (int i = tid; i < 16 * ANR; i += 256) {
-      const int cq = i >> 7, r = i & 127;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (r0 + r < na) v = g4[i];
-      G[r][4 * cq] = v.x, G[r][4 * cq + 1] = v.y, G[r][4 * cq + 2] = v.z, G[r][4 * cq + 3] = v.w;
-    }
-  } else {
-    for (int i = tid; i < ANR * 64; i += 256) {
-      const int r = i >> 6, c = i & 63;
-      G[r][c] = (r0 + r < na) ? gang0[(size_t)(r0 + r) * 64 + c] : 0.f;
-    }
+  for (int i = tid; i < ANR * 64; i += 256) {
+    const int r = i >> 6, c = i & 63;
+    G[r][c] = (r0 + r < na) ? gang0[(size_t)(r0 + r) * 64 + c] : 0.f;
   }
   __syncthreads();
   for (int i = tid; i < ANR * 9; i += 256) {
@@ -1209,12 +1229,12 @@ __global__ void __launch_bounds__(256) k_angle_init_bwd(int64_t na, const int* _
 }
 constexpr size_t kAngleBwdSmem = (size_t)(ANR * 65 + ANR * 12 + 576) * sizeof(float);
 void launch_angle_init_bwd(cudaStream_t st, int64_t na, const int* a_in, const int* a_out, const float4* b_vec,
-                           const float* fa, const float* Wae, const float* gang0, float* gbvec, bool interleaved) {
+                           const float* fa, const float* Wae, const float* gang0, float* gbvec) {
   if (na <= 0) return;
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_)
     B2M_CK(cudaFuncSetAttribute(k_angle_init_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAngleBwdSmem));
-  k_angle_init_bwd<<<cdiv(na, ANR), 256, kAngleBwdSmem, st>>>(na, a_in, a_out, b_vec, fa, Wae, gang0, gbvec, interleaved ? 1 : 0);
+  k_angle_init_bwd<<<cdiv(na, ANR), 256, kAngleBwdSmem, st>>>(na, a_in, a_out, b_vec, fa, Wae, gang0, gbvec);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }

@@ -1,4 +1,4 @@
-// kernels.cuh -- launch-side declarations of the CHGNet hot-path kernels (sm_100a).
+// kernels.cuh -- launch-side declarations of the CHGNet hot-path kernels (sm_90a).
 //
 // Formulation (verified against autograd in oracle/manual_ref.py):
 //   first layer of every GatedMLP is split by input block, so the per-edge / per-angle work is
@@ -31,17 +31,8 @@ void launch_gemm(cudaStream_t st, const float* A, int lda, const float* B, float
 void launch_embed(cudaStream_t st, int n, const int* type, const float* emb, float* x0);
 void launch_bond_init(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp, const float* W /*[64][9]*/,
                       float* out /*[nb,64]*/);
-// Angle features (ang^l, and their adjoint gang) are touched only by the line-graph kernels, whose TMEM-imposed
-// thread = row mapping makes every 16-byte access of a row-major [A][64] tensor its own L1 wavefront (LSU 49-63 % busy,
-// profiles/r02k).  On the tcgen05 path they are therefore stored TILE-INTERLEAVED like the other kernel-private tensors:
-//   float4 index ((tile * 16 + c/4) * 128 + r), tile = row / 128, r = row % 128   (a tile is one contiguous 32 KB block)
-// The FP32-FFMA generation keeps row-major; `interleaved` selects the layout in the two kernels both paths share.
-__host__ __device__ inline size_t ang_index(int64_t row, int c, int interleaved) {
-  return interleaved ? ((size_t)((row >> 7) * 16 + (c >> 2)) * 128 + (size_t)(row & 127)) * 4 + (size_t)(c & 3)
-                     : (size_t)row * 64 + (size_t)c;
-}
 void launch_angle_init(cudaStream_t st, int64_t na, const int* a_in, const int* a_out, const float4* b_vec,
-                       const float* fa /*[5]*/, const float* Wae /*[64][9]*/, float* ang0, bool interleaved);
+                       const float* fa /*[5]*/, const float* Wae /*[64][9]*/, float* ang0 /*[A,64]*/);
 void launch_silu(cudaStream_t st, int64_t n, const float* pre, float* out);
 void launch_dsilu_mul(cudaStream_t st, int64_t n, const float* pre, float* g);  // g *= dsilu(pre)
 void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats);
@@ -57,8 +48,10 @@ struct AtomConvArgs {
   const float* Cproj;  // [n_own,128]  x @ W1t^T + b1
   const float* Qproj;  // [B_own,128]  h @ W1e^T   (nullptr for layer 0)
   const float* M;      // [128][9]     W1e @ W_be
-  const float* W2k;    // [2][64][64]  k-major second layers (L then G)
-  const float* W2raw;  // [2][64][64]  as stored [out][in] (backward)
+  // second layers (L then G) as wgmma B operands: per branch the canonical K-major core-matrix image of a [64 n][64 k]
+  // matrix, tf32 hi plane then lo plane (8192 floats per branch; engine.cu canon_split)
+  const float* W2can;   // B[n][k] = W2[n][k]   (forward: hid . W2^T)
+  const float* W2Tcan;  // B[n][k] = W2[k][n]   (backward: g . W2)
   const float* b2;     // [128]
   const float* Wabw;   // [64][9]
   RadialParams rp;
@@ -70,13 +63,7 @@ struct AtomConvArgs {
   float* gC;          // [n_own,128] (+=)
   float* gQ;          // [B_own,128] (=)
   float* gd;          // [E] (+=)
-  // tcgen05 path: second-layer pre-activations (u | v) saved by the forward for the backward
-  float* uv_save;       // [E,128] or nullptr (forward)
-  const float* uv;      // [E,128] (backward)
-  const float* be;      // [E,12] radial basis (9 used), computed once per step by launch_edge_basis
-  const float* dbe;     // [E,12] d(be)/dd
 };
-void launch_edge_basis(cudaStream_t st, int64_t E, const float4* e_vec, RadialParams rp, float* be, float* dbe);
 void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a);
 void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a);
 
@@ -90,10 +77,11 @@ struct LineArgs {
   const float* Ha;    // [B_loc,128]
   const float* Hb;    // [B_own,128] (+bias folded)
   const float* Xc;    // [n_loc,128]
-  const float* Wgk;   // [2][64][64] k-major angle block of the first layer
-  const float* Wgraw; // [128][64]   as stored (backward)
-  const float* W2k;   // hidden only
-  const float* W2raw;
+  // wgmma B operands (canonical core-matrix images, tf32 hi plane then lo plane; engine.cu canon_split)
+  const float* Wgcan;   // per branch [64 n][64 k]: B[n][k] = Wg[br*64 + n][k]  (angle block of the first layer)
+  const float* WgTcan;  // [64 n][128 k]: B[n][k] = Wg[k][n]                     (backward: gang += gpre . Wg)
+  const float* W2can;   // hidden only, as AtomConvArgs
+  const float* W2Tcan;
   const float* b2;
   // forward outputs
   float* aggB;     // HIDDEN: [B_own,64] (+=)
@@ -104,11 +92,6 @@ struct LineArgs {
   float* gHa;          // [B_loc,128] (+=)
   float* gHb;          // [B_own,128] (+=)
   float* gXc;          // [n_loc,128] (+=)
-  // tcgen05 path: tensors saved by the forward for the backward
-  float* uv_save;       // [A,128] last-layer pre-activations (u | v)
-  float* ds_save;       // [A,128] silu'(first-layer pre-activation)   (HIDDEN only)
-  const float* uv;
-  const float* ds;
 };
 void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden);
 void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden);
@@ -124,7 +107,7 @@ void launch_h0_bwd(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp
                    float* gdb);
 // theta / Fourier backward: gbvec[a], gbvec[b] += ...
 void launch_angle_init_bwd(cudaStream_t st, int64_t na, const int* a_in, const int* a_out, const float4* b_vec,
-                           const float* fa, const float* Wae, const float* gang0, float* gbvec, bool interleaved);
+                           const float* fa, const float* Wae, const float* gang0, float* gbvec);
 
 // -------- readout --------
 // e_atom = y2 @ F2 + c2 (+elem ref); energy (double) += sum; site = x @ Ws + bs
@@ -148,22 +131,11 @@ void launch_scatter_add_rows(cudaStream_t st, int n, int width, const int* idx, 
 }  // namespace b2m
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 (5th-gen tensor core) variants.  3xTF32 split (hi*hi + lo*hi + hi*lo, fp32 accumulate in
-// TMEM) keeps fp32-level accuracy.  Weights are pre-formatted on the host into the canonical
-// K-major / no-swizzle core-matrix layout (8 rows x 16 B), hi and lo planes (see engine.cu: canon()).
+// Row GEMMs on the Hopper tensor cores (kernels_wg.cu, wgmma).  3xTF32 split (hi*hi + lo*hi + hi*lo, fp32 accumulate)
+// keeps fp32-level accuracy.  Weights are pre-formatted on the host into the canonical K-major / no-swizzle
+// core-matrix layout (8 rows x 16 B), hi and lo planes (see engine.cu: canon_split()).
 // ---------------------------------------------------------------------------------------------
 namespace b2m {
-struct AtomConvTcW {
-  const float* W2can;   // [4][4096]: W2L hi, W2L lo, W2G hi, W2G lo   (N=64, K=64)
-  const float* Mcan;    // [2][2048]: M hi, M lo                        (N=128, K=16; k>=9 zero)
-  const float* W2Tcan;  // [4][4096]: W2L^T hi, lo, W2G^T hi, lo        (backward: ghid = g . W2)
-  int l2pf = 0;         // set by the launcher: prefetch the next tile's streamed blocks into L2
-};
-void launch_atomconv_fwd_tc(cudaStream_t st, const AtomConvArgs& a, const AtomConvTcW& w, int num_sms);
-void launch_atomconv_bwd_tc(cudaStream_t st, const AtomConvArgs& a, const AtomConvTcW& w, int num_sms);
-// third generation (kernels_ac3.cu): cp.async-staged gathers one tile ahead, no saved pre-activations unless uv_save
-void launch_atomconv_fwd_v3(cudaStream_t st, const AtomConvArgs& a, const AtomConvTcW& w, int num_sms);
-void launch_atomconv_bwd_v3(cudaStream_t st, const AtomConvArgs& a, const AtomConvTcW& w, int num_sms);
 // C[M,N] = (R | accum C | 0) + A[M,K] @ B + bias, B given as canonical hi/lo planes of its [N][K] view.
 // (K,N) in {(64,128), (64,64), (128,64)}.
 void launch_gemm_tc(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N,
@@ -173,15 +145,6 @@ void launch_gemm_tc(cudaStream_t st, const float* A, int lda, const float* Bcan,
 void launch_gemm_tc_epi(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N,
                         int K, const float* bias, bool accum, int epi, float* Cpre, const float* Pre, int ldp,
                         int num_sms);
-struct LineTcW {
-  const float* Wgcan;   // [2][8192]: first-layer angle block (N=128, K=64) hi, lo
-  const float* W2can;   // [4][4096]: second layers (HIDDEN)
-  const float* W2Tcan;  // [4][4096]: transposed second layers (HIDDEN, backward)
-  const float* WgTcan;  // [4][4096]: per branch (N=64 angle cols, K=64 first-layer cols): L hi, L lo, G hi, G lo
-  int l2pf = 0;         // set by the launcher: prefetch the next tile's streamed blocks into L2
-};
-void launch_line_fwd_tc(cudaStream_t st, const LineArgs& a, const LineTcW& w, bool hidden, int num_sms);
-void launch_line_bwd_tc(cudaStream_t st, const LineArgs& a, const LineTcW& w, bool hidden, int num_sms);
 }  // namespace b2m
 
 // ---------------------------------------------------------------------------------------------

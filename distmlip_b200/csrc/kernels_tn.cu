@@ -10,7 +10,7 @@
 // element-wise tensor algebra is one thread per (atom, channel), coalesced over channels; aggregations walk the
 // CSR-by-destination rows (no atomics in the forward); the reverse pass scatters to sources with red.add.
 // First generation of this path.  The edge-level products (edge MLP 32 -> 64 -> 128 -> 192 and the three distance
-// projections, 49 % of a step) run on the tcgen05 row GEMM of the CHGNet path (kernels_tc.cu, k_gemm_tc_pipe with a
+// projections) run on the wgmma row GEMM of the CHGNet path (kernels_wg.cu, k_gemm_wg with a
 // SiLU / SiLU' epilogue; engine_tn.inl composes the 192-wide layers from its 64/128 shapes); the node-level products
 // (channel mixes, scalar MLPs, readout) use the FP32-FFMA tile kernel below, which also serves the edge level under
 // B2M_TN_FFMA=1 (A/B checks).  DESIGN.md 8 lists what comes next.

@@ -20,7 +20,7 @@ class EngineBackedModel:
     def from_existing(cls, model, dtype=distmlip_b200.float_th):
         """chgnet.py:551-560 / tensornet.py:206-217: takes the matgl model (any nn.Module with that attribute tree)."""
         if dtype not in (torch.float, torch.float32):
-            raise ValueError("the sm_100a engine computes in fp32 only")
+            raise ValueError("the sm_90a engine computes in fp32 only")
         model.to("cpu")
         dist_model = cls.__new__(cls)
         dist_model.__dict__ = model.__dict__.copy()

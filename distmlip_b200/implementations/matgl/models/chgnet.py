@@ -25,7 +25,7 @@ from ._base import EngineBackedModel
 
 
 class CHGNet_Dist(EngineBackedModel):
-    """Main CHGNet model (B200 engine behind the reference's wrapper API)."""
+    """Main CHGNet model (H100 engine behind the reference's wrapper API)."""
 
     __version__ = 1
     _has_site = True

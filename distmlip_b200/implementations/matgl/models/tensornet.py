@@ -22,7 +22,7 @@ from ._base import EngineBackedModel
 
 
 class TensorNet_Dist(EngineBackedModel):
-    """TensorNet model (B200 engine behind the reference's wrapper API)."""
+    """TensorNet model (H100 engine behind the reference's wrapper API)."""
 
     __version__ = 1
 

@@ -1,5 +1,5 @@
 /*
- * b200mlip.h -- C-ABI of libb200mlip.so: the B200-native (sm_100a) engine behind the
+ * b200mlip.h -- C-ABI of libb200mlip.so: the H100-native (sm_90a) engine behind the
  * DistMLIP-compatible CHGNet hot path.  Plain C, no CPython / NumPy / torch types.
  *
  * What each entry point replaces in the reference (AegisIK/DistMLIP @ 9824cd4):
@@ -125,6 +125,9 @@ int b2m_compute(b2m_handle h, int want_forces, int want_stress, double* energy, 
 /* Same arithmetic, graph already resident; runs `reps` passes and returns device time (ms) of
  * the last one measured with CUDA events on the compute stream. Used by bench.py `value`. */
 int b2m_compute_resident(b2m_handle h, int want_forces, int want_stress, int reps, double* energy, float* ms);
+/* Results of the last evaluation (b2m_compute or b2m_compute_resident) without running another one: energy,
+ * forces [natoms][3] and stress [3][3] (GPa), as b2m_compute returns them; any pointer may be NULL. */
+int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9);
 
 /* site-wise readout (magmom) for all atoms, [natoms] */
 int b2m_get_sitewise(b2m_handle h, float* out);

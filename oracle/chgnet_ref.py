@@ -7,11 +7,11 @@ Pure-PyTorch (CPU) restatement of the arithmetic behind the reference's CHGNet h
                                                  DistMLIP/implementations/matgl/pes.py:50-146
                                                  DistMLIP/distributed/dist.py:277-358, 635-702
   layer internals ............................... matgl @ git 5171392 (pyproject.toml:26-28), NOT in
-                                                 /root/reference and NOT installable here (no network):
+                                                 the reference repository and not installed with it:
                                                  restated from SURVEY.md §9 "(RECALLED-matgl)".
 
 PARITY UNPINNED: the reference ships no tests / golden vectors for the model arithmetic and
-matgl+dgl cannot be imported in this image, so nothing in this file has been checked against a
+matgl+dgl are not available to the tests, so nothing in this file has been checked against a
 run of the real reference.  What *is* pinned: the graph side (oracle/graph_ref.py vs oracle/_ref).
 
 The module's attribute tree and state_dict keys mirror matgl's `CHGNet` (SURVEY.md §8c) so that

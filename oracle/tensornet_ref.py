@@ -8,12 +8,12 @@ Pure-PyTorch (CPU) restatement of the arithmetic behind the reference's TensorNe
                                                  `matgl.layers.TensorEmbedding`, `TensorNetInteraction`, `BondExpansion`,
                                                  `WeightedReadOut`, `matgl.utils.maths.{decompose_tensor, tensor_norm,
                                                  vector_to_skewtensor, vector_to_symtensor}`, `matgl.utils.cutoff.
-                                                 cosine_cutoff` -- NOT in /root/reference and NOT installable here:
+                                                 cosine_cutoff` -- NOT in the reference repository:
                                                  restated from memory of that code ("RECALLED-matgl"), which itself
                                                  follows the published TensorNet architecture (Simeon & De Fabritiis 2023).
 
-PARITY UNPINNED: the reference ships no tests / golden vectors for the model arithmetic and matgl + dgl cannot be
-imported in this image (profiles/r02_reference_deps_probe.txt), so nothing in this file has been checked against a run
+PARITY UNPINNED: the reference ships no tests / golden vectors for the model arithmetic and matgl + dgl are not
+available to the tests, so nothing in this file has been checked against a run
 of the real reference.
 
 The attribute tree and `state_dict` keys mirror matgl's `TensorNet` as `TensorNet_Dist.enable_distributed_mode`

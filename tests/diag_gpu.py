@@ -1,5 +1,5 @@
 """Stage-by-stage GPU diagnostic (not a pytest file): prints max errors of every tap vs the oracle.
-Usage on the GPU box:  python tests/diag_gpu.py [ncells]"""
+Usage on a GPU machine:  python tests/diag_gpu.py [ncells]"""
 import os
 import sys
 

@@ -1,11 +1,12 @@
-"""Generates tests/golden/graph_golden.json from the reference's own C graph builder (oracle/_ref,
-compiled from /root/reference by oracle/Makefile).  Run in the build container:
+"""Generates tests/golden/graph_golden.json and tests/golden/live_reference.json from the reference's own C graph
+builder (oracle/_ref, compiled from the reference sources by oracle/Makefile; REF=<reference checkout>):
 
-    make -C oracle && python tests/golden/make_golden.py
+    make -C oracle REF=<reference checkout> && python tests/golden/make_golden.py
 
-Each case stores order-independent integer digests of what get_subgraphs_fast returned
-(subgraph_creation_fast.c:403-422), so the numpy restatement (oracle/graph_ref.py) and the CUDA graph
-builder can be checked without the reference being present (it does not exist on the GPU box).
+Each case of graph_golden.json stores order-independent integer digests of what get_subgraphs_fast returned
+(subgraph_creation_fast.c:403-422); live_reference.json stores ORDER-dependent digests of the sorted edge list and of
+the partition lists, and a seeded sample of the distances.  The numpy restatement (oracle/graph_ref.py) and the CUDA
+graph builder are checked against these without the reference being present.
 """
 import json
 import os
@@ -85,8 +86,40 @@ def describe(atoms, P):
     return d
 
 
+def ordered_digest(x):
+    """digest that also pins the order of the rows"""
+    x = np.asarray(x, dtype=np.int64)
+    if x.size == 0:
+        return digest(x)
+    x = x.reshape(len(x), -1)
+    return digest(np.column_stack([np.arange(len(x)), x]))
+
+
+def live_case():
+    """what tests/test_oracle.py::test_graph_oracle_matches_live_reference compares: 2016 atoms, two slabs"""
+    atoms = si_diamond(6, nz=7, seed=11)
+    cart, lat, pbc = atoms.get_positions(), atoms.get_cell(), atoms.get_pbc().astype(np.int64)
+    t = G.ref_get_subgraphs(cart, atoms.get_scaled_positions(wrap=True), lat, pbc, 2, 5.0, 3.0, True)
+    c = G.canon_from_ref_tuple(t, 2)
+    order = np.lexsort((c["off"][:, 2], c["off"][:, 1], c["off"][:, 0], c["i2"], c["i1"]))
+    i1, i2, off, dist = c["i1"][order], c["i2"][order], c["off"][order], c["dist"][order]
+    sample = np.sort(np.random.default_rng(0).choice(len(dist), size=min(500, len(dist)), replace=False))
+    d = {"edges": ordered_digest(np.column_stack([i1, i2, off])), "dist_index": sample.tolist(),
+         "dist": [float(x) for x in dist[sample]], "parts": []}
+    for p in range(2):
+        part = c["parts"][p]
+        d["parts"].append({"to": [ordered_digest(part["to"][q]) for q in range(2)],
+                           "from": [ordered_digest(part["from"][q]) for q in range(2)],
+                           "edges": ordered_digest(np.column_stack(part["edges"][:2])),
+                           "n_angles": int(len(part["line_src"]))})
+    return d
+
+
 if __name__ == "__main__":
+    here = os.path.dirname(os.path.abspath(__file__))
     res = {k: describe(a, P) for k, (a, P) in cases().items()}
-    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "graph_golden.json"), "w") as f:
+    with open(os.path.join(here, "graph_golden.json"), "w") as f:
         json.dump(res, f, indent=1)
     print({k: (v["natoms"], v["edges"][0]) for k, v in res.items()})
+    with open(os.path.join(here, "live_reference.json"), "w") as f:
+        json.dump(live_case(), f)

@@ -1,8 +1,8 @@
 """CPU-side checks of bench.py's output contract (no GPU): the reference arm's JSON line and the clock sampler.
 
-The product arm needs a B200 and is exercised by the driver; what can be pinned here is that the reference arm
-(`--impl reference`, which times the reference's C graph builder from oracle/_ref plus the CPU restatement) prints one
-JSON line with every key the driver reads, and that the nvidia-smi sampler keeps only rows inside the timed window.
+The product arm needs an H100; what can be pinned here is that the reference arm (`--impl reference`, which times the
+reference's C graph builder from oracle/_ref, or its numpy restatement where that is not built, plus the CPU
+restatement of the model) prints one JSON line with every key a reader of the results uses, and that the nvidia-smi sampler keeps only rows inside the timed window.
 """
 import json
 import os

@@ -1,4 +1,4 @@
-"""N>1 on real GPUs: only runs where at least two B200s are visible (skipped on the 1-GPU box)."""
+"""N>1 on real GPUs: only runs where at least two H100s are visible (skipped with one GPU)."""
 import os
 import subprocess
 import sys

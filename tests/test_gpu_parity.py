@@ -1,4 +1,4 @@
-"""GPU parity tests (run with `-m gpu` on a B200): the CUDA path through the C-ABI vs the oracle.
+"""GPU parity tests (run with `-m gpu` on an H100): the CUDA path through the C-ABI vs the oracle.
 
 Tolerances: BASELINE.json's north_star asks for 1e-4 eV/atom and 1e-3 eV/A; with random-init weights the
 forces are ~1e-2 eV/A, so the tests hold the engine to much tighter bounds (fp32 round-off level):
@@ -64,9 +64,9 @@ def test_energy_forces_stress_match_oracle(eng, model, n):
 
 
 def test_many_tiles_per_cta_match_oracle(eng, model):
-    """8 000 atoms = 1 750 edge tiles and 750 angle tiles: every persistent CTA (grid = 2 x 148) runs 5-6 tiles, so the
-    mbarrier phase flips, the TMEM reuse across tiles and the destination runs that straddle tile boundaries are checked
-    against the oracle directly (not only through self-consistency properties)."""
+    """8 000 atoms = 1 750 edge tiles and 750 angle tiles, several per SM, so the reuse of shared-memory stages across
+    tiles and the destination runs that straddle tile boundaries are checked against the oracle directly (not only
+    through self-consistency properties)."""
     atoms = si_diamond(10, seed=31)
     check_vs_oracle(eng, model, atoms)
     c = eng.counts()
@@ -309,8 +309,8 @@ def test_axis_permutation_symmetry(eng, model):
 
 
 # ------------------------------------------------------------------ the two kernel generations agree on the device
-def test_tcgen05_and_ffma_paths_agree(model):
-    """default path = tcgen05 (3xTF32 in TMEM); B2M_LEGACY_FFMA=1 selects the FP32-FFMA tile kernels."""
+def test_wgmma_and_ffma_row_gemms_agree(model):
+    """default path = row GEMMs on wgmma (3xTF32); B2M_LEGACY_FFMA=1 selects the FP32-FFMA GEMM tiles."""
     atoms = si_diamond(4, seed=23)
     old = os.environ.get("B2M_LEGACY_FFMA")
     try:

@@ -1,6 +1,6 @@
 """CPU tests that pin the oracle (test infrastructure) before anything is checked against it:
   * oracle/graph_ref.py  == committed golden digests generated from the reference's own C code
-  * oracle/graph_ref.py  == the live compiled reference (oracle/_ref) when it is present
+  * oracle/graph_ref.py  == order-dependent digests of the compiled reference's output on one more cell
   * oracle/manual_ref.py (factorised forward + hand-derived backward) == autograd of chgnet_ref.py
 """
 import json
@@ -35,29 +35,25 @@ def test_graph_oracle_matches_golden(name):
 
 
 def test_graph_oracle_matches_live_reference():
-    if G.load_ref_extension() is None:
-        if os.path.isdir("/root/reference/DistMLIP/distributed"):
-            import subprocess
-            subprocess.run(["make", "-C", os.path.join(os.path.dirname(HERE), "oracle")], check=True)
-        else:
-            pytest.skip("oracle/_ref not built and /root/reference absent")
+    """the reference's own C graph builder on a 2016-atom cell, two slabs: its sorted edge list, distances and partition
+    lists as stored in tests/golden/live_reference.json (tests/golden/make_golden.py)"""
+    from tests.golden.make_golden import ordered_digest
+
+    ref = json.load(open(os.path.join(HERE, "golden", "live_reference.json")))
     atoms = si_diamond(6, nz=7, seed=11)
     cart, lat, pbc = atoms.get_positions(), atoms.get_cell(), atoms.get_pbc().astype(np.int64)
-    t = G.ref_get_subgraphs(cart, atoms.get_scaled_positions(wrap=True), lat, pbc, 2, 5.0, 3.0, True)
-    c = G.canon_from_ref_tuple(t, 2)
     o = G.GraphOracle(cart, lat, pbc, 2, 5.0, 3.0, True)
-    order = np.lexsort((c["off"][:, 2], c["off"][:, 1], c["off"][:, 0], c["i2"], c["i1"]))
-    assert np.array_equal(o.i1, c["i1"][order]) and np.array_equal(o.i2, c["i2"][order])
-    assert np.array_equal(o.off, c["off"][order])
-    assert np.allclose(np.sqrt(o.d2), c["dist"][order], atol=1e-12)
+    assert ordered_digest(np.column_stack([o.i1, o.i2, o.off])) == ref["edges"]
+    idx = np.asarray(ref["dist_index"])
+    assert np.allclose(np.sqrt(o.d2)[idx], np.asarray(ref["dist"]), atol=1e-12)
     for p in range(2):
-        part = c["parts"][p]
+        part = ref["parts"][p]
         for q in range(2):
-            assert np.array_equal(part["to"][q], o.to_list(p, q))
-            assert np.array_equal(part["from"][q], o.from_list(p, q))
+            assert ordered_digest(o.to_list(p, q)) == part["to"][q]
+            assert ordered_digest(o.from_list(p, q)) == part["from"][q]
         s, d, of = o.edges_of(p)
-        assert np.array_equal(s, part["edges"][0]) and np.array_equal(d, part["edges"][1])
-        assert len(o.angles_of(p)) == len(part["line_src"])
+        assert ordered_digest(np.column_stack([s, d])) == part["edges"]
+        assert len(o.angles_of(p)) == part["n_angles"]
 
 
 def test_reference_rejects_thin_slabs_and_so_does_oracle():
