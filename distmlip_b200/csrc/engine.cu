@@ -684,7 +684,7 @@ static void atom_layer_fwd(b2m_engine* e, int l) {
   B2M_CK(cudaEventCreate(&e0));
   B2M_CK(cudaEventCreate(&e1));
   B2M_CK(cudaEventRecord(e0, e->st));
-  launch_atomconv_fwd(e->st, a);
+  launch_atomconv_fwd(e->st, a, e->num_sms);
   B2M_CK(cudaEventRecord(e1, e->st));
   e->gather_ev.push_back({e0, e1});
   gemm(e, e->agg.p, D, w.Wout_k, e->x[l + 1].p, D, g.n_own, D, D, nullptr, e->x[l].p, D, false);
@@ -704,7 +704,7 @@ static void atom_layer_bwd(b2m_engine* e, int l) {
     launch_zero_rows(e->st, e->gC.p, (int64_t)g.n_own * D2);
     a.gA = e->gA.p, a.gC = e->gC.p, a.gQ = e->gQ.p;
   }
-  launch_atomconv_bwd(e->st, a);
+  launch_atomconv_bwd(e->st, a, e->num_sms);
   if (need_gx) {
     gemm(e, e->gA.p, D2, w.W1s_raw, e->gx.p, D, g.n_loc, D, D2, nullptr, nullptr, 0, true);
     gemm(e, e->gC.p, D2, w.W1t_raw, e->gx.p, D, g.n_own, D, D2, nullptr, nullptr, 0, true);

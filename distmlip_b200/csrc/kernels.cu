@@ -4,6 +4,8 @@
 #include "kernels.cuh"
 #include "wgmma.cuh"
 
+#include <algorithm>
+
 namespace b2m {
 
 std::atomic<long long> g_launch_count{0};
@@ -52,6 +54,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "r"(addr), "r"(parity)
         : "memory");
   } while (!ok);
+}
+// a double-buffered stage: tile number `it` of a CTA sits in buffer it & 1, whose mbarrier completes one phase per fill,
+// so that tile's consumer waits on parity (it >> 1) & 1
+__device__ __forceinline__ uint32_t stage_parity(int it) { return (uint32_t)(it >> 1) & 1u; }
+// one thread: a weight image (bytes a multiple of 16 KB) as 16 KB bulk copies completing on `bar`
+__device__ __forceinline__ void bulk_g2s_image(float* dst, const float* src, uint32_t bytes, uint64_t* bar) {
+  mbar_expect_tx(bar, bytes);
+  for (uint32_t o = 0; o < bytes; o += 16384u) bulk_g2s(dst + o / 4, src + o / 4, 16384u, bar);
 }
 
 __device__ __forceinline__ float ipowf(float x, int n) {
@@ -384,149 +394,210 @@ void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats) {
 }
 
 // ============================================================================================
-// atom conv: forward
+// atom conv: shared pieces of the persistent forward and backward
 // ============================================================================================
-struct AtomSmemFwd {
-  static constexpr int kTile = 32;  // float offset of tile (128 B for the mbarrier)
-  static constexpr int kW = kTile + TM * LD;      // wgmma images of W2 (2 branches x hi | lo)
-  static constexpr int kBe = kW + 16384;
-  static constexpr int kWab = kBe + TM * 12;
-  static constexpr int kB2 = kWab + 576;
-  static constexpr int kD = kB2 + 128;
-  static constexpr int kIdx = kD + TM;
-  static constexpr int kTotal = kIdx + 3 * TM;
-  static constexpr size_t bytes = (size_t)kTotal * 4;
+// Both kernels run one CTA per SM (grid = min(tiles, SMs)); CTA c takes tiles c, c + grid, c + 2 grid, ...  Every
+// tile's A[src] rows arrive by per-row bulk copies into one of two [TM][LD] buffers, tile number `it` of the CTA in
+// buffer it & 1 (its mbarrier: stage_parity(it)).  The copies of tile it + 1 are issued while tile it is computed;
+// its index loads one tile earlier still, into registers (EdgeRow).
+struct EdgeRow {
+  int src, dst, bond;
+  float d;
 };
-
-__global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
-  extern __shared__ __align__(128) float smem[];
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);
-  float* tile = smem + AtomSmemFwd::kTile;
-  float* Wsm = smem + AtomSmemFwd::kW;
-  float* be_s = smem + AtomSmemFwd::kBe;
-  float* wabW = smem + AtomSmemFwd::kWab;
-  float* b2s = smem + AtomSmemFwd::kB2;
-  float* s_d = smem + AtomSmemFwd::kD;
-  int* s_src = reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx);
-  int* s_dst = s_src + TM;
-  int* s_bond = s_dst + TM;
-
+__device__ __forceinline__ EdgeRow edge_row(const AtomConvArgs& a, int64_t e) {
+  EdgeRow r{-1, -1, -1, 1.f};
+  if (threadIdx.x < TM && e < a.E) {
+    r.src = a.e_src[e];
+    r.dst = a.e_dst[e];
+    r.bond = a.e_bond[e];
+    r.d = a.e_vec[e].w;
+  }
+  return r;
+}
+// threads 0..TM-1 publish their row of tile t (indices, distance) and start its A[src] copy into `buf`; the caller has
+// made sure, with a barrier, that nobody reads `buf` or the index arrays of this stage any more
+__device__ __forceinline__ void issue_gather(const AtomConvArgs& a, int64_t t, const EdgeRow& row, float* buf,
+                                             uint64_t* bar, int* s_src, int* s_dst, int* s_bond, float* s_d) {
   const int tid = threadIdx.x;
-  const int64_t e0 = (int64_t)blockIdx.x * TM;
-  const int nvalid = (int)min((int64_t)TM, a.E - e0);
-
+  if (tid == 0) mbar_expect_tx(bar, (uint32_t)min((int64_t)TM, a.E - t * TM) * 512u);
   if (tid < TM) {
-    int src = -1, dst = -1, bond = -1;
-    float d = 1.f;
-    if (tid < nvalid) {
-      const int64_t e = e0 + tid;
-      src = a.e_src[e];
-      dst = a.e_dst[e];
-      bond = a.e_bond[e];
-      d = a.e_vec[e].w;
-    }
-    s_src[tid] = src;
-    s_dst[tid] = dst;
-    s_bond[tid] = bond;
-    s_d[tid] = d;
+    if (s_src != nullptr) s_src[tid] = row.src;
+    s_dst[tid] = row.dst;
+    s_bond[tid] = row.bond;
+    s_d[tid] = row.d;
+    if (row.src >= 0) bulk_g2s(buf + tid * LD, a.Aproj + (size_t)row.src * D2, 512u, bar);
   }
-  if (tid == 0) {
-    mbar_init(mbar, 1);
-    fence_barrier_init();
+}
+// be_k(d_r) (and d be_k / dd) of the tile's rows, both warpgroups (rows r, radial halves)
+__device__ __forceinline__ void radial_rows(const AtomConvArgs& a, const float* s_d, int nvalid, float* be_s,
+                                            float* dbe_s) {
+  const int r = threadIdx.x & 127, half = threadIdx.x >> 7;
+  const float d = s_d[r];
+  const int k0 = half ? 5 : 0, k1 = half ? 9 : 5;
+  for (int k = k0; k < k1; k++) {
+    float be = 0.f, dbe = 0.f;
+    if (r < nvalid) rbf_env_k(d, a.rp.freq[k], a.rp, be, dbe);
+    be_s[r * 12 + k] = be;
+    if (dbe_s != nullptr) dbe_s[r * 12 + k] = dbe;
   }
-  __syncthreads();
-  // TMA row gather: A[src] (512 B per edge) straight into the tile
-  if (tid == 0) mbar_expect_tx(mbar, (uint32_t)nvalid * 512u);
-  if (tid < nvalid) bulk_g2s(tile + tid * LD, a.Aproj + (size_t)s_src[tid] * D2, 512u, mbar);
-  stage_w(Wsm, a.W2can, 4096);
-  for (int i = tid; i < 576; i += NT) wabW[i] = a.Wabw[i];
-  if (tid < 128) b2s[tid] = a.b2[tid];
-  {
-    const int r = tid & 127, half = tid >> 7;
-    const float d = s_d[r];
-    const int k0 = half ? 5 : 0, k1 = half ? 9 : 5;
-    for (int k = k0; k < k1; k++) {
-      float be = 0.f, dbe;
-      if (r < nvalid) rbf_env_k(d, a.rp.freq[k], a.rp, be, dbe);
-      be_s[r * 12 + k] = be;
-    }
-  }
-  mbar_wait(mbar, 0);
-  __syncthreads();
-  // pre = A[src] + C[dst] + (M.be | Q[bond]);  hid = silu(pre)
-  {
-    const int j = tid & 127, rh = tid >> 7;
-    float Mj[9];
+}
+// pre[r][j] = A[src] (in the tile) + C[dst] + (Q[bond] | M.be) for this thread's column j = tid & 127 and rows
+// r = tid >> 7 + 2 i, handed to f(r, pre) (rows r >= nvalid: f(r, 0)).  The C / Q rows of 16 rows are loaded together
+// before any is used, so a thread has 32 loads in flight instead of one round trip per row.
+template <class F>
+__device__ __forceinline__ void first_layer(const AtomConvArgs& a, const float* tile, const int* s_dst,
+                                            const int* s_bond, const float* be_s, const float (&Mj)[9], int nvalid,
+                                            F&& f) {
+  const int j = threadIdx.x & 127, rh = threadIdx.x >> 7;
+  const bool useQ = a.Qproj != nullptr;
+#pragma unroll 1
+  for (int i0 = 0; i0 < 64; i0 += 16) {
+    float cv[16], qv[16];
 #pragma unroll
-    for (int k = 0; k < 9; k++) Mj[k] = a.M[j * 9 + k];
-    for (int i = 0; i < 64; i++) {
-      const int r = rh + 2 * i;
-      float v = 0.f;
+    for (int u = 0; u < 16; u++) {
+      const int r = rh + 2 * (i0 + u);
+      const int dst = s_dst[r], bond = s_bond[r];
+      cv[u] = dst >= 0 ? __ldg(&a.Cproj[(size_t)dst * D2 + j]) : 0.f;
+      qv[u] = (useQ && bond >= 0) ? __ldg(&a.Qproj[(size_t)bond * D2 + j]) : 0.f;
+    }
+#pragma unroll
+    for (int u = 0; u < 16; u++) {
+      const int r = rh + 2 * (i0 + u);
+      float p = 0.f;
       if (r < nvalid) {
-        const int dst = s_dst[r], bond = s_bond[r];
-        float t;
-        if (a.Qproj != nullptr && bond >= 0) {
-          t = a.Qproj[(size_t)bond * D2 + j];
-        } else {
+        float t = qv[u];
+        if (!(useQ && s_bond[r] >= 0)) {
           t = 0.f;
 #pragma unroll
           for (int k = 0; k < 9; k++) t = fmaf(be_s[r * 12 + k], Mj[k], t);
         }
-        v = silu_f(tile[r * LD + j] + a.Cproj[(size_t)dst * D2 + j] + t);
+        p = tile[r * LD + j] + cv[u] + t;
       }
-      tile[r * LD + j] = v;
+      f(r, p);
     }
-  }
-  __syncthreads();
-  const Map m;
-  float acc[AR][AC];
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-  gemm64(tile, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-#pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
-      acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
-    }
-  __syncthreads();
-  if (m.branch == 1) {
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int j = 0; j < AC; j++) tile[m.row(i) * LD + m.col(j)] = acc[i][j];
-  }
-  __syncthreads();
-  if (m.branch == 0) {
-#pragma unroll
-    for (int i = 0; i < AR; i++) {
-      const int r = m.row(i);
-#pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const int c = m.col(j);
-        float wab = 0.f;
-#pragma unroll
-        for (int k = 0; k < 9; k++) wab = fmaf(be_s[r * 12 + k], wabW[c * 9 + k], wab);
-        tile[r * LD + c] = acc[i][j] * tile[r * LD + c] * wab;
-      }
-    }
-  }
-  __syncthreads();
-  {
-    const int c = tid & 63, part = tid >> 6;
-    seg_flush(tile, LD, c, part * 32, part * 32 + 32, s_dst, a.agg, D);
   }
 }
 
-void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a) {
+__device__ __forceinline__ void red_add_v4(float* p, float4 v) {
+  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+               : "memory");
+}
+
+// ============================================================================================
+// atom conv: forward
+// ============================================================================================
+struct AtomSmemFwd {
+  static constexpr int kTile = 32;                  // two [TM][LD] gather buffers (first 128 B: their mbarriers)
+  static constexpr int kW = kTile + 2 * TM * LD;    // wgmma images of W2 (2 branches x hi | lo), staged once
+  static constexpr int kBe = kW + 16384;
+  static constexpr int kWab = kBe + TM * 12;
+  static constexpr int kB2 = kWab + 576;
+  static constexpr int kD = kB2 + 128;              // [2][TM] per buffer
+  static constexpr int kIdx = kD + 2 * TM;          // dst [2][TM], bond [2][TM]
+  static constexpr int kTotal = kIdx + 4 * TM;
+  static constexpr size_t bytes = (size_t)kTotal * 4;
+};
+static_assert(AtomSmemFwd::bytes <= 232448, "atom-conv forward shared memory");
+
+__global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
+  extern __shared__ __align__(128) float smem[];
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);  // [2]
+  float* Wsm = smem + AtomSmemFwd::kW;
+  float* be_s = smem + AtomSmemFwd::kBe;
+  float* wabW = smem + AtomSmemFwd::kWab;
+  float* b2s = smem + AtomSmemFwd::kB2;
+
+  const int tid = threadIdx.x;
+  const int64_t ntiles = (a.E + TM - 1) / TM, step = gridDim.x;
+  auto tile_of = [&](int s) { return smem + AtomSmemFwd::kTile + s * TM * LD; };
+  auto d_of = [&](int s) { return smem + AtomSmemFwd::kD + s * TM; };
+  auto dst_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + s * TM; };
+  auto bond_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + (2 + s) * TM; };
+
+  if (tid == 0) {
+    mbar_init(&mbar[0], 1);
+    mbar_init(&mbar[1], 1);
+    fence_barrier_init();
+  }
+  EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
+  // loop-invariant operands, once per CTA
+  stage_w(Wsm, a.W2can, 4096);
+  for (int i = tid; i < 576; i += NT) wabW[i] = a.Wabw[i];
+  if (tid < 128) b2s[tid] = a.b2[tid];
+  float Mj[9];
+#pragma unroll
+  for (int k = 0; k < 9; k++) Mj[k] = a.M[(tid & 127) * 9 + k];
+  __syncthreads();
+  issue_gather(a, blockIdx.x, nxt, tile_of(0), &mbar[0], nullptr, dst_of(0), bond_of(0), d_of(0));
+  nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid);
+
+  int it = 0;
+  for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
+    const int s = it & 1;
+    float* tile = tile_of(s);
+    const int* s_dst = dst_of(s);
+    const int* s_bond = bond_of(s);
+    const int nvalid = (int)min((int64_t)TM, a.E - t * TM);
+    fence_proxy_async_smem();  // this thread's generic accesses of the other buffer come before its bulk refill
+    __syncthreads();           // the previous tile is done with the other buffer and be_s
+    if (t + step < ntiles) {
+      issue_gather(a, t + step, nxt, tile_of(s ^ 1), &mbar[s ^ 1], nullptr, dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
+      nxt = edge_row(a, (t + 2 * step) * TM + tid);
+    }
+    radial_rows(a, d_of(s), nvalid, be_s, nullptr);
+    mbar_wait(&mbar[s], stage_parity(it));
+    __syncthreads();
+    // pre = A[src] + C[dst] + (M.be | Q[bond]);  hid = silu(pre)
+    first_layer(a, tile, s_dst, s_bond, be_s, Mj, nvalid,
+                [&](int r, float p) { tile[r * LD + (tid & 127)] = r < nvalid ? silu_f(p) : 0.f; });
+    __syncthreads();
+    const Map m;
+    float acc[AR][AC];
+    gemm64(tile, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+#pragma unroll
+    for (int i = 0; i < AR; i++)
+#pragma unroll
+      for (int j = 0; j < AC; j++) {
+        const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
+        acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
+      }
+    __syncthreads();
+    if (m.branch == 1) {
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) tile[m.row(i) * LD + m.col(j)] = acc[i][j];
+    }
+    __syncthreads();
+    if (m.branch == 0) {
+#pragma unroll
+      for (int i = 0; i < AR; i++) {
+        const int r = m.row(i);
+#pragma unroll
+        for (int j = 0; j < AC; j++) {
+          const int c = m.col(j);
+          float wab = 0.f;
+#pragma unroll
+          for (int k = 0; k < 9; k++) wab = fmaf(be_s[r * 12 + k], wabW[c * 9 + k], wab);
+          tile[r * LD + c] = acc[i][j] * tile[r * LD + c] * wab;
+        }
+      }
+    }
+    __syncthreads();
+    {
+      const int c = tid & 63, part = tid >> 6;
+      seg_flush(tile, LD, c, part * 32, part * 32 + 32, s_dst, a.agg, D);
+    }
+  }
+}
+
+void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
   if (a.E <= 0) return;
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_) {
     B2M_CK(cudaFuncSetAttribute(k_atomconv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AtomSmemFwd::bytes));
   }
-  k_atomconv_fwd<<<cdiv(a.E, TM), NT, AtomSmemFwd::bytes, st>>>(a);
+  k_atomconv_fwd<<<std::min(cdiv(a.E, TM), num_sms), NT, AtomSmemFwd::bytes, st>>>(a);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }
@@ -534,27 +605,32 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a) {
 // ============================================================================================
 // atom conv: backward (recompute forward in-tile, then hand-derived reverse pass)
 // ============================================================================================
+// Shared memory holds one weight image (64 KB) and two [TM][LD] tiles whose roles alternate: the tile's gathered rows
+// arrive in buffer it & 1, which becomes P (pre-activations, then their adjoints); the other buffer is H (hidden
+// activations, then the second-layer adjoints).  Once g.W2 has read H and the W2^T image, both are refilled by bulk
+// copies -- H with the next tile's A[src] rows, the image with W2 -- which land while this tile's scatter phase runs.
+// The W2^T image is loaded right after the recompute product, under the elementwise reverse.  The weight barrier
+// completes two phases per tile (W2^T, then W2), waited on in that order.
 struct AtomSmemBwd {
-  static constexpr int kP = 32;
-  static constexpr int kH = kP + TM * LD;
-  static constexpr int kGw = kH + TM * LD;     // dE/dw_ab . W_ab per (row, radial k) [TM][12]
-  static constexpr int kW = kGw + TM * 12;     // wgmma images of W2 / W2^T (2 branches x hi | lo)
+  static constexpr int kBuf = 32;               // two [TM][LD] tiles (first 128 B: 2 gather mbarriers + weight mbarrier)
+  static constexpr int kGw = kBuf + 2 * TM * LD;  // dE/dw_ab . W_ab per (row, radial k) [TM][12]
+  static constexpr int kW = kGw + TM * 12;        // wgmma image of W2 or W2^T (2 branches x hi | lo)
   static constexpr int kBe = kW + 16384;
   static constexpr int kDbe = kBe + TM * 12;
   static constexpr int kWab = kDbe + TM * 12;
   static constexpr int kM = kWab + 576;
   static constexpr int kB2 = kM + 1152;
-  static constexpr int kD = kB2 + 128;
-  static constexpr int kIdx = kD + TM;
-  static constexpr int kTotal = kIdx + 3 * TM;
+  static constexpr int kD = kB2 + 128;          // [2][TM]
+  static constexpr int kIdx = kD + 2 * TM;      // src, dst, bond: [2][TM] each
+  static constexpr int kTotal = kIdx + 6 * TM;
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
+static_assert(AtomSmemBwd::bytes <= 232448, "atom-conv backward shared memory");
 
 __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);
-  float* tileP = smem + AtomSmemBwd::kP;
-  float* tileH = smem + AtomSmemBwd::kH;
+  uint64_t* gbar = reinterpret_cast<uint64_t*>(smem);  // [2]: gather buffers
+  uint64_t* wbar = gbar + 2;                            // weight image
   float* gws = smem + AtomSmemBwd::kGw;
   float* Wsm = smem + AtomSmemBwd::kW;
   float* be_s = smem + AtomSmemBwd::kBe;
@@ -562,205 +638,215 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   float* wabW = smem + AtomSmemBwd::kWab;
   float* Msm = smem + AtomSmemBwd::kM;
   float* b2s = smem + AtomSmemBwd::kB2;
-  float* s_d = smem + AtomSmemBwd::kD;
-  int* s_src = reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx);
-  int* s_dst = s_src + TM;
-  int* s_bond = s_dst + TM;
 
   const int tid = threadIdx.x;
-  const int64_t e0 = (int64_t)blockIdx.x * TM;
-  const int nvalid = (int)min((int64_t)TM, a.E - e0);
+  const int64_t ntiles = (a.E + TM - 1) / TM, step = gridDim.x;
   const bool useQ = a.Qproj != nullptr;
+  auto buf_of = [&](int s) { return smem + AtomSmemBwd::kBuf + s * TM * LD; };
+  auto d_of = [&](int s) { return smem + AtomSmemBwd::kD + s * TM; };
+  auto src_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + s * TM; };
+  auto dst_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + (2 + s) * TM; };
+  auto bond_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + (4 + s) * TM; };
 
-  if (tid < TM) {
-    int src = -1, dst = -1, bond = -1;
-    float d = 1.f;
-    if (tid < nvalid) {
-      const int64_t e = e0 + tid;
-      src = a.e_src[e];
-      dst = a.e_dst[e];
-      bond = a.e_bond[e];
-      d = a.e_vec[e].w;
-    }
-    s_src[tid] = src;
-    s_dst[tid] = dst;
-    s_bond[tid] = bond;
-    s_d[tid] = d;
-  }
   if (tid == 0) {
-    mbar_init(mbar, 1);
+    mbar_init(&gbar[0], 1);
+    mbar_init(&gbar[1], 1);
+    mbar_init(wbar, 1);
     fence_barrier_init();
   }
-  __syncthreads();
-  if (tid == 0) mbar_expect_tx(mbar, (uint32_t)nvalid * 512u);
-  if (tid < nvalid) bulk_g2s(tileP + tid * LD, a.Aproj + (size_t)s_src[tid] * D2, 512u, mbar);
-  stage_w(Wsm, a.W2can, 4096);
+  EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
   for (int i = tid; i < 576; i += NT) wabW[i] = a.Wabw[i];
   for (int i = tid; i < 1152; i += NT) Msm[i] = a.M[i];
   if (tid < 128) b2s[tid] = a.b2[tid];
-  {
-    const int r = tid & 127, half = tid >> 7;
-    const float d = s_d[r];
-    const int k0 = half ? 5 : 0, k1 = half ? 9 : 5;
-    for (int k = k0; k < k1; k++) {
-      float be = 0.f, dbe = 0.f;
-      if (r < nvalid) rbf_env_k(d, a.rp.freq[k], a.rp, be, dbe);
-      be_s[r * 12 + k] = be;
-      dbe_s[r * 12 + k] = dbe;
-    }
-  }
-  mbar_wait(mbar, 0);
-  __syncthreads();
-  {
-    const int j = tid & 127, rh = tid >> 7;
-    for (int i = 0; i < 64; i++) {
-      const int r = rh + 2 * i;
-      float p = 0.f;
-      if (r < nvalid) {
-        const int dst = s_dst[r], bond = s_bond[r];
-        float t;
-        if (useQ && bond >= 0) {
-          t = a.Qproj[(size_t)bond * D2 + j];
-        } else {
-          t = 0.f;
+  float Mj[9];
 #pragma unroll
-          for (int k = 0; k < 9; k++) t = fmaf(be_s[r * 12 + k], Msm[j * 9 + k], t);
-        }
-        p = tileP[r * LD + j] + a.Cproj[(size_t)dst * D2 + j] + t;
-      }
+  for (int k = 0; k < 9; k++) Mj[k] = a.M[(tid & 127) * 9 + k];
+  __syncthreads();
+  if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
+  issue_gather(a, blockIdx.x, nxt, buf_of(0), &gbar[0], src_of(0), dst_of(0), bond_of(0), d_of(0));
+  nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid);
+  uint32_t wpar = 0;
+
+  int it = 0;
+  for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
+    const int s = it & 1;
+    float* tileP = buf_of(s);
+    float* tileH = buf_of(s ^ 1);
+    const int* s_src = src_of(s);
+    const int* s_dst = dst_of(s);
+    const int* s_bond = bond_of(s);
+    const int64_t e0 = t * TM;
+    const int nvalid = (int)min((int64_t)TM, a.E - e0);
+    __syncthreads();  // the previous tile's scatter phase is done with tileH (its P), gws, be_s, dbe_s
+    radial_rows(a, d_of(s), nvalid, be_s, dbe_s);
+    mbar_wait(&gbar[s], stage_parity(it));
+    mbar_wait(wbar, wpar);  // W2
+    wpar ^= 1;
+    __syncthreads();
+    first_layer(a, tileP, s_dst, s_bond, be_s, Mj, nvalid, [&](int r, float p) {
+      const int j = tid & 127;
       tileP[r * LD + j] = p;
       tileH[r * LD + j] = r < nvalid ? silu_f(p) : 0.f;
-    }
-  }
-  __syncthreads();
-  const Map m;
-  float acc[AR][AC];
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-  gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-#pragma unroll
-    for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];  // u (L) / v (G)
-  __syncthreads();  // hid + W2k no longer needed
-  // exchange activations between the two branches through tileH
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-#pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const float u = acc[i][j];
-      tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
-    }
-  stage_w(Wsm, a.W2Tcan, 4096);
-  __syncthreads();
-  float gw[AR][9];  // branch 0: this thread's columns of sum_c dE/dw_ab[r][c] W_ab[c][k]
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-#pragma unroll
-    for (int k = 0; k < 9; k++) gw[i][k] = 0.f;
-#pragma unroll
-  for (int i = 0; i < AR; i++) {
-    const int r = m.row(i);
-    const int dst = s_dst[r];
-#pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const int c = m.col(j);
-      const float u = acc[i][j];
-      const float po = tileH[r * LD + (1 - m.branch) * 64 + c];  // partner activation
-      float g = 0.f;
-      if (dst >= 0) {
-        const float gm = a.gagg[(size_t)dst * D + c];
-        float wab = 0.f;
-#pragma unroll
-        for (int k = 0; k < 9; k++) wab = fmaf(be_s[r * 12 + k], wabW[c * 9 + k], wab);
-        if (m.branch == 0) {
-          const float s = sigm(u);
-          const float oL = u * s;
-          const float gwv = gm * oL * po;                    // d/d w_ab
-#pragma unroll
-          for (int k = 0; k < 9; k++) gw[i][k] = fmaf(gwv, wabW[c * 9 + k], gw[i][k]);
-          g = gm * po * wab * (s * (1.f + u * (1.f - s)));    // d/du
-        } else {
-          const float oG = sigm(u);
-          g = gm * po * wab * oG * (1.f - oG);               // d/dv
-        }
-      }
-      acc[i][j] = g;
-    }
-  }
-  if (m.branch == 0) {  // the four lanes l/4 = const of a warp own one row's 64 columns
+    });
+    __syncthreads();
+    const Map m;
+    float acc[AR][AC];
+    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
 #pragma unroll
     for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int k = 0; k < 9; k++) {
-        float v = gw[i][k];
-        v += __shfl_xor_sync(0xffffffffu, v, 1);
-        v += __shfl_xor_sync(0xffffffffu, v, 2);
-        if ((threadIdx.x & 3) == 0) gws[m.row(i) * 12 + k] = v;
+      for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];  // u (L) / v (G)
+    __syncthreads();  // hid + the W2 image no longer needed
+    if (tid == 0) bulk_g2s_image(Wsm, a.W2Tcan, 16384 * 4, wbar);
+    // exchange activations between the two branches through tileH
+#pragma unroll
+    for (int i = 0; i < AR; i++)
+#pragma unroll
+      for (int j = 0; j < AC; j++) {
+        const float u = acc[i][j];
+        tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
       }
-  }
-  __syncthreads();
+    __syncthreads();
+    float gw[AR][9];  // branch 0: this thread's columns of sum_c dE/dw_ab[r][c] W_ab[c][k]
 #pragma unroll
-  for (int i = 0; i < AR; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int j = 0; j < AC; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
-  __syncthreads();
-  // ghid = [gu @ W2L, gv @ W2G];  gpre = ghid * dsilu(pre)
+      for (int k = 0; k < 9; k++) gw[i][k] = 0.f;
 #pragma unroll
-  for (int i = 0; i < AR; i++)
-    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-  gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+    for (int i = 0; i < AR; i++) {
+      const int r = m.row(i);
+      const int dst = s_dst[r];
+      float2 gm2[AC / 2];  // this row's 16 dE/dagg values, loaded before any is used
 #pragma unroll
-  for (int i = 0; i < AR; i++)
+      for (int jj = 0; jj < AC / 2; jj++)
+        gm2[jj] = dst >= 0 ? __ldg(reinterpret_cast<const float2*>(&a.gagg[(size_t)dst * D + m.col(2 * jj)]))
+                           : make_float2(0.f, 0.f);
 #pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
-      tileP[idx] = acc[i][j] * dsilu_f(tileP[idx]);
-    }
-  __syncthreads();
-  // ---- scatter phase ----
-  {  // d E / d d_e through the radial basis (w_ab weights and, unless a bond row fed by Q, M.be)
-    const int r = tid >> 1, kh = tid & 1;
-    float part = 0.f;
-    if (r < nvalid) {
-      const int k0 = kh ? 5 : 0, k1 = kh ? 9 : 5;
-      const bool viaM = !(useQ && s_bond[r] >= 0);
-      for (int k = k0; k < k1; k++) {
-        float s = gws[r * 12 + k];
-        if (viaM)
-          for (int j = 0; j < 128; j++) s = fmaf(tileP[r * LD + j], Msm[j * 9 + k], s);
-        part = fmaf(s, dbe_s[r * 12 + k], part);
+      for (int j = 0; j < AC; j++) {
+        const int c = m.col(j);
+        const float u = acc[i][j];
+        const float po = tileH[r * LD + (1 - m.branch) * 64 + c];  // partner activation
+        float g = 0.f;
+        if (dst >= 0) {
+          const float gm = (j & 1) ? gm2[j >> 1].y : gm2[j >> 1].x;
+          float wab = 0.f;
+#pragma unroll
+          for (int k = 0; k < 9; k++) wab = fmaf(be_s[r * 12 + k], wabW[c * 9 + k], wab);
+          if (m.branch == 0) {
+            const float sg = sigm(u);
+            const float oL = u * sg;
+            const float gwv = gm * oL * po;                    // d/d w_ab
+#pragma unroll
+            for (int k = 0; k < 9; k++) gw[i][k] = fmaf(gwv, wabW[c * 9 + k], gw[i][k]);
+            g = gm * po * wab * (sg * (1.f + u * (1.f - sg)));  // d/du
+          } else {
+            const float oG = sigm(u);
+            g = gm * po * wab * oG * (1.f - oG);               // d/dv
+          }
+        }
+        acc[i][j] = g;
       }
     }
-    part += __shfl_xor_sync(0xffffffffu, part, 1);
-    if (kh == 0 && r < nvalid) a.gd[e0 + r] += part;
-  }
-  {
-    const int j = tid & 127, rh = tid >> 7;
-    if (useQ && a.gQ != nullptr) {
-      for (int i = 0; i < 64; i++) {
-        const int r = rh + 2 * i;
-        if (r < nvalid && s_bond[r] >= 0) a.gQ[(size_t)s_bond[r] * D2 + j] = tileP[r * LD + j];
+    if (m.branch == 0) {  // the four lanes l/4 = const of a warp own one row's 64 columns
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int k = 0; k < 9; k++) {
+          float v = gw[i][k];
+          v += __shfl_xor_sync(0xffffffffu, v, 1);
+          v += __shfl_xor_sync(0xffffffffu, v, 2);
+          if ((threadIdx.x & 3) == 0) gws[m.row(i) * 12 + k] = v;
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < AR; i++)
+#pragma unroll
+      for (int j = 0; j < AC; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+    mbar_wait(wbar, wpar);  // W2^T
+    wpar ^= 1;
+    __syncthreads();
+    // ghid = [gu @ W2L, gv @ W2G];  gpre = ghid * dsilu(pre)
+    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+#pragma unroll
+    for (int i = 0; i < AR; i++)
+#pragma unroll
+      for (int j = 0; j < AC; j++) {
+        const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
+        tileP[idx] = acc[i][j] * dsilu_f(tileP[idx]);
+      }
+    fence_proxy_async_smem();  // this thread's generic accesses of tileH come before its bulk refill
+    __syncthreads();           // tileH and the W2^T image are free
+    if (t + step < ntiles) {
+      if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
+      issue_gather(a, t + step, nxt, tileH, &gbar[s ^ 1], src_of(s ^ 1), dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
+      nxt = edge_row(a, (t + 2 * step) * TM + tid);
+    }
+    // ---- scatter phase (reads tileP and this tile's index arrays only) ----
+    {  // d E / d d_e through the radial basis (w_ab weights and, unless a bond row fed by Q, M.be): warpgroup h sums
+       // sum_j gpre[r][j] M[j][k] over j in [64 h, 64 h + 64) for row r = tid & 127, all k at once
+      const int r = tid & 127, h = tid >> 7;
+      float sk[9];
+#pragma unroll
+      for (int k = 0; k < 9; k++) sk[k] = 0.f;
+      const bool viaM = r < nvalid && !(useQ && s_bond[r] >= 0);
+      if (viaM) {
+#pragma unroll 4
+        for (int jq = 0; jq < 16; jq++) {
+          const float4 p = *reinterpret_cast<const float4*>(&tileP[r * LD + 64 * h + 4 * jq]);
+          const float* Mq = Msm + (64 * h + 4 * jq) * 9;
+#pragma unroll
+          for (int k = 0; k < 9; k++) {
+            float v = sk[k];
+            v = fmaf(p.x, Mq[k], v);
+            v = fmaf(p.y, Mq[9 + k], v);
+            v = fmaf(p.z, Mq[18 + k], v);
+            v = fmaf(p.w, Mq[27 + k], v);
+            sk[k] = v;
+          }
+        }
+      }
+      if (h == 1) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) be_s[r * 12 + k] = sk[k];  // be_s is free until the next tile
+      }
+      __syncthreads();
+      if (h == 0 && r < nvalid) {
+        float part = 0.f;
+#pragma unroll
+        for (int k = 0; k < 9; k++) part = fmaf(gws[r * 12 + k] + (sk[k] + be_s[r * 12 + k]), dbe_s[r * 12 + k], part);
+        a.gd[e0 + r] += part;
       }
     }
-    if (a.gA != nullptr) {
-      seg_flush(tileP, LD, j, rh * 64, rh * 64 + 64, s_dst, a.gC, D2);
-      for (int i = 0; i < 64; i++) {
-        const int r = rh + 2 * i;
-        if (r < nvalid) atomicAdd(&a.gA[(size_t)s_src[r] * D2 + j], tileP[r * LD + j]);
+    {
+      const int j = tid & 127, rh = tid >> 7;
+      if (useQ && a.gQ != nullptr) {
+        for (int i = 0; i < 64; i++) {
+          const int r = rh + 2 * i;
+          if (r < nvalid && s_bond[r] >= 0) a.gQ[(size_t)s_bond[r] * D2 + j] = tileP[r * LD + j];
+        }
+      }
+      if (a.gA != nullptr) seg_flush(tileP, LD, j, rh * 64, rh * 64 + 64, s_dst, a.gC, D2);
+    }
+    if (a.gA != nullptr) {  // gA[src] += gpre: a 4-wide reduction per (row, column quad), a warp per row
+      const int q = tid & 31, rg = tid >> 5;
+#pragma unroll 4
+      for (int i = 0; i < TM / 8; i++) {
+        const int r = rg + 8 * i;
+        if (r < nvalid)
+          red_add_v4(&a.gA[(size_t)s_src[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&tileP[r * LD + 4 * q]));
       }
     }
   }
 }
 
-void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a) {
+void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
   if (a.E <= 0) return;
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_) {
     B2M_CK(cudaFuncSetAttribute(k_atomconv_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AtomSmemBwd::bytes));
   }
-  k_atomconv_bwd<<<cdiv(a.E, TM), NT, AtomSmemBwd::bytes, st>>>(a);
+  k_atomconv_bwd<<<std::min(cdiv(a.E, TM), num_sms), NT, AtomSmemBwd::bytes, st>>>(a);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }

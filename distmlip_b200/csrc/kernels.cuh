@@ -64,8 +64,9 @@ struct AtomConvArgs {
   float* gQ;          // [B_own,128] (=)
   float* gd;          // [E] (+=)
 };
-void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a);
-void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a);
+// persistent: min(tiles, num_sms) CTAs loop over the 128-edge tiles
+void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms);
+void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a, int num_sms);
 
 // -------- bond conv ("node" phase, HIDDEN) and angle update ("edge" phase, !HIDDEN) --------
 struct LineArgs {
