@@ -18,6 +18,7 @@ SYMBOLS = [
     "b2m_finalize_weights", "b2m_set_scaling", "b2m_comm_unique_id", "b2m_comm_init", "b2m_set_partition", "b2m_set_structure", "b2m_compute",
     "b2m_compute_resident", "b2m_get_results", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
     "b2m_debug_tensor", "b2m_last_timings", "b2m_release_workspace", "b2m_set_view", "b2m_create_tensornet",
+    "b2m_set_atomic", "b2m_get_atomic",
 ]
 
 
@@ -83,6 +84,8 @@ def load_library():
     lib.b2m_last_timings.argtypes = [vp, P(dbl), i32]
     lib.b2m_release_workspace.argtypes = [vp]
     lib.b2m_set_view.argtypes = [vp, i32]
+    lib.b2m_set_atomic.argtypes = [vp, i32]
+    lib.b2m_get_atomic.argtypes = [vp, P(dbl), P(C.c_float)]
     for s in SYMBOLS:
         if s not in ("b2m_last_error", "b2m_get_partition_info"):
             getattr(lib, s).restype = C.c_int
@@ -218,6 +221,20 @@ class Engine:
         out = np.empty(self.natoms, dtype=np.float32)
         self._ck(self.lib.b2m_get_sitewise(self.h, out.ctypes.data_as(C.POINTER(C.c_float))))
         return out
+
+    def set_atomic(self, on):
+        """per-atom energies and virials in the following evaluations (off by default: no buffers, no extra work)"""
+        self._ck(self.lib.b2m_set_atomic(self.h, int(bool(on))))
+
+    def atomic(self, virials=True):
+        """per-atom energies [natoms] f64 (eV, summing to the energy) and per-atom virials [natoms, 3, 3] f32 (eV,
+        summing to the strain derivative of the energy) of the last evaluation, which must have run with
+        set_atomic(True); the virials need a backward (forces or stress).  `virials=False` returns (energies, None)."""
+        e = np.empty(self.natoms, dtype=np.float64)
+        w = np.empty((self.natoms, 3, 3), dtype=np.float32) if virials else None
+        self._ck(self.lib.b2m_get_atomic(self.h, e.ctypes.data_as(C.POINTER(C.c_double)),
+                                         w.ctypes.data_as(C.POINTER(C.c_float)) if virials else None))
+        return e, w
 
     def set_view(self, part):
         """single-process group: the partition that counts() / partition_info() describe"""

@@ -22,6 +22,7 @@
 
 #include <algorithm>
 
+#include "atomic_virial.cuh"
 #include "graph.cuh"
 #include "kernels.cuh"
 #include "tn_state.cuh"
@@ -172,6 +173,14 @@ struct b2m_engine {
   DBuf<float> gx, gh, gang, gA, gC, gQ, gHa, gHb, gXc, gagg, gupd, gaggB, gd, gdb, gbvec, gy1, gy2;
   DBuf<float> forces, sendbuf, recvbuf, site_full;
   DBuf<double> scal;  // [0]=energy, [1..9]=virial
+  // per-atom energies and virials (b2m_set_atomic; DESIGN.md "Per-atom energies and virials"): allocated on the first
+  // evaluation with the flag on, indexed by global atom id like `forces`
+  bool atomic = false;
+  int atomic_last = 0;      // what the last evaluation left in them: 0 nothing, 1 energies, 2 energies and virials
+  DBuf<double> atom_e;      // [N]
+  DBuf<float> atom_vir;     // [N][kVirPitch]
+  DBuf<double> aesum, aetmp;  // leader of a group: the summed energies / staging of a peer's array
+  DBuf<float> avsum, avtmp;   // same for the virials
   // timings
   cudaEvent_t ev[8] = {nullptr};
   double t_graph = 0, t_fwd = 0, t_bwd = 0, t_gather = 0, t_total = 0;
@@ -802,7 +811,7 @@ static void forward(b2m_engine* e) {
   launch_silu(e->st, (int64_t)g.n_own * D, e->y2p.p, e->y2.p);
   B2M_CK(cudaMemsetAsync(e->scal.p, 0, 16 * sizeof(double), e->st));
   launch_rowdot(e->st, g.n_own, e->y2.p, e->d_F2, e->c2, e->e_atom.p, e->scal.p, g.type.p, e->d_eref,
-                (float)e->desc.data_std);
+                (float)e->desc.data_std, g.gid.p, e->atomic ? e->atom_e.p : nullptr, e->desc.data_mean / g.N);
 }
 
 static void backward(b2m_engine* e) {
@@ -842,10 +851,11 @@ static void backward(b2m_engine* e) {
   // geometry: h0 = W_be be(d_b), theta/Fourier, then edges -> forces and virial
   launch_h0_bwd(e->st, g.B_loc, g.b_vec.p, e->rp2, e->d_Wbe, e->gh.p, e->gdb.p);
   launch_angle_init_bwd(e->st, g.A, g.a_in.p, g.a_out.p, g.b_vec.p, e->d_fa, e->d_Wae, e->gang.p, e->gbvec.p);
+  float* avir = e->atomic ? e->atom_vir.p : nullptr;
   launch_edge_final(e->st, g.E, g.e_src.p, g.e_dst.p, g.e_bond.p, g.e_vec.p, g.gid.p, e->gd.p, e->gdb.p, e->gbvec.p,
-                    e->forces.p, e->scal.p + 1);
+                    e->forces.p, e->scal.p + 1, avir);
   launch_halo_bond_final(e->st, g.B_own, g.B_loc, g.b_src_gid.p, g.b_dst.p, g.b_vec.p, g.gid.p, e->gdb.p, e->gbvec.p,
-                         e->forces.p, e->scal.p + 1);
+                         e->forces.p, e->scal.p + 1, avir);
 }
 
 static void run(b2m_engine* e, bool grads) {
@@ -862,6 +872,16 @@ static void run(b2m_engine* e, bool grads) {
   const long long l0 = g_launch_count;
   B2M_CK(cudaEventRecord(e->ev[0], e->st));
   e->want_grads = grads;
+  const size_t N = (size_t)e->g.N;
+  if (e->atomic) {  // zeroed here, before the readout writes the energies and the backward accumulates the virials
+    e->atom_e.ensure(N + 64);
+    e->atom_e.zero(N, e->st);
+    if (grads) {
+      e->atom_vir.ensure(N * kVirPitch + 64);
+      e->atom_vir.zero(N * kVirPitch, e->st);
+    }
+  }
+  e->atomic_last = 0;
   if (e->kind == 1) tn_forward(e); else forward(e);
   B2M_CK(cudaEventRecord(e->ev[1], e->st));
   if (grads) {
@@ -871,10 +891,16 @@ static void run(b2m_engine* e, bool grads) {
     NCCL_CK(g_nccl.AllReduce(e->scal.p, e->scal.p, 10, ncclFloat64, ncclSum, e->comm, e->st));
     if (grads)
       NCCL_CK(g_nccl.AllReduce(e->forces.p, e->forces.p, (size_t)e->g.N * 3, ncclFloat32, ncclSum, e->comm, e->st));
+    if (e->atomic) {
+      NCCL_CK(g_nccl.AllReduce(e->atom_e.p, e->atom_e.p, N, ncclFloat64, ncclSum, e->comm, e->st));
+      if (grads)
+        NCCL_CK(g_nccl.AllReduce(e->atom_vir.p, e->atom_vir.p, N * kVirPitch, ncclFloat32, ncclSum, e->comm, e->st));
+    }
   }
   B2M_CK(cudaEventRecord(e->ev[2], e->st));
   B2M_CK(cudaStreamSynchronize(e->st));
   e->launches_last = g_launch_count - l0;
+  e->atomic_last = e->atomic ? (grads ? 2 : 1) : 0;
   float ms;
   B2M_CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]));
   e->t_fwd = ms;
@@ -916,6 +942,10 @@ static void ensure_pinned(void*& p, size_t& cap, size_t bytes) {
 }
 
 __global__ void k_add_inplace(int64_t n, const float* __restrict__ src, float* __restrict__ dst) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) dst[i] += src[i];
+}
+__global__ void k_add_inplace_f64(int64_t n, const double* __restrict__ src, double* __restrict__ dst) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i < n) dst[i] += src[i];
 }
@@ -1002,6 +1032,42 @@ static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) 
   if (energy) *energy = e->last_energy;
   if (stress9)
     for (int k = 0; k < 9; k++) stress9[k] = (float)(hs[1 + k] / e->g.volume * 160.21766208);  // pes.py:140-145
+}
+
+// per-atom energies [N] and virials [N][9] of the last evaluation; a group sums its partitions' arrays on the leader's
+// device (energies: each atom has one owner; virials: every partition adds the edges and bond parts it holds), a
+// multi-process run has all-reduced them in run()
+static void fetch_atomic(b2m_engine* e, double* energies, float* virials) {
+  const size_t N = (size_t)e->g.N;
+  const double* esrc = e->atom_e.p;
+  const float* vsrc = e->atom_vir.p;
+  if (!e->parts.empty()) {
+    auto sum = [&](auto& total, auto& tmp, auto member_buf, size_t n, auto add) {
+      total.ensure(n + 64);
+      tmp.ensure(n + 64);
+      B2M_CK(cudaMemcpyAsync(total.p, member_buf(e).p, n * sizeof(*total.p), cudaMemcpyDeviceToDevice, e->st));
+      for (size_t p = 1; p < e->parts.size(); p++) {
+        B2M_CK(cudaMemcpyAsync(tmp.p, member_buf(e->parts[p]).p, n * sizeof(*total.p), cudaMemcpyDefault, e->st));
+        add<<<cdiv((int64_t)n, 256), 256, 0, e->st>>>((int64_t)n, tmp.p, total.p);
+        B2M_CK(cudaGetLastError());
+      }
+      return total.p;
+    };
+    if (energies) esrc = sum(e->aesum, e->aetmp, [](b2m_engine* m) -> DBuf<double>& { return m->atom_e; }, N, k_add_inplace_f64);
+    if (virials)
+      vsrc = sum(e->avsum, e->avtmp, [](b2m_engine* m) -> DBuf<float>& { return m->atom_vir; }, N * kVirPitch, k_add_inplace);
+  }
+  const size_t vbytes = N * kVirPitch * sizeof(float);
+  if (virials) {
+    ensure_pinned(e->pin_out, e->pin_out_cap, vbytes);
+    B2M_CK(cudaMemcpyAsync(e->pin_out, vsrc, vbytes, cudaMemcpyDeviceToHost, e->st));
+  }
+  if (energies) B2M_CK(cudaMemcpyAsync(energies, esrc, N * sizeof(double), cudaMemcpyDeviceToHost, e->st));
+  B2M_CK(cudaStreamSynchronize(e->st));
+  if (virials) {
+    const float* w = static_cast<const float*>(e->pin_out);
+    for (size_t i = 0; i < N; i++) memcpy(virials + i * 9, w + i * kVirPitch, 9 * sizeof(float));
+  }
 }
 
 }  // namespace b2m
@@ -1290,6 +1356,7 @@ static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart,
     species = reinterpret_cast<const int32_t*>((const char*)h->pin_in + cb);
   }
   B2M_CK(cudaEventRecord(h->ev[3], h->st));
+  h->atomic_last = 0;  // per-atom results of an earlier structure are gone
   h->g.build(h->st, natoms, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff, tol, h->rank,
              h->world);
   if (h->kind == 1) tn_alloc_workspace(h); else alloc_workspace(h);
@@ -1334,6 +1401,23 @@ int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9)
   API_BEGIN
   B2M_REQUIRE(h->have_graph, B2M_ERR_STATE, "no structure");
   fetch(h, energy, forces, stress9);
+  API_END
+}
+
+int b2m_set_atomic(b2m_handle h, int on) {
+  API_BEGIN
+  each_member(h, [&](b2m_engine* e) { e->atomic = on != 0; });
+  API_END
+}
+
+int b2m_get_atomic(b2m_handle h, double* energies, float* virials) {
+  API_BEGIN
+  B2M_REQUIRE(h->have_graph, B2M_ERR_STATE, "no structure");
+  B2M_REQUIRE(h->atomic_last > 0, B2M_ERR_STATE,
+              "the last evaluation ran without per-atom energies and virials (b2m_set_atomic(h, 1) first)");
+  B2M_REQUIRE(virials == nullptr || h->atomic_last == 2, B2M_ERR_STATE,
+              "per-atom virials need an evaluation with a backward (want_forces or want_stress)");
+  fetch_atomic(h, energies, virials);
   API_END
 }
 
@@ -1458,8 +1542,11 @@ int b2m_release_workspace(b2m_handle h) {
     for (auto* b : {&e->Ha, &e->Hb, &e->Xc, &e->agg, &e->aggB, &e->y1p, &e->y1, &e->y2p, &e->y2,
                     &e->e_atom, &e->site, &e->gx, &e->gh, &e->gang, &e->gA, &e->gC, &e->gQ, &e->gHa, &e->gHb, &e->gXc,
                     &e->gagg, &e->gupd, &e->gaggB, &e->gd, &e->gdb, &e->gbvec, &e->gy1, &e->gy2, &e->forces,
-                    &e->sendbuf, &e->recvbuf, &e->site_full, &e->precv[0], &e->precv[1], &e->ftmp, &e->fsum})
+                    &e->sendbuf, &e->recvbuf, &e->site_full, &e->precv[0], &e->precv[1], &e->ftmp, &e->fsum,
+                    &e->atom_vir, &e->avsum, &e->avtmp})
       drop(*b);
+    for (auto* b : {&e->atom_e, &e->aesum, &e->aetmp}) drop(*b);
+    e->atomic_last = 0;
     tn_release(e);
     e->g.~Graph();  // the resident graph goes too
     new (&e->g) Graph();

@@ -1,6 +1,7 @@
 // kernels.cu -- hand-written sm_90a kernels of the CHGNet hot path (fp32 FFMA math,
 // cp.async.bulk (TMA) row gathers into shared memory, segmented scatter-adds).
 // See kernels.cuh for the formulation; oracle/manual_ref.py is the CPU mirror of every stage.
+#include "atomic_virial.cuh"
 #include "kernels.cuh"
 #include "wgmma.cuh"
 
@@ -1328,10 +1329,13 @@ void launch_angle_init_bwd(cudaStream_t st, int64_t na, const int* a_in, const i
 // ============================================================================================
 // readout
 // ============================================================================================
+// kAtomic: also the per-atom energy of every row, atom_e[gid[row]] = scale * v + elem_ref + mean_per_atom
+template <bool kAtomic>
 __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__ X, const float* __restrict__ w,
                                                 float bias, float* __restrict__ out, double* __restrict__ sum,
                                                 const int* __restrict__ type, const double* __restrict__ elem_ref,
-                                                float scale) {
+                                                float scale, const int* __restrict__ gid, double* __restrict__ atom_e,
+                                                double mean_per_atom) {
   // one warp per row
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   float v = 0.f;
@@ -1348,6 +1352,7 @@ __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__
     if (out) out[warp] = v;
     contrib = (double)scale * (double)v;
     if (elem_ref) contrib += elem_ref[type[warp]];
+    if constexpr (kAtomic) atom_e[gid[warp]] = contrib + mean_per_atom;
   }
   if (sum) {
     if (lane == 0) part[threadIdx.x >> 5] = contrib;
@@ -1360,9 +1365,15 @@ __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__
   }
 }
 void launch_rowdot(cudaStream_t st, int n, const float* X, const float* w, float bias, float* out, double* sum,
-                   const int* type, const double* elem_ref, float scale) {
+                   const int* type, const double* elem_ref, float scale, const int* gid, double* atom_e,
+                   double mean_per_atom) {
   if (n <= 0) return;
-  k_rowdot<<<cdiv((int64_t)n * 32, 256), 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale);
+  if (atom_e)
+    k_rowdot<true><<<cdiv((int64_t)n * 32, 256), 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid,
+                                                               atom_e, mean_per_atom);
+  else
+    k_rowdot<false><<<cdiv((int64_t)n * 32, 256), 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid,
+                                                                atom_e, mean_per_atom);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }
@@ -1398,16 +1409,19 @@ __device__ __forceinline__ void virial_reduce(const float (&v)[9], double* __res
   }
 }
 
+// kAtomic: also 1/2 v (x) g into both endpoints' rows of the per-atom virial array (atomic_virial.cuh)
+template <bool kAtomic>
 __global__ void __launch_bounds__(256) k_edge_final(int64_t E, const int* __restrict__ e_src,
                                                     const int* __restrict__ e_dst, const int* __restrict__ e_bond,
                                                     const float4* __restrict__ e_vec, const int* __restrict__ gid,
                                                     const float* __restrict__ gd, const float* __restrict__ gdb,
                                                     const float* __restrict__ gbvec, float* __restrict__ forces,
-                                                    double* __restrict__ virial) {
+                                                    double* __restrict__ virial, float* __restrict__ atom_vir) {
   const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   float vir[9];
 #pragma unroll
   for (int k = 0; k < 9; k++) vir[k] = 0.f;
+  int asrc = 0, adst = -1;
   if (e < E) {
     const float4 v = e_vec[e];
     float g = gd[e];
@@ -1431,23 +1445,38 @@ __global__ void __launch_bounds__(256) k_edge_final(int64_t E, const int* __rest
     vir[0] = v.x * gx, vir[1] = v.x * gy, vir[2] = v.x * gz;
     vir[3] = v.y * gx, vir[4] = v.y * gy, vir[5] = v.y * gz;
     vir[6] = v.z * gx, vir[7] = v.z * gy, vir[8] = v.z * gz;
+    if constexpr (kAtomic) asrc = gsrc, adst = gdst;
+  }
+  if constexpr (kAtomic) {
+    float w[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) w[k] = 0.5f * vir[k];
+    red_add_edge_virial(atom_vir, asrc, adst, w);
   }
   virial_reduce(vir, virial);
 }
 void launch_edge_final(cudaStream_t st, int64_t E, const int* e_src, const int* e_dst, const int* e_bond,
                        const float4* e_vec, const int* gid, const float* gd, const float* gdb, const float* gbvec,
-                       float* forces, double* virial) {
+                       float* forces, double* virial, float* atom_vir) {
   if (E <= 0) return;
-  k_edge_final<<<cdiv(E, 256), 256, 0, st>>>(E, e_src, e_dst, e_bond, e_vec, gid, gd, gdb, gbvec, forces, virial);
+  if (atom_vir)
+    k_edge_final<true><<<cdiv(E, 256), 256, 0, st>>>(E, e_src, e_dst, e_bond, e_vec, gid, gd, gdb, gbvec, forces, virial,
+                                                     atom_vir);
+  else
+    k_edge_final<false><<<cdiv(E, 256), 256, 0, st>>>(E, e_src, e_dst, e_bond, e_vec, gid, gd, gdb, gbvec, forces, virial,
+                                                      atom_vir);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }
 
+// kAtomic: also 1/2 v (x) g of this partition's part of g into both endpoints' per-atom virial rows (the bond's
+// owner adds its own part in k_edge_final, so the sum over partitions is exact)
+template <bool kAtomic>
 __global__ void __launch_bounds__(256) k_halo_bond_final(int b0, int b1, const int* __restrict__ b_src_gid,
                                                          const int* __restrict__ b_dst, const float4* __restrict__ b_vec,
                                                          const int* __restrict__ gid, const float* __restrict__ gdb,
                                                          const float* __restrict__ gbvec, float* __restrict__ forces,
-                                                         double* __restrict__ virial) {
+                                                         double* __restrict__ virial, float* __restrict__ atom_vir) {
   const int b = b0 + blockIdx.x * blockDim.x + threadIdx.x;
   float vir[9];
 #pragma unroll
@@ -1467,15 +1496,26 @@ __global__ void __launch_bounds__(256) k_halo_bond_final(int b0, int b1, const i
     vir[0] = v.x * gx, vir[1] = v.x * gy, vir[2] = v.x * gz;
     vir[3] = v.y * gx, vir[4] = v.y * gy, vir[5] = v.y * gz;
     vir[6] = v.z * gx, vir[7] = v.z * gy, vir[8] = v.z * gz;
+    if constexpr (kAtomic) {
+      float w[9];
+#pragma unroll
+      for (int k = 0; k < 9; k++) w[k] = 0.5f * vir[k];
+      red_add_virial(atom_vir, gdst, w);
+      red_add_virial(atom_vir, gsrc, w);
+    }
   }
   virial_reduce(vir, virial);
 }
 void launch_halo_bond_final(cudaStream_t st, int b0, int b1, const int* b_src_gid, const int* b_dst,
                             const float4* b_vec, const int* gid, const float* gdb, const float* gbvec, float* forces,
-                            double* virial) {
+                            double* virial, float* atom_vir) {
   if (b1 <= b0) return;
-  k_halo_bond_final<<<cdiv(b1 - b0, 256), 256, 0, st>>>(b0, b1, b_src_gid, b_dst, b_vec, gid, gdb, gbvec, forces,
-                                                        virial);
+  if (atom_vir)
+    k_halo_bond_final<true><<<cdiv(b1 - b0, 256), 256, 0, st>>>(b0, b1, b_src_gid, b_dst, b_vec, gid, gdb, gbvec,
+                                                                forces, virial, atom_vir);
+  else
+    k_halo_bond_final<false><<<cdiv(b1 - b0, 256), 256, 0, st>>>(b0, b1, b_src_gid, b_dst, b_vec, gid, gdb, gbvec,
+                                                                 forces, virial, atom_vir);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }

@@ -16,6 +16,7 @@
 // B2M_TN_FFMA=1 (A/B checks).  DESIGN.md 8 lists what comes next.
 #include <math_constants.h>
 
+#include "atomic_virial.cuh"
 #include "kernels.cuh"
 
 namespace b2m {
@@ -596,11 +597,14 @@ __global__ void k_tn_invariants_bwd(int n, const float* __restrict__ X, const fl
   store10(gX + (size_t)t * TW, c, v);
 }
 // last layer of both readout chains (width W -> 1), product, energy sum; one warp per atom
+// kAtomic: also the per-atom energy of every row, atom_e[gid[row]] = scale * L * G + eref + mean_per_atom
+template <bool kAtomic>
 __global__ void k_tn_readout_final(int n, int W, const float* __restrict__ hL, const float* __restrict__ wL, float bL,
                                    const float* __restrict__ hG, const float* __restrict__ wG, float bG,
                                    const int* __restrict__ type, const double* __restrict__ eref, float scale,
                                    float* __restrict__ lout, float* __restrict__ gout, float* __restrict__ e_atom,
-                                   double* __restrict__ energy) {
+                                   double* __restrict__ energy, const int* __restrict__ gid, double* __restrict__ atom_e,
+                                   double mean_per_atom) {
   const int r = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (r >= n) return;
   float a = 0.f, b = 0.f;
@@ -617,6 +621,7 @@ __global__ void k_tn_readout_final(int n, int W, const float* __restrict__ hL, c
     lout[r] = L, gout[r] = Gt, e_atom[r] = L * Gt;
     double ev = (double)scale * (double)(L * Gt);
     if (eref) ev += eref[type[r]];
+    if constexpr (kAtomic) atom_e[gid[r]] = ev + mean_per_atom;
     atomicAdd(energy, ev);
   }
 }
@@ -651,16 +656,20 @@ __device__ __forceinline__ void virial_reduce_tn(const float (&v)[9], double* __
     atomicAdd(&virial[threadIdx.x], s);
   }
 }
+// kAtomic: also 1/2 v (x) g into both endpoints' rows of the per-atom virial array (atomic_virial.cuh)
+template <bool kAtomic>
 __global__ void __launch_bounds__(256) k_tn_edge_final(int64_t E, const int* __restrict__ e_src,
                                                        const int* __restrict__ e_dst, const float4* __restrict__ e_vec,
                                                        const int* __restrict__ gid, TnRadial rp,
                                                        const float* __restrict__ g_rbf, const float* __restrict__ gC,
                                                        const float* __restrict__ gvh, float* __restrict__ gd_out,
-                                                       float* __restrict__ forces, double* __restrict__ virial) {
+                                                       float* __restrict__ forces, double* __restrict__ virial,
+                                                       float* __restrict__ atom_vir) {
   const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   float vir[9];
 #pragma unroll
   for (int k = 0; k < 9; k++) vir[k] = 0.f;
+  int asrc = 0, adst = -1;
   if (e < E) {
     const float4 v = e_vec[e];
     const float d = v.w, rd = 1.f / d;
@@ -686,6 +695,13 @@ __global__ void __launch_bounds__(256) k_tn_edge_final(int64_t E, const int* __r
     vir[0] = v.x * gx, vir[1] = v.x * gy, vir[2] = v.x * gz;  // strain_bar[a][b] = sum vec[a] g[b]  (pes.py:140-145)
     vir[3] = v.y * gx, vir[4] = v.y * gy, vir[5] = v.y * gz;
     vir[6] = v.z * gx, vir[7] = v.z * gy, vir[8] = v.z * gz;
+    if constexpr (kAtomic) asrc = gsrc, adst = gdst;
+  }
+  if constexpr (kAtomic) {
+    float w[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) w[k] = 0.5f * vir[k];
+    red_add_edge_virial(atom_vir, asrc, adst, w);
   }
   virial_reduce_tn(vir, virial);
 }
@@ -771,9 +787,14 @@ void launch_tn_invariants_bwd(cudaStream_t st, int n, const float* X, const floa
 }
 void launch_tn_readout_final(cudaStream_t st, int n, int W, const float* hL, const float* wL, float bL, const float* hG,
                              const float* wG, float bG, const int* type, const double* eref, float scale, float* lout,
-                             float* gout, float* e_atom, double* energy) {
-  TN_LAUNCH(k_tn_readout_final, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout,
-            e_atom, energy);
+                             float* gout, float* e_atom, double* energy, const int* gid, double* atom_e,
+                             double mean_per_atom) {
+  if (atom_e)
+    TN_LAUNCH(k_tn_readout_final<true>, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout,
+              e_atom, energy, gid, atom_e, mean_per_atom);
+  else
+    TN_LAUNCH(k_tn_readout_final<false>, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout,
+              gout, e_atom, energy, gid, atom_e, mean_per_atom);
 }
 void launch_tn_readout_seed(cudaStream_t st, int n, int W, const float* lout, const float* gout, float scale,
                             const float* wL, const float* wG, const float* preL, const float* preG, float* gL,
@@ -782,8 +803,12 @@ void launch_tn_readout_seed(cudaStream_t st, int n, int W, const float* lout, co
 }
 void launch_tn_edge_final(cudaStream_t st, int64_t E, const int* e_src, const int* e_dst, const float4* e_vec,
                           const int* gid, const TnRadial& rp, const float* g_rbf, const float* gC, const float* gvh,
-                          float* gd, float* forces, double* virial) {
-  TN_LAUNCH(k_tn_edge_final, E, st, E, e_src, e_dst, e_vec, gid, rp, g_rbf, gC, gvh, gd, forces, virial);
+                          float* gd, float* forces, double* virial, float* atom_vir) {
+  if (atom_vir)
+    TN_LAUNCH(k_tn_edge_final<true>, E, st, E, e_src, e_dst, e_vec, gid, rp, g_rbf, gC, gvh, gd, forces, virial, atom_vir);
+  else
+    TN_LAUNCH(k_tn_edge_final<false>, E, st, E, e_src, e_dst, e_vec, gid, rp, g_rbf, gC, gvh, gd, forces, virial,
+              atom_vir);
 }
 
 }  // namespace b2m

@@ -29,6 +29,7 @@ class Distributed:
         self.total_num_edges = None  # global count needs a reduction over ranks; see num_atom_edges
         self.forces = None
         self.stress = None
+        self.atomic = None  # (per-atom energies, per-atom virials) when the Potential asks for them
 
     @staticmethod
     def cartesian_to_wrapped_fractional(positions_cartesian, lattice, pbc):

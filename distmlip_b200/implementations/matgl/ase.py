@@ -18,6 +18,12 @@ try:  # pragma: no cover - ASE is absent in the build image
 except Exception:  # noqa: BLE001
     _HAVE_ASE = False
     _all_changes = ["positions", "numbers", "cell", "pbc", "initial_charges", "initial_magmoms"]
+try:  # pragma: no cover
+    from ase.calculators.calculator import PropertyNotImplementedError as _PropertyNotImplementedError
+except Exception:  # noqa: BLE001
+
+    class _PropertyNotImplementedError(NotImplementedError):
+        """ase.calculators.calculator.PropertyNotImplementedError where ASE is absent"""
 
     class _Calculator:  # minimal stand-in with the attributes PESCalculator_Dist touches
         def __init__(self, **kwargs):
@@ -57,11 +63,20 @@ class PESCalculator_Dist(_Calculator):
         self.state_attr = state_attr
         self.use_voigt = use_voigt
         self.last_count = None
+        # per-atom energies / stresses only exist when the potential computes them; the class attribute stays the
+        # reference's tuple
+        self.compute_atomic = bool(getattr(potential, "calc_atomic", False))
+        if self.compute_atomic:
+            self.implemented_properties = tuple(PESCalculator_Dist.implemented_properties) + ("energies", "stresses")
 
     def calculate(self, atoms, properties=None, system_changes=None):
         """ase.py:80-127."""
         properties = properties or ["energy"]
         system_changes = system_changes or _all_changes
+        missing = [p for p in ("energies", "stresses") if p in properties and not self.compute_atomic]
+        if missing:
+            raise _PropertyNotImplementedError(
+                f"{missing} need a potential built with Potential_Dist(..., calc_atomic=True)")
         _Calculator.calculate(self, atoms=atoms, properties=properties, system_changes=system_changes)
         calc_result = self.potential(atoms, self.state_attr)
         self.results.update(
@@ -74,6 +89,14 @@ class PESCalculator_Dist(_Calculator):
             self.results.update(stress=(_voigt6(st) if self.use_voigt else st) * self.stress_weight)
         if self.compute_magmom:
             self.results.update(magmoms=calc_result[4].detach().cpu().numpy())
+        if self.compute_atomic:
+            self.results.update(energies=self.potential.atomic_energies.detach().cpu().numpy())
+            if self.compute_stress and self.potential.atomic_stresses is not None:
+                st = self.potential.atomic_stresses.detach().cpu().numpy()  # [N,3,3] GPa, sums to `stress`
+                if self.use_voigt:
+                    st = np.stack([st[:, 0, 0], st[:, 1, 1], st[:, 2, 2], (st[:, 1, 2] + st[:, 2, 1]) / 2,
+                                   (st[:, 0, 2] + st[:, 2, 0]) / 2, (st[:, 0, 1] + st[:, 1, 0]) / 2], axis=1)
+                self.results.update(stresses=st * self.stress_weight)
 
 
 class TrajectoryObserver:

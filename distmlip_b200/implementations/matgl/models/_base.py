@@ -123,12 +123,19 @@ class EngineBackedModel:
     def potential_forward_dist(self, dist_info, atoms, lattice_matrix, calc_stresses, calc_forces, calc_hessian,
                                state_attr=None):
         """Seam of chgnet.py:21-30,199-206 / tensornet.py:10-19.  Returns (node_types, positions, strain, (E, site_wise));
-        forces / stress of the same evaluation are left on `dist_info` (no autograd graph exists)."""
+        forces / stress of the same evaluation are left on `dist_info` (no autograd graph exists), and so are the
+        per-atom (energies, virials) when `_want_atomic` is set (else None)."""
         if calc_hessian:
             raise NotImplementedError("Calculating hessians is not implemented for distributed inference.")
         eng = self._engine
+        # per-atom energies / virials only when the Potential asks for them (buffers and reductions exist only then)
+        want_atomic = bool(self.__dict__.get("_want_atomic", False))
+        if want_atomic != self.__dict__.get("_atomic_on", False):
+            eng.set_atomic(want_atomic)
+            self._atomic_on = want_atomic
         e, f, s = eng.compute(forces=calc_forces, stress=calc_stresses)
         dist_info.forces, dist_info.stress = f, s
+        dist_info.atomic = eng.atomic(virials=calc_forces or calc_stresses) if want_atomic else None
         node_types = torch.as_tensor(dist_info.species, dtype=distmlip_b200.int_th)
         positions = torch.from_numpy(dist_info.cart)  # zero-copy view (f64); no autograd graph hangs off it here
         strain = torch.zeros(1, 3, 3, dtype=distmlip_b200.float_th)

@@ -1,7 +1,9 @@
 """Potential_Dist -- drop-in for DistMLIP.implementations.matgl.pes.Potential_Dist (pes.py:13-146).
 
 Same constructor kwargs and call convention: `potential(atoms, state_attr=None, tol=1e-8)` returns
-`(energies, forces, stresses(GPa, 3x3), hessian=None[, site_wise])` as torch tensors.  Differences, all
+`(energies, forces, stresses(GPa, 3x3), hessian=None[, site_wise])` as torch tensors.  With `calc_atomic=True` (not in
+the reference) each call also sets `atomic_energies` (f64 [N], eV, summing to the energy) and `atomic_stresses` (f32
+[N,3,3], GPa, summing to the stress; None without forces and stress), see DESIGN.md for the convention.  Differences, all
 deliberate: one partition is allowed (the reference asserts > 1 GPU, pes.py:40-42); energy, forces and
 stress come out of one b2m_compute call (hand-written backward) instead of torch.autograd.backward
 (pes.py:122-124); results are CPU tensors (the ASE calculator immediately calls .cpu().numpy()).
@@ -23,7 +25,7 @@ class Potential_Dist:
 
     def __init__(self, model=None, num_threads=None, data_mean=0.0, data_std=1.0, element_refs=None,
                  calc_forces=True, calc_stresses=True, calc_hessian=False, calc_site_wise=False, debug_mode=False,
-                 calc_repuls=False, zbl_trainable=False, **kwargs):
+                 calc_repuls=False, zbl_trainable=False, calc_atomic=False, **kwargs):
         if model is None:
             raise ValueError("model is required")
         self.model = model
@@ -35,6 +37,8 @@ class Potential_Dist:
         self.calc_stresses = calc_stresses
         self.calc_hessian = calc_hessian
         self.calc_site_wise = calc_site_wise
+        self.calc_atomic = calc_atomic
+        self.atomic_energies = self.atomic_stresses = None
         self.debug_mode = debug_mode
         self.data_mean = float(torch.as_tensor(data_mean).item()) if data_mean is not None else 0.0
         self.data_std = float(torch.as_tensor(data_std).item()) if data_std is not None else 1.0
@@ -62,6 +66,7 @@ class Potential_Dist:
         model = self.model
         species = model._species_of(atoms)
         model._want_site = bool(self.calc_site_wise)
+        model._want_atomic = bool(self.calc_atomic)
         model._finalize(self.data_mean, self.data_std, self.element_refs)
         dist_info = Distributed.create_distributed(
             cart_coords=cart_coords, frac_coords=None, lattice_matrix=lattice_matrix,
@@ -77,6 +82,13 @@ class Potential_Dist:
             print("Debug mode true, returning early")
             return model_out[-1]
         _node_types, _positions, _strain, (total_energies, site_wise) = model_out
+        if self.calc_atomic:
+            energies, virials = dist_info.atomic
+            self.atomic_energies = torch.from_numpy(energies)
+            self.atomic_stresses = None
+            if virials is not None:  # w_i / V, in the unit and sign of `stresses` (pes.py:140-145)
+                vol = abs(np.linalg.det(lattice_matrix))
+                self.atomic_stresses = torch.from_numpy((virials.astype(np.float64) * (160.21766208 / vol)).astype(np.float32))
         forces = torch.as_tensor(dist_info.forces) if self.calc_forces else None
         stresses = torch.as_tensor(dist_info.stress) if self.calc_stresses else None
         hessian = None

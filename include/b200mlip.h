@@ -129,6 +129,18 @@ int b2m_compute_resident(b2m_handle h, int want_forces, int want_stress, int rep
  * forces [natoms][3] and stress [3][3] (GPa), as b2m_compute returns them; any pointer may be NULL. */
 int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9);
 
+/* Per-atom energies and virials (DESIGN.md "Per-atom energies and virials"), off by default.  With on != 0 the
+ * following evaluations (b2m_compute, b2m_compute_resident) also produce, for every atom i,
+ *   energies[i] = data_std * e_i + element_ref[Z_i] + data_mean / natoms   (eV; sums to the energy)
+ *   virials[i]  = 1/2 sum over the edges e with endpoint i of v_e (x) dE/dv_e   (eV, 3x3 row-major, not symmetrised;
+ *                 sums to the strain derivative of the energy, i.e. stress * volume / 160.21766208)
+ * With the flag off no buffer is allocated and no extra kernel or collective runs. */
+int b2m_set_atomic(b2m_handle h, int on);
+/* Per-atom results of the last evaluation (energies [natoms] or NULL, virials [natoms][9] or NULL), every partition
+ * layout, both model families.  B2M_ERR_STATE if that evaluation ran with the flag off, or if virials are asked for
+ * after an evaluation without a backward (want_forces = want_stress = 0). */
+int b2m_get_atomic(b2m_handle h, double* energies, float* virials);
+
 /* site-wise readout (magmom) for all atoms, [natoms] */
 int b2m_get_sitewise(b2m_handle h, float* out);
 
