@@ -16,9 +16,11 @@ import torch
 GPA_PER_EV_A3 = 160.21766208
 
 
-def atomic_ref(model, atoms, data_mean=0.0, data_std=1.0, element_refs=None, dtype=torch.float64):
+def atomic_ref(model, atoms, data_mean=0.0, data_std=1.0, element_refs=None, dtype=torch.float64, edges=False):
     """Returns a dict of torch tensors: energies [N], virials [N,3,3] (eV), energy (scalar), strain_virial [3,3]
-    (dE/d strain, eV), stress [3,3] (GPa), forces [N,3]."""
+    (dE/d strain, eV), stress [3,3] (GPa), forces [N,3].  With `edges=True` also the per-edge parts the virials are
+    made of, in the neighbour list's order: edge_src [E], edge_dst [E], edge_off [E,3] (int64 image of dst) and
+    edge_half [E,3,3] = 1/2 v_e (x) g_e, which goes once to each endpoint."""
     from oracle.graph_ref import neighbor_list
 
     tensornet = hasattr(model, "tensor_embedding")
@@ -59,5 +61,48 @@ def atomic_ref(model, atoms, data_mean=0.0, data_std=1.0, element_refs=None, dty
     half = 0.5 * vec.detach()[:, :, None] * g[:, None, :]  # [E,3,3]: 1/2 v_e (x) g_e
     vir = torch.zeros(n, 3, 3, dtype=dtype).index_add_(0, src, half).index_add_(0, dst, half)
     vol = abs(np.linalg.det(lattice_np))
-    return dict(energies=eps, virials=vir, energy=total.detach(), strain_virial=strain.grad.detach(),
-                stress=strain.grad.detach() / vol * GPA_PER_EV_A3, forces=-pos.grad.detach())
+    out = dict(energies=eps, virials=vir, energy=total.detach(), strain_virial=strain.grad.detach(),
+               stress=strain.grad.detach() / vol * GPA_PER_EV_A3, forces=-pos.grad.detach())
+    if edges:
+        out.update(edge_src=src, edge_dst=dst, edge_off=t(off), edge_half=half)
+    return out
+
+
+def routing_mutants(src, dst, half, n, order=None):
+    """Per-atom virials [N,3,3] of plausible routing bugs of a kernel that walks the edges in `order` (default: sorted
+    by destination, stably) one edge per lane, 32 lanes per warp, and adds the destination halves once per run of
+    equal destinations.  Returns {name: virials}; "next atom" is the destination of the following run (cyclically).
+
+      last_edge_to_next   the last edge of every run adds its destination half to the next atom
+      run_to_next         every run adds its destination halves to the next atom
+      all_to_dst          the source half goes to the destination as well
+      src_transposed      the source receives (1/2 v (x) g)^T
+      straddle_to_next    a run cut by a multiple of 32: the part before the last cut goes to the next atom
+    """
+    src, dst = torch.as_tensor(src), torch.as_tensor(dst)
+    if order is None:
+        order = torch.argsort(dst, stable=True)
+    order = torch.as_tensor(order)
+    s, d, h = src[order], dst[order], half[order]
+    E = len(d)
+    pos = torch.arange(E)
+    start = torch.ones(E, dtype=torch.bool)
+    start[1:] = d[1:] != d[:-1]
+    end = torch.ones(E, dtype=torch.bool)
+    end[:-1] = start[1:]
+    run = torch.cumsum(start.long(), 0) - 1
+    next_atom = d[start].roll(-1)[run]  # per edge: the destination of the following run
+    last = pos[end][run]                # per edge: position of its run's last edge
+    z = lambda: torch.zeros(n, 3, 3, dtype=h.dtype)
+    src_part = z().index_add_(0, s, h)
+
+    def with_dst(target):
+        return src_part + z().index_add_(0, target, h)
+
+    return {
+        "last_edge_to_next": with_dst(torch.where(pos == last, next_atom, d)),
+        "run_to_next": with_dst(next_atom),
+        "all_to_dst": z().index_add_(0, d, 2 * h),
+        "src_transposed": z().index_add_(0, s, h.transpose(1, 2)) + z().index_add_(0, d, h),
+        "straddle_to_next": with_dst(torch.where(pos // 32 < last // 32, next_atom, d)),
+    }

@@ -135,3 +135,41 @@ def test_calculator_energies_and_stresses():
     # the class attribute stays the reference's tuple
     assert mase.PESCalculator_Dist.implemented_properties == cls_props
     assert cls_props == ("energy", "free_energy", "forces", "stress", "hessian", "magmoms")
+
+
+# ------------------------------------------------------------------ the GPU tolerances against routing bugs
+# A kernel that adds an edge's half (or an atom's energy) to the wrong atom keeps both sum rules; only the per-atom
+# comparison of tests/test_gpu_atomic.py sees it.  Its tolerances must stay far below what such bugs do.  The bugs are
+# built from the oracle's per-edge halves in destination-sorted order (oracle.atomic_ref.routing_mutants); the
+# 4000-atom GPU test repeats this in the engine's own edge order.
+def gpu_structures():
+    from tests.test_gpu_atomic import STRUCTURES, calculator_cell, irregular, slab
+
+    return dict(STRUCTURES, slab=slab, calculator=calculator_cell, irregular=irregular)
+
+
+@pytest.mark.parametrize("family", ["chgnet", "tensornet"])
+@pytest.mark.parametrize("structure", ["diamond64", "diamond512", "rough", "slab", "calculator", "irregular"])
+def test_gpu_tolerances_are_far_below_routing_bugs(family, structure):
+    from oracle.atomic_ref import routing_mutants
+    from tests.test_gpu_atomic import TOL_EPS, TOL_W
+
+    # fp32 round-off, not accuracy targets: no looser than 1e-3 of max |w| and 2e-6 eV, whatever the margins below allow
+    assert TOL_W[family] <= 1e-3 and TOL_EPS <= 2e-6
+    atoms = gpu_structures()[structure]()
+    model = model_of(family)
+    r = atomic_ref(model, atoms, element_refs=refs(model), edges=True, **SCALING)
+    w, src, dst, half = r["virials"], r["edge_src"], r["edge_dst"], r["edge_half"]
+    bound = TOL_W[family] * float(w.abs().max())  # eV: the largest per-atom virial error the GPU tests accept
+    errs = {name: float((wm - w).abs().max()) for name, wm in routing_mutants(src, dst, half, len(atoms)).items()}
+    if family == "chgnet":
+        # CHGNet's per-atom virials are symmetric to 1e-4 of max |w|: only TensorNet can show a transposition
+        assert errs.pop("src_transposed") < 1e-3 * float(w.abs().max())
+    for name, err in errs.items():
+        assert err >= 10 * bound, (name, err, bound)
+    # a single misrouted edge of median size is 10x above the tolerance
+    edge = half.abs().amax((1, 2))
+    assert bound <= 0.1 * float(edge.median()), (bound, float(edge.median()))
+    # an atom's energy on one of its neighbours: 10x above the tolerance for 90 % of the edges
+    eps = r["energies"]
+    assert TOL_EPS <= 0.1 * float((eps[src] - eps[dst]).abs().quantile(0.1))
