@@ -18,7 +18,7 @@ SYMBOLS = [
     "b2m_finalize_weights", "b2m_set_scaling", "b2m_comm_unique_id", "b2m_comm_init", "b2m_set_partition", "b2m_set_structure", "b2m_compute",
     "b2m_compute_resident", "b2m_get_results", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
     "b2m_debug_tensor", "b2m_last_timings", "b2m_release_workspace", "b2m_set_view", "b2m_create_tensornet",
-    "b2m_set_atomic", "b2m_get_atomic",
+    "b2m_set_atomic", "b2m_get_atomic", "b2m_set_heat_flux", "b2m_compute_heat_flux",
 ]
 
 
@@ -86,6 +86,8 @@ def load_library():
     lib.b2m_set_view.argtypes = [vp, i32]
     lib.b2m_set_atomic.argtypes = [vp, i32]
     lib.b2m_get_atomic.argtypes = [vp, P(dbl), P(C.c_float)]
+    lib.b2m_set_heat_flux.argtypes = [vp, dbl]
+    lib.b2m_compute_heat_flux.argtypes = [vp, P(dbl), P(dbl), P(C.c_float), P(C.c_float), P(dbl)]
     for s in SYMBOLS:
         if s not in ("b2m_last_error", "b2m_get_partition_info"):
             getattr(lib, s).restype = C.c_int
@@ -235,6 +237,24 @@ class Engine:
         self._ck(self.lib.b2m_get_atomic(self.h, e.ctypes.data_as(C.POINTER(C.c_double)),
                                          w.ctypes.data_as(C.POINTER(C.c_float)) if virials else None))
         return e, w
+
+    def set_heat_flux(self, reach):
+        """reach > 0 (Angstrom): the following set_structure calls build the unfolded cell (images within `reach`), on
+        which compute() returns the periodic results and compute_heat_flux() the flux; 0 switches back"""
+        self._ck(self.lib.b2m_set_heat_flux(self.h, float(reach)))
+
+    def compute_heat_flux(self, velocities):
+        """energy, forces [natoms, 3], stress [3, 3] and (J_pot [3], J_conv [3]) in eV * velocity unit (not divided
+        by the volume) for velocities [natoms, 3]"""
+        v = np.ascontiguousarray(velocities, dtype=np.float64).reshape(self.natoms, 3)
+        e = C.c_double()
+        f = np.empty((self.natoms, 3), dtype=np.float32)
+        s = np.empty(9, dtype=np.float32)
+        j = np.empty(6, dtype=np.float64)
+        self._ck(self.lib.b2m_compute_heat_flux(
+            self.h, v.ctypes.data_as(C.POINTER(C.c_double)), C.byref(e), f.ctypes.data_as(C.POINTER(C.c_float)),
+            s.ctypes.data_as(C.POINTER(C.c_float)), j.ctypes.data_as(C.POINTER(C.c_double))))
+        return e.value, f, s.reshape(3, 3), (j[:3].copy(), j[3:].copy())
 
     def set_view(self, part):
         """single-process group: the partition that counts() / partition_info() describe"""

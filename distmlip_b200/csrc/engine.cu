@@ -181,6 +181,17 @@ struct b2m_engine {
   DBuf<float> atom_vir;     // [N][kVirPitch]
   DBuf<double> aesum, aetmp;  // leader of a group: the summed energies / staging of a peer's array
   DBuf<float> avsum, avtmp;   // same for the virials
+  // heat flux (b2m_set_heat_flux; DESIGN.md §10): with hf_reach > 0 b2m_set_structure builds the unfolded cell (`uf`) and
+  // the graph of it without periodicity; every readout then weights atom j's energy by hf_w[j]
+  double hf_reach = 0;
+  Unfold uf;
+  int64_t hf_n = 0;       // cell atoms of the resident unfolded graph; 0: the graph is the structure itself
+  int hf_seed = -1;       // weight of the next evaluation: -1 the cell mask (1 / 0), 0..2 the seed (r_j - c)_alpha
+  double hf_c[3] = {0, 0, 0};  // cell centre
+  DBuf<float> hf_w;       // [N] readout weight of every unfolded atom
+  DBuf<float> hf_G;       // leader: [3][N][3] forces of the three seeded passes
+  DBuf<float> hf_fold;    // leader: folded forces [n][3] or virials [n][kVirPitch]
+  DBuf<double> hf_vel, hf_out;
   // timings
   cudaEvent_t ev[8] = {nullptr};
   double t_graph = 0, t_fwd = 0, t_bwd = 0, t_gather = 0, t_total = 0;
@@ -195,6 +206,9 @@ struct b2m_engine {
 };
 
 namespace b2m {
+
+// atoms of the structure the caller passed: the graph's atoms, or the cell atoms of an unfolded graph
+static int64_t cell_atoms(const b2m_engine* e) { return e->hf_n ? e->hf_n : e->g.N; }
 
 static const std::vector<float>& W(b2m_engine* e, const std::string& k, std::vector<int64_t> shape) {
   auto it = e->host_w.find(k);
@@ -811,7 +825,8 @@ static void forward(b2m_engine* e) {
   launch_silu(e->st, (int64_t)g.n_own * D, e->y2p.p, e->y2.p);
   B2M_CK(cudaMemsetAsync(e->scal.p, 0, 16 * sizeof(double), e->st));
   launch_rowdot(e->st, g.n_own, e->y2.p, e->d_F2, e->c2, e->e_atom.p, e->scal.p, g.type.p, e->d_eref,
-                (float)e->desc.data_std, g.gid.p, e->atomic ? e->atom_e.p : nullptr, e->desc.data_mean / g.N);
+                (float)e->desc.data_std, g.gid.p, e->atomic ? e->atom_e.p : nullptr, e->desc.data_mean / cell_atoms(e),
+                e->hf_n ? e->hf_w.p : nullptr);
 }
 
 static void backward(b2m_engine* e) {
@@ -825,7 +840,8 @@ static void backward(b2m_engine* e) {
   launch_zero_rows(e->st, e->gx.p, (int64_t)g.n_loc * D);
   launch_zero_rows(e->st, e->forces.p, g.N * 3);
   // readout backward
-  launch_readout_seed(e->st, g.n_own, e->y2p.p, e->d_F2, (float)e->desc.data_std, e->gy2.p);
+  launch_readout_seed(e->st, g.n_own, e->y2p.p, e->d_F2, (float)e->desc.data_std, e->gy2.p, g.gid.p,
+                      e->hf_n ? e->hf_w.p : nullptr);
   gemm(e, e->gy2.p, D, e->d_F1raw, e->gy1.p, D, g.n_own, D, D, nullptr, nullptr, 0, false);
   launch_dsilu_mul(e->st, (int64_t)g.n_own * D, e->y1p.p, e->gy1.p);
   gemm(e, e->gy1.p, D, e->d_F0raw, e->gx.p, D, g.n_own, D, D, nullptr, nullptr, 0, false);
@@ -858,6 +874,73 @@ static void backward(b2m_engine* e) {
                          e->forces.p, e->scal.p + 1, avir);
 }
 
+// ------------------------------------------------------------------------------------------
+// heat flux (DESIGN.md §10)
+#define LAUNCH_HF(kern, n, st, ...)                              \
+  do {                                                           \
+    if ((n) > 0) {                                               \
+      kern<<<cdiv((n), 256), 256, 0, st>>>(__VA_ARGS__);         \
+      B2M_CK(cudaGetLastError());                                \
+      g_launch_count++;                                          \
+    }                                                            \
+  } while (0)
+
+// readout weight of every unfolded atom: images 0; cell atoms 1 (alpha < 0, the mask) or (r_j - c)_alpha (a seed)
+__global__ void k_hf_weights(int64_t N, int64_t n, const double* __restrict__ cart, double cx, double cy, double cz,
+                             int alpha, float* __restrict__ w) {
+  const int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (j >= N) return;
+  const double c = alpha == 0 ? cx : alpha == 1 ? cy : cz;
+  w[j] = j >= n ? 0.f : alpha < 0 ? 1.f : (float)(cart[3 * j + alpha] - c);
+}
+
+// out[image_of[j]][k] += src[j][k], k < width, rows of `pitch` floats (out zeroed before)
+__global__ void k_hf_fold(int64_t N, const int* __restrict__ image_of, int width, int pitch,
+                          const float* __restrict__ src, float* __restrict__ out) {
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t >= N * width) return;
+  const int64_t j = t / width;
+  const int k = (int)(t - j * width);
+  atomicAdd(&out[(int64_t)image_of[j] * pitch + k], src[j * pitch + k]);
+}
+
+// J_pot^a = sum_j [ -F^a_j . v_j + (r_j - c)_a (F_j . v_j) ] over all unfolded atoms (F^a: forces of seed a, i.e. -G^a;
+// F: forces of the masked pass; v_j the velocity of the cell atom j is an image of), J_conv^a = sum_{i<n} eps_i v_i,a.
+// out[0..2] = J_pot, out[3..5] = J_conv, accumulated in f64.
+__global__ void __launch_bounds__(256) k_hf_contract(int64_t N, int64_t n, const double* __restrict__ cart, double cx,
+                                                     double cy, double cz, const int* __restrict__ image_of,
+                                                     const double* __restrict__ vel, const float* __restrict__ F,
+                                                     const float* __restrict__ FS, const double* __restrict__ eps,
+                                                     double* __restrict__ out) {
+  double acc[6] = {0, 0, 0, 0, 0, 0};
+  for (int64_t j = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; j < N; j += (int64_t)gridDim.x * blockDim.x) {
+    const int i = image_of[j];
+    const double v[3] = {vel[3 * i], vel[3 * i + 1], vel[3 * i + 2]};
+    const double fv = F[3 * j] * v[0] + F[3 * j + 1] * v[1] + F[3 * j + 2] * v[2];
+    const double r[3] = {cart[3 * j] - cx, cart[3 * j + 1] - cy, cart[3 * j + 2] - cz};
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      const float* Fa = FS + (size_t)a * N * 3 + 3 * j;
+      acc[a] += r[a] * fv - (Fa[0] * v[0] + Fa[1] * v[1] + Fa[2] * v[2]);
+      if (j < n) acc[3 + a] += eps[j] * v[a];
+    }
+  }
+  __shared__ double red[6][8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < 6; k++) {
+    double x = acc[k];
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    if (lane == 0) red[k][warp] = x;
+  }
+  __syncthreads();
+  if (threadIdx.x < 6) {
+    double s = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += red[threadIdx.x][w];
+    atomicAdd(&out[threadIdx.x], s);
+  }
+}
+
 static void run(b2m_engine* e, bool grads) {
   B2M_REQUIRE(e->finalized, B2M_ERR_STATE, "weights not finalized");
   B2M_REQUIRE(e->have_graph, B2M_ERR_STATE, "b2m_set_structure has not been called");
@@ -882,6 +965,10 @@ static void run(b2m_engine* e, bool grads) {
     }
   }
   e->atomic_last = 0;
+  if (e->hf_n) {
+    LAUNCH_HF(k_hf_weights, e->g.N, e->st, e->g.N, e->hf_n, e->g.cart.p, e->hf_c[0], e->hf_c[1], e->hf_c[2], e->hf_seed,
+              e->hf_w.p);
+  }
   if (e->kind == 1) tn_forward(e); else forward(e);
   B2M_CK(cudaEventRecord(e->ev[1], e->st));
   if (grads) {
@@ -997,23 +1084,37 @@ static void run_any(b2m_engine* e, bool grads) {
   e->launches_last = launches;
 }
 
+// forces [N][3] of the whole structure on the leader's device: a group sums its partitions' arrays, a multi-process run
+// has all-reduced them in run()
+static const float* summed_forces(b2m_engine* e) {
+  if (e->parts.empty()) return e->forces.p;
+  const size_t n = (size_t)e->g.N * 3;
+  e->ftmp.ensure(n + 64);
+  e->fsum.ensure(n + 64);
+  B2M_CK(cudaMemcpyAsync(e->fsum.p, e->forces.p, n * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
+  for (size_t p = 1; p < e->parts.size(); p++) {
+    B2M_CK(cudaMemcpyAsync(e->ftmp.p, e->parts[p]->forces.p, n * sizeof(float), cudaMemcpyDefault, e->st));
+    k_add_inplace<<<cdiv((int64_t)n, 256), 256, 0, e->st>>>((int64_t)n, e->ftmp.p, e->fsum.p);
+    B2M_CK(cudaGetLastError());
+  }
+  return e->fsum.p;
+}
+
+// unfolded graph: rows [N][pitch] of every unfolded atom summed onto their cell atoms -> [n][pitch] (hf_fold)
+static const float* fold_rows(b2m_engine* e, const float* src, int width, int pitch) {
+  const int64_t N = e->g.N, n = e->hf_n;
+  e->hf_fold.ensure((size_t)n * pitch + 64);
+  e->hf_fold.zero((size_t)n * pitch, e->st);
+  LAUNCH_HF(k_hf_fold, N * width, e->st, N, e->uf.image_of.p, width, pitch, src, e->hf_fold.p);
+  return e->hf_fold.p;
+}
+
 static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) {
   double hs[10];
   B2M_CK(cudaMemcpyAsync(hs, e->scal.p, 10 * sizeof(double), cudaMemcpyDeviceToHost, e->st));
-  const float* fsrc = e->forces.p;
-  if (!e->parts.empty() && forces) {  // group: sum the partitions' force arrays on the leader's device
-    const size_t n = (size_t)e->g.N * 3;
-    e->ftmp.ensure(n + 64);
-    e->fsum.ensure(n + 64);
-    B2M_CK(cudaMemcpyAsync(e->fsum.p, e->forces.p, n * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
-    for (size_t p = 1; p < e->parts.size(); p++) {
-      B2M_CK(cudaMemcpyAsync(e->ftmp.p, e->parts[p]->forces.p, n * sizeof(float), cudaMemcpyDefault, e->st));
-      k_add_inplace<<<cdiv((int64_t)n, 256), 256, 0, e->st>>>((int64_t)n, e->ftmp.p, e->fsum.p);
-      B2M_CK(cudaGetLastError());
-    }
-    fsrc = e->fsum.p;
-  }
-  const size_t fbytes = (size_t)e->g.N * 3 * sizeof(float);
+  const float* fsrc = forces ? summed_forces(e) : nullptr;
+  if (forces && e->hf_n) fsrc = fold_rows(e, fsrc, 3, 3);  // periodic forces F_i = sum of F~ over i and its images
+  const size_t fbytes = (size_t)cell_atoms(e) * 3 * sizeof(float);
   if (forces) {
     ensure_pinned(e->pin_out, e->pin_out_cap, fbytes);
     B2M_CK(cudaMemcpyAsync(e->pin_out, fsrc, fbytes, cudaMemcpyDeviceToHost, e->st));
@@ -1038,7 +1139,7 @@ static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) 
 // device (energies: each atom has one owner; virials: every partition adds the edges and bond parts it holds), a
 // multi-process run has all-reduced them in run()
 static void fetch_atomic(b2m_engine* e, double* energies, float* virials) {
-  const size_t N = (size_t)e->g.N;
+  const size_t N = (size_t)cell_atoms(e), NG = (size_t)e->g.N;  // unfolded graph: cell atoms out, all atoms summed
   const double* esrc = e->atom_e.p;
   const float* vsrc = e->atom_vir.p;
   if (!e->parts.empty()) {
@@ -1053,10 +1154,12 @@ static void fetch_atomic(b2m_engine* e, double* energies, float* virials) {
       }
       return total.p;
     };
-    if (energies) esrc = sum(e->aesum, e->aetmp, [](b2m_engine* m) -> DBuf<double>& { return m->atom_e; }, N, k_add_inplace_f64);
+    if (energies) esrc = sum(e->aesum, e->aetmp, [](b2m_engine* m) -> DBuf<double>& { return m->atom_e; }, NG, k_add_inplace_f64);
     if (virials)
-      vsrc = sum(e->avsum, e->avtmp, [](b2m_engine* m) -> DBuf<float>& { return m->atom_vir; }, N * kVirPitch, k_add_inplace);
+      vsrc = sum(e->avsum, e->avtmp, [](b2m_engine* m) -> DBuf<float>& { return m->atom_vir; }, NG * kVirPitch, k_add_inplace);
   }
+  // images carry no energy (weight 0); their virial halves belong to the cell atoms they are images of
+  if (virials && e->hf_n) vsrc = fold_rows(e, vsrc, 9, kVirPitch);
   const size_t vbytes = N * kVirPitch * sizeof(float);
   if (virials) {
     ensure_pinned(e->pin_out, e->pin_out_cap, vbytes);
@@ -1068,6 +1171,60 @@ static void fetch_atomic(b2m_engine* e, double* energies, float* virials) {
     const float* w = static_cast<const float*>(e->pin_out);
     for (size_t i = 0; i < N; i++) memcpy(virials + i * 9, w + i * kVirPitch, 9 * sizeof(float));
   }
+}
+
+// One forward + backward per readout weight: the three seeds (r_j - c)_alpha, then the cell mask, so that the handle is
+// left holding the masked (periodic) evaluation for fetch / b2m_get_results / b2m_get_atomic.  Every pass re-runs the
+// forward: the backward recomputes its projection buffers in place, so a second backward on the same forward state is
+// not possible without keeping copies of them.
+static void heat_flux(b2m_engine* h, const double* vel, double* flux6) {
+  const int64_t N = h->g.N, n = h->hf_n;
+  const std::vector<b2m_engine*> members = h->parts.empty() ? std::vector<b2m_engine*>{h} : h->parts;
+  std::vector<bool> atomic_flag;
+  for (auto* e : members) atomic_flag.push_back(e->atomic);
+  auto restore = [&] {  // the handle's own state: masked readout, its b2m_set_atomic flag
+    for (size_t k = 0; k < members.size(); k++) members[k]->hf_seed = -1, members[k]->atomic = atomic_flag[k];
+  };
+  try {
+    h->hf_G.ensure((size_t)N * 9 + 64);
+    for (int a = 0; a < 3; a++) {
+      for (auto* e : members) e->hf_seed = a;
+      run_any(h, true);
+      B2M_CK(cudaMemcpyAsync(h->hf_G.p + (size_t)a * N * 3, summed_forces(h), (size_t)N * 3 * sizeof(float),
+                             cudaMemcpyDeviceToDevice, h->st));
+    }
+    // the masked pass also writes the per-atom energies (J_conv) whatever the handle's b2m_set_atomic flag
+    for (auto* e : members) e->hf_seed = -1, e->atomic = true;
+    run_any(h, true);
+  } catch (...) {
+    restore();
+    throw;
+  }
+  restore();
+  const float* F = summed_forces(h);
+  const double* eps = h->atom_e.p;
+  if (!h->parts.empty()) {
+    h->aesum.ensure(N + 64);
+    h->aetmp.ensure(N + 64);
+    B2M_CK(cudaMemcpyAsync(h->aesum.p, h->atom_e.p, N * sizeof(double), cudaMemcpyDeviceToDevice, h->st));
+    for (size_t p = 1; p < h->parts.size(); p++) {
+      B2M_CK(cudaMemcpyAsync(h->aetmp.p, h->parts[p]->atom_e.p, N * sizeof(double), cudaMemcpyDefault, h->st));
+      k_add_inplace_f64<<<cdiv(N, 256), 256, 0, h->st>>>(N, h->aetmp.p, h->aesum.p);
+      B2M_CK(cudaGetLastError());
+    }
+    eps = h->aesum.p;
+  }
+  h->hf_vel.ensure((size_t)n * 3 + 64);
+  h->hf_out.ensure(64);
+  B2M_CK(cudaMemcpyAsync(h->hf_vel.p, vel, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->st));
+  h->hf_out.zero(6, h->st);
+  const int grid = std::max(1, std::min(cdiv(N, 256), 4 * h->num_sms));
+  k_hf_contract<<<grid, 256, 0, h->st>>>(N, n, h->g.cart.p, h->hf_c[0], h->hf_c[1], h->hf_c[2], h->uf.image_of.p,
+                                         h->hf_vel.p, F, h->hf_G.p, eps, h->hf_out.p);
+  B2M_CK(cudaGetLastError());
+  g_launch_count++;
+  B2M_CK(cudaMemcpyAsync(flux6, h->hf_out.p, 6 * sizeof(double), cudaMemcpyDeviceToHost, h->st));
+  B2M_CK(cudaStreamSynchronize(h->st));
 }
 
 }  // namespace b2m
@@ -1357,8 +1514,22 @@ static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart,
   }
   B2M_CK(cudaEventRecord(h->ev[3], h->st));
   h->atomic_last = 0;  // per-atom results of an earlier structure are gone
-  h->g.build(h->st, natoms, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff, tol, h->rank,
-             h->world);
+  h->hf_n = 0, h->hf_seed = -1;
+  if (h->hf_reach > 0) {
+    // heat flux: the unfolded cell, built on the device, is the graph's input; no periodicity
+    h->uf.build(h->st, natoms, cart, species, lattice9, pbc3, h->hf_reach);
+    const int no_pbc[3] = {0, 0, 0};
+    h->g.walls_from_min = true;
+    h->g.build(h->st, h->uf.N, h->uf.cart.p, lattice9, h->uf.species.p, no_pbc, h->desc.cutoff,
+               h->desc.three_body_cutoff, tol, h->rank, h->world);
+    h->hf_n = natoms;
+    h->hf_w.ensure((size_t)h->uf.N + 64);
+    for (int m = 0; m < 3; m++) h->hf_c[m] = 0.5 * (lattice9[m] + lattice9[3 + m] + lattice9[6 + m]);
+  } else {
+    h->g.walls_from_min = false;
+    h->g.build(h->st, natoms, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff, tol, h->rank,
+               h->world);
+  }
   if (h->kind == 1) tn_alloc_workspace(h); else alloc_workspace(h);
   B2M_CK(cudaEventRecord(h->ev[4], h->st));
   B2M_CK(cudaStreamSynchronize(h->st));
@@ -1404,6 +1575,25 @@ int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9)
   API_END
 }
 
+int b2m_set_heat_flux(b2m_handle h, double reach) {
+  API_BEGIN
+  B2M_REQUIRE(reach >= 0 && std::isfinite(reach), B2M_ERR_INVALID, "heat-flux reach must be >= 0");
+  each_member(h, [&](b2m_engine* e) { e->hf_reach = reach; });
+  API_END
+}
+
+int b2m_compute_heat_flux(b2m_handle h, const double* vel, double* energy, float* forces, float* stress9,
+                          double* flux6) {
+  API_BEGIN
+  B2M_REQUIRE(vel && flux6, B2M_ERR_INVALID, "velocities and flux6 are required");
+  B2M_REQUIRE(h->hf_reach > 0, B2M_ERR_STATE, "heat flux is off (b2m_set_heat_flux(h, reach > 0) first)");
+  B2M_REQUIRE(h->have_graph && h->hf_n > 0, B2M_ERR_STATE,
+              "the resident structure is not unfolded (b2m_set_structure after b2m_set_heat_flux)");
+  heat_flux(h, vel, flux6);
+  fetch(h, energy, forces, stress9);
+  API_END
+}
+
 int b2m_set_atomic(b2m_handle h, int on) {
   API_BEGIN
   each_member(h, [&](b2m_engine* e) { e->atomic = on != 0; });
@@ -1443,7 +1633,7 @@ int b2m_get_sitewise(b2m_handle h, float* out) {
     B2M_CK(cudaMemcpyAsync(full.data(), h->site_full.p, g.N * sizeof(float), cudaMemcpyDeviceToHost, h->st));
     B2M_CK(cudaStreamSynchronize(h->st));
   }
-  memcpy(out, full.data(), g.N * sizeof(float));
+  memcpy(out, full.data(), cell_atoms(h) * sizeof(float));  // unfolded graph: the cell atoms come first
   API_END
 }
 
@@ -1543,10 +1733,13 @@ int b2m_release_workspace(b2m_handle h) {
                     &e->e_atom, &e->site, &e->gx, &e->gh, &e->gang, &e->gA, &e->gC, &e->gQ, &e->gHa, &e->gHb, &e->gXc,
                     &e->gagg, &e->gupd, &e->gaggB, &e->gd, &e->gdb, &e->gbvec, &e->gy1, &e->gy2, &e->forces,
                     &e->sendbuf, &e->recvbuf, &e->site_full, &e->precv[0], &e->precv[1], &e->ftmp, &e->fsum,
-                    &e->atom_vir, &e->avsum, &e->avtmp})
+                    &e->atom_vir, &e->avsum, &e->avtmp, &e->hf_w, &e->hf_G, &e->hf_fold})
       drop(*b);
-    for (auto* b : {&e->atom_e, &e->aesum, &e->aetmp}) drop(*b);
+    for (auto* b : {&e->atom_e, &e->aesum, &e->aetmp, &e->hf_vel, &e->hf_out}) drop(*b);
     e->atomic_last = 0;
+    e->hf_n = 0;
+    e->uf.~Unfold();
+    new (&e->uf) Unfold();
     tn_release(e);
     e->g.~Graph();  // the resident graph goes too
     new (&e->g) Graph();

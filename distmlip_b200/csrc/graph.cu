@@ -492,6 +492,65 @@ __global__ void k_fill_i(int64_t n, int* p, int v) {
 }
 
 // ---------------------------------------------------------------------------------------------
+// unfolded cell (heat flux)
+struct UnfoldBox {
+  double lat[9], inv[9];
+  double lo[3], hi[3];  // admitted fractional range per axis
+  int smin[3], smax[3];  // image shifts to try (0, 0 along non-periodic axes)
+};
+
+__global__ void k_unfold_frac(int64_t n, const double* __restrict__ cart, UnfoldBox b, double* __restrict__ frac) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  for (int j = 0; j < 3; j++)
+    frac[3 * i + j] = cart[3 * i] * b.inv[j] + cart[3 * i + 1] * b.inv[3 + j] + cart[3 * i + 2] * b.inv[6 + j];
+}
+
+__device__ __forceinline__ bool unfold_admits(const UnfoldBox& b, int k, double f, int s) {
+  if (b.smin[k] == 0 && b.smax[k] == 0) return s == 0;  // non-periodic axis (or no room for an image)
+  const double g = f + s;
+  return g >= b.lo[k] && g <= b.hi[k];
+}
+
+// cnt[i] = number of images of atom i (shift s != 0 with every coordinate admitted)
+__global__ void k_unfold_count(int64_t n, const double* __restrict__ frac, UnfoldBox b, int* __restrict__ cnt) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int c[3];
+  for (int k = 0; k < 3; k++) {
+    c[k] = 0;
+    for (int s = b.smin[k]; s <= b.smax[k]; s++) c[k] += unfold_admits(b, k, frac[3 * i + k], s) ? 1 : 0;
+  }
+  cnt[i] = c[0] * c[1] * c[2] - 1;  // the atom itself (s = 0) is always admitted
+}
+
+// the cell atom at row i, its images at rows n + off[i] + (0, 1, ...) in (s0, s1, s2) lexicographic order
+__global__ void k_unfold_fill(int64_t n, const double* __restrict__ cart0, const int* __restrict__ spec0,
+                              const double* __restrict__ frac, const int* __restrict__ off, UnfoldBox b,
+                              double* __restrict__ cart, int* __restrict__ spec, int* __restrict__ image_of) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double x = cart0[3 * i], y = cart0[3 * i + 1], z = cart0[3 * i + 2];
+  const int sp = spec0[i];
+  cart[3 * i] = x, cart[3 * i + 1] = y, cart[3 * i + 2] = z;
+  spec[i] = sp, image_of[i] = (int)i;
+  int64_t o = n + off[i];
+  for (int s0 = b.smin[0]; s0 <= b.smax[0]; s0++) {
+    if (!unfold_admits(b, 0, frac[3 * i], s0)) continue;
+    for (int s1 = b.smin[1]; s1 <= b.smax[1]; s1++) {
+      if (!unfold_admits(b, 1, frac[3 * i + 1], s1)) continue;
+      for (int s2 = b.smin[2]; s2 <= b.smax[2]; s2++) {
+        if (!unfold_admits(b, 2, frac[3 * i + 2], s2) || (s0 == 0 && s1 == 0 && s2 == 0)) continue;
+        for (int m = 0; m < 3; m++)
+          cart[3 * o + m] = (m == 0 ? x : m == 1 ? y : z) + s0 * b.lat[m] + s1 * b.lat[3 + m] + s2 * b.lat[6 + m];
+        spec[o] = sp, image_of[o] = (int)i;
+        o++;
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 static void inv3(const double* m, double* o, double& det) {
   det = m[0] * (m[4] * m[8] - m[5] * m[7]) - m[1] * (m[3] * m[8] - m[5] * m[6]) + m[2] * (m[3] * m[7] - m[4] * m[6]);
   double id = 1.0 / det;
@@ -570,8 +629,9 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   tmp_i2.ensure(N + 1);
   tmp_i3.ensure(N + 1);
   tmp_flag.ensure(2 * N + 16);
-  B2M_CK(cudaMemcpyAsync(cart.p, h_cart, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
-  B2M_CK(cudaMemcpyAsync(species.p, h_species, N * sizeof(int), cudaMemcpyHostToDevice, st));
+  // host staging, or the device arrays of an Unfold
+  B2M_CK(cudaMemcpyAsync(cart.p, h_cart, 3 * N * sizeof(double), cudaMemcpyDefault, st));
+  B2M_CK(cudaMemcpyAsync(species.p, h_species, N * sizeof(int), cudaMemcpyDefault, st));
   for (int k = 0; k < 3; k++) {
     gp.nc[k] = 1;
     gp.reach[k] = 1;
@@ -629,7 +689,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     }
     // check_partition_size (:1512-1529): lattice *column* of the axis, width = walls[0] * |col|
     double col[3] = {lat[longest], lat[longest + 3], lat[longest + 6]};
-    double width = wl.w[0] * sqrt(col[0] * col[0] + col[1] * col[1] + col[2] * col[2]);
+    double width = (wl.w[0] - (walls_from_min ? fmn : 0.0)) * sqrt(col[0] * col[0] + col[1] * col[1] + col[2] * col[2]);
     double need = 2 * (rcut + rbond);
     if (width <= need) {
       char buf[256];
@@ -1008,6 +1068,60 @@ int64_t Graph::export_info(cudaStream_t st, int which, int64_t* out, int64_t cap
     default:
       throw Error(B2M_ERR_INVALID, "unknown partition-info selector");
   }
+}
+
+void Unfold::build(cudaStream_t st, int64_t natoms, const double* h_cart, const int32_t* h_species,
+                   const double* h_lat, const int* h_pbc, double reach) {
+  B2M_REQUIRE(natoms > 0 && natoms < (1LL << 31) / 4, B2M_ERR_INVALID, "natoms out of range");
+  B2M_REQUIRE(reach > 0, B2M_ERR_INVALID, "heat-flux reach must be > 0");
+  n = natoms;
+  UnfoldBox b;
+  double det;
+  memcpy(b.lat, h_lat, sizeof b.lat);
+  inv3(b.lat, b.inv, det);
+  B2M_REQUIRE(fabs(det) > 1e-12, B2M_ERR_INVALID, "singular lattice");
+  cart0.ensure(3 * n);
+  frac0.ensure(3 * n);
+  species0.ensure(n);
+  cnt.ensure(n + 1);
+  off.ensure(n + 1);
+  B2M_CK(cudaMemcpyAsync(cart0.p, h_cart, 3 * n * sizeof(double), cudaMemcpyDefault, st));
+  B2M_CK(cudaMemcpyAsync(species0.p, h_species, n * sizeof(int), cudaMemcpyDefault, st));
+  LAUNCH1D(k_unfold_frac, n, st, n, cart0.p, b, frac0.p);
+  // fractional bounding box of the cell atoms (k_minmax's Cartesian half reads the positions and is not used)
+  const int RB = 256;
+  red_tmp.ensure(RB * 12);
+  k_minmax<<<RB, 256, 0, st>>>(n, cart0.p, frac0.p, red_tmp.p);
+  B2M_CK(cudaGetLastError());
+  std::vector<double> hred(RB * 12);
+  B2M_CK(cudaMemcpyAsync(hred.data(), red_tmp.p, RB * 12 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaStreamSynchronize(st));
+  for (int k = 0; k < 3; k++) {
+    double fmn = 1e300, fmx = -1e300;
+    for (int r = 0; r < RB; r++) {
+      fmn = std::min(fmn, hred[r * 12 + 3 + k]);
+      fmx = std::max(fmx, hred[r * 12 + 9 + k]);
+    }
+    b.smin[k] = b.smax[k] = 0;
+    b.lo[k] = fmn, b.hi[k] = fmx;
+    if (h_pbc[k]) {
+      // reach / h_k in fractional units: |column k of inv| = 1 / h_k
+      const double pad = reach * sqrt(b.inv[k] * b.inv[k] + b.inv[3 + k] * b.inv[3 + k] + b.inv[6 + k] * b.inv[6 + k]);
+      b.lo[k] = fmn - pad, b.hi[k] = fmx + pad;
+      b.smin[k] = (int)ceil(b.lo[k] - fmx), b.smax[k] = (int)floor(b.hi[k] - fmn);
+      B2M_REQUIRE(b.smax[k] - b.smin[k] < 4096, B2M_ERR_INVALID, "heat-flux reach far larger than the cell");
+    }
+  }
+  LAUNCH1D(k_unfold_count, n, st, n, frac0.p, b, cnt.p);
+  B2M_CK(cudaMemsetAsync(cnt.p + n, 0, sizeof(int), st));
+  excl_scan(cub_tmp, cnt.p, off.p, n + 1, st);
+  const int64_t n_img = read_int(off.p + n, st);
+  N = n + n_img;
+  B2M_REQUIRE(N < (1LL << 31) / 4, B2M_ERR_INVALID, "unfolded cell too large");
+  cart.ensure(3 * N);
+  species.ensure(N);
+  image_of.ensure(N);
+  LAUNCH1D(k_unfold_fill, n, st, n, cart0.p, species0.p, frac0.p, off.p, b, cart.p, species.p, image_of.p);
 }
 
 }  // namespace b2m

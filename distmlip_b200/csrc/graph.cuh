@@ -75,11 +75,31 @@ struct Graph {
   DBuf<int> e_src_gid;
   DBuf<unsigned char> keys_out;  // persistent scratch: no cudaMalloc/cudaFree on the per-step path
   DBuf<int> sel_out, nsel;
+  // unfolded (heat-flux) structures: slab walls are measured from the lowest fractional coordinate, not from 0, because
+  // the periodic images put atoms below 0 along the partition axis
+  bool walls_from_min = false;
 
   void build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
              const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,
              int rank_, int world_);
   int64_t export_info(cudaStream_t st, int which, int64_t* out, int64_t cap);
+};
+
+// Unfolded cell of the heat flux (DESIGN.md §10): the n cell atoms at their given positions, followed by every periodic
+// image j + s.L (s integer, nonzero, zero along non-periodic axes) whose fractional coordinates lie in the cell atoms'
+// fractional bounding box widened by reach / h_k along each periodic axis k (h_k: the cell's height across lattice
+// plane k).  Every atom within `reach` Angstrom of a cell atom is inside that box.  Built on the GPU as count / scan /
+// fill; the result stays on the device and is the input of a non-periodic Graph::build.
+struct Unfold {
+  int64_t n = 0, N = 0;   // cell atoms, cell atoms + images
+  DBuf<double> cart;      // [N,3]
+  DBuf<int> species;      // [N]
+  DBuf<int> image_of;     // [N] cell atom of every unfolded atom (image_of[i] = i for i < n)
+  DBuf<double> cart0, frac0, red_tmp;
+  DBuf<int> species0, cnt, off;
+  DBuf<char> cub_tmp;
+  void build(cudaStream_t st, int64_t natoms, const double* h_cart, const int32_t* h_species, const double* h_lat,
+             const int* h_pbc, double reach);
 };
 
 }  // namespace b2m

@@ -1330,12 +1330,13 @@ void launch_angle_init_bwd(cudaStream_t st, int64_t na, const int* a_in, const i
 // readout
 // ============================================================================================
 // kAtomic: also the per-atom energy of every row, atom_e[gid[row]] = scale * v + elem_ref + mean_per_atom
-template <bool kAtomic>
+// kWeighted: every row's energy (and per-atom energy) times wgt[gid[row]] (heat flux: cell mask or position seed)
+template <bool kAtomic, bool kWeighted = false>
 __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__ X, const float* __restrict__ w,
                                                 float bias, float* __restrict__ out, double* __restrict__ sum,
                                                 const int* __restrict__ type, const double* __restrict__ elem_ref,
                                                 float scale, const int* __restrict__ gid, double* __restrict__ atom_e,
-                                                double mean_per_atom) {
+                                                double mean_per_atom, const float* __restrict__ wgt) {
   // one warp per row
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   float v = 0.f;
@@ -1352,6 +1353,11 @@ __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__
     if (out) out[warp] = v;
     contrib = (double)scale * (double)v;
     if (elem_ref) contrib += elem_ref[type[warp]];
+    if constexpr (kWeighted) {
+      const double wt = (double)wgt[gid[warp]];
+      contrib *= wt;
+      mean_per_atom *= wt;
+    }
     if constexpr (kAtomic) atom_e[gid[warp]] = contrib + mean_per_atom;
   }
   if (sum) {
@@ -1366,26 +1372,40 @@ __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__
 }
 void launch_rowdot(cudaStream_t st, int n, const float* X, const float* w, float bias, float* out, double* sum,
                    const int* type, const double* elem_ref, float scale, const int* gid, double* atom_e,
-                   double mean_per_atom) {
+                   double mean_per_atom, const float* wgt) {
   if (n <= 0) return;
-  if (atom_e)
-    k_rowdot<true><<<cdiv((int64_t)n * 32, 256), 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid,
-                                                               atom_e, mean_per_atom);
+  const int nb = cdiv((int64_t)n * 32, 256);
+  if (wgt && atom_e)
+    k_rowdot<true, true><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e,
+                                             mean_per_atom, wgt);
+  else if (wgt)
+    k_rowdot<false, true><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e,
+                                              mean_per_atom, wgt);
+  else if (atom_e)
+    k_rowdot<true><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e, mean_per_atom,
+                                       wgt);
   else
-    k_rowdot<false><<<cdiv((int64_t)n * 32, 256), 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid,
-                                                                atom_e, mean_per_atom);
+    k_rowdot<false><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e, mean_per_atom,
+                                        wgt);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }
+// kWeighted: row r's seed times wgt[gid[r]]
+template <bool kWeighted = false>
 __global__ void k_readout_seed(int n, const float* __restrict__ pre, const float* __restrict__ w, float scale,
-                               float* __restrict__ g) {
+                               float* __restrict__ g, const int* __restrict__ gid, const float* __restrict__ wgt) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= (int64_t)n * 64) return;
+  if constexpr (kWeighted) scale *= wgt[gid[i >> 6]];
   g[i] = scale * w[i & 63] * dsilu_f(pre[i]);
 }
-void launch_readout_seed(cudaStream_t st, int n, const float* pre, const float* w, float scale, float* g) {
+void launch_readout_seed(cudaStream_t st, int n, const float* pre, const float* w, float scale, float* g,
+                         const int* gid, const float* wgt) {
   if (n <= 0) return;
-  k_readout_seed<<<cdiv((int64_t)n * 64, 256), 256, 0, st>>>(n, pre, w, scale, g);
+  if (wgt)
+    k_readout_seed<true><<<cdiv((int64_t)n * 64, 256), 256, 0, st>>>(n, pre, w, scale, g, gid, wgt);
+  else
+    k_readout_seed<<<cdiv((int64_t)n * 64, 256), 256, 0, st>>>(n, pre, w, scale, g, gid, wgt);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }

@@ -115,9 +115,10 @@ void launch_angle_init_bwd(cudaStream_t st, int64_t na, const int* a_in, const i
 // atom_e != nullptr: also atom_e[gid[row]] = scale * e_atom + elem ref + mean_per_atom (per-atom energies, double)
 void launch_rowdot(cudaStream_t st, int n, const float* X, const float* w, float bias, float* out, double* sum,
                    const int* type, const double* elem_ref, float scale, const int* gid = nullptr,
-                   double* atom_e = nullptr, double mean_per_atom = 0.0);
-// g[r][c] = scale * w[c] * dsilu(pre[r][c])
-void launch_readout_seed(cudaStream_t st, int n, const float* pre, const float* w, float scale, float* g);
+                   double* atom_e = nullptr, double mean_per_atom = 0.0, const float* wgt = nullptr);
+// g[r][c] = scale * w[c] * dsilu(pre[r][c])   (wgt != nullptr: times wgt[gid[r]])
+void launch_readout_seed(cudaStream_t st, int n, const float* pre, const float* w, float scale, float* g,
+                         const int* gid = nullptr, const float* wgt = nullptr);
 
 // -------- final geometry backward --------
 // atom_vir != nullptr: also the per-atom virials, [N][12] f32 by global id (atomic_virial.cuh)
@@ -212,10 +213,10 @@ void launch_tn_invariants_bwd(cudaStream_t st, int n, const float* X, const floa
 void launch_tn_readout_final(cudaStream_t st, int n, int W, const float* hL, const float* wL, float bL, const float* hG,
                              const float* wG, float bG, const int* type, const double* eref, float scale, float* lout,
                              float* gout, float* e_atom, double* energy, const int* gid = nullptr,
-                             double* atom_e = nullptr, double mean_per_atom = 0.0);
+                             double* atom_e = nullptr, double mean_per_atom = 0.0, const float* wgt = nullptr);
 void launch_tn_readout_seed(cudaStream_t st, int n, int W, const float* lout, const float* gout, float scale,
                             const float* wL, const float* wG, const float* preL, const float* preG, float* gL,
-                            float* gG);
+                            float* gG, const int* gid = nullptr, const float* wgt = nullptr);
 void launch_tn_edge_final(cudaStream_t st, int64_t E, const int* e_src, const int* e_dst, const float4* e_vec,
                           const int* gid, const TnRadial& rp, const float* g_rbf, const float* gC, const float* gvh,
                           float* gd, float* forces, double* virial, float* atom_vir = nullptr);

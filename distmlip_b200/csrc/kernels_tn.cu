@@ -598,13 +598,14 @@ __global__ void k_tn_invariants_bwd(int n, const float* __restrict__ X, const fl
 }
 // last layer of both readout chains (width W -> 1), product, energy sum; one warp per atom
 // kAtomic: also the per-atom energy of every row, atom_e[gid[row]] = scale * L * G + eref + mean_per_atom
-template <bool kAtomic>
+// kWeighted: every row's energy (and per-atom energy) times wgt[gid[row]] (heat flux: cell mask or position seed)
+template <bool kAtomic, bool kWeighted = false>
 __global__ void k_tn_readout_final(int n, int W, const float* __restrict__ hL, const float* __restrict__ wL, float bL,
                                    const float* __restrict__ hG, const float* __restrict__ wG, float bG,
                                    const int* __restrict__ type, const double* __restrict__ eref, float scale,
                                    float* __restrict__ lout, float* __restrict__ gout, float* __restrict__ e_atom,
                                    double* __restrict__ energy, const int* __restrict__ gid, double* __restrict__ atom_e,
-                                   double mean_per_atom) {
+                                   double mean_per_atom, const float* __restrict__ wgt) {
   const int r = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (r >= n) return;
   float a = 0.f, b = 0.f;
@@ -621,18 +622,27 @@ __global__ void k_tn_readout_final(int n, int W, const float* __restrict__ hL, c
     lout[r] = L, gout[r] = Gt, e_atom[r] = L * Gt;
     double ev = (double)scale * (double)(L * Gt);
     if (eref) ev += eref[type[r]];
+    if constexpr (kWeighted) {
+      const double wt = (double)wgt[gid[r]];
+      ev *= wt;
+      mean_per_atom *= wt;
+    }
     if constexpr (kAtomic) atom_e[gid[r]] = ev + mean_per_atom;
     atomicAdd(energy, ev);
   }
 }
 // adjoints of the last hidden activations of both chains, already times SiLU'(pre) of that layer
+// kWeighted: row r's seed times wgt[gid[r]]
+template <bool kWeighted = false>
 __global__ void k_tn_readout_seed(int n, int W, const float* __restrict__ lout, const float* __restrict__ gout,
                                   float scale, const float* __restrict__ wL, const float* __restrict__ wG,
                                   const float* __restrict__ preL, const float* __restrict__ preG,
-                                  float* __restrict__ gL, float* __restrict__ gG) {
+                                  float* __restrict__ gL, float* __restrict__ gG, const int* __restrict__ gid,
+                                  const float* __restrict__ wgt) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= (int64_t)n * W) return;
   const int r = (int)(i / W), c = (int)(i % W);
+  if constexpr (kWeighted) scale *= wgt[gid[r]];
   const float L = lout[r], Gt = gout[r];
   gL[i] = scale * Gt * wL[c] * dsilu_f(preL[i]);
   gG[i] = scale * L * Gt * (1.f - Gt) * wG[c] * dsilu_f(preG[i]);
@@ -788,18 +798,30 @@ void launch_tn_invariants_bwd(cudaStream_t st, int n, const float* X, const floa
 void launch_tn_readout_final(cudaStream_t st, int n, int W, const float* hL, const float* wL, float bL, const float* hG,
                              const float* wG, float bG, const int* type, const double* eref, float scale, float* lout,
                              float* gout, float* e_atom, double* energy, const int* gid, double* atom_e,
-                             double mean_per_atom) {
-  if (atom_e)
+                             double mean_per_atom, const float* wgt) {
+  const auto k_weighted_atomic = k_tn_readout_final<true, true>;
+  const auto k_weighted = k_tn_readout_final<false, true>;
+  if (wgt && atom_e)
+    TN_LAUNCH(k_weighted_atomic, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout,
+              e_atom, energy, gid, atom_e, mean_per_atom, wgt);
+  else if (wgt)
+    TN_LAUNCH(k_weighted, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout, e_atom,
+              energy, gid, atom_e, mean_per_atom, wgt);
+  else if (atom_e)
     TN_LAUNCH(k_tn_readout_final<true>, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout,
-              e_atom, energy, gid, atom_e, mean_per_atom);
+              e_atom, energy, gid, atom_e, mean_per_atom, wgt);
   else
     TN_LAUNCH(k_tn_readout_final<false>, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout,
-              gout, e_atom, energy, gid, atom_e, mean_per_atom);
+              gout, e_atom, energy, gid, atom_e, mean_per_atom, wgt);
 }
 void launch_tn_readout_seed(cudaStream_t st, int n, int W, const float* lout, const float* gout, float scale,
                             const float* wL, const float* wG, const float* preL, const float* preG, float* gL,
-                            float* gG) {
-  TN_LAUNCH(k_tn_readout_seed, (int64_t)n * W, st, n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG);
+                            float* gG, const int* gid, const float* wgt) {
+  if (wgt)
+    TN_LAUNCH(k_tn_readout_seed<true>, (int64_t)n * W, st, n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG, gid,
+              wgt);
+  else
+    TN_LAUNCH(k_tn_readout_seed, (int64_t)n * W, st, n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG, gid, wgt);
 }
 void launch_tn_edge_final(cudaStream_t st, int64_t E, const int* e_src, const int* e_dst, const float4* e_vec,
                           const int* gid, const TnRadial& rp, const float* g_rbf, const float* gC, const float* gvh,

@@ -30,6 +30,7 @@ class Distributed:
         self.forces = None
         self.stress = None
         self.atomic = None  # (per-atom energies, per-atom virials) when the Potential asks for them
+        self.heat_flux = None  # (J_pot, J_conv) when the Potential asks for the heat flux
 
     @staticmethod
     def cartesian_to_wrapped_fractional(positions_cartesian, lattice, pbc):

@@ -68,6 +68,10 @@ class PESCalculator_Dist(_Calculator):
         self.compute_atomic = bool(getattr(potential, "calc_atomic", False))
         if self.compute_atomic:
             self.implemented_properties = tuple(PESCalculator_Dist.implemented_properties) + ("energies", "stresses")
+        # likewise the heat flux (J, eV * Angstrom / ASE time unit, not divided by the volume) of a potential built with
+        # calc_heat_flux=True
+        if getattr(potential, "calc_heat_flux", False):
+            self.implemented_properties = tuple(self.implemented_properties) + ("heat_flux", "heat_flux_potential")
 
     def calculate(self, atoms, properties=None, system_changes=None):
         """ase.py:80-127."""
@@ -77,6 +81,10 @@ class PESCalculator_Dist(_Calculator):
         if missing:
             raise _PropertyNotImplementedError(
                 f"{missing} need a potential built with Potential_Dist(..., calc_atomic=True)")
+        missing = [p for p in ("heat_flux", "heat_flux_potential") if p in properties and
+                   not getattr(self.potential, "calc_heat_flux", False)]
+        if missing:
+            raise _PropertyNotImplementedError(f"{missing} need Potential_Dist(..., calc_heat_flux=True)")
         _Calculator.calculate(self, atoms=atoms, properties=properties, system_changes=system_changes)
         calc_result = self.potential(atoms, self.state_attr)
         self.results.update(
@@ -97,6 +105,9 @@ class PESCalculator_Dist(_Calculator):
                     st = np.stack([st[:, 0, 0], st[:, 1, 1], st[:, 2, 2], (st[:, 1, 2] + st[:, 2, 1]) / 2,
                                    (st[:, 0, 2] + st[:, 2, 0]) / 2, (st[:, 0, 1] + st[:, 1, 0]) / 2], axis=1)
                 self.results.update(stresses=st * self.stress_weight)
+        if getattr(self.potential, "calc_heat_flux", False) and self.potential.heat_flux is not None:
+            self.results.update(heat_flux=self.potential.heat_flux["total"].copy(),
+                                heat_flux_potential=self.potential.heat_flux["potential"].copy())
 
 
 class TrajectoryObserver:

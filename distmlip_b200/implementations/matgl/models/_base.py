@@ -120,6 +120,19 @@ class EngineBackedModel:
         eng.finalize()
         self._engine_finalized, self._final_key = True, key
 
+    def heat_flux_reach(self):
+        """Receptive-field radius (Angstrom) of an atom's energy: the unfolded cell of the heat flux must hold every
+        periodic image within this distance of the cell (DESIGN.md §10)."""
+        raise NotImplementedError
+
+    def _set_heat_flux(self, reach, velocities):
+        """reach > 0: the next graph build unfolds the cell and the next potential_forward_dist computes the heat flux
+        for `velocities`; 0: plain periodic evaluation (the engine is only told when the reach changes)"""
+        if float(reach) != self.__dict__.get("_hf_reach", 0.0):
+            self._engine.set_heat_flux(float(reach))
+            self._hf_reach = float(reach)
+        self._hf_velocities = velocities if reach > 0 else None
+
     def potential_forward_dist(self, dist_info, atoms, lattice_matrix, calc_stresses, calc_forces, calc_hessian,
                                state_attr=None):
         """Seam of chgnet.py:21-30,199-206 / tensornet.py:10-19.  Returns (node_types, positions, strain, (E, site_wise));
@@ -133,7 +146,12 @@ class EngineBackedModel:
         if want_atomic != self.__dict__.get("_atomic_on", False):
             eng.set_atomic(want_atomic)
             self._atomic_on = want_atomic
-        e, f, s = eng.compute(forces=calc_forces, stress=calc_stresses)
+        velocities = self.__dict__.get("_hf_velocities")
+        if velocities is not None:  # heat flux: the masked pass returns what compute would, plus (J_pot, J_conv)
+            e, f, s, dist_info.heat_flux = eng.compute_heat_flux(velocities)
+            self._hf_velocities = None
+        else:
+            e, f, s = eng.compute(forces=calc_forces, stress=calc_stresses)
         dist_info.forces, dist_info.stress = f, s
         dist_info.atomic = eng.atomic(virials=calc_forces or calc_stresses) if want_atomic else None
         node_types = torch.as_tensor(dist_info.species, dtype=distmlip_b200.int_th)

@@ -30,6 +30,12 @@ class CHGNet_Dist(EngineBackedModel):
     __version__ = 1
     _has_site = True
 
+    def heat_flux_reach(self):
+        """max(n_blocks * r_cut, r_cut + (n_blocks - 1) * r_bond): a message moves r_cut per atom conv or r_bond per
+        bond conv, and a bond feature reaches the atom graph only at its own bond's endpoint (DESIGN.md §10)"""
+        nb, rc, rb = int(self._attr("n_blocks")), float(self._attr("cutoff")), float(self._attr("three_body_cutoff"))
+        return max(nb * rc, rc + (nb - 1) * rb)
+
     def enable_distributed_mode(self, gpus):
         """chgnet.py:455-549. `gpus`: CUDA ordinals, one per partition."""
         gpus, rank, world, group = self._process_layout(gpus)

@@ -26,6 +26,11 @@ class TensorNet_Dist(EngineBackedModel):
 
     __version__ = 1
 
+    def heat_flux_reach(self):
+        """(n_blocks + 1) * r_cut: the embedding aggregates one hop, every interaction layer one more"""
+        nblocks = len({int(k.split(".")[1]) for k in self._state_dict if k.startswith("layers.")})
+        return (nblocks + 1) * float(self._attr("cutoff"))
+
     def enable_distributed_mode(self, gpus):
         """tensornet.py:163-204. `gpus`: CUDA ordinals, one per partition."""
         gpus, rank, world, group = self._process_layout(gpus)

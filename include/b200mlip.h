@@ -141,6 +141,25 @@ int b2m_set_atomic(b2m_handle h, int on);
  * after an evaluation without a backward (want_forces = want_stress = 0). */
 int b2m_get_atomic(b2m_handle h, double* energies, float* virials);
 
+/* Heat flux of the model (DESIGN.md "Heat flux"), off by default (reach = 0).  With reach > 0 (Angstrom, at least the
+ * model's receptive field: n_blocks * r_cut for CHGNet, (n_blocks + 1) * r_cut for TensorNet) the following
+ * b2m_set_structure calls build the unfolded cell: the natoms cell atoms, then every periodic image within `reach` of
+ * them along the periodic axes, evaluated without periodicity with the energy U = sum of the cell atoms' energies.
+ * On such a handle b2m_compute (and b2m_compute_resident, b2m_get_results) returns the periodic energy, forces [natoms][3]
+ * (the forces of an atom's images summed onto it) and stress, and b2m_get_atomic the cell atoms' values: an MD loop pays
+ * for the flux only on the steps that call b2m_compute_heat_flux.  reach = 0 switches back at the next
+ * b2m_set_structure. */
+int b2m_set_heat_flux(b2m_handle h, double reach);
+/* One masked and three position-seeded evaluations of the unfolded cell.  vel: [natoms][3] Angstrom / (unit time), f64.
+ * energy / forces / stress9 as b2m_compute (any may be NULL).  flux6 (f64):
+ *   flux6[0..2] = J_pot  = sum_{i<n} sum_j r_ij (dU_i/dr_j . v_j),  r_ij = r_i - r_j, j over every unfolded atom
+ *   flux6[3..5] = J_conv = sum_{i<n} e_i v_i  (e_i: the per-atom energies of b2m_set_atomic)
+ * in eV * (velocity unit), not divided by the volume (LAMMPS compute heat/flux); the kinetic part sum 1/2 m v^2 v is the
+ * caller's.  Afterwards b2m_get_atomic returns the per-atom energies and virials of the masked evaluation.
+ * B2M_ERR_STATE when the reach is 0 or the resident structure was set before it. */
+int b2m_compute_heat_flux(b2m_handle h, const double* vel, double* energy, float* forces, float* stress9,
+                          double* flux6);
+
 /* site-wise readout (magmom) for all atoms, [natoms] */
 int b2m_get_sitewise(b2m_handle h, float* out);
 
