@@ -776,7 +776,7 @@ static void line_bwd_common(b2m_engine* e, int l, bool hidden, LineArgs& a) {
   launch_zero_rows(e->st, e->gHb.p, (int64_t)g.B_own * D2);
   launch_zero_rows(e->st, e->gXc.p, (int64_t)g.n_loc * D2);
   a.gang = e->gang.p, a.gHa = e->gHa.p, a.gHb = e->gHb.p, a.gXc = e->gXc.p;
-  launch_line_bwd(e->st, a, hidden);
+  launch_line_bwd(e->st, a, hidden, e->num_sms);
   gemm(e, e->gHa.p, D2, hidden ? w.W1a_raw : w.WAa_raw, e->gh.p, D, g.B_loc, D, D2, nullptr, nullptr, 0, true);
   gemm(e, e->gHb.p, D2, hidden ? w.W1b_raw : w.WAb_raw, e->gh.p, D, g.B_own, D, D2, nullptr, nullptr, 0, true);
   gemm(e, e->gXc.p, D2, hidden ? w.W1c_raw : w.WAc_raw, e->gx.p, D, g.n_loc, D, D2, nullptr, nullptr, 0, true);
@@ -799,7 +799,7 @@ static void forward(b2m_engine* e) {
     launch_zero_rows(e->st, e->aggB.p, (int64_t)g.B_own * D);
     LineArgs a = line_args(e, l, true);
     a.aggB = e->aggB.p;
-    launch_line_fwd(e->st, a, true);
+    launch_line_fwd(e->st, a, true, e->num_sms);
     gemm(e, e->aggB.p, D, w.Wout_k, e->upd[l].p, D, g.B_own, D, D, nullptr, nullptr, 0, false);
     launch_bond_update_fwd(e->st, g.B_own, g.b_vec.p, e->rp3, e->d_W3bw, e->h[l].p, e->upd[l].p, e->h[l + 1].p);
     if (l < nb - 2) {
@@ -812,7 +812,7 @@ static void forward(b2m_engine* e) {
       line_proj_Ha(e, l, false);
       LineArgs b = line_args(e, l, false);
       b.ang_out = e->ang[l + 1].p;
-      launch_line_fwd(e->st, b, false);
+      launch_line_fwd(e->st, b, false, e->num_sms);
     }
   }
   // site-wise readout after block n-2 (chgnet.py:392-398)

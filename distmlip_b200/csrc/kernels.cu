@@ -855,310 +855,405 @@ void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
 // ============================================================================================
 // line-graph kernels: bond conv (HIDDEN) and angle update (!HIDDEN)
 // ============================================================================================
+// Persistent like the atom conv: min(tiles, SMs) CTAs, CTA c takes tiles c, c + grid, ...  Two [TM][LD] buffers
+// alternate: tile number `it` of a CTA has its Ha[a] rows in buffer it & 1 (P) and its own angle rows in columns
+// 64..127 of the other buffer (Q; pitch LD, so the A fragments of ang.Wg^T read conflict-free).  Each copy completes on
+// the barrier of its tile's stage (hbar / abar [it & 1], parity stage_parity(it)).  One 64 KB weight slot holds the
+// image the next product needs; images that share it are refilled by bulk copies as soon as the product before has
+// read the slot, and waited on (wbar, one phase per fill, in fill order) just before the product that reads them.
 struct LineSmem {
-  static constexpr int kP = 32;
-  static constexpr int kAng = kP + TM * LD;   // [TM][LDA] angle rows; the backward's tileH [TM][LD] aliases them
-  static constexpr int kH = kAng;             // (backward only, first written after the angle rows have been read)
-  static constexpr int kW = kAng + TM * LD;   // wgmma images of the weights (2 branches x hi | lo, or Wg^T hi | lo)
+  static constexpr int kBuf = 32;              // two [TM][LD] buffers (first 128 B: hbar[2], abar[2], wbar)
+  static constexpr int kW = kBuf + 2 * TM * LD;  // one weight image (2 branches x hi | lo, or Wg^T hi | lo)
   static constexpr int kB2 = kW + 16384;
-  static constexpr int kIdx = kB2 + 128;
-  static constexpr int kFwdTotal = kIdx + 3 * TM;
-  static constexpr int kBwdTotal = kFwdTotal;
-  static constexpr size_t fwd_bytes = (size_t)kFwdTotal * 4;
-  static constexpr size_t bwd_bytes = (size_t)kBwdTotal * 4;
+  static constexpr int kIdx = kB2 + 128;       // a_in, a_out, a_ctr: [2][TM] each
+  static constexpr int kTotal = kIdx + 6 * TM;
+  static constexpr size_t bytes = (size_t)kTotal * 4;
+};
+static_assert(LineSmem::bytes <= 232448, "line-graph shared memory");
+
+struct LineSm {
+  float* smem;
+  __device__ __forceinline__ uint64_t* hbar() const { return reinterpret_cast<uint64_t*>(smem); }
+  __device__ __forceinline__ uint64_t* abar() const { return hbar() + 2; }
+  __device__ __forceinline__ uint64_t* wbar() const { return hbar() + 4; }
+  __device__ __forceinline__ float* buf(int s) const { return smem + LineSmem::kBuf + s * TM * LD; }
+  __device__ __forceinline__ float* W() const { return smem + LineSmem::kW; }
+  __device__ __forceinline__ float* b2() const { return smem + LineSmem::kB2; }
+  __device__ __forceinline__ int* idx(int s, int k) const {  // k: 0 a_in, 1 a_out, 2 a_ctr
+    return reinterpret_cast<int*>(smem + LineSmem::kIdx) + (2 * k + s) * TM;
+  }
 };
 
-// common prologue: indices, TMA gathers of Ha[a] rows and the tile's own angle rows, Wg staging
-__device__ __forceinline__ int line_prologue(const LineArgs& a, float* smem, int64_t r0) {
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);
-  float* tileP = smem + LineSmem::kP;
-  float* angT = smem + LineSmem::kAng;
-  float* Wsm = smem + LineSmem::kW;
-  float* b2s = smem + LineSmem::kB2;
-  int* s_a = reinterpret_cast<int*>(smem + LineSmem::kIdx);
-  int* s_b = s_a + TM;
-  int* s_c = s_b + TM;
-  const int tid = threadIdx.x;
-  const int nvalid = (int)min((int64_t)TM, a.A - r0);
-  if (tid < TM) {
-    int ia = -1, ib = -1, ic = -1;
-    if (tid < nvalid) {
-      ia = a.a_in[r0 + tid];
-      ib = a.a_out[r0 + tid];
-      ic = a.a_ctr[r0 + tid];
-    }
-    s_a[tid] = ia;
-    s_b[tid] = ib;
-    s_c[tid] = ic;
+struct AngleIdx {
+  int a, b, c;
+};
+__device__ __forceinline__ AngleIdx angle_idx(const LineArgs& a, int64_t r) {
+  AngleIdx x{-1, -1, -1};
+  if (threadIdx.x < TM && r < a.A) {
+    x.a = a.a_in[r];
+    x.b = a.a_out[r];
+    x.c = a.a_ctr[r];
   }
+  return x;
+}
+// threads 0..TM-1 publish their row of tile t into stage s's index arrays and start its Ha[a] copy into `buf`; the
+// caller has made sure, with a proxy fence and a barrier, that nobody reads `buf` or those arrays any more
+__device__ __forceinline__ void line_issue_ha(const LineArgs& a, const LineSm& sm, int64_t t, const AngleIdx& x,
+                                             float* buf, int s) {
+  const int tid = threadIdx.x;
+  if (tid == 0) mbar_expect_tx(&sm.hbar()[s], (uint32_t)min((int64_t)TM, a.A - t * TM) * 512u);
+  if (tid < TM) {
+    sm.idx(s, 0)[tid] = x.a;
+    sm.idx(s, 1)[tid] = x.b;
+    sm.idx(s, 2)[tid] = x.c;
+    if (x.a >= 0) bulk_g2s(buf + tid * LD, a.Ha + (size_t)x.a * D2, 512u, &sm.hbar()[s]);
+  }
+}
+// the 256 B angle rows of tile t into columns 64..127 of `buf`, completing on abar[s]
+__device__ __forceinline__ void line_issue_ang(const LineArgs& a, const LineSm& sm, int64_t t, float* buf, int s) {
+  const int tid = threadIdx.x;
+  const int nvalid = (int)min((int64_t)TM, a.A - t * TM);
+  if (tid == 0) mbar_expect_tx(&sm.abar()[s], (uint32_t)nvalid * 256u);
+  if (tid < nvalid) bulk_g2s(buf + tid * LD + 64, a.ang + (size_t)(t * TM + tid) * D, 256u, &sm.abar()[s]);
+}
+// barriers, b2, the first weight image and the copies of the CTA's first tile (Ha into buffer 0, angles into buffer 1)
+__device__ __forceinline__ AngleIdx line_prologue(const LineArgs& a, const LineSm& sm) {
+  const int tid = threadIdx.x;
   if (tid == 0) {
-    mbar_init(mbar, 1);
+    for (int i = 0; i < 5; i++) mbar_init(&sm.hbar()[i], 1);
     fence_barrier_init();
   }
+  AngleIdx x = angle_idx(a, (int64_t)blockIdx.x * TM + tid);
+  if (tid < 128) sm.b2()[tid] = a.b2 ? a.b2[tid] : 0.f;
   __syncthreads();
-  if (tid == 0) mbar_expect_tx(mbar, (uint32_t)nvalid * 768u);
-  if (tid < nvalid) {
-    bulk_g2s(tileP + tid * LD, a.Ha + (size_t)s_a[tid] * D2, 512u, mbar);
-    bulk_g2s(angT + tid * LDA, a.ang + (size_t)(r0 + tid) * D, 256u, mbar);
-  } else if (tid < TM) {
-    for (int k = 0; k < 64; k++) angT[tid * LDA + k] = 0.f;
-    for (int k = 0; k < 128; k++) tileP[tid * LD + k] = 0.f;
+  if (tid == 0) bulk_g2s_image(sm.W(), a.Wgcan, 16384 * 4, sm.wbar());
+  line_issue_ha(a, sm, blockIdx.x, x, sm.buf(0), 0);
+  line_issue_ang(a, sm, blockIdx.x, sm.buf(1), 0);
+  return angle_idx(a, ((int64_t)blockIdx.x + gridDim.x) * TM + tid);
+}
+
+// pre = Ha[a] (in tile P) + ang.Wg^T (acc) + Hb[b] + Xc[c] on this thread's accumulator elements, handed to f(i, j, pre)
+// (rows r >= nvalid: f(i, j, 0)).  A row's 16 Hb and 16 Xc values are loaded as float2 pairs before any is used.
+template <class F>
+__device__ __forceinline__ void line_first_layer(const LineArgs& a, const Map& m, const float* P, const int* s_b,
+                                                 const int* s_c, int nvalid, const float (&acc)[AR][AC], F&& f) {
+#pragma unroll
+  for (int i = 0; i < AR; i++) {
+    const int r = m.row(i);
+    const bool ok = r < nvalid;
+    const float* hb = a.Hb + (size_t)(ok ? s_b[r] : 0) * D2 + m.branch * 64;
+    const float* xc = a.Xc + (size_t)(ok ? s_c[r] : 0) * D2 + m.branch * 64;
+    float2 hv[AC / 2], xv[AC / 2];
+#pragma unroll
+    for (int jj = 0; jj < AC / 2; jj++) {
+      hv[jj] = ok ? __ldg(reinterpret_cast<const float2*>(hb + m.col(2 * jj))) : make_float2(0.f, 0.f);
+      xv[jj] = ok ? __ldg(reinterpret_cast<const float2*>(xc + m.col(2 * jj))) : make_float2(0.f, 0.f);
+    }
+#pragma unroll
+    for (int j = 0; j < AC; j++) {
+      const int col = m.branch * 64 + m.col(j);
+      float p = 0.f;
+      if (ok) p = P[r * LD + col] + acc[i][j] + ((j & 1) ? hv[j >> 1].y : hv[j >> 1].x) + ((j & 1) ? xv[j >> 1].y : xv[j >> 1].x);
+      f(i, j, p);
+    }
   }
-  stage_w(Wsm, a.Wgcan, 4096);
-  if (tid < 128) b2s[tid] = a.b2 ? a.b2[tid] : 0.f;
-  mbar_wait(mbar, 0);
-  __syncthreads();
-  return nvalid;
 }
 
 template <bool HIDDEN>
 __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
   extern __shared__ __align__(128) float smem[];
-  float* tileP = smem + LineSmem::kP;
-  float* angT = smem + LineSmem::kAng;
-  float* Wsm = smem + LineSmem::kW;
-  float* b2s = smem + LineSmem::kB2;
-  int* s_a = reinterpret_cast<int*>(smem + LineSmem::kIdx);
-  int* s_b = s_a + TM;
-  int* s_c = s_b + TM;
-  const int64_t r0 = (int64_t)blockIdx.x * TM;
-  const int nvalid = line_prologue(a, smem, r0);
-  (void)s_a;
-  const Map m;
-  float acc[AR][AC];
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-  gemm64(angT, LDA, 0, Wsm + m.branch * 8192, acc);
-#pragma unroll
-  for (int i = 0; i < AR; i++) {
-    const int r = m.row(i);
-    const int ib = s_b[r], ic = s_c[r];
-#pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const int col = m.branch * 64 + m.col(j);
-      float p = 0.f;
-      if (r < nvalid) p = tileP[r * LD + col] + acc[i][j] + a.Hb[(size_t)ib * D2 + col] + a.Xc[(size_t)ic * D2 + col];
+  const LineSm sm{smem};
+  const float* b2s = sm.b2();
+  const int tid = threadIdx.x;
+  const int64_t ntiles = (a.A + TM - 1) / TM, step = gridDim.x;
+  AngleIdx nxt = line_prologue(a, sm);
+  uint32_t wpar = 0;
+
+  int it = 0;
+  for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
+    const int s = it & 1;
+    float* P = sm.buf(s);
+    float* Q = sm.buf(s ^ 1);
+    const int* s_b = sm.idx(s, 1);
+    const int* s_c = sm.idx(s, 2);
+    const int64_t r0 = t * TM;
+    const int nvalid = (int)min((int64_t)TM, a.A - r0);
+    const bool more = t + step < ntiles;
+    const Map m;
+    float acc[AR][AC];
+    // ang . Wg^T (angle rows in Q)
+    mbar_wait(&sm.abar()[s], stage_parity(it));
+    mbar_wait(sm.wbar(), wpar);  // Wg
+    if (HIDDEN) wpar ^= 1;       // (!HIDDEN: Wg stays, its only phase is complete)
+    gemm64(Q, LD, 64, sm.W() + m.branch * 8192, acc);
+    fence_proxy_async_smem();  // this thread's generic accesses of Q come before its bulk refill
+    __syncthreads();           // Q (angle rows, the previous tile's gates) and its index arrays are free; so is Wg
+    if (more) {
+      line_issue_ha(a, sm, t + step, nxt, Q, s ^ 1);
+      nxt = angle_idx(a, (t + 2 * step) * TM + tid);
+    }
+    if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.W2can, 16384 * 4, sm.wbar());
+    mbar_wait(&sm.hbar()[s], stage_parity(it));
+    line_first_layer(a, m, P, s_b, s_c, nvalid, acc, [&](int i, int j, float p) {
       if (HIDDEN) {
-        tileP[r * LD + col] = r < nvalid ? silu_f(p) : 0.f;
+        P[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.row(i) < nvalid ? silu_f(p) : 0.f;
       } else {
         acc[i][j] = m.branch == 0 ? silu_f(p) : sigm(p);
       }
+    });
+    fence_proxy_async_smem();
+    __syncthreads();  // (!HIDDEN: the Ha rows in P have been read, its columns 64..127 are free)
+    if (HIDDEN) {
+      mbar_wait(sm.wbar(), wpar);  // W2
+      wpar ^= 1;
+      gemm64(P, LD, m.branch * 64, sm.W() + m.branch * 8192, acc);
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) {
+          const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
+          acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
+        }
+      fence_proxy_async_smem();
+      __syncthreads();  // columns 64..127 of P are free (and so is W2)
     }
-  }
-  __syncthreads();
-  if (HIDDEN) {
-    stage_w(Wsm, a.W2can, 4096);
+    if (more) {
+      line_issue_ang(a, sm, t + step, P, s ^ 1);
+      if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.Wgcan, 16384 * 4, sm.wbar());
+    }
+    if (m.branch == 1) {
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) P[m.row(i) * LD + m.col(j)] = acc[i][j];
+    }
     __syncthreads();
+    if (m.branch == 0) {
 #pragma unroll
-    for (int i = 0; i < AR; i++)
-      for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-    gemm64(tileP, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
-        acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
-      }
-    __syncthreads();
-  }
-  if (m.branch == 1) {
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int j = 0; j < AC; j++)
-        tileP[m.row(i) * LD + m.col(j)] = acc[i][j];
-  }
-  __syncthreads();
-  if (m.branch == 0) {
-#pragma unroll
-    for (int i = 0; i < AR; i++) {
-      const int r = m.row(i);
-#pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const int c = m.col(j);
-        const float mv = acc[i][j] * tileP[r * LD + c];
+      for (int i = 0; i < AR; i++) {
+        const int r = m.row(i);
         if (HIDDEN) {
-          tileP[r * LD + c] = mv;
-        } else if (r < nvalid) {
-          a.ang_out[(size_t)(r0 + r) * D + c] = angT[r * LDA + c] + mv;
+#pragma unroll
+          for (int j = 0; j < AC; j++) P[r * LD + m.col(j)] = acc[i][j] * P[r * LD + m.col(j)];
+        } else if (r < nvalid) {  // ang_out = ang + m, the angle rows re-read (L2) as float2 pairs
+          const float* ang = a.ang + (size_t)(r0 + r) * D;
+          float* out = a.ang_out + (size_t)(r0 + r) * D;
+          float2 av[AC / 2];
+#pragma unroll
+          for (int jj = 0; jj < AC / 2; jj++) av[jj] = __ldg(reinterpret_cast<const float2*>(ang + m.col(2 * jj)));
+#pragma unroll
+          for (int jj = 0; jj < AC / 2; jj++) {
+            const int c = m.col(2 * jj);
+            const float2 v = make_float2(av[jj].x + acc[i][2 * jj] * P[r * LD + c],
+                                         av[jj].y + acc[i][2 * jj + 1] * P[r * LD + c + 1]);
+            *reinterpret_cast<float2*>(out + c) = v;
+          }
         }
       }
     }
-  }
-  if (HIDDEN) {
-    __syncthreads();
-    const int c = threadIdx.x & 63, part = threadIdx.x >> 6;
-    seg_flush(tileP, LD, c, part * 32, part * 32 + 32, s_b, a.aggB, D);
+    if (HIDDEN) {
+      __syncthreads();
+      const int c = tid & 63, part = tid >> 6;
+      seg_flush(P, LD, c, part * 32, part * 32 + 32, s_b, a.aggB, D);
+    }
   }
 }
 
+// Backward: P (buffer it & 1) holds the tile's Ha rows, then its pre-activations, then their adjoints; H (the other
+// buffer) holds the angle rows, then the hidden activations and the second-layer adjoints.  Once H has been read for the
+// last time (HIDDEN: by g.W2, !HIDDEN: by the elementwise reverse), the next tile's Ha rows are copied into it (H becomes
+// the next tile's P); once the scatter phase and gang += gpre.Wg have read P, the next tile's angle rows go into its
+// columns 64..127 (P becomes the next tile's H).  Weight images through the one slot: HIDDEN Wg -> W2 -> W2^T -> Wg^T
+// per tile, !HIDDEN Wg -> Wg^T.
 template <bool HIDDEN>
 __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
   extern __shared__ __align__(128) float smem[];
-  float* tileP = smem + LineSmem::kP;
-  float* angT = smem + LineSmem::kAng;
-  float* Wsm = smem + LineSmem::kW;
-  float* b2s = smem + LineSmem::kB2;
-  float* tileH = smem + LineSmem::kH;
-  int* s_a = reinterpret_cast<int*>(smem + LineSmem::kIdx);
-  int* s_b = s_a + TM;
-  int* s_c = s_b + TM;
+  const LineSm sm{smem};
+  const float* b2s = sm.b2();
   const int tid = threadIdx.x;
-  const int64_t r0 = (int64_t)blockIdx.x * TM;
-  const int nvalid = line_prologue(a, smem, r0);
-  const Map m;
-  float acc[AR][AC];
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-    for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-  gemm64(angT, LDA, 0, Wsm + m.branch * 8192, acc);
-  __syncthreads();  // both warpgroups have read the angle rows: tileH (aliasing them) may be written
-#pragma unroll
-  for (int i = 0; i < AR; i++) {
-    const int r = m.row(i);
-    const int ib = s_b[r], ic = s_c[r];
-#pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const int col = m.branch * 64 + m.col(j);
-      float p = 0.f;
-      if (r < nvalid) p = tileP[r * LD + col] + acc[i][j] + a.Hb[(size_t)ib * D2 + col] + a.Xc[(size_t)ic * D2 + col];
+  const int64_t ntiles = (a.A + TM - 1) / TM, step = gridDim.x;
+  AngleIdx nxt = line_prologue(a, sm);
+  uint32_t wpar = 0;
+
+  int it = 0;
+  for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
+    const int s = it & 1;
+    float* P = sm.buf(s);
+    float* H = sm.buf(s ^ 1);
+    const int* s_a = sm.idx(s, 0);
+    const int* s_b = sm.idx(s, 1);
+    const int* s_c = sm.idx(s, 2);
+    const int64_t r0 = t * TM;
+    const int nvalid = (int)min((int64_t)TM, a.A - r0);
+    const bool more = t + step < ntiles;
+    const Map m;
+    float acc[AR][AC];
+    mbar_wait(&sm.abar()[s], stage_parity(it));
+    mbar_wait(sm.wbar(), wpar);  // Wg
+    wpar ^= 1;
+    gemm64(H, LD, 64, sm.W() + m.branch * 8192, acc);
+    __syncthreads();  // both warpgroups have read the angle rows and Wg: H and the slot may be written
+    if (tid == 0) bulk_g2s_image(sm.W(), HIDDEN ? a.W2can : a.WgTcan, 16384 * 4, sm.wbar());
+    mbar_wait(&sm.hbar()[s], stage_parity(it));
+    line_first_layer(a, m, P, s_b, s_c, nvalid, acc, [&](int i, int j, float p) {
       if (HIDDEN) {
-        tileP[r * LD + col] = p;
-        tileH[r * LD + col] = r < nvalid ? silu_f(p) : 0.f;
+        const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
+        P[idx] = p;
+        H[idx] = m.row(i) < nvalid ? silu_f(p) : 0.f;
       } else {
         acc[i][j] = p;
       }
-    }
-  }
-  __syncthreads();
-  if (HIDDEN) {
-    stage_w(Wsm, a.W2can, 4096);
+    });
     __syncthreads();
+    if (HIDDEN) {
+      mbar_wait(sm.wbar(), wpar);  // W2
+      wpar ^= 1;
+      gemm64(H, LD, m.branch * 64, sm.W() + m.branch * 8192, acc);
 #pragma unroll
-    for (int i = 0; i < AR; i++)
-      for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+      for (int i = 0; i < AR; i++)
 #pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
-    __syncthreads();
-  }
-  // acc = pre-activation of the last layer of this GatedMLP (u | v).  Exchange activations.
-#pragma unroll
-  for (int i = 0; i < AR; i++)
-#pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const float u = acc[i][j];
-      tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
+        for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
+      __syncthreads();  // H and W2 have been read
+      if (tid == 0) bulk_g2s_image(sm.W(), a.W2Tcan, 16384 * 4, sm.wbar());
     }
-  if (HIDDEN) stage_w(Wsm, a.W2Tcan, 4096);
-  __syncthreads();
-#pragma unroll
-  for (int i = 0; i < AR; i++) {
-    const int r = m.row(i);
-    const int ib = s_b[r];
-#pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const int c = m.col(j);
-      const float u = acc[i][j];
-      const float po = tileH[r * LD + (1 - m.branch) * 64 + c];
-      float g = 0.f;
-      if (r < nvalid) {
-        const float gm = HIDDEN ? a.gaggB[(size_t)ib * D + c] : a.gang[(size_t)(r0 + r) * D + c];
-        if (m.branch == 0) {
-          const float s = sigm(u);
-          g = gm * po * (s * (1.f + u * (1.f - s)));
-        } else {
-          const float oG = sigm(u);
-          g = gm * po * oG * (1.f - oG);
-        }
-      }
-      acc[i][j] = g;
-    }
-  }
-  __syncthreads();
-  if (HIDDEN) {
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int j = 0; j < AC; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-      for (int j = 0; j < AC; j++) acc[i][j] = 0.f;
-    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+    // acc = pre-activation of the last layer of this GatedMLP (u | v).  Exchange activations.
 #pragma unroll
     for (int i = 0; i < AR; i++)
 #pragma unroll
       for (int j = 0; j < AC; j++) {
-        const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
-        tileP[idx] = acc[i][j] * dsilu_f(tileP[idx]);
+        const float u = acc[i][j];
+        H[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
       }
-  } else {
+    __syncthreads();
 #pragma unroll
-    for (int i = 0; i < AR; i++)
+    for (int i = 0; i < AR; i++) {
+      const int r = m.row(i);
+      const bool ok = r < nvalid;
+      // this row's 16 upstream gradients, loaded as float2 pairs before any is used
+      const float* gsrc = HIDDEN ? a.gaggB + (size_t)(ok ? s_b[r] : 0) * D : a.gang + (size_t)(r0 + (ok ? r : 0)) * D;
+      float2 gm2[AC / 2];
 #pragma unroll
-      for (int j = 0; j < AC; j++) tileP[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
-  }
-  __syncthreads();
-  // gang += gpre @ Wg   (K = 128, N = 64) on the tensor cores: warpgroup w takes rows 64 w .. 64 w + 63
-  stage_w(Wsm, a.WgTcan, 4096);
-  __syncthreads();
-  {
-    float d[32];
-    const uint32_t bh = s_u32(Wsm), bl = bh + 64u * 128u * 4u;
-    wg_mm64(tileP, LD, 64 * m.branch, 0, bh, bl, 0, false, d);
-    wg_mm64(tileP, LD, 64 * m.branch, 64, bh, bl, 64, true, d);
+      for (int jj = 0; jj < AC / 2; jj++)
+        gm2[jj] = ok ? *reinterpret_cast<const float2*>(gsrc + m.col(2 * jj)) : make_float2(0.f, 0.f);
 #pragma unroll
-    for (int q = 0; q < 32; q += 2) {
-      const int r = 64 * m.branch + m.rb + 8 * ((q >> 1) & 1), c = 8 * (q >> 2) + m.cb;
-      if (r < nvalid) {
-        float2* gp = reinterpret_cast<float2*>(&a.gang[(size_t)(r0 + r) * D + c]);
-        float2 v = *gp;
-        v.x += d[q], v.y += d[q + 1];
-        *gp = v;
+      for (int j = 0; j < AC; j++) {
+        const int c = m.col(j);
+        const float u = acc[i][j];
+        const float po = H[r * LD + (1 - m.branch) * 64 + c];
+        float g = 0.f;
+        if (ok) {
+          const float gm = (j & 1) ? gm2[j >> 1].y : gm2[j >> 1].x;
+          if (m.branch == 0) {
+            const float sg = sigm(u);
+            g = gm * po * (sg * (1.f + u * (1.f - sg)));
+          } else {
+            const float oG = sigm(u);
+            g = gm * po * oG * (1.f - oG);
+          }
+        }
+        acc[i][j] = g;
       }
     }
-  }
-  {
-    const int j = tid & 127, rh = tid >> 7;
-    seg_flush(tileP, LD, j, rh * 64, rh * 64 + 64, s_b, a.gHb, D2);
-    seg_flush(tileP, LD, j, rh * 64, rh * 64 + 64, s_c, a.gXc, D2);
-    for (int i = 0; i < 64; i++) {
-      const int r = rh + 2 * i;
-      if (r < nvalid) atomicAdd(&a.gHa[(size_t)s_a[r] * D2 + j], tileP[r * LD + j]);
+    __syncthreads();
+    if (HIDDEN) {
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) H[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+      mbar_wait(sm.wbar(), wpar);  // W2^T
+      wpar ^= 1;
+      __syncthreads();
+      gemm64(H, LD, m.branch * 64, sm.W() + m.branch * 8192, acc);
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) {
+          const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
+          P[idx] = acc[i][j] * dsilu_f(P[idx]);
+        }
+    } else {
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) P[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+    }
+    fence_proxy_async_smem();  // this thread's generic accesses of H come before its bulk refill
+    __syncthreads();           // H, its stage's index arrays and (HIDDEN) W2^T are free; P holds gpre
+    if (more) {
+      line_issue_ha(a, sm, t + step, nxt, H, s ^ 1);
+      nxt = angle_idx(a, (t + 2 * step) * TM + tid);
+    }
+    if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.WgTcan, 16384 * 4, sm.wbar());
+    // ---- scatter phase (reads P and this tile's index arrays) ----
+    {
+      const int j = tid & 127, rh = tid >> 7;
+      seg_flush(P, LD, j, rh * 64, rh * 64 + 64, s_b, a.gHb, D2);
+      seg_flush(P, LD, j, rh * 64, rh * 64 + 64, s_c, a.gXc, D2);
+    }
+    {  // gHa[a] += gpre: a 4-wide reduction per (row, column quad), a warp per row
+      const int q = tid & 31, rg = tid >> 5;
+#pragma unroll 4
+      for (int i = 0; i < TM / 8; i++) {
+        const int r = rg + 8 * i;
+        if (r < nvalid)
+          red_add_v4(&a.gHa[(size_t)s_a[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&P[r * LD + 4 * q]));
+      }
+    }
+    // gang += gpre @ Wg   (K = 128, N = 64) on the tensor cores: warpgroup w takes rows 64 w .. 64 w + 63
+    mbar_wait(sm.wbar(), wpar);  // Wg^T
+    wpar ^= 1;
+    {
+      float d[32];
+      const uint32_t bh = s_u32(sm.W()), bl = bh + 64u * 128u * 4u;
+      wg_mm64(P, LD, 64 * m.branch, 0, bh, bl, 0, false, d);
+      wg_mm64(P, LD, 64 * m.branch, 64, bh, bl, 64, true, d);
+#pragma unroll
+      for (int q = 0; q < 32; q += 2) {
+        const int r = 64 * m.branch + m.rb + 8 * ((q >> 1) & 1), c = 8 * (q >> 2) + m.cb;
+        if (r < nvalid) {
+          float2* gp = reinterpret_cast<float2*>(&a.gang[(size_t)(r0 + r) * D + c]);
+          float2 v = *gp;
+          v.x += d[q], v.y += d[q + 1];
+          *gp = v;
+        }
+      }
+    }
+    fence_proxy_async_smem();  // this thread's generic accesses of P come before its bulk refill
+    __syncthreads();           // P and Wg^T are free
+    if (more) {
+      line_issue_ang(a, sm, t + step, P, s ^ 1);
+      if (tid == 0) bulk_g2s_image(sm.W(), a.Wgcan, 16384 * 4, sm.wbar());
     }
   }
 }
 
-void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden) {
+void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms) {
   if (a.A <= 0) return;
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_) {
-    B2M_CK(cudaFuncSetAttribute(k_line_fwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::fwd_bytes));
-    B2M_CK(cudaFuncSetAttribute(k_line_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::fwd_bytes));
+    B2M_CK(cudaFuncSetAttribute(k_line_fwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
+    B2M_CK(cudaFuncSetAttribute(k_line_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
   }
+  const int grid = std::min(cdiv(a.A, TM), num_sms);
   if (hidden)
-    k_line_fwd<true><<<cdiv(a.A, TM), NT, LineSmem::fwd_bytes, st>>>(a);
+    k_line_fwd<true><<<grid, NT, LineSmem::bytes, st>>>(a);
   else
-    k_line_fwd<false><<<cdiv(a.A, TM), NT, LineSmem::fwd_bytes, st>>>(a);
+    k_line_fwd<false><<<grid, NT, LineSmem::bytes, st>>>(a);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }
-void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden) {
+void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms) {
   if (a.A <= 0) return;
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_) {
-    B2M_CK(cudaFuncSetAttribute(k_line_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bwd_bytes));
-    B2M_CK(cudaFuncSetAttribute(k_line_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bwd_bytes));
+    B2M_CK(cudaFuncSetAttribute(k_line_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
+    B2M_CK(cudaFuncSetAttribute(k_line_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
   }
+  const int grid = std::min(cdiv(a.A, TM), num_sms);
   if (hidden)
-    k_line_bwd<true><<<cdiv(a.A, TM), NT, LineSmem::bwd_bytes, st>>>(a);
+    k_line_bwd<true><<<grid, NT, LineSmem::bytes, st>>>(a);
   else
-    k_line_bwd<false><<<cdiv(a.A, TM), NT, LineSmem::bwd_bytes, st>>>(a);
+    k_line_bwd<false><<<grid, NT, LineSmem::bytes, st>>>(a);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }

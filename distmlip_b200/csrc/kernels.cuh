@@ -94,8 +94,9 @@ struct LineArgs {
   float* gHb;          // [B_own,128] (+=)
   float* gXc;          // [n_loc,128] (+=)
 };
-void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden);
-void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden);
+// persistent: min(tiles, num_sms) CTAs loop over the 128-angle tiles
+void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms);
+void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms);
 
 // -------- bond update: h' = h + upd * w3b(d_b) --------
 void launch_bond_update_fwd(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp3, const float* W3bw,
