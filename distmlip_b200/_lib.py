@@ -18,7 +18,7 @@ SYMBOLS = [
     "b2m_finalize_weights", "b2m_set_scaling", "b2m_comm_unique_id", "b2m_comm_init", "b2m_set_partition", "b2m_set_structure", "b2m_compute",
     "b2m_compute_resident", "b2m_get_results", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
     "b2m_debug_tensor", "b2m_last_timings", "b2m_release_workspace", "b2m_set_view", "b2m_create_tensornet",
-    "b2m_set_atomic", "b2m_get_atomic", "b2m_set_heat_flux", "b2m_compute_heat_flux",
+    "b2m_set_atomic", "b2m_get_atomic", "b2m_set_heat_flux", "b2m_compute_heat_flux", "b2m_create_mace",
 ]
 
 
@@ -36,6 +36,15 @@ class TensorNetDesc(C.Structure):
         ("n_elem", C.c_int32), ("units", C.c_int32), ("num_rbf", C.c_int32), ("n_blocks", C.c_int32),
         ("so3", C.c_int32), ("reserved", C.c_int32),
         ("cutoff", C.c_double), ("rbf_width", C.c_double), ("data_mean", C.c_double), ("data_std", C.c_double),
+    ]
+
+
+class MaceDesc(C.Structure):
+    _fields_ = [
+        ("n_elem", C.c_int32), ("channels", C.c_int32), ("max_ell", C.c_int32), ("correlation", C.c_int32),
+        ("num_interactions", C.c_int32), ("num_bessel", C.c_int32), ("num_polynomial_cutoff", C.c_int32),
+        ("mlp_hidden", C.c_int32), ("residual_mask", C.c_int32), ("reserved", C.c_int32),
+        ("r_max", C.c_double), ("c_act", C.c_double), ("avg_num_neighbors", C.c_double * 8),
     ]
 
 
@@ -62,6 +71,7 @@ def load_library():
     P = C.POINTER
     lib.b2m_create.argtypes = [P(ModelDesc), P(C.c_int), i32, P(vp)]
     lib.b2m_create_tensornet.argtypes = [P(TensorNetDesc), P(C.c_int), i32, P(vp)]
+    lib.b2m_create_mace.argtypes = [P(MaceDesc), P(C.c_int), i32, P(vp)]
     lib.b2m_destroy.argtypes = [vp]
     lib.b2m_last_error.argtypes = [vp]
     lib.b2m_last_error.restype = C.c_char_p
@@ -109,15 +119,19 @@ class Engine:
     job) or a list of ordinals = a single-process group with one partition per entry (ordinals may repeat)."""
 
     def __init__(self, *, n_elem, dim=64, max_n=9, max_f=4, n_blocks, cutoff, three_body_cutoff=0.0, cutoff_exponent=0,
-                 data_mean=0.0, data_std=1.0, device=0, tensornet=None):
+                 data_mean=0.0, data_std=1.0, device=0, tensornet=None, mace=None):
         """`tensornet`: None for CHGNet, else dict(units=, num_rbf=, so3=, rbf_width=) for a TensorNet handle
-        (b2m_create_tensornet); everything after construction is the same."""
+        (b2m_create_tensornet); `mace`: a MaceDesc for a MACE handle (b2m_create_mace, which takes n_elem, n_blocks and
+        the cutoff from it); everything after construction is the same."""
         self.lib = load_library()
         self.h = C.c_void_p()
         devs = [int(d) for d in device] if isinstance(device, (list, tuple)) else [int(device)]
         dev = (C.c_int * len(devs))(*devs)
-        self.kind = "chgnet" if tensornet is None else "tensornet"
-        if tensornet is None:
+        self.kind = "mace" if mace is not None else ("chgnet" if tensornet is None else "tensornet")
+        if mace is not None:
+            self.desc = mace
+            rc = self.lib.b2m_create_mace(C.byref(self.desc), dev, len(devs), C.byref(self.h))
+        elif tensornet is None:
             self.desc = ModelDesc(n_elem, dim, max_n, max_f, n_blocks, cutoff_exponent, cutoff, three_body_cutoff,
                                   data_mean, data_std)
             rc = self.lib.b2m_create(C.byref(self.desc), dev, len(devs), C.byref(self.h))

@@ -25,6 +25,7 @@
 #include "atomic_virial.cuh"
 #include "graph.cuh"
 #include "kernels.cuh"
+#include "mace_state.cuh"
 #include "tn_state.cuh"
 
 namespace b2m {
@@ -115,8 +116,9 @@ struct GroupSync {
 
 struct b2m_engine {
   b2m_model_desc desc;
-  int kind = 0;                   // 0: CHGNet (b2m_create), 1: TensorNet (b2m_create_tensornet)
+  int kind = 0;                   // 0: CHGNet (b2m_create), 1: TensorNet (b2m_create_tensornet), 2: MACE (b2m_create_mace)
   b2m::TnState* tn = nullptr;     // TensorNet weights and workspace (kind 1)
+  b2m::MaceState* mace = nullptr;  // MACE weights and workspace (kind 2)
   int device = 0;
   cudaStream_t st = nullptr;
   cudaStream_t cst = nullptr;            // halo traffic of the forward pass (overlaps the projections that do not need it)
@@ -552,10 +554,15 @@ static void alloc_workspace(b2m_engine* e) {
 // rows (forward) or copies its halo adjoints into the owner's receive buffer (backward); a CUDA event per exchange point
 // orders the receiver's stream behind the sender's.
 // kind 0: atom rows x[l] | 1: bond rows h[l] | 2: TensorNet atom tensors X[l] (10 x 64 floats per atom)
+//      3: MACE node features h[l] (C floats per atom)
 static float* halo_buffer(b2m_engine* e, int kind, int l) {
+  if (kind == 3) return e->mace->h[l].p;
   return kind == 1 ? e->h[l].p : (kind == 2 ? e->tn->X[l].p : e->x[l].p);
 }
-static int halo_width(int kind) { return kind == 2 ? 10 * D : D; }
+static int halo_width(const b2m_engine* e, int kind) {
+  if (kind == 3) return e->mace->C;
+  return kind == 2 ? 10 * D : D;
+}
 
 static cudaEvent_t next_halo_event(b2m_engine* e) {
   // the events are created in b2m_create: a neighbour's thread reads hev[k] concurrently, so the vector never grows here
@@ -572,7 +579,7 @@ static void halo_forward_begin(b2m_engine* e, int kind, int l) {
   if (e->world <= 1 || e->debug_no_halo) return;
   Graph& g = e->g;
   const bool bonds = kind == 1;
-  const size_t W = (size_t)halo_width(kind);
+  const size_t W = (size_t)halo_width(e, kind);
   float* buf = halo_buffer(e, kind, l);
   const int* nto = bonds ? g.nb_to : g.n_to;
   const int* toff = bonds ? g.bto_off : g.to_off;
@@ -674,6 +681,7 @@ static void halo_backward(b2m_engine* e, float* gbuf, bool bonds, int width = D)
 }
 
 #include "engine_tn.inl"
+#include "engine_mace.inl"
 
 static AtomConvArgs atom_args(b2m_engine* e, int l) {
   Graph& g = e->g;
@@ -969,10 +977,14 @@ static void run(b2m_engine* e, bool grads) {
     LAUNCH_HF(k_hf_weights, e->g.N, e->st, e->g.N, e->hf_n, e->g.cart.p, e->hf_c[0], e->hf_c[1], e->hf_c[2], e->hf_seed,
               e->hf_w.p);
   }
-  if (e->kind == 1) tn_forward(e); else forward(e);
+  if (e->kind == 1) tn_forward(e);
+  else if (e->kind == 2) mace_forward(e);
+  else forward(e);
   B2M_CK(cudaEventRecord(e->ev[1], e->st));
   if (grads) {
-    if (e->kind == 1) tn_backward(e); else backward(e);
+    if (e->kind == 1) tn_backward(e);
+    else if (e->kind == 2) mace_backward(e);
+    else backward(e);
   }
   if (e->world > 1 && e->leader == nullptr && !e->debug_no_halo) {
     NCCL_CK(g_nccl.AllReduce(e->scal.p, e->scal.p, 10, ncclFloat64, ncclSum, e->comm, e->st));
@@ -1298,12 +1310,25 @@ static b2m_engine* create_one(const b2m_model_desc* desc, int device, int count)
 }
 
 static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdesc, const int* devices, int ndev,
-                      b2m_handle* out) {
+                      b2m_handle* out, const b2m_mace_desc* mdesc = nullptr) {
   if (!desc || !devices || !out) return B2M_ERR_INVALID;
   std::vector<b2m_engine*> made;
   try {
     B2M_REQUIRE(ndev >= 1 && ndev <= MAXP, B2M_ERR_PARTITIONS, "ndev must be in [1,16]");
-    if (tdesc) {
+    if (mdesc) {
+      B2M_REQUIRE(mdesc->channels >= 32 && mdesc->channels <= 128 && mdesc->channels % 32 == 0, B2M_ERR_INVALID,
+                  "MACE engine supports hidden_irreps = C x 0e with C a multiple of 32, C <= 128");
+      B2M_REQUIRE(mdesc->max_ell >= 0 && mdesc->max_ell <= 3, B2M_ERR_INVALID, "MACE engine supports max_ell <= 3");
+      B2M_REQUIRE(mdesc->correlation >= 1 && mdesc->correlation <= 3, B2M_ERR_INVALID, "MACE engine supports correlation <= 3");
+      B2M_REQUIRE(mdesc->num_interactions >= 1 && mdesc->num_interactions <= kMaceMaxLayers, B2M_ERR_INVALID,
+                  "num_interactions must be in [1,8]");
+      B2M_REQUIRE(mdesc->num_bessel >= 1 && mdesc->num_bessel <= 64, B2M_ERR_INVALID, "num_bessel must be in [1,64]");
+      B2M_REQUIRE(mdesc->mlp_hidden >= 1 && mdesc->mlp_hidden <= 256, B2M_ERR_INVALID, "readout MLP width must be in [1,256]");
+      B2M_REQUIRE(mdesc->num_polynomial_cutoff >= 1 && mdesc->r_max > 0 && mdesc->c_act > 0, B2M_ERR_INVALID,
+                  "r_max, the cutoff exponent and c_act must be positive");
+      for (int t = 0; t < mdesc->num_interactions; t++)
+        B2M_REQUIRE(mdesc->avg_num_neighbors[t] > 0, B2M_ERR_INVALID, "avg_num_neighbors must be positive");
+    } else if (tdesc) {
       B2M_REQUIRE(tdesc->units == D, B2M_ERR_INVALID, "TensorNet engine supports units = 64");
       B2M_REQUIRE(tdesc->num_rbf >= 1 && tdesc->num_rbf <= 64, B2M_ERR_INVALID, "num_rbf must be in [1,64]");
       B2M_REQUIRE(tdesc->n_blocks >= 1 && tdesc->n_blocks <= 16, B2M_ERR_INVALID, "nblocks must be in [1,16]");
@@ -1322,7 +1347,19 @@ static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdes
                                     cudaGetErrorString(ce));
     for (int p = 0; p < ndev; p++) {
       made.push_back(create_one(desc, devices[p], count));
-      if (tdesc) {
+      if (mdesc) {
+        b2m_engine* m = made.back();
+        m->kind = 2;
+        m->mace = new MaceState();
+        MaceState& M = *m->mace;
+        M.Cr = mdesc->channels, M.C = (mdesc->channels + 63) / 64 * 64;
+        M.L1 = mdesc->max_ell + 1, M.nsh = M.L1 * M.L1, M.T = mdesc->num_interactions;
+        M.correlation = mdesc->correlation, M.H = mdesc->mlp_hidden, M.c_act = mdesc->c_act;
+        M.rp.nb = mdesc->num_bessel, M.rp.nbp = 64, M.rp.p = mdesc->num_polynomial_cutoff;
+        M.rp.r_max = (float)mdesc->r_max, M.rp.pref = (float)std::sqrt(2.0 / mdesc->r_max);
+        for (int t = 0; t < M.T; t++)
+          M.interaction_residual[t] = (mdesc->residual_mask >> t) & 1, M.avg_nb[t] = mdesc->avg_num_neighbors[t];
+      } else if (tdesc) {
         b2m_engine* m = made.back();
         m->kind = 1;
         m->tn = new TnState();
@@ -1359,6 +1396,7 @@ static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdes
   } catch (const b2m::Error& ex) {
     for (auto* m : made) {
       delete m->tn;
+      delete m->mace;
       delete m;
     }
     g_create_err = ex.what();
@@ -1382,9 +1420,21 @@ int b2m_create_tensornet(const b2m_tensornet_desc* tdesc, const int* devices, in
   return create_any(&d, tdesc, devices, ndev, out);
 }
 
+int b2m_create_mace(const b2m_mace_desc* mdesc, const int* devices, int ndev, b2m_handle* out) {
+  if (!mdesc) return B2M_ERR_INVALID;
+  // the shared part of the engine (graph build, transport) reads the CHGNet-shaped description: no bond graph, r_max as
+  // the cutoff, no Potential scaling (scale, shift and E0 are part of the model)
+  b2m_model_desc d;
+  memset(&d, 0, sizeof d);
+  d.n_elem = mdesc->n_elem, d.dim = D, d.max_n = NR, d.max_f = 4, d.n_blocks = mdesc->num_interactions;
+  d.cutoff = mdesc->r_max, d.three_body_cutoff = 0.0, d.data_mean = 0.0, d.data_std = 1.0;
+  return create_any(&d, nullptr, devices, ndev, out, mdesc);
+}
+
 static void destroy_one(b2m_engine* h) {
   cudaSetDevice(h->device);
   delete h->tn;  // frees its device buffers
+  delete h->mace;
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
   for (auto& p : h->gather_ev) {
     cudaEventDestroy(p.first);
@@ -1428,6 +1478,7 @@ int b2m_load_weights(b2m_handle h, const char* name, const float* host_ptr, cons
 
 int b2m_set_element_refs(b2m_handle h, const double* offsets, int n) {
   API_BEGIN
+  B2M_REQUIRE(h->kind != 2, B2M_ERR_INVALID, "a MACE model carries its own atomic energies (atomic_energies_fn)");
   B2M_REQUIRE(offsets == nullptr || n == 0 || n == h->desc.n_elem, B2M_ERR_INVALID, "element_refs length must equal n_elem");
   each_member(h, [&](b2m_engine* e) {
     if (offsets == nullptr || n == 0) {  // clear: a later Potential without element_refs must not inherit the old offsets
@@ -1443,6 +1494,7 @@ int b2m_set_element_refs(b2m_handle h, const double* offsets, int n) {
 
 int b2m_set_scaling(b2m_handle h, double data_mean, double data_std) {
   API_BEGIN
+  B2M_REQUIRE(h->kind != 2, B2M_ERR_INVALID, "a MACE model carries its own scale and shift (scale_shift)");
   each_member(h, [&](b2m_engine* e) {
     e->desc.data_mean = data_mean;
     e->desc.data_std = data_std;
@@ -1453,7 +1505,9 @@ int b2m_set_scaling(b2m_handle h, double data_mean, double data_std) {
 int b2m_finalize_weights(b2m_handle h) {
   API_BEGIN
   each_member(h, [&](b2m_engine* e) {
-    if (e->kind == 1) tn_finalize_weights(e); else finalize_weights(e);
+    if (e->kind == 1) tn_finalize_weights(e);
+    else if (e->kind == 2) mace_finalize_weights(e);
+    else finalize_weights(e);
   });
   API_END
 }
@@ -1530,7 +1584,9 @@ static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart,
     h->g.build(h->st, natoms, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff, tol, h->rank,
                h->world);
   }
-  if (h->kind == 1) tn_alloc_workspace(h); else alloc_workspace(h);
+  if (h->kind == 1) tn_alloc_workspace(h);
+  else if (h->kind == 2) mace_alloc_workspace(h);
+  else alloc_workspace(h);
   B2M_CK(cudaEventRecord(h->ev[4], h->st));
   B2M_CK(cudaStreamSynchronize(h->st));
   float ms;
@@ -1578,6 +1634,7 @@ int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9)
 int b2m_set_heat_flux(b2m_handle h, double reach) {
   API_BEGIN
   B2M_REQUIRE(reach >= 0 && std::isfinite(reach), B2M_ERR_INVALID, "heat-flux reach must be >= 0");
+  B2M_REQUIRE(h->kind != 2, B2M_ERR_INVALID, "the heat flux is not implemented for MACE");
   each_member(h, [&](b2m_engine* e) { e->hf_reach = reach; });
   API_END
 }
@@ -1614,7 +1671,7 @@ int b2m_get_atomic(b2m_handle h, double* energies, float* virials) {
 int b2m_get_sitewise(b2m_handle h, float* out) {
   API_BEGIN
   B2M_REQUIRE(h->have_graph && out, B2M_ERR_STATE, "no structure");
-  B2M_REQUIRE(h->kind == 0, B2M_ERR_INVALID, "the site-wise readout belongs to CHGNet (TensorNet has none)");
+  B2M_REQUIRE(h->kind == 0, B2M_ERR_INVALID, "the site-wise readout belongs to CHGNet (TensorNet and MACE have none)");
   std::vector<float> full(h->g.N, 0.f);
   auto collect = [&](b2m_engine* e) {  // owned rows of one partition -> global order
     Graph& g = e->g;
@@ -1680,6 +1737,8 @@ int b2m_debug_tensor(b2m_handle h, const char* name, float* out, int64_t cap, in
   auto idx = [&](const std::string& pre) { return atoi(n.c_str() + pre.size()); };
   if (h->kind == 1) {
     B2M_REQUIRE(tn_debug_lookup(h, n, src, r, c), B2M_ERR_INVALID, "unknown debug tensor: " + n);
+  } else if (h->kind == 2) {
+    B2M_REQUIRE(mace_debug_lookup(h, n, src, r, c), B2M_ERR_INVALID, "unknown debug tensor: " + n);
   } else if (n[0] == 'x' && isdigit(n[1])) {
     int l = idx("x");
     B2M_REQUIRE(l >= 0 && l < (int)h->x.size(), B2M_ERR_INVALID, "bad layer");
@@ -1741,6 +1800,7 @@ int b2m_release_workspace(b2m_handle h) {
     e->uf.~Unfold();
     new (&e->uf) Unfold();
     tn_release(e);
+    mace_release(e);
     e->g.~Graph();  // the resident graph goes too
     new (&e->g) Graph();
   });

@@ -1,0 +1,441 @@
+// kernels_mace.cu -- MACE with scalar hidden features (hidden_irreps = C x 0e) on the same partitioned CSR graph as the
+// CHGNet and TensorNet paths.  Arithmetic as oracle/mace_ref.py states it (the conventions are written down there once);
+// engine_mace.inl runs these kernels stage by stage.
+//
+// First generation: the node- and edge-level products (radial MLP, linear_up, the per-l mixes, the product linear) run
+// on the wgmma row GEMM of the other paths (kernels_wg.cu, engine_mace.inl tc_mm); the element-dependent mixes
+// (skip_tp) read the element's C x C block per atom; the symmetric contraction is one thread per (atom, channel) that
+// walks the nonzero terms of U, which every channel shares.  Aggregations walk the CSR-by-destination rows (no atomics
+// in the forward); the reverse scatters to sources with atomics.
+#include "atomic_virial.cuh"
+#include "mace_state.cuh"
+
+namespace b2m {
+
+namespace {
+
+__device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + __expf(-x)); }
+__device__ __forceinline__ float silu_f(float x) { return x * sigm(x); }
+__device__ __forceinline__ float dsilu_f(float x) {
+  const float s = sigm(x);
+  return s * (1.f + x * (1.f - s));
+}
+
+#define MACE_LAUNCH(kern, nitems, bs, st, ...)                \
+  do {                                                        \
+    if ((nitems) > 0) {                                       \
+      kern<<<cdiv((nitems), (bs)), (bs), 0, st>>>(__VA_ARGS__); \
+      B2M_CK(cudaGetLastError());                             \
+      g_launch_count++;                                       \
+    }                                                         \
+  } while (0)
+
+// ============================================================================================
+// edge geometry: spherical harmonics (oracle/mace_ref.py sh_basis) and Bessel x polynomial cutoff
+// ============================================================================================
+// value and gradient (w.r.t. the unit vector's components) carried together
+struct Dual {
+  float v, x, y, z;
+};
+__device__ __forceinline__ Dual operator*(Dual a, Dual b) {
+  return {a.v * b.v, a.x * b.v + a.v * b.x, a.y * b.v + a.v * b.y, a.z * b.v + a.v * b.z};
+}
+__device__ __forceinline__ Dual operator*(float s, Dual a) { return {s * a.v, s * a.x, s * a.y, s * a.z}; }
+__device__ __forceinline__ Dual operator-(Dual a, Dual b) { return {a.v - b.v, a.x - b.x, a.y - b.y, a.z - b.z}; }
+
+template <class T>
+__device__ __forceinline__ T smul(float s, T a) { return s * a; }
+
+// Y[0..nsh) of the unit vector (x, y, z); T = float or Dual
+template <class T>
+__device__ __forceinline__ void sh16(T x, T y, T z, T one, int nsh, T* Y) {
+  Y[0] = one;
+  if (nsh <= 1) return;
+  const float s3 = 1.7320508075688772f;
+  Y[1] = smul(s3, x), Y[2] = smul(s3, y), Y[3] = smul(s3, z);
+  if (nsh <= 4) return;
+  const float s15 = 3.872983346207417f, s5h = 1.118033988749895f, s15h = 1.9364916731037085f;
+  const T xx = x * x, yy = y * y, zz = z * z;
+  Y[4] = smul(s15, x * y), Y[5] = smul(s15, y * z), Y[6] = smul(s5h, smul(2.f, zz) - xx - yy), Y[7] = smul(s15, x * z);
+  Y[8] = smul(s15h, xx - yy);
+  if (nsh <= 9) return;
+  const float a = 2.091650066335189f, b = 10.246950765959598f, c = 1.6201851746019651f, d = 1.3228756555322954f;
+  const T q = smul(4.f, zz) - xx - yy;
+  Y[9] = smul(a, y * (smul(3.f, xx) - yy));
+  Y[10] = smul(b, x * y * z);
+  Y[11] = smul(c, y * q);
+  Y[12] = smul(d, z * (smul(2.f, zz) - smul(3.f, xx) - smul(3.f, yy)));
+  Y[13] = smul(c, x * q);
+  Y[14] = smul(0.5f * b, z * (xx - yy));
+  Y[15] = smul(a, x * (xx - smul(3.f, yy)));
+}
+
+// polynomial cutoff and its derivative in d
+__device__ __forceinline__ void poly_cut(float d, const MaceRadial& rp, float& f, float& df) {
+  const float x = d / rp.r_max;
+  if (x >= 1.f) {
+    f = 0.f, df = 0.f;
+    return;
+  }
+  const float p = (float)rp.p;
+  const float xp1 = __powf(x, p - 1.f), xp = xp1 * x, xp1p = xp * x, xp2 = xp1p * x;
+  f = 1.f - 0.5f * (p + 1.f) * (p + 2.f) * xp + p * (p + 2.f) * xp1p - 0.5f * p * (p + 1.f) * xp2;
+  df = (-0.5f * (p + 1.f) * (p + 2.f) * p * xp1 + p * (p + 2.f) * (p + 1.f) * xp - 0.5f * p * (p + 1.f) * (p + 2.f) * xp1p) /
+       rp.r_max;
+}
+
+__global__ void k_mace_edge_geom(int64_t E, const float4* __restrict__ e_vec, MaceRadial rp, int nsh,
+                                 float* __restrict__ Y, float* __restrict__ eb) {
+  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const float4 v = e_vec[e];
+  const float d = v.w, rd = 1.f / d;
+  float y[kMaceMaxNsh];
+  sh16<float>(v.x * rd, v.y * rd, v.z * rd, 1.f, nsh, y);
+#pragma unroll
+  for (int k = 0; k < kMaceMaxNsh; k++) Y[e * kMaceMaxNsh + k] = k < nsh ? y[k] : 0.f;
+  float f, df;
+  poly_cut(d, rp, f, df);
+  for (int n = 0; n < rp.nbp; n++) eb[e * rp.nbp + n] = n < rp.nb ? rp.pref * sinf(rp.w[n] * d) * rd * f : 0.f;
+}
+
+__global__ void k_mace_embed(int n, int C, const int* __restrict__ type, const float* __restrict__ W,
+                             float* __restrict__ h0) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n * C) return;
+  const int r = (int)(i / C), c = (int)(i % C);
+  h0[i] = W[(size_t)type[r] * C + c];
+}
+
+// A[lm][t][c] = sum_{e -> t} R[e][l(lm) C + c] Y[e][lm] u[src(e)][c]
+__global__ void k_mace_msg(int n_own, int C, int L1, const int* __restrict__ row_ptr, const int* __restrict__ e_src,
+                           const float* __restrict__ R, const float* __restrict__ Y, const float* __restrict__ u,
+                           float* __restrict__ A) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;
+  const int t = (int)(i / C), c = (int)(i % C), nsh = L1 * L1, RW = L1 * C;
+  float acc[kMaceMaxNsh];
+#pragma unroll
+  for (int k = 0; k < kMaceMaxNsh; k++) acc[k] = 0.f;
+  for (int e = row_ptr[t]; e < row_ptr[t + 1]; e++) {
+    const float uc = u[(size_t)e_src[e] * C + c];
+    const float* re = R + (size_t)e * RW + c;
+    const float* ye = Y + (size_t)e * kMaceMaxNsh;
+#pragma unroll
+    for (int l = 0; l < 4; l++) {
+      if (l >= L1) break;
+      const float r = re[l * C] * uc;
+      for (int m = l * l; m < (l + 1) * (l + 1); m++) acc[m] = fmaf(r, ye[m], acc[m]);
+    }
+  }
+  const size_t plane = (size_t)n_own * C;
+#pragma unroll
+  for (int k = 0; k < kMaceMaxNsh; k++)
+    if (k < nsh) A[k * plane + i] = acc[k];
+}
+
+// reverse of k_mace_msg: gR[e][l C + c] = u sum_{m in l} gA[m] Y[m] ; gY[e][m] += sum_c gA[m] R[l] u (warp sums over
+// 32 channels of one destination, then one atomic) ; gu[src][c] += sum_m gA[m] R[l(m)] Y[m]
+__global__ void k_mace_msg_bwd(int n_own, int C, int L1, const int* __restrict__ row_ptr, const int* __restrict__ e_src,
+                               const float* __restrict__ R, const float* __restrict__ Y, const float* __restrict__ u,
+                               const float* __restrict__ gA, float* __restrict__ gR, float* __restrict__ gY,
+                               float* __restrict__ gu) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;  // n_own * C is a multiple of 32: whole warps leave together
+  const int t = (int)(i / C), c = (int)(i % C), nsh = L1 * L1, RW = L1 * C, lane = threadIdx.x & 31;
+  const size_t plane = (size_t)n_own * C;
+  float ga[kMaceMaxNsh];
+#pragma unroll
+  for (int k = 0; k < kMaceMaxNsh; k++) ga[k] = k < nsh ? gA[k * plane + i] : 0.f;
+  for (int e = row_ptr[t]; e < row_ptr[t + 1]; e++) {
+    const int s = e_src[e];
+    const float uc = u[(size_t)s * C + c];
+    const float* re = R + (size_t)e * RW + c;
+    const float* ye = Y + (size_t)e * kMaceMaxNsh;
+    float gus = 0.f;
+#pragma unroll
+    for (int l = 0; l < 4; l++) {
+      if (l >= L1) break;
+      const float r = re[l * C];
+      float gr = 0.f;
+      for (int m = l * l; m < (l + 1) * (l + 1); m++) {
+        const float y = ye[m];
+        gr = fmaf(ga[m], y, gr);
+        float gy = ga[m] * r * uc;
+        for (int o = 16; o > 0; o >>= 1) gy += __shfl_xor_sync(0xffffffffu, gy, o);
+        if (lane == 0) atomicAdd(&gY[(size_t)e * kMaceMaxNsh + m], gy);
+      }
+      gR[(size_t)e * RW + l * C + c] = gr * uc;
+      gus = fmaf(gr, r, gus);
+    }
+    atomicAdd(&gu[(size_t)s * C + c], gus);
+  }
+}
+
+// out[lm][i][:] (+)= in[lm][i][:] @ W[type[i]][l(lm)] : one block of C threads per row i; each weight element is read
+// once per row and applied to the 2l + 1 components of its l
+__global__ void k_mace_elem_mix(int n, int C, int L1, int nsh, const int* __restrict__ type, const float* __restrict__ W,
+                                const float* __restrict__ in, float* __restrict__ out, int accum) {
+  __shared__ float x[7][128];
+  const int i = blockIdx.x, c2 = threadIdx.x;
+  const int z = type[i];
+  const size_t plane = (size_t)n * C;
+  const int Lw = nsh == 1 ? 1 : L1;
+  for (int l = 0; l < Lw; l++) {
+    const int m0 = l * l, nm = 2 * l + 1;
+    __syncthreads();
+    for (int m = 0; m < nm; m++) x[m][c2] = in[(m0 + m) * plane + (size_t)i * C + c2];
+    __syncthreads();
+    const float* Wb = W + ((size_t)z * Lw + l) * C * C + c2;
+    float acc[7] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    for (int c = 0; c < C; c++) {
+      const float w = Wb[(size_t)c * C];
+#pragma unroll
+      for (int m = 0; m < 7; m++)
+        if (m < nm) acc[m] = fmaf(w, x[m][c], acc[m]);
+    }
+    for (int m = 0; m < nm; m++) {
+      float* o = out + (m0 + m) * plane + (size_t)i * C + c2;
+      *o = accum ? *o + acc[m] : acc[m];
+    }
+  }
+}
+
+// symmetric contraction, one thread per (atom, channel): the channel's 16 components of A sit in shared memory (column
+// per thread), the terms are read by every thread of the warp at the same address
+template <bool kBwd>
+__global__ void __launch_bounds__(128) k_mace_symc(int n_own, int C, int nsh, int Ktot, const int* __restrict__ type,
+                                                   const float* __restrict__ A, const MaceTerm* __restrict__ terms,
+                                                   int nterms, const float* __restrict__ w, const float* __restrict__ gB,
+                                                   float* __restrict__ out) {
+  __shared__ float a[kMaceMaxNsh][128];
+  __shared__ float ga[kBwd ? kMaceMaxNsh : 1][128];
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;
+  const int tid = threadIdx.x, t = (int)(i / C), c = (int)(i % C);
+  const size_t plane = (size_t)n_own * C;
+#pragma unroll
+  for (int k = 0; k < kMaceMaxNsh; k++) {
+    a[k][tid] = k < nsh ? A[k * plane + i] : 0.f;
+    if constexpr (kBwd) ga[k][tid] = 0.f;
+  }
+  const float* wz = w + (size_t)type[t] * Ktot * C + c;
+  const float g = kBwd ? gB[i] : 0.f;
+  float acc = 0.f;
+  for (int j = 0; j < nterms; j++) {
+    const MaceTerm tm = terms[j];
+    const int nu = tm.idx >> 24, i1 = tm.idx & 255, i2 = (tm.idx >> 8) & 255, i3 = (tm.idx >> 16) & 255;
+    const float cw = tm.coef * wz[(size_t)tm.kg * C];
+    const float a1 = a[i1][tid], a2 = nu >= 2 ? a[i2][tid] : 1.f, a3 = nu >= 3 ? a[i3][tid] : 1.f;
+    if constexpr (!kBwd) {
+      acc = fmaf(cw, a1 * a2 * a3, acc);
+    } else {
+      const float s = cw * g;
+      ga[i1][tid] += s * a2 * a3;
+      if (nu >= 2) ga[i2][tid] += s * a1 * a3;
+      if (nu >= 3) ga[i3][tid] += s * a1 * a2;
+    }
+  }
+  if constexpr (!kBwd) {
+    out[i] = acc;
+  } else {
+#pragma unroll
+    for (int k = 0; k < kMaceMaxNsh; k++)
+      if (k < nsh) out[k * plane + i] = ga[k][tid];
+  }
+}
+
+// ============================================================================================
+// readouts
+// ============================================================================================
+__global__ void k_mace_readout_lin(int n_own, int C, const float* __restrict__ h, const float* __restrict__ w,
+                                   float* __restrict__ e_lin) {
+  const int r = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (r >= n_own) return;
+  float s = 0.f;
+  for (int c = lane; c < C; c += 32) s = fmaf(h[(size_t)r * C + c], w[c], s);
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) e_lin[r] += s;
+}
+
+template <bool kAtomic>
+__global__ void k_mace_readout_final(int n_own, int C, int H, const float* __restrict__ h, const float* __restrict__ W1,
+                                     const float* __restrict__ w2, const float* __restrict__ e_lin,
+                                     const int* __restrict__ type, const double* __restrict__ E0, double scale,
+                                     double shift, float* __restrict__ pre, double* __restrict__ energy,
+                                     const int* __restrict__ gid, double* __restrict__ atom_e) {
+  const int r = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (r >= n_own) return;
+  float e = 0.f;
+  for (int j = 0; j < H; j++) {
+    float s = 0.f;
+    for (int c = lane; c < C; c += 32) s = fmaf(h[(size_t)r * C + c], W1[(size_t)c * H + j], s);
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) pre[(size_t)r * H + j] = s;
+    e = fmaf(silu_f(s), w2[j], e);
+  }
+  if (lane == 0) {
+    const double eps = E0[type[r]] + scale * ((double)e_lin[r] + (double)e) + shift;
+    if constexpr (kAtomic) atom_e[gid[r]] = eps;
+    atomicAdd(energy, eps);
+  }
+}
+
+__global__ void k_mace_readout_seed(int n_own, int C, int H, const float* __restrict__ pre, const float* __restrict__ W1,
+                                    const float* __restrict__ w2, float scale, float* __restrict__ gh) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;
+  const int r = (int)(i / C), c = (int)(i % C);
+  float s = 0.f;
+  for (int j = 0; j < H; j++) s = fmaf(W1[(size_t)c * H + j] * w2[j], dsilu_f(pre[(size_t)r * H + j]), s);
+  gh[i] = scale * s;
+}
+
+__global__ void k_mace_add_row(int n_own, int C, const float* __restrict__ w, float scale, float* __restrict__ gh) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;
+  gh[i] += scale * w[i % C];
+}
+
+// ============================================================================================
+// final geometry reverse: dE/dv from the adjoints of the radial basis (g_eb) and of the harmonics (gY)
+// ============================================================================================
+__device__ __forceinline__ void virial_reduce_mace(const float (&v)[9], double* __restrict__ virial) {
+  __shared__ float red[9][8];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int k = 0; k < 9; k++) {
+    float x = v[k];
+    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+    if (lane == 0) red[k][warp] = x;
+  }
+  __syncthreads();
+  if (threadIdx.x < 9) {
+    double s = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += (double)red[threadIdx.x][w];
+    atomicAdd(&virial[threadIdx.x], s);
+  }
+}
+template <bool kAtomic>
+__global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, const int* __restrict__ e_src,
+                                                         const int* __restrict__ e_dst, const float4* __restrict__ e_vec,
+                                                         const int* __restrict__ gid, MaceRadial rp,
+                                                         const float* __restrict__ g_eb, const float* __restrict__ gY,
+                                                         float* __restrict__ forces, double* __restrict__ virial,
+                                                         float* __restrict__ atom_vir) {
+  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  float vir[9];
+#pragma unroll
+  for (int k = 0; k < 9; k++) vir[k] = 0.f;
+  int asrc = 0, adst = -1;
+  if (e < E) {
+    const float4 v = e_vec[e];
+    const float d = v.w, rd = 1.f / d;
+    const float x = v.x * rd, y = v.y * rd, z = v.z * rd;
+    float f, df;
+    poly_cut(d, rp, f, df);
+    float gd = 0.f;
+    for (int n = 0; n < rp.nb; n++) {
+      float sn, cn;
+      sincosf(rp.w[n] * d, &sn, &cn);  // w_n d reaches num_bessel * pi: the accurate range reduction
+      const float b = rp.pref * sn * rd, db = rp.pref * (rp.w[n] * cn - sn * rd) * rd;
+      gd = fmaf(g_eb[(size_t)e * rp.nbp + n], db * f + b * df, gd);
+    }
+    Dual Yd[kMaceMaxNsh];
+    sh16<Dual>(Dual{x, 1.f, 0.f, 0.f}, Dual{y, 0.f, 1.f, 0.f}, Dual{z, 0.f, 0.f, 1.f}, Dual{1.f, 0.f, 0.f, 0.f}, nsh, Yd);
+    float hx = 0.f, hy = 0.f, hz = 0.f;
+    for (int m = 1; m < nsh; m++) {
+      const float gy = gY[(size_t)e * kMaceMaxNsh + m];
+      hx = fmaf(gy, Yd[m].x, hx), hy = fmaf(gy, Yd[m].y, hy), hz = fmaf(gy, Yd[m].z, hz);
+    }
+    const float pr = hx * x + hy * y + hz * z;
+    const float gx = gd * x + (hx - pr * x) * rd, gyv = gd * y + (hy - pr * y) * rd, gz = gd * z + (hz - pr * z) * rd;
+    // vec = x_dst + off.L - x_src :  dE/dx_dst += g, dE/dx_src -= g ; F = -dE/dx
+    const int gdst = gid[e_dst[e]], gsrc = gid[e_src[e]];
+    atomicAdd(&forces[(size_t)gdst * 3], -gx);
+    atomicAdd(&forces[(size_t)gdst * 3 + 1], -gyv);
+    atomicAdd(&forces[(size_t)gdst * 3 + 2], -gz);
+    atomicAdd(&forces[(size_t)gsrc * 3], gx);
+    atomicAdd(&forces[(size_t)gsrc * 3 + 1], gyv);
+    atomicAdd(&forces[(size_t)gsrc * 3 + 2], gz);
+    vir[0] = v.x * gx, vir[1] = v.x * gyv, vir[2] = v.x * gz;
+    vir[3] = v.y * gx, vir[4] = v.y * gyv, vir[5] = v.y * gz;
+    vir[6] = v.z * gx, vir[7] = v.z * gyv, vir[8] = v.z * gz;
+    if constexpr (kAtomic) asrc = gsrc, adst = gdst;
+  }
+  if constexpr (kAtomic) {
+    float w[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) w[k] = 0.5f * vir[k];
+    red_add_edge_virial(atom_vir, asrc, adst, w);
+  }
+  virial_reduce_mace(vir, virial);
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------------------------
+// launchers
+// ---------------------------------------------------------------------------------------------
+void launch_mace_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const MaceRadial& rp, int nsh, float* Y,
+                           float* eb) {
+  MACE_LAUNCH(k_mace_edge_geom, E, 256, st, E, e_vec, rp, nsh, Y, eb);
+}
+void launch_mace_embed(cudaStream_t st, int n, int C, const int* type, const float* W, float* h0) {
+  MACE_LAUNCH(k_mace_embed, (int64_t)n * C, 256, st, n, C, type, W, h0);
+}
+void launch_mace_msg(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
+                     const float* Y, const float* u, float* A) {
+  MACE_LAUNCH(k_mace_msg, (int64_t)n_own * C, 256, st, n_own, C, L1, row_ptr, e_src, R, Y, u, A);
+}
+void launch_mace_msg_bwd(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
+                         const float* Y, const float* u, const float* gA, float* gR, float* gY, float* gu) {
+  MACE_LAUNCH(k_mace_msg_bwd, (int64_t)n_own * C, 256, st, n_own, C, L1, row_ptr, e_src, R, Y, u, gA, gR, gY, gu);
+}
+void launch_mace_elem_mix(cudaStream_t st, int n, int C, int L1, int nsh, const int* type, const float* W,
+                          const float* in, float* out, bool accum) {
+  if (n <= 0) return;
+  B2M_REQUIRE(C <= 128, B2M_ERR_INVALID, "mace elem mix: C <= 128");
+  k_mace_elem_mix<<<n, C, 0, st>>>(n, C, L1, nsh, type, W, in, out, accum ? 1 : 0);
+  B2M_CK(cudaGetLastError());
+  g_launch_count++;
+}
+void launch_mace_symc(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                      const MaceTerm* terms, int nterms, const float* w, float* B) {
+  MACE_LAUNCH(k_mace_symc<false>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, nullptr, B);
+}
+void launch_mace_symc_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                          const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA) {
+  MACE_LAUNCH(k_mace_symc<true>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, gB, gA);
+}
+void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, const float* h, const float* w, float* e_lin) {
+  MACE_LAUNCH(k_mace_readout_lin, (int64_t)n_own * 32, 256, st, n_own, C, h, w, e_lin);
+}
+void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
+                               const float* e_lin, const int* type, const double* E0, double scale, double shift,
+                               float* pre, double* energy, const int* gid, double* atom_e) {
+  if (atom_e)
+    MACE_LAUNCH(k_mace_readout_final<true>, (int64_t)n_own * 32, 256, st, n_own, C, H, h, W1, w2, e_lin, type, E0, scale,
+                shift, pre, energy, gid, atom_e);
+  else
+    MACE_LAUNCH(k_mace_readout_final<false>, (int64_t)n_own * 32, 256, st, n_own, C, H, h, W1, w2, e_lin, type, E0, scale,
+                shift, pre, energy, gid, atom_e);
+}
+void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const float* pre, const float* W1,
+                              const float* w2, float scale, float* gh) {
+  MACE_LAUNCH(k_mace_readout_seed, (int64_t)n_own * C, 256, st, n_own, C, H, pre, W1, w2, scale, gh);
+}
+void launch_mace_add_row(cudaStream_t st, int n_own, int C, const float* w, float scale, float* gh) {
+  MACE_LAUNCH(k_mace_add_row, (int64_t)n_own * C, 256, st, n_own, C, w, scale, gh);
+}
+void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
+                            const int* gid, const MaceRadial& rp, const float* g_eb, const float* gY, float* forces,
+                            double* virial, float* atom_vir) {
+  if (atom_vir)
+    MACE_LAUNCH(k_mace_edge_final<true>, E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial,
+                atom_vir);
+  else
+    MACE_LAUNCH(k_mace_edge_final<false>, E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial,
+                atom_vir);
+}
+
+}  // namespace b2m

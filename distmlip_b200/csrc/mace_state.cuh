@@ -1,0 +1,103 @@
+// mace_state.cuh -- kernels (kernels_mace.cu), weights and workspace of the MACE path (engine_mace.inl).
+// Layouts: node features h [n][C]; the l-resolved atom basis A [nsh][n_own][C] (lm-major, so that the rows of one l form
+// one contiguous [(2l+1) n_own][C] block for the per-l channel mixes); edge quantities [E][...].
+#pragma once
+#include <vector>
+
+#include "kernels.cuh"
+
+namespace b2m {
+
+constexpr int kMaceMaxLayers = 8;
+constexpr int kMaceMaxNsh = 16;  // max_ell <= 3
+
+struct MaceRadial {
+  int nb;       // Bessel functions in use
+  int nbp;      // row pitch of the basis buffers (64, padding columns zero)
+  int p;        // polynomial cutoff exponent
+  float r_max;
+  float pref;   // sqrt(2 / r_max)
+  float w[64];  // Bessel frequencies
+};
+
+// one term coef * A[i1] A[i2] A[i3] (first nu factors) of the symmetric contraction, weighted by w[z][kg][c]
+struct MaceTerm {
+  int idx;  // i1 | i2 << 8 | i3 << 16 | nu << 24
+  int kg;   // row of the element-channel weight table (all nu concatenated)
+  float coef;
+};
+
+void launch_mace_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const MaceRadial& rp, int nsh, float* Y,
+                           float* eb);
+void launch_mace_embed(cudaStream_t st, int n, int C, const int* type, const float* W, float* h0);
+void launch_mace_msg(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
+                     const float* Y, const float* u, float* A);
+void launch_mace_msg_bwd(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
+                         const float* Y, const float* u, const float* gA, float* gR, float* gY, float* gu);
+// out[lm][i][:] (+)= in[lm][i][:] @ W[type[i]][l(lm)]  (W [n_elem][L1][C][C]); nsh = 1 for a plain [n][C] row block
+void launch_mace_elem_mix(cudaStream_t st, int n, int C, int L1, int nsh, const int* type, const float* W,
+                          const float* in, float* out, bool accum);
+void launch_mace_symc(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A, const MaceTerm* terms,
+                      int nterms, const float* w, float* B);
+void launch_mace_symc_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                          const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA);
+// e_lin[i] += h[i] . w   (linear readouts; w carries 1 / sqrt(C))
+void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, const float* h, const float* w, float* e_lin);
+// eps_i = E0[z] + scale * (e_lin + act(h W1) . w2) + shift; pre [n][H] kept for the reverse; energy += sum eps
+// atom_e != nullptr: atom_e[gid[i]] = eps_i
+void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
+                               const float* e_lin, const int* type, const double* E0, double scale, double shift,
+                               float* pre, double* energy, const int* gid, double* atom_e);
+// gh[i][c] = scale * sum_j W1[c][j] w2[j] SiLU'(pre[i][j])
+void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const float* pre, const float* W1,
+                              const float* w2, float scale, float* gh);
+// gh[i][c] += scale * w[c]
+void launch_mace_add_row(cudaStream_t st, int n_own, int C, const float* w, float scale, float* gh);
+void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
+                            const int* gid, const MaceRadial& rp, const float* g_eb, const float* gY, float* forces,
+                            double* virial, float* atom_vir = nullptr);
+
+// A [K][N] weight (y = x W) as operands of the wgmma row GEMM (kernels_wg.cu): blocks of K x N = 64 x 128, 64 x 64 or
+// 128 x 64 in the order engine_mace.inl's tc_blocks visits them, each the canonical hi/lo image of its [N][K] view
+struct TcW {
+  int K = 0, N = 0;
+  std::vector<const float*> blk;
+};
+
+struct MaceLayerW {
+  bool residual = true;
+  TcW Wup, WupT;              // [C][C] / sqrt(C) and its transpose
+  std::vector<TcW> mlp, mlpT;  // radial MLP layers (scaled, c_act folded, padded to multiples of 64) and transposes
+  TcW Wlin[4], WlinT[4];       // per l [C][C] / (avg_num_neighbors sqrt(C))
+  const float *Wskip = nullptr, *WskipT = nullptr;  // [n_elem][L1 or 1][C][C] / sqrt(C n_elem)
+  TcW Wprod, WprodT;          // [C][C] / sqrt(C)
+  const float* wsym = nullptr;                              // [n_elem][Ktot][C]
+  const MaceTerm* terms = nullptr;
+  int nterms = 0, Ktot = 0;
+  const float* wread = nullptr;                             // linear readout [C] / sqrt(C) (all layers but the last)
+};
+
+struct MaceState {
+  // C: row pitch of every per-atom array, the model's channel count Cr rounded up to a multiple of 64 (the wgmma GEMM
+  // shapes); the padding channels carry zero weights and stay zero
+  int C = 128, Cr = 128, L1 = 4, nsh = 16, T = 2, correlation = 3, H = 16;
+  double c_act = 1.0, scale = 1.0, shift = 0.0;
+  MaceRadial rp{};
+  std::vector<int> hid;   // radial MLP hidden widths, padded to 64
+  int interaction_residual[kMaceMaxLayers] = {0};
+  double avg_nb[kMaceMaxLayers] = {0};
+  // weights
+  const float* Wemb = nullptr;  // [n_elem][C] / sqrt(n_elem)
+  std::vector<MaceLayerW> L;
+  const float *W1 = nullptr, *w2 = nullptr;  // non-linear readout: [C][H] / sqrt(C), [H] c_act / sqrt(H)
+  const double* E0 = nullptr;
+  DBuf<double> e0buf;
+  // workspace
+  DBuf<float> Y, eb, R, e_lin, pre_out, B, Am, sc;
+  std::vector<DBuf<float>> h, u, A, pre;  // h: T + 1, u / A: T, pre: radial MLP hidden layers
+  DBuf<float> act[2];
+  // reverse
+  DBuf<float> gY, g_eb, gR, gB, gA, gAm, gh, ghn, gu, gact[2];
+};
+
+}  // namespace b2m

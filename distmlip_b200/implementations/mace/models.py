@@ -1,0 +1,154 @@
+"""ScaleShiftMACE_Dist -- a mace `ScaleShiftMACE` with scalar hidden features on the sm_90a engine.
+
+`from_existing` takes any object with mace's attribute tree and `state_dict()` (mace itself need not be importable, so
+the model is recognised by structure, not by `isinstance`); `enable_distributed_mode(gpus)` validates the
+configuration and creates the engine (b2m_create_mace).  The arithmetic, with every e3nn / mace convention it relies on,
+is stated in oracle/mace_ref.py; the kernels are csrc/kernels_mace.cu.
+
+Supported configuration (anything else raises NotImplementedError in enable_distributed_mode): ScaleShiftMACE with one
+head, hidden_irreps = C x 0e (C a multiple of 32, C <= 128), max_ell <= 3, correlation <= 3, Bessel radial basis
+(num_bessel <= 64) times PolynomialCutoff, a FullyConnectedNet radial MLP (hidden widths <= 64),
+RealAgnosticResidualInteractionBlock or RealAgnosticInteractionBlock per layer, LinearReadoutBlock on every layer but the
+last and NonLinearReadoutBlock (gated SiLU) on the last; no pair repulsion, no distance transform.
+"""
+from __future__ import annotations
+
+import numpy as np
+import torch
+
+from distmlip_b200 import _lib
+from distmlip_b200.implementations.matgl.models._base import EngineBackedModel
+
+# e3nn normalize2mom(SiLU), 1 / sqrt(E[SiLU(z)^2]) for z ~ N(0, 1): used when the model does not carry its own constant
+SILU_2MOM = 1.6765324703310909
+
+_RESIDUAL = "RealAgnosticResidualInteractionBlock"
+_PLAIN = "RealAgnosticInteractionBlock"
+
+
+def _act_cst(module, default=SILU_2MOM):
+    act = getattr(module, "act", None) or getattr(module, "non_linearity", None)
+    cst = getattr(act, "cst", None)
+    return float(cst) if cst is not None else default
+
+
+class ScaleShiftMACE_Dist(EngineBackedModel):
+    """mace ScaleShiftMACE (H100 engine behind DistMLIP's wrapper API)."""
+
+    __version__ = 1
+
+    @classmethod
+    def from_existing(cls, model, dtype=torch.float32):
+        for name in ("atomic_numbers", "r_max", "interactions", "products", "readouts", "radial_embedding",
+                     "node_embedding", "scale_shift", "atomic_energies_fn"):
+            if not hasattr(model, name):
+                raise TypeError(f"not a mace ScaleShiftMACE: no attribute {name!r}")
+        return super().from_existing(model, dtype)
+
+    def heat_flux_reach(self):
+        raise NotImplementedError("the heat flux is not implemented for MACE")
+
+    def _describe(self):
+        """b2m_mace_desc fields of the model, or NotImplementedError naming the first unsupported option"""
+        sd = self._state_dict
+        heads = self._attr("heads", None)
+        if heads is not None and len(heads) > 1:
+            raise NotImplementedError(f"multi-head models are not supported (heads={list(heads)})")
+        if self._attr("pair_repulsion", False) or any(k.startswith("pair_repulsion_fn.") for k in sd):
+            raise NotImplementedError("pair_repulsion (ZBL) is not supported")
+        rad = self._attr("radial_embedding")
+        if getattr(rad, "distance_transform", None) is not None or any(".distance_transform." in k for k in sd):
+            raise NotImplementedError("radial distance_transform is not supported")
+        if any(k.startswith("radial_embedding.") and k.split(".")[1] not in ("bessel_fn", "cutoff_fn") for k in sd):
+            raise NotImplementedError("radial_type other than the Bessel basis is not supported")
+        if "radial_embedding.bessel_fn.bessel_weights" not in sd:
+            raise NotImplementedError("radial_type other than the Bessel basis is not supported")
+        if any("dipole" in k for k in sd):
+            raise NotImplementedError("dipole models are not supported")
+        z = [int(a) for a in torch.as_tensor(self._attr("atomic_numbers")).tolist()]
+        n_elem = len(z)
+        C = int(sd["node_embedding.linear.weight"].numel()) // n_elem
+        if C % 32 or C > 128:
+            raise NotImplementedError(f"hidden_irreps = {C}x0e: C must be a multiple of 32 and at most 128")
+        inters = list(self._attr("interactions"))
+        T = len(inters)
+        if T > 8:
+            raise NotImplementedError(f"num_interactions={T}: at most 8")
+        pc = "products.0.symmetric_contractions.contractions.0."
+        if "products.0.symmetric_contractions.contractions.1.weights_max" in sd:
+            raise NotImplementedError("hidden_irreps with l > 0 (equivariant hidden features) are not supported")
+        correlation = sum(1 for k in sd if k.startswith(pc + "U_matrix_"))
+        if not 1 <= correlation <= 3:
+            raise NotImplementedError(f"correlation={correlation}: 1..3 supported")
+        if sd[pc + "U_matrix_1"].dim() != 2:
+            raise NotImplementedError("hidden_irreps with l > 0 (equivariant hidden features) are not supported")
+        nsh = int(sd[pc + "U_matrix_1"].shape[0])
+        max_ell = int(round(nsh ** 0.5)) - 1
+        if (max_ell + 1) ** 2 != nsh or max_ell > 3:
+            raise NotImplementedError(f"edge spherical harmonics with {nsh} components: max_ell <= 3 supported")
+        residual = 0
+        avg = [0.0] * 8
+        for t, it in enumerate(inters):
+            name = type(it).__name__
+            if name == _RESIDUAL:
+                residual |= 1 << t
+            elif name != _PLAIN:
+                raise NotImplementedError(f"interactions.{t} is a {name}: only {_RESIDUAL} and {_PLAIN} are supported")
+            avg[t] = float(getattr(it, "avg_num_neighbors"))
+            hs = [int(sd[k].shape[1]) for k in sorted(
+                (k for k in sd if k.startswith(f"interactions.{t}.conv_tp_weights.layer")),
+                key=lambda k: int(k.split(".")[3][5:]))]
+            if any(h > 64 for h in hs[:-1]):
+                raise NotImplementedError(f"radial MLP hidden widths {hs[:-1]}: at most 64")
+        readouts = list(self._attr("readouts"))
+        for t, ro in enumerate(readouts):
+            want = "NonLinearReadoutBlock" if t == T - 1 else "LinearReadoutBlock"
+            if type(ro).__name__ != want:
+                raise NotImplementedError(f"readouts.{t} is a {type(ro).__name__}: {want} expected")
+        if f"readouts.{T - 1}.linear_2.weight" not in sd:
+            raise NotImplementedError("the last readout must be a NonLinearReadoutBlock")
+        H = int(sd[f"readouts.{T - 1}.linear_2.weight"].numel())
+        first_mlp = getattr(inters[0], "conv_tp_weights", None)
+        c_act = _act_cst(getattr(first_mlp, "layer0", None)) if first_mlp is not None else SILU_2MOM
+        return _lib.MaceDesc(
+            n_elem=n_elem, channels=C, max_ell=max_ell, correlation=correlation, num_interactions=T,
+            num_bessel=int(sd["radial_embedding.bessel_fn.bessel_weights"].numel()),
+            num_polynomial_cutoff=int(round(float(sd["radial_embedding.cutoff_fn.p"]))),
+            mlp_hidden=H, residual_mask=residual, reserved=0, r_max=float(sd["r_max"]), c_act=c_act,
+            avg_num_neighbors=(_lib.C.c_double * 8)(*avg))
+
+    def enable_distributed_mode(self, gpus):
+        """mace.py / models.py of the reference: `gpus` are CUDA ordinals, one per partition (a single-process group
+        when one process gets several, one rank per GPU under torchrun, a replica for a single GPU)."""
+        desc = self._describe()
+        gpus, rank, world, group = self._process_layout(gpus)
+        from distmlip_b200.structures import Z_OF
+
+        sym_of = {z: s for s, z in Z_OF.items()}
+        self.__dict__["element_types"] = tuple(sym_of[int(z)] for z in torch.as_tensor(self._attr("atomic_numbers")).tolist())
+        self.__dict__["_e0"] = self._state_dict["atomic_energies_fn.atomic_energies"].double().numpy().reshape(-1)
+        eng = _lib.Engine(n_elem=desc.n_elem, n_blocks=desc.num_interactions, cutoff=desc.r_max, mace=desc,
+                          device=[int(g) for g in gpus] if group else int(gpus[rank]))
+        self._attach_engine(eng, gpus, rank, world, group)
+        eng.finalize()
+        self._engine_finalized = True
+
+    def evaluate(self, atoms, forces=True, stress=True, atomic=False):
+        """One evaluation on the engine: (energy, forces [n, 3] eV/A, stress [3, 3] GPa, per-atom energies or None,
+        per-atom virials [n, 3, 3] eV or None)."""
+        if not self.__dict__.get("dist_enabled"):
+            raise RuntimeError("call enable_distributed_mode(gpus) first")
+        eng = self._engine
+        if bool(atomic) != self.__dict__.get("_atomic_on", False):
+            eng.set_atomic(bool(atomic))
+            self._atomic_on = bool(atomic)
+        eng.set_structure(np.asarray(atoms.get_positions(wrap=False), dtype=np.float64), np.array(atoms.get_cell()),
+                          self._species_of(atoms), np.asarray(atoms.get_pbc(), dtype=np.int32))
+        e, f, s = eng.compute(forces=forces, stress=stress)
+        ae = av = None
+        if atomic:
+            ae, av = eng.atomic(virials=forces or stress)
+        return e, f, s, ae, av
+
+    def dist_forward(self, *args, **kwargs):
+        raise NotImplementedError("dist_forward over torch graphs does not exist here; use MACECalculator_Dist")

@@ -97,6 +97,31 @@ typedef struct {
 } b2m_tensornet_desc;
 int b2m_create_tensornet(const b2m_tensornet_desc* desc, const int* devices, int ndev, b2m_handle* out);
 
+/* MACE (DESIGN.md §11): the same handle type and calls, for a mace ScaleShiftMACE with scalar hidden features
+ * (hidden_irreps = C x 0e), loaded key by key from its state_dict (arithmetic and conventions: oracle/mace_ref.py).
+ * Supported: one head, C a multiple of 32 with C <= 128, max_ell <= 3, correlation <= 3, Bessel basis x polynomial cutoff,
+ * an e3nn FullyConnectedNet radial MLP (hidden widths <= 64), RealAgnostic(Residual)InteractionBlock per layer, linear
+ * readouts and a gated non-linear last readout.  Edges are every periodic image closer than r_max (no bond graph).
+ * Scale, shift and the atomic energies E0 come from the state_dict: b2m_set_scaling and b2m_set_element_refs return
+ * B2M_ERR_INVALID on such a handle, as do b2m_get_sitewise and b2m_set_heat_flux.  b2m_set_atomic / b2m_get_atomic give
+ * energies[i] = E0[z_i] + scale * e_i + shift and the per-atom virials. */
+typedef struct {
+  int32_t n_elem;                 /* len(atomic_numbers)                                                 */
+  int32_t channels;               /* C of hidden_irreps = C x 0e                                         */
+  int32_t max_ell;                /* edge spherical harmonics 0..max_ell                                 */
+  int32_t correlation;            /* symmetric-contraction order                                         */
+  int32_t num_interactions;       /* <= 8                                                                */
+  int32_t num_bessel;             /* radial Bessel functions                                             */
+  int32_t num_polynomial_cutoff;  /* PolynomialCutoff exponent p                                         */
+  int32_t mlp_hidden;             /* width of the non-linear readout                                     */
+  int32_t residual_mask;          /* bit t: interactions.t is a RealAgnosticResidualInteractionBlock     */
+  int32_t reserved;
+  double r_max;                   /* cutoff (Angstrom)                                                   */
+  double c_act;                   /* e3nn normalize2mom(SiLU) constant of the radial MLP and the readout */
+  double avg_num_neighbors[8];    /* per interaction                                                     */
+} b2m_mace_desc;
+int b2m_create_mace(const b2m_mace_desc* desc, const int* devices, int ndev, b2m_handle* out);
+
 /* One call per state_dict key of the matgl CHGNet attribute tree (SURVEY.md 8c), fp32 row-major. */
 int b2m_load_weights(b2m_handle h, const char* name, const float* host_ptr, const int64_t* shape, int ndim);
 /* Optional per-element energy offsets (Potential.element_refs), length n_elem. */
