@@ -43,7 +43,7 @@ class MaceDesc(C.Structure):
     _fields_ = [
         ("n_elem", C.c_int32), ("channels", C.c_int32), ("max_ell", C.c_int32), ("correlation", C.c_int32),
         ("num_interactions", C.c_int32), ("num_bessel", C.c_int32), ("num_polynomial_cutoff", C.c_int32),
-        ("mlp_hidden", C.c_int32), ("residual_mask", C.c_int32), ("reserved", C.c_int32),
+        ("mlp_hidden", C.c_int32), ("residual_mask", C.c_int32), ("hidden_max_l", C.c_int32),
         ("r_max", C.c_double), ("c_act", C.c_double), ("avg_num_neighbors", C.c_double * 8),
     ]
 

@@ -21,6 +21,7 @@
 #include <vector>
 
 #include <algorithm>
+#include <array>
 
 #include "atomic_virial.cuh"
 #include "graph.cuh"
@@ -554,13 +555,13 @@ static void alloc_workspace(b2m_engine* e) {
 // rows (forward) or copies its halo adjoints into the owner's receive buffer (backward); a CUDA event per exchange point
 // orders the receiver's stream behind the sender's.
 // kind 0: atom rows x[l] | 1: bond rows h[l] | 2: TensorNet atom tensors X[l] (10 x 64 floats per atom)
-//      3: MACE node features h[l] (C floats per atom)
+//      3: MACE node features h[l] (C floats per atom, 4 C for 0e+1o features)
 static float* halo_buffer(b2m_engine* e, int kind, int l) {
   if (kind == 3) return e->mace->h[l].p;
   return kind == 1 ? e->h[l].p : (kind == 2 ? e->tn->X[l].p : e->x[l].p);
 }
-static int halo_width(const b2m_engine* e, int kind) {
-  if (kind == 3) return e->mace->C;
+static int halo_width(const b2m_engine* e, int kind, int l) {
+  if (kind == 3) return e->mace->hw[l];
   return kind == 2 ? 10 * D : D;
 }
 
@@ -579,7 +580,7 @@ static void halo_forward_begin(b2m_engine* e, int kind, int l) {
   if (e->world <= 1 || e->debug_no_halo) return;
   Graph& g = e->g;
   const bool bonds = kind == 1;
-  const size_t W = (size_t)halo_width(e, kind);
+  const size_t W = (size_t)halo_width(e, kind, l);
   float* buf = halo_buffer(e, kind, l);
   const int* nto = bonds ? g.nb_to : g.n_to;
   const int* toff = bonds ? g.bto_off : g.to_off;
@@ -1317,7 +1318,11 @@ static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdes
     B2M_REQUIRE(ndev >= 1 && ndev <= MAXP, B2M_ERR_PARTITIONS, "ndev must be in [1,16]");
     if (mdesc) {
       B2M_REQUIRE(mdesc->channels >= 32 && mdesc->channels <= 128 && mdesc->channels % 32 == 0, B2M_ERR_INVALID,
-                  "MACE engine supports hidden_irreps = C x 0e with C a multiple of 32, C <= 128");
+                  "MACE engine supports hidden_irreps = C x 0e (+ C x 1o) with C a multiple of 32, C <= 128");
+      B2M_REQUIRE(mdesc->hidden_max_l == 0 || mdesc->hidden_max_l == 1, B2M_ERR_INVALID,
+                  "MACE engine supports hidden_max_l 0 (C x 0e) or 1 (C x 0e + C x 1o)");
+      B2M_REQUIRE(mdesc->hidden_max_l == 0 || mdesc->max_ell >= 1, B2M_ERR_INVALID,
+                  "0e+1o hidden features need max_ell >= 1");
       B2M_REQUIRE(mdesc->max_ell >= 0 && mdesc->max_ell <= 3, B2M_ERR_INVALID, "MACE engine supports max_ell <= 3");
       B2M_REQUIRE(mdesc->correlation >= 1 && mdesc->correlation <= 3, B2M_ERR_INVALID, "MACE engine supports correlation <= 3");
       B2M_REQUIRE(mdesc->num_interactions >= 1 && mdesc->num_interactions <= kMaceMaxLayers, B2M_ERR_INVALID,
@@ -1355,6 +1360,9 @@ static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdes
         M.Cr = mdesc->channels, M.C = (mdesc->channels + 63) / 64 * 64;
         M.L1 = mdesc->max_ell + 1, M.nsh = M.L1 * M.L1, M.T = mdesc->num_interactions;
         M.correlation = mdesc->correlation, M.H = mdesc->mlp_hidden, M.c_act = mdesc->c_act;
+        M.hidden_max_l = mdesc->hidden_max_l;
+        M.hw.assign(M.T + 1, M.C);  // h[t] of 0 < t < T carries 0e+1o when hidden_max_l = 1
+        for (int t = 1; t < M.T; t++) M.hw[t] = M.hidden_max_l ? 4 * M.C : M.C;
         M.rp.nb = mdesc->num_bessel, M.rp.nbp = 64, M.rp.p = mdesc->num_polynomial_cutoff;
         M.rp.r_max = (float)mdesc->r_max, M.rp.pref = (float)std::sqrt(2.0 / mdesc->r_max);
         for (int t = 0; t < M.T; t++)
@@ -1464,7 +1472,8 @@ const char* b2m_last_error(b2m_handle h) { return h ? h->err.c_str() : g_create_
 
 int b2m_load_weights(b2m_handle h, const char* name, const float* host_ptr, const int64_t* shape, int ndim) {
   API_BEGIN
-  B2M_REQUIRE(name && host_ptr && shape && ndim >= 1 && ndim <= 4, B2M_ERR_INVALID, "bad weight arguments");
+  // up to 5 dimensions: the 1o symmetric-contraction tensor U_matrix_3 of MACE is [3, nsh, nsh, nsh, K]
+  B2M_REQUIRE(name && host_ptr && shape && ndim >= 1 && ndim <= 5, B2M_ERR_INVALID, "bad weight arguments");
   size_t n = 1;
   std::vector<int64_t> sh(shape, shape + ndim);
   for (auto s : sh) n *= (size_t)s;

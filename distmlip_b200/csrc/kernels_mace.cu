@@ -1,5 +1,6 @@
-// kernels_mace.cu -- MACE with scalar hidden features (hidden_irreps = C x 0e) on the same partitioned CSR graph as the
-// CHGNet and TensorNet paths.  Arithmetic as oracle/mace_ref.py states it (the conventions are written down there once);
+// kernels_mace.cu -- MACE with hidden features C x 0e or C x 0e + C x 1o on the same partitioned CSR graph as the
+// CHGNet and TensorNet paths.  Arithmetic as oracle/mace_ref.py and, for 0e+1o features, tests/mace_eq_ref.py state it
+// (the conventions are written down there once);
 // engine_mace.inl runs these kernels stage by stage.
 //
 // First generation: the node- and edge-level products (radial MLP, linear_up, the per-l mixes, the product linear) run
@@ -8,6 +9,7 @@
 // walks the nonzero terms of U, which every channel shares.  Aggregations walk the CSR-by-destination rows (no atomics
 // in the forward); the reverse scatters to sources with atomics.
 #include "atomic_virial.cuh"
+#include "mace_cg.cuh"
 #include "mace_state.cuh"
 
 namespace b2m {
@@ -246,14 +248,203 @@ __global__ void __launch_bounds__(128) k_mace_symc(int n_own, int C, int nsh, in
 }
 
 // ============================================================================================
+// 0e+1o node features (layers t >= 1 of a model with hidden_irreps C x 0e + C x 1o)
+// ============================================================================================
+// the coupling list of one max_ell (mace_cg.cuh), expanded with X
+#define MACE_CG_EXPAND(L, X) \
+  if constexpr ((L) == 1) { MACE_CG_1(X) } else if constexpr ((L) == 2) { MACE_CG_2(X) } else { MACE_CG_3(X) }
+
+// Am[slot(l_out, m, j)] = sum_{e -> t} R[e][p] sum CG u[src][l_in m1] Y[e][l_sh m2] over the paths p of conv_paths,
+// one thread per (atom, channel) with the 4 + npaths + nsh operands of an edge in registers; no atomics
+template <int kL>
+__global__ void __launch_bounds__(256) k_mace_msg_eq(int n_own, int C, const int* __restrict__ row_ptr,
+                                                     const int* __restrict__ e_src, const float* __restrict__ R,
+                                                     const float* __restrict__ Y, const float* __restrict__ u,
+                                                     float* __restrict__ Am) {
+  constexpr int NP = mace_npaths(kL), NS = mace_nslots(kL), NSH = (kL + 1) * (kL + 1);
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;
+  const int t = (int)(i / C), c = (int)(i % C);
+  float acc[NS];
+#pragma unroll
+  for (int k = 0; k < NS; k++) acc[k] = 0.f;
+  for (int e = row_ptr[t]; e < row_ptr[t + 1]; e++) {
+    const float* us = u + (size_t)e_src[e] * 4 * C + c;
+    const float uu[4] = {us[0], us[C], us[2 * C], us[3 * C]};
+    const float* re = R + (size_t)e * NP * C + c;
+    float r[NP];
+#pragma unroll
+    for (int p = 0; p < NP; p++) r[p] = re[p * C];
+    const float* ye = Y + (size_t)e * kMaceMaxNsh;
+    float y[NSH];
+#pragma unroll
+    for (int k = 0; k < NSH; k++) y[k] = ye[k];
+#define MACE_X(p, iu, iy, s, cf) acc[s] = fmaf((cf) * r[p], uu[iu] * y[iy], acc[s]);
+    MACE_CG_EXPAND(kL, MACE_X)
+#undef MACE_X
+  }
+  int s = 0;
+#pragma unroll
+  for (int l = 0; l <= kL; l++) {
+    const int np = mace_np_l(kL, l);
+    float* blk = Am + (size_t)mace_slot_base(kL, l) * n_own * C;
+#pragma unroll
+    for (int m = 0; m < 2 * l + 1; m++)
+#pragma unroll
+      for (int j = 0; j < np; j++) blk[(((size_t)m * n_own + t) * np + j) * C + c] = acc[s++];
+  }
+}
+
+// reverse of k_mace_msg_eq: gR over R in place (the thread of (dst, c) is the only reader and writer of R[e][.][c] for
+// its edges), gY[e][k] += the warp's 32 channels (one atomic per warp), gu[src][4][c] += (atomics)
+template <int kL>
+__global__ void __launch_bounds__(256) k_mace_msg_eq_bwd(int n_own, int C, const int* __restrict__ row_ptr,
+                                                         const int* __restrict__ e_src, float* __restrict__ R,
+                                                         const float* __restrict__ Y, const float* __restrict__ u,
+                                                         const float* __restrict__ gAm, float* __restrict__ gY,
+                                                         float* __restrict__ gu) {
+  constexpr int NP = mace_npaths(kL), NS = mace_nslots(kL), NSH = (kL + 1) * (kL + 1);
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;  // n_own * C is a multiple of 32: whole warps leave together
+  const int t = (int)(i / C), c = (int)(i % C), lane = threadIdx.x & 31;
+  float ga[NS];
+  {
+    int s = 0;
+#pragma unroll
+    for (int l = 0; l <= kL; l++) {
+      const int np = mace_np_l(kL, l);
+      const float* blk = gAm + (size_t)mace_slot_base(kL, l) * n_own * C;
+#pragma unroll
+      for (int m = 0; m < 2 * l + 1; m++)
+#pragma unroll
+        for (int j = 0; j < np; j++) ga[s++] = blk[(((size_t)m * n_own + t) * np + j) * C + c];
+    }
+  }
+  for (int e = row_ptr[t]; e < row_ptr[t + 1]; e++) {
+    const int src = e_src[e];
+    const float* us = u + (size_t)src * 4 * C + c;
+    const float uu[4] = {us[0], us[C], us[2 * C], us[3 * C]};
+    float* re = R + (size_t)e * NP * C + c;
+    float r[NP], gr[NP];
+#pragma unroll
+    for (int p = 0; p < NP; p++) r[p] = re[p * C], gr[p] = 0.f;
+    const float* ye = Y + (size_t)e * kMaceMaxNsh;
+    float y[NSH], gy[NSH];
+#pragma unroll
+    for (int k = 0; k < NSH; k++) y[k] = ye[k], gy[k] = 0.f;
+    float g4[4] = {0.f, 0.f, 0.f, 0.f};
+#define MACE_X(p, iu, iy, s, cf)                  \
+  {                                               \
+    const float g = (cf) * ga[s];                 \
+    gr[p] = fmaf(g, uu[iu] * y[iy], gr[p]);       \
+    const float gq = g * r[p];                    \
+    g4[iu] = fmaf(gq, y[iy], g4[iu]);             \
+    gy[iy] = fmaf(gq, uu[iu], gy[iy]);            \
+  }
+    MACE_CG_EXPAND(kL, MACE_X)
+#undef MACE_X
+#pragma unroll
+    for (int p = 0; p < NP; p++) re[p * C] = gr[p];
+#pragma unroll
+    for (int k = 1; k < NSH; k++) {  // Y[0] = 1 carries no gradient
+      float v = gy[k];
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) atomicAdd(&gY[(size_t)e * kMaceMaxNsh + k], v);
+    }
+    float* gs = gu + (size_t)src * 4 * C + c;
+#pragma unroll
+    for (int k = 0; k < 4; k++) atomicAdd(gs + k * C, g4[k]);
+  }
+}
+
+// out[i][m][:] (+)= in[i][m][:] @ W[type[i]][l(m)], m < ncomp (1 or 4), rows of pitch ldi / ldo: one block of C threads
+// per row, each weight element read once per row and applied to the components of its l
+__global__ void k_mace_elem_mix_rows(int n, int C, int ncomp, int ldi, int ldo, const int* __restrict__ type,
+                                     const float* __restrict__ W, const float* __restrict__ in, float* __restrict__ out,
+                                     int accum) {
+  __shared__ float x[4][128];
+  const int i = blockIdx.x, c2 = threadIdx.x;
+  const int z = type[i], Lw = ncomp == 4 ? 2 : 1;
+  for (int m = 0; m < ncomp; m++) x[m][c2] = in[(size_t)i * ldi + m * C + c2];
+  __syncthreads();
+  const float* W0 = W + (size_t)z * Lw * C * C + c2;
+  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+  if (ncomp == 4) {
+    const float* W1 = W0 + (size_t)C * C;
+    for (int c = 0; c < C; c++) {
+      const float w0 = W0[(size_t)c * C], w1 = W1[(size_t)c * C];
+      a0 = fmaf(w0, x[0][c], a0), a1 = fmaf(w1, x[1][c], a1), a2 = fmaf(w1, x[2][c], a2), a3 = fmaf(w1, x[3][c], a3);
+    }
+  } else {
+    for (int c = 0; c < C; c++) a0 = fmaf(W0[(size_t)c * C], x[0][c], a0);
+  }
+  const float a[4] = {a0, a1, a2, a3};
+  for (int m = 0; m < ncomp; m++) {
+    float* o = out + (size_t)i * ldo + m * C + c2;
+    *o = accum ? *o + a[m] : a[m];
+  }
+}
+
+// symmetric contraction with a 1o output: as k_mace_symc, with the term's output slot o (MaceTerm) selecting one of four
+// accumulators (forward) or upstream adjoints (reverse); B / gB [4][n_own][C]
+template <bool kBwd>
+__global__ void __launch_bounds__(128) k_mace_symc_eq(int n_own, int C, int nsh, int Ktot, const int* __restrict__ type,
+                                                      const float* __restrict__ A, const MaceTerm* __restrict__ terms,
+                                                      int nterms, const float* __restrict__ w,
+                                                      const float* __restrict__ gB, float* __restrict__ out) {
+  __shared__ float a[kMaceMaxNsh][128];
+  __shared__ float ga[kBwd ? kMaceMaxNsh : 1][128];
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;
+  const int tid = threadIdx.x, t = (int)(i / C), c = (int)(i % C);
+  const size_t plane = (size_t)n_own * C;
+#pragma unroll
+  for (int k = 0; k < kMaceMaxNsh; k++) {
+    a[k][tid] = k < nsh ? A[k * plane + i] : 0.f;
+    if constexpr (kBwd) ga[k][tid] = 0.f;
+  }
+  const float* wz = w + (size_t)type[t] * Ktot * C + c;
+  float g[4] = {0.f, 0.f, 0.f, 0.f};
+  if constexpr (kBwd) {
+#pragma unroll
+    for (int o = 0; o < 4; o++) g[o] = gB[o * plane + i];
+  }
+  float acc[4] = {0.f, 0.f, 0.f, 0.f};
+  for (int j = 0; j < nterms; j++) {
+    const MaceTerm tm = terms[j];
+    const int nu = (tm.idx >> 24) & 3, o = (tm.idx >> 28) & 3;
+    const int i1 = tm.idx & 255, i2 = (tm.idx >> 8) & 255, i3 = (tm.idx >> 16) & 255;
+    const float cw = tm.coef * wz[(size_t)tm.kg * C];
+    const float a1 = a[i1][tid], a2 = nu >= 2 ? a[i2][tid] : 1.f, a3 = nu >= 3 ? a[i3][tid] : 1.f;
+    if constexpr (!kBwd) {
+      const float v = cw * (a1 * a2 * a3);  // the same o for the whole warp: the selects do not diverge
+      acc[0] += o == 0 ? v : 0.f, acc[1] += o == 1 ? v : 0.f, acc[2] += o == 2 ? v : 0.f, acc[3] += o == 3 ? v : 0.f;
+    } else {
+      const float s = cw * (o == 0 ? g[0] : o == 1 ? g[1] : o == 2 ? g[2] : g[3]);
+      ga[i1][tid] += s * a2 * a3;
+      if (nu >= 2) ga[i2][tid] += s * a1 * a3;
+      if (nu >= 3) ga[i3][tid] += s * a1 * a2;
+    }
+  }
+  if constexpr (!kBwd) {
+#pragma unroll
+    for (int o = 0; o < 4; o++) out[o * plane + i] = acc[o];
+  } else {
+#pragma unroll
+    for (int k = 0; k < kMaceMaxNsh; k++)
+      if (k < nsh) out[k * plane + i] = ga[k][tid];
+  }
+}
+
+// ============================================================================================
 // readouts
 // ============================================================================================
-__global__ void k_mace_readout_lin(int n_own, int C, const float* __restrict__ h, const float* __restrict__ w,
+__global__ void k_mace_readout_lin(int n_own, int C, int ld, const float* __restrict__ h, const float* __restrict__ w,
                                    float* __restrict__ e_lin) {
   const int r = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (r >= n_own) return;
   float s = 0.f;
-  for (int c = lane; c < C; c += 32) s = fmaf(h[(size_t)r * C + c], w[c], s);
+  for (int c = lane; c < C; c += 32) s = fmaf(h[(size_t)r * ld + c], w[c], s);
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) e_lin[r] += s;
 }
@@ -291,10 +482,11 @@ __global__ void k_mace_readout_seed(int n_own, int C, int H, const float* __rest
   gh[i] = scale * s;
 }
 
-__global__ void k_mace_add_row(int n_own, int C, const float* __restrict__ w, float scale, float* __restrict__ gh) {
+__global__ void k_mace_add_row(int n_own, int C, int ld, const float* __restrict__ w, float scale,
+                               float* __restrict__ gh) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= (int64_t)n_own * C) return;
-  gh[i] += scale * w[i % C];
+  gh[(i / C) * ld + i % C] += scale * w[i % C];
 }
 
 // ============================================================================================
@@ -407,8 +599,8 @@ void launch_mace_symc_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, 
                           const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA) {
   MACE_LAUNCH(k_mace_symc<true>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, gB, gA);
 }
-void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, const float* h, const float* w, float* e_lin) {
-  MACE_LAUNCH(k_mace_readout_lin, (int64_t)n_own * 32, 256, st, n_own, C, h, w, e_lin);
+void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, int ld, const float* h, const float* w, float* e_lin) {
+  MACE_LAUNCH(k_mace_readout_lin, (int64_t)n_own * 32, 256, st, n_own, C, ld, h, w, e_lin);
 }
 void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
                                const float* e_lin, const int* type, const double* E0, double scale, double shift,
@@ -424,8 +616,42 @@ void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const fl
                               const float* w2, float scale, float* gh) {
   MACE_LAUNCH(k_mace_readout_seed, (int64_t)n_own * C, 256, st, n_own, C, H, pre, W1, w2, scale, gh);
 }
-void launch_mace_add_row(cudaStream_t st, int n_own, int C, const float* w, float scale, float* gh) {
-  MACE_LAUNCH(k_mace_add_row, (int64_t)n_own * C, 256, st, n_own, C, w, scale, gh);
+void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh) {
+  MACE_LAUNCH(k_mace_add_row, (int64_t)n_own * C, 256, st, n_own, C, ld, w, scale, gh);
+}
+void launch_mace_msg_eq(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
+                        const float* R, const float* Y, const float* u, float* Am) {
+  if (max_ell == 1) MACE_LAUNCH(k_mace_msg_eq<1>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, Am);
+  else if (max_ell == 2) MACE_LAUNCH(k_mace_msg_eq<2>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, Am);
+  else if (max_ell == 3) MACE_LAUNCH(k_mace_msg_eq<3>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, Am);
+  else throw Error(B2M_ERR_INVALID, "mace message with 0e+1o features: max_ell must be 1..3");
+}
+void launch_mace_msg_eq_bwd(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
+                            float* R, const float* Y, const float* u, const float* gAm, float* gY, float* gu) {
+  if (max_ell == 1)
+    MACE_LAUNCH(k_mace_msg_eq_bwd<1>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
+  else if (max_ell == 2)
+    MACE_LAUNCH(k_mace_msg_eq_bwd<2>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
+  else if (max_ell == 3)
+    MACE_LAUNCH(k_mace_msg_eq_bwd<3>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
+  else throw Error(B2M_ERR_INVALID, "mace message with 0e+1o features: max_ell must be 1..3");
+}
+void launch_mace_elem_mix_rows(cudaStream_t st, int n, int C, int ncomp, int ldi, int ldo, const int* type,
+                               const float* W, const float* in, float* out, bool accum) {
+  if (n <= 0) return;
+  B2M_REQUIRE(C <= 128 && (ncomp == 1 || ncomp == 4), B2M_ERR_INVALID, "mace elem mix: C <= 128, 1 or 4 components");
+  k_mace_elem_mix_rows<<<n, C, 0, st>>>(n, C, ncomp, ldi, ldo, type, W, in, out, accum ? 1 : 0);
+  B2M_CK(cudaGetLastError());
+  g_launch_count++;
+}
+void launch_mace_symc_eq(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                         const MaceTerm* terms, int nterms, const float* w, float* B) {
+  MACE_LAUNCH(k_mace_symc_eq<false>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, nullptr,
+              B);
+}
+void launch_mace_symc_eq_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                             const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA) {
+  MACE_LAUNCH(k_mace_symc_eq<true>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, gB, gA);
 }
 void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
                             const int* gid, const MaceRadial& rp, const float* g_eb, const float* gY, float* forces,

@@ -1,6 +1,7 @@
 // mace_state.cuh -- kernels (kernels_mace.cu), weights and workspace of the MACE path (engine_mace.inl).
-// Layouts: node features h [n][C]; the l-resolved atom basis A [nsh][n_own][C] (lm-major, so that the rows of one l form
-// one contiguous [(2l+1) n_own][C] block for the per-l channel mixes); edge quantities [E][...].
+// Layouts: node features h [n][C], or [n][4][C] (0e, then 1o m = 0..2) for 0e+1o layers, so that a halo row is one
+// contiguous span; the l-resolved atom basis A [nsh][n_own][C] (lm-major, so that the rows of one l form one contiguous
+// [(2l+1) n_own][C] block for the per-l channel mixes); edge quantities [E][...].
 #pragma once
 #include <vector>
 
@@ -20,12 +21,24 @@ struct MaceRadial {
   float w[64];  // Bessel frequencies
 };
 
-// one term coef * A[i1] A[i2] A[i3] (first nu factors) of the symmetric contraction, weighted by w[z][kg][c]
+// one term coef * A[i1] A[i2] A[i3] (first nu factors) of the symmetric contraction, weighted by w[z][kg][c], added to
+// output slot o (0: the 0e output; 1 + m: component m of the 1o output; always 0 on layers with scalar output)
 struct MaceTerm {
-  int idx;  // i1 | i2 << 8 | i3 << 16 | nu << 24
+  int idx;  // i1 | i2 << 8 | i3 << 16 | nu << 24 | o << 28
   int kg;   // row of the element-channel weight table (all nu concatenated)
   float coef;
 };
+
+// conv_tp with 0e+1o node features (tests/mace_eq_ref.py conv_paths): paths per output l, all paths, and the message
+// accumulators, ordered (l_out, m_out, j) with j the path's place among those of its l_out.  The message buffer Am of a
+// 0e+1o layer holds, per l_out, a [(2 l_out + 1)][n_own][np(l_out) C] block (slot_base(l_out) n_own C floats in)
+__host__ __device__ constexpr int mace_np_l(int max_ell, int l) { return l == 0 ? 2 : (l < max_ell ? 3 : 2); }
+__host__ __device__ constexpr int mace_slot_base(int max_ell, int l) {
+  return l == 0 ? 0 : mace_slot_base(max_ell, l - 1) + (2 * l - 1) * mace_np_l(max_ell, l - 1);
+}
+__host__ __device__ constexpr int mace_npaths(int max_ell) { return 3 * max_ell + 1; }
+__host__ __device__ constexpr int mace_nslots(int max_ell) { return mace_slot_base(max_ell, max_ell + 1); }
+constexpr int kMaceMaxSlots = mace_nslots(3);  // 40
 
 void launch_mace_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const MaceRadial& rp, int nsh, float* Y,
                            float* eb);
@@ -34,6 +47,21 @@ void launch_mace_msg(cudaStream_t st, int n_own, int C, int L1, const int* row_p
                      const float* Y, const float* u, float* A);
 void launch_mace_msg_bwd(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
                          const float* Y, const float* u, const float* gA, float* gR, float* gY, float* gu);
+// 0e+1o node features: Am (layout above) from u [n][4][C], R [E][npaths C], Y
+void launch_mace_msg_eq(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
+                        const float* R, const float* Y, const float* u, float* Am);
+// its reverse: R is overwritten with gR (each (atom, channel) thread owns its edges' entries); gY, gu [n][4][C] accumulate
+void launch_mace_msg_eq_bwd(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
+                            float* R, const float* Y, const float* u, const float* gAm, float* gY, float* gu);
+// out[i][m][:] (+)= in[i][m][:] @ W[type[i]][l(m)] for the first ncomp (1 or 4) components of rows of pitch ldi / ldo
+// (the node-feature layout; W [n_elem][1 or 2][C][C])
+void launch_mace_elem_mix_rows(cudaStream_t st, int n, int C, int ncomp, int ldi, int ldo, const int* type,
+                               const float* W, const float* in, float* out, bool accum);
+// symmetric contraction with a 1o output: B [4][n_own][C] (slot 0: 0e, 1..3: 1o) and its reverse (gB in the same layout)
+void launch_mace_symc_eq(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                         const MaceTerm* terms, int nterms, const float* w, float* B);
+void launch_mace_symc_eq_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                             const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA);
 // out[lm][i][:] (+)= in[lm][i][:] @ W[type[i]][l(lm)]  (W [n_elem][L1][C][C]); nsh = 1 for a plain [n][C] row block
 void launch_mace_elem_mix(cudaStream_t st, int n, int C, int L1, int nsh, const int* type, const float* W,
                           const float* in, float* out, bool accum);
@@ -41,8 +69,8 @@ void launch_mace_symc(cudaStream_t st, int n_own, int C, int nsh, int Ktot, cons
                       int nterms, const float* w, float* B);
 void launch_mace_symc_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
                           const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA);
-// e_lin[i] += h[i] . w   (linear readouts; w carries 1 / sqrt(C))
-void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, const float* h, const float* w, float* e_lin);
+// e_lin[i] += h[i][0:C] . w   (linear readouts; w carries 1 / sqrt(C); rows of pitch ld)
+void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, int ld, const float* h, const float* w, float* e_lin);
 // eps_i = E0[z] + scale * (e_lin + act(h W1) . w2) + shift; pre [n][H] kept for the reverse; energy += sum eps
 // atom_e != nullptr: atom_e[gid[i]] = eps_i
 void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
@@ -51,8 +79,8 @@ void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const f
 // gh[i][c] = scale * sum_j W1[c][j] w2[j] SiLU'(pre[i][j])
 void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const float* pre, const float* W1,
                               const float* w2, float scale, float* gh);
-// gh[i][c] += scale * w[c]
-void launch_mace_add_row(cudaStream_t st, int n_own, int C, const float* w, float scale, float* gh);
+// gh[i][c] += scale * w[c]  (c < C, rows of pitch ld)
+void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh);
 void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
                             const int* gid, const MaceRadial& rp, const float* g_eb, const float* gY, float* forces,
                             double* virial, float* atom_vir = nullptr);
@@ -66,12 +94,16 @@ struct TcW {
 
 struct MaceLayerW {
   bool residual = true;
+  int Lin = 0, Lout = 0;      // node features 0e (0) or 0e+1o (1) in and out
+  int NP = 0;                 // conv_tp paths (max_ell + 1 for 0e input)
   TcW Wup, WupT;              // [C][C] / sqrt(C) and its transpose
+  TcW Wup1, Wup1T, Wprod1, Wprod1T;  // the 1o blocks of linear_up (Lin) and of the product linear (Lout)
   std::vector<TcW> mlp, mlpT;  // radial MLP layers (scaled, c_act folded, padded to multiples of 64) and transposes
-  TcW Wlin[4], WlinT[4];       // per l [C][C] / (avg_num_neighbors sqrt(C))
-  const float *Wskip = nullptr, *WskipT = nullptr;  // [n_elem][L1 or 1][C][C] / sqrt(C n_elem)
+  TcW Wlin[4], WlinT[4];       // per l [np(l) C][C] / (avg_num_neighbors sqrt(np(l) C)), np(l) = 1 for 0e input
+  const float *Wskip = nullptr, *WskipT = nullptr;  // [n_elem][L1, 1 or 2][C][C] / sqrt(C n_elem)
+  int Lskip = 1;                                    // l blocks of a residual skip
   TcW Wprod, WprodT;          // [C][C] / sqrt(C)
-  const float* wsym = nullptr;                              // [n_elem][Ktot][C]
+  const float* wsym = nullptr;                              // [n_elem][Ktot][C] (contractions.0, then .1)
   const MaceTerm* terms = nullptr;
   int nterms = 0, Ktot = 0;
   const float* wread = nullptr;                             // linear readout [C] / sqrt(C) (all layers but the last)
@@ -81,6 +113,8 @@ struct MaceState {
   // C: row pitch of every per-atom array, the model's channel count Cr rounded up to a multiple of 64 (the wgmma GEMM
   // shapes); the padding channels carry zero weights and stay zero
   int C = 128, Cr = 128, L1 = 4, nsh = 16, T = 2, correlation = 3, H = 16;
+  int hidden_max_l = 0;   // 1: hidden features 0e+1o (layers 0 < t and t < T - 1 carry 1o)
+  std::vector<int> hw;    // row pitch of h[t], t = 0..T: C or 4 C
   double c_act = 1.0, scale = 1.0, shift = 0.0;
   MaceRadial rp{};
   std::vector<int> hid;   // radial MLP hidden widths, padded to 64

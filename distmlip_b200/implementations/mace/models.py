@@ -1,12 +1,14 @@
-"""ScaleShiftMACE_Dist -- a mace `ScaleShiftMACE` with scalar hidden features on the sm_90a engine.
+"""ScaleShiftMACE_Dist -- a mace `ScaleShiftMACE` with hidden features C x 0e or C x 0e + C x 1o on the sm_90a engine.
 
 `from_existing` takes any object with mace's attribute tree and `state_dict()` (mace itself need not be importable, so
 the model is recognised by structure, not by `isinstance`); `enable_distributed_mode(gpus)` validates the
 configuration and creates the engine (b2m_create_mace).  The arithmetic, with every e3nn / mace convention it relies on,
-is stated in oracle/mace_ref.py; the kernels are csrc/kernels_mace.cu.
+is stated in oracle/mace_ref.py (scalar hidden features) and tests/mace_eq_ref.py (0e+1o); the kernels are
+csrc/kernels_mace.cu.
 
 Supported configuration (anything else raises NotImplementedError in enable_distributed_mode): ScaleShiftMACE with one
-head, hidden_irreps = C x 0e (C a multiple of 32, C <= 128), max_ell <= 3, correlation <= 3, Bessel radial basis
+head, hidden_irreps = C x 0e or C x 0e + C x 1o (C a multiple of 32, C <= 128; the shapes of MACE-MP-0 "small" and
+"medium"), max_ell <= 3 (>= 1 with 1o), correlation <= 3, Bessel radial basis
 (num_bessel <= 64) times PolynomialCutoff, a FullyConnectedNet radial MLP (hidden widths <= 64),
 RealAgnosticResidualInteractionBlock or RealAgnosticInteractionBlock per layer, LinearReadoutBlock on every layer but the
 last and NonLinearReadoutBlock (gated SiLU) on the last; no pair repulsion, no distance transform.
@@ -24,6 +26,22 @@ SILU_2MOM = 1.6765324703310909
 
 _RESIDUAL = "RealAgnosticResidualInteractionBlock"
 _PLAIN = "RealAgnosticInteractionBlock"
+
+
+def _parse_irreps(text):
+    """'128x0e+128x1o' -> [(128, 0, 'e'), (128, 1, 'o')] (str() of an e3nn Irreps)"""
+    out = []
+    for part in str(text).replace(" ", "").split("+"):
+        mul, ir = part.split("x") if "x" in part else ("1", part)
+        out.append((int(mul), int(ir[:-1]), ir[-1]))
+    return out
+
+
+def conv_paths(max_ell, hidden_l):
+    """(l_in, l_sh, l_out) of conv_tp in mace's order (tests/mace_eq_ref.py conv_paths, csrc/engine_mace.inl)"""
+    paths = [(li, ls, lo) for li in range(hidden_l + 1) for ls in range(max_ell + 1)
+             for lo in range(abs(li - ls), min(li + ls, max_ell) + 1) if (li + ls + lo) % 2 == 0]
+    return sorted(paths, key=lambda p: p[2])
 
 
 def _act_cst(module, default=SILU_2MOM):
@@ -75,17 +93,17 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
         if T > 8:
             raise NotImplementedError(f"num_interactions={T}: at most 8")
         pc = "products.0.symmetric_contractions.contractions.0."
-        if "products.0.symmetric_contractions.contractions.1.weights_max" in sd:
-            raise NotImplementedError("hidden_irreps with l > 0 (equivariant hidden features) are not supported")
         correlation = sum(1 for k in sd if k.startswith(pc + "U_matrix_"))
         if not 1 <= correlation <= 3:
             raise NotImplementedError(f"correlation={correlation}: 1..3 supported")
         if sd[pc + "U_matrix_1"].dim() != 2:
-            raise NotImplementedError("hidden_irreps with l > 0 (equivariant hidden features) are not supported")
+            raise NotImplementedError("equivariant hidden features: contractions.0 (the 0e output) must have U_matrix_1 "
+                                      f"[nsh, K], not {list(sd[pc + 'U_matrix_1'].shape)}")
         nsh = int(sd[pc + "U_matrix_1"].shape[0])
         max_ell = int(round(nsh ** 0.5)) - 1
         if (max_ell + 1) ** 2 != nsh or max_ell > 3:
             raise NotImplementedError(f"edge spherical harmonics with {nsh} components: max_ell <= 3 supported")
+        hidden_l = self._hidden_l(sd, inters, C, T, n_elem, nsh, max_ell, correlation)
         residual = 0
         avg = [0.0] * 8
         for t, it in enumerate(inters):
@@ -114,8 +132,80 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
             n_elem=n_elem, channels=C, max_ell=max_ell, correlation=correlation, num_interactions=T,
             num_bessel=int(sd["radial_embedding.bessel_fn.bessel_weights"].numel()),
             num_polynomial_cutoff=int(round(float(sd["radial_embedding.cutoff_fn.p"]))),
-            mlp_hidden=H, residual_mask=residual, reserved=0, r_max=float(sd["r_max"]), c_act=c_act,
+            mlp_hidden=H, residual_mask=residual, hidden_max_l=hidden_l, r_max=float(sd["r_max"]), c_act=c_act,
             avg_num_neighbors=(_lib.C.c_double * 8)(*avg))
+
+    @staticmethod
+    def _hidden_l(sd, inters, C, T, n_elem, nsh, max_ell, correlation):
+        """0 for hidden_irreps C x 0e, 1 for C x 0e + C x 1o, from the interactions' `hidden_irreps` when they carry it
+        and from the state_dict shapes, each checked against what conv_tp's path rule predicts per layer"""
+        hl = 0
+        irreps = getattr(inters[0], "hidden_irreps", None) if inters else None
+        if irreps is not None:
+            ir = _parse_irreps(irreps)
+            if any(l > 1 for _, l, _ in ir):
+                raise NotImplementedError(f"hidden_irreps = {irreps}: equivariant hidden features with l > 1 "
+                                          "(MACE-MP-0 'large') are not supported")
+            if len({m for m, _, _ in ir}) > 1:
+                raise NotImplementedError(f"hidden_irreps = {irreps}: unequal multiplicities across l are not supported")
+            if [(l, p) for _, l, p in ir] not in ([(0, "e")], [(0, "e"), (1, "o")]):
+                raise NotImplementedError(f"hidden_irreps = {irreps}: equivariant hidden features other than 0e and 0e+1o "
+                                          "(parity: only 1o) are not supported")
+            hl = len(ir) - 1
+        pre = "products.{}.symmetric_contractions.contractions.{}."
+        if any(k.startswith("products.") and ".symmetric_contractions.contractions." in k and
+               int(k.split(".")[4]) >= 2 for k in sd):
+            raise NotImplementedError("equivariant hidden features with l > 1 (a third contraction) are not supported")
+        has1 = [any(k.startswith(pre.format(t, 1)) for k in sd) for t in range(T)]
+        if any(has1):
+            for t in range(T):
+                u1 = sd.get(pre.format(t, 1) + "U_matrix_1")
+                if has1[t] and (u1 is None or u1.dim() != 3):
+                    raise NotImplementedError(f"equivariant hidden features: products.{t} has contractions.1 without a "
+                                              "[3, nsh, K] U_matrix_1 (malformed state_dict)")
+                if u1 is not None and u1.shape[0] != 3:
+                    raise NotImplementedError(f"equivariant hidden features: contractions.1 of products.{t} gives "
+                                              f"{u1.shape[0]} components; only 1o (3) is supported (l > 1 is not)")
+            if irreps is not None and hl == 0:
+                raise NotImplementedError("equivariant hidden features: contractions.1 on a C x 0e model")
+            hl = 1
+        if hl and max_ell < 1:
+            raise NotImplementedError("equivariant hidden features need max_ell >= 1")
+        for t in range(T):
+            lin, lout = int(hl and t > 0), int(hl and t < T - 1)
+            npaths = len(conv_paths(max_ell, lin))
+            up = int(sd[f"interactions.{t}.linear_up.weight"].numel())
+            if up != (1 + lin) * C * C:
+                c1 = round(max(up - C * C, 0) ** 0.5)
+                if lin and c1 * c1 == up - C * C:
+                    raise NotImplementedError(f"interactions.{t}.linear_up maps {C}x0e+{c1}x1o: unequal multiplicities "
+                                              "across l are not supported")
+                raise NotImplementedError(f"interactions.{t}.linear_up has {up} weights, {(1 + lin) * C * C} expected for "
+                                          f"hidden_irreps {C}x0e" + (f"+{C}x1o" if hl else "") + " (equivariant hidden "
+                                          "features other than 0e+1o are not supported)")
+            last = max((k for k in sd if k.startswith(f"interactions.{t}.conv_tp_weights.layer")),
+                       key=lambda k: int(k.split(".")[3][5:]))
+            if int(sd[last].shape[1]) != npaths * C:
+                raise NotImplementedError(f"{last} has {int(sd[last].shape[1])} outputs, {npaths} paths x {C} expected: "
+                                          "equivariant hidden features other than 0e+1o (parity: only 1o) are not supported")
+            if int(sd[f"interactions.{t}.linear.weight"].numel()) != npaths * C * C:
+                raise NotImplementedError(f"interactions.{t}.linear does not match the {npaths} conv_tp paths of "
+                                          "0e" + ("+1o" if lin else "") + " node features")
+            if int(sd[f"products.{t}.linear.weight"].numel()) != (1 + lout) * C * C:
+                raise NotImplementedError(f"products.{t}.linear has {int(sd[f'products.{t}.linear.weight'].numel())} "
+                                          f"weights, {(1 + lout) * C * C} expected (unequal multiplicities across l or "
+                                          "l > 1 are not supported)")
+            if has1[t] != bool(lout):
+                raise NotImplementedError(f"equivariant hidden features: products.{t} " +
+                                          ("lacks" if lout else "has") + " contractions.1 (only the last layer is 0e)")
+            if lout:
+                w = sd.get(pre.format(t, 1) + "weights_max")
+                if w is None or w.dim() != 3 or int(w.shape[0]) != n_elem or int(w.shape[2]) != C:
+                    raise NotImplementedError(f"products.{t} contractions.1 weights_max is not [{n_elem}, K, {C}] "
+                                              "(unequal multiplicities across l are not supported)")
+                if sum(1 for k in sd if k.startswith(pre.format(t, 1) + "U_matrix_")) != correlation:
+                    raise NotImplementedError(f"products.{t}: contractions.1 and contractions.0 differ in correlation")
+        return hl
 
     def enable_distributed_mode(self, gpus):
         """mace.py / models.py of the reference: `gpus` are CUDA ordinals, one per partition (a single-process group

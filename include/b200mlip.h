@@ -97,8 +97,10 @@ typedef struct {
 } b2m_tensornet_desc;
 int b2m_create_tensornet(const b2m_tensornet_desc* desc, const int* devices, int ndev, b2m_handle* out);
 
-/* MACE (DESIGN.md §11): the same handle type and calls, for a mace ScaleShiftMACE with scalar hidden features
- * (hidden_irreps = C x 0e), loaded key by key from its state_dict (arithmetic and conventions: oracle/mace_ref.py).
+/* MACE (DESIGN.md §11): the same handle type and calls, for a mace ScaleShiftMACE with hidden features C x 0e
+ * (hidden_max_l = 0, MACE-MP-0 "small") or C x 0e + C x 1o (hidden_max_l = 1, MACE-MP-0 "medium"; then max_ell >= 1),
+ * loaded key by key from its state_dict (arithmetic and conventions: oracle/mace_ref.py and, for 0e+1o,
+ * tests/mace_eq_ref.py).
  * Supported: one head, C a multiple of 32 with C <= 128, max_ell <= 3, correlation <= 3, Bessel basis x polynomial cutoff,
  * an e3nn FullyConnectedNet radial MLP (hidden widths <= 64), RealAgnostic(Residual)InteractionBlock per layer, linear
  * readouts and a gated non-linear last readout.  Edges are every periodic image closer than r_max (no bond graph).
@@ -107,7 +109,7 @@ int b2m_create_tensornet(const b2m_tensornet_desc* desc, const int* devices, int
  * energies[i] = E0[z_i] + scale * e_i + shift and the per-atom virials. */
 typedef struct {
   int32_t n_elem;                 /* len(atomic_numbers)                                                 */
-  int32_t channels;               /* C of hidden_irreps = C x 0e                                         */
+  int32_t channels;               /* C of hidden_irreps = C x 0e (+ C x 1o)                              */
   int32_t max_ell;                /* edge spherical harmonics 0..max_ell                                 */
   int32_t correlation;            /* symmetric-contraction order                                         */
   int32_t num_interactions;       /* <= 8                                                                */
@@ -115,7 +117,7 @@ typedef struct {
   int32_t num_polynomial_cutoff;  /* PolynomialCutoff exponent p                                         */
   int32_t mlp_hidden;             /* width of the non-linear readout                                     */
   int32_t residual_mask;          /* bit t: interactions.t is a RealAgnosticResidualInteractionBlock     */
-  int32_t reserved;
+  int32_t hidden_max_l;           /* 0: hidden_irreps C x 0e; 1: C x 0e + C x 1o (other values invalid)  */
   double r_max;                   /* cutoff (Angstrom)                                                   */
   double c_act;                   /* e3nn normalize2mom(SiLU) constant of the radial MLP and the readout */
   double avg_num_neighbors[8];    /* per interaction                                                     */
