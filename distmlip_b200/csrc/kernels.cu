@@ -398,9 +398,17 @@ void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats) {
 // atom conv: shared pieces of the persistent forward and backward
 // ============================================================================================
 // Both kernels run one CTA per SM (grid = min(tiles, SMs)); CTA c takes tiles c, c + grid, c + 2 grid, ...  Every
-// tile's A[src] rows arrive by per-row bulk copies into one of two [TM][LD] buffers, tile number `it` of the CTA in
+// tile's A[src] rows arrive by per-row bulk copies into one of two [TM][LDE] buffers, tile number `it` of the CTA in
 // buffer it & 1 (its mbarrier: stage_parity(it)).  The copies of tile it + 1 are issued while tile it is computed;
 // its index loads one tile earlier still, into registers (EdgeRow).
+//
+// Every per-element phase works in the accumulator layout (Map): warpgroup b owns first-layer columns 64 b .. 64 b + 63
+// (the hidden columns its branch's second layer reads) and the branch's 64 outputs, and a thread owns 4 rows x 16
+// columns of both.  Such a thread touches the tile only at its own positions (row(i), 64 b + col(j)), as float2 pairs
+// (col(2 jj), col(2 jj) + 1); the pitch LDE = 136 (8 mod 32 floats) puts the 8 rows x 4 pairs of a half-warp on 32
+// distinct banks.
+constexpr int LDE = 136;
+
 struct EdgeRow {
   int src, dst, bond;
   float d;
@@ -426,7 +434,7 @@ __device__ __forceinline__ void issue_gather(const AtomConvArgs& a, int64_t t, c
     s_dst[tid] = row.dst;
     s_bond[tid] = row.bond;
     s_d[tid] = row.d;
-    if (row.src >= 0) bulk_g2s(buf + tid * LD, a.Aproj + (size_t)row.src * D2, 512u, bar);
+    if (row.src >= 0) bulk_g2s(buf + tid * LDE, a.Aproj + (size_t)row.src * D2, 512u, bar);
   }
 }
 // be_k(d_r) (and d be_k / dd) of the tile's rows, both warpgroups (rows r, radial halves)
@@ -442,40 +450,116 @@ __device__ __forceinline__ void radial_rows(const AtomConvArgs& a, const float* 
     if (dbe_s != nullptr) dbe_s[r * 12 + k] = dbe;
   }
 }
-// pre[r][j] = A[src] (in the tile) + C[dst] + (Q[bond] | M.be) for this thread's column j = tid & 127 and rows
-// r = tid >> 7 + 2 i, handed to f(r, pre) (rows r >= nvalid: f(r, 0)).  The C / Q rows of 16 rows are loaded together
-// before any is used, so a thread has 32 loads in flight instead of one round trip per row.
-template <class F>
-__device__ __forceinline__ void first_layer(const AtomConvArgs& a, const float* tile, const int* s_dst,
-                                            const int* s_bond, const float* be_s, const float (&Mj)[9], int nvalid,
-                                            F&& f) {
-  const int j = threadIdx.x & 127, rh = threadIdx.x >> 7;
-  const bool useQ = a.Qproj != nullptr;
-#pragma unroll 1
-  for (int i0 = 0; i0 < 64; i0 += 16) {
-    float cv[16], qv[16];
+// the radial operands live in shared memory at a row pitch of 12 floats (k < 9 used): a row is two float4 and a float
+__device__ __forceinline__ void stage_pitch12(float* dst, const float* __restrict__ src, int rows) {
+  for (int i = threadIdx.x; i < rows * 12; i += NT) {
+    const int r = i / 12, k = i % 12;
+    dst[i] = k < 9 ? src[r * 9 + k] : 0.f;
+  }
+}
+__device__ __forceinline__ void ld9(const float* p, float (&v)[9]) {
+  const float4 x = *reinterpret_cast<const float4*>(p), y = *reinterpret_cast<const float4*>(p + 4);
+  v[0] = x.x, v[1] = x.y, v[2] = x.z, v[3] = x.w, v[4] = y.x, v[5] = y.y, v[6] = y.z, v[7] = y.w, v[8] = p[8];
+}
+__device__ __forceinline__ float dot9(const float (&x)[9], const float (&y)[9]) {
+  float s = 0.f;
 #pragma unroll
-    for (int u = 0; u < 16; u++) {
-      const int r = rh + 2 * (i0 + u);
-      const int dst = s_dst[r], bond = s_bond[r];
-      cv[u] = dst >= 0 ? __ldg(&a.Cproj[(size_t)dst * D2 + j]) : 0.f;
-      qv[u] = (useQ && bond >= 0) ? __ldg(&a.Qproj[(size_t)bond * D2 + j]) : 0.f;
+  for (int k = 0; k < 9; k++) s = fmaf(x[k], y[k], s);
+  return s;
+}
+__device__ __forceinline__ float2 ld_f2(const float* p) { return *reinterpret_cast<const float2*>(p); }
+__device__ __forceinline__ void st_f2(float* p, float x, float y) { *reinterpret_cast<float2*>(p) = make_float2(x, y); }
+
+// pre of this thread's rows of 64-row half h (acc[2h], acc[2h + 1], Map layout): A[src] (in the tile) + C[dst] +
+// (Q[bond] | M.be), summed in that order; rows r >= nvalid are 0.  Index work is per row; the C / Q values of both rows
+// (32 float2 loads) are in flight before any is used.  Msm: M as [128][12], be_s: [TM][12].
+__device__ __forceinline__ void first_layer_half(const AtomConvArgs& a, const Map& m, int h, const float* tile,
+                                                 const int* s_dst, const int* s_bond, const float* be_s,
+                                                 const float* Msm, int nvalid, float (&acc)[AR][AC]) {
+  const int c0 = 64 * m.branch + m.cb;
+  float2 cv[2][AC / 2], qv[2][AC / 2];
+  float be[2][9];
+  bool viaQ[2], ok[2];
+#pragma unroll
+  for (int ii = 0; ii < 2; ii++) {
+    const int r = m.row(2 * h + ii);
+    const int dst = s_dst[r], bond = s_bond[r];
+    ok[ii] = r < nvalid;
+    viaQ[ii] = a.Qproj != nullptr && bond >= 0;
+    const float* cp = a.Cproj + (size_t)max(dst, 0) * D2 + c0;
+#pragma unroll
+    for (int jj = 0; jj < AC / 2; jj++) cv[ii][jj] = dst >= 0 ? __ldg(reinterpret_cast<const float2*>(cp + 8 * jj)) : make_float2(0.f, 0.f);
+    if (viaQ[ii]) {
+      const float* qp = a.Qproj + (size_t)bond * D2 + c0;
+#pragma unroll
+      for (int jj = 0; jj < AC / 2; jj++) qv[ii][jj] = __ldg(reinterpret_cast<const float2*>(qp + 8 * jj));
+    } else {
+#pragma unroll
+      for (int jj = 0; jj < AC / 2; jj++) qv[ii][jj] = make_float2(0.f, 0.f);
     }
+    ld9(be_s + r * 12, be[ii]);
+  }
 #pragma unroll
-    for (int u = 0; u < 16; u++) {
-      const int r = rh + 2 * (i0 + u);
-      float p = 0.f;
-      if (r < nvalid) {
-        float t = qv[u];
-        if (!(useQ && s_bond[r] >= 0)) {
-          t = 0.f;
+  for (int j = 0; j < AC; j++) {
+    float mk[9];
+    ld9(Msm + (64 * m.branch + m.col(j)) * 12, mk);
 #pragma unroll
-          for (int k = 0; k < 9; k++) t = fmaf(be_s[r * 12 + k], Mj[k], t);
-        }
-        p = tile[r * LD + j] + cv[u] + t;
-      }
-      f(r, p);
+    for (int ii = 0; ii < 2; ii++) {
+      const int r = m.row(2 * h + ii);
+      const float x = tile[r * LDE + 64 * m.branch + m.col(j)];
+      const float2 c2 = cv[ii][j >> 1], q2 = qv[ii][j >> 1];
+      const float t = viaQ[ii] ? ((j & 1) ? q2.y : q2.x) : dot9(be[ii], mk);
+      acc[2 * h + ii][j] = ok[ii] ? x + ((j & 1) ? c2.y : c2.x) + t : 0.f;
     }
+  }
+}
+
+// acc rows of half h (2h, 2h + 1) = x rows of half h . B^T on the tensor cores (warpgroup-collective), 3xTF32 (hi.hi +
+// lo.hi + hi.lo, fp32 accumulate).  x is in the accumulator layout and is the register A fragment as it stands: in k
+// block ks a thread holds columns 8 ks + 2 (l%4) and + 1, which fill the fragment's k slots l%4 and l%4 + 4.  So B (the
+// branch's canonical image, hi plane of 4096 floats, then lo) has its k index permuted within each block of 8 (slot q
+// <- column 2q, slot q + 4 <- column 2q + 1; engine.cu: second_layer_can).  x and acc may be the same array.
+__device__ __forceinline__ void wg_mm64_acc(const float (&x)[AR][AC], int h, const float* Bcan, float (&acc)[AR][AC]) {
+  constexpr uint32_t LBO = 8 * 128;  // byte step between core matrices along K (N = 64)
+  const uint32_t b_hi = s_u32(Bcan), b_lo = b_hi + 4096u * 4u;
+  uint32_t ah[8][4], al[8][4];
+#pragma unroll
+  for (int ks = 0; ks < 8; ks++) {
+    const float v[4] = {x[2 * h][2 * ks], x[2 * h + 1][2 * ks], x[2 * h][2 * ks + 1], x[2 * h + 1][2 * ks + 1]};
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      ah[ks][q] = tf32_hi_bits(v[q]);
+      al[ks][q] = __float_as_uint(v[q] - __uint_as_float(ah[ks][q]));
+    }
+  }
+  float d[32];
+  acc_fence(d);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 8; ks++) {
+#pragma unroll
+    for (int term = 0; term < 3; term++) {
+      const uint64_t bd = gmma_desc((term == 2 ? b_lo : b_hi) + ks * 2 * LBO, LBO, 128u);
+      wgmma_tf32_n64_rA(d, term == 1 ? al[ks] : ah[ks], bd, (ks > 0 || term > 0) ? 1 : 0);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+  acc_fence(d);
+#pragma unroll
+  for (int q = 0; q < 32; q++) acc[2 * h + ((q >> 1) & 1)][2 * (q >> 2) + (q & 1)] = d[q];
+}
+
+// v[ii][k] of the rows of half h (i = 2h + ii) summed over the 4 lanes of a quad (they share rows): lane l takes the sum
+// of row i = l & 3 into out when that row is in half h
+__device__ __forceinline__ void quad_reduce_half(const float (&v)[2][9], int h, float (&out)[9]) {
+  const int l = threadIdx.x & 3;
+  const bool b0 = l & 1, mine = (l >> 1) == h;
+#pragma unroll
+  for (int k = 0; k < 9; k++) {
+    float w = (b0 ? v[1][k] : v[0][k]) + __shfl_xor_sync(0xffffffffu, b0 ? v[0][k] : v[1][k], 1);
+    w += __shfl_xor_sync(0xffffffffu, w, 2);
+    if (mine) out[k] = w;
   }
 }
 
@@ -488,29 +572,34 @@ __device__ __forceinline__ void red_add_v4(float* p, float4 v) {
 // atom conv: forward
 // ============================================================================================
 struct AtomSmemFwd {
-  static constexpr int kTile = 32;                  // two [TM][LD] gather buffers (first 128 B: their mbarriers)
-  static constexpr int kW = kTile + 2 * TM * LD;    // wgmma images of W2 (2 branches x hi | lo), staged once
-  static constexpr int kBe = kW + 16384;
-  static constexpr int kWab = kBe + TM * 12;
-  static constexpr int kB2 = kWab + 576;
+  static constexpr int kTile = 32;                  // two [TM][LDE] gather buffers (first 128 B: their mbarriers)
+  static constexpr int kW = kTile + 2 * TM * LDE;   // wgmma images of W2 (2 branches x hi | lo, k permuted), staged once
+  static constexpr int kBe = kW + 16384;            // be [TM][12]
+  static constexpr int kM = kBe + TM * 12;          // M [128][12]
+  static constexpr int kWab = kM + 128 * 12;        // W_ab [64][12]
+  static constexpr int kB2 = kWab + 64 * 12;
   static constexpr int kD = kB2 + 128;              // [2][TM] per buffer
   static constexpr int kIdx = kD + 2 * TM;          // dst [2][TM], bond [2][TM]
   static constexpr int kTotal = kIdx + 4 * TM;
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
 static_assert(AtomSmemFwd::bytes <= 232448, "atom-conv forward shared memory");
+static_assert(AtomSmemFwd::kW % 4 == 0 && AtomSmemFwd::kBe % 4 == 0 && AtomSmemFwd::kM % 4 == 0 &&
+                  AtomSmemFwd::kWab % 4 == 0,
+              "16-byte aligned images and pitch-12 rows");
 
 __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
   uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);  // [2]
   float* Wsm = smem + AtomSmemFwd::kW;
   float* be_s = smem + AtomSmemFwd::kBe;
+  float* Msm = smem + AtomSmemFwd::kM;
   float* wabW = smem + AtomSmemFwd::kWab;
   float* b2s = smem + AtomSmemFwd::kB2;
 
   const int tid = threadIdx.x;
   const int64_t ntiles = (a.E + TM - 1) / TM, step = gridDim.x;
-  auto tile_of = [&](int s) { return smem + AtomSmemFwd::kTile + s * TM * LD; };
+  auto tile_of = [&](int s) { return smem + AtomSmemFwd::kTile + s * TM * LDE; };
   auto d_of = [&](int s) { return smem + AtomSmemFwd::kD + s * TM; };
   auto dst_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + s * TM; };
   auto bond_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + (2 + s) * TM; };
@@ -523,15 +612,14 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
   EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
   // loop-invariant operands, once per CTA
   stage_w(Wsm, a.W2can, 4096);
-  for (int i = tid; i < 576; i += NT) wabW[i] = a.Wabw[i];
+  stage_pitch12(Msm, a.M, 128);
+  stage_pitch12(wabW, a.Wabw, 64);
   if (tid < 128) b2s[tid] = a.b2[tid];
-  float Mj[9];
-#pragma unroll
-  for (int k = 0; k < 9; k++) Mj[k] = a.M[(tid & 127) * 9 + k];
   __syncthreads();
   issue_gather(a, blockIdx.x, nxt, tile_of(0), &mbar[0], nullptr, dst_of(0), bond_of(0), d_of(0));
   nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid);
 
+  const Map m;
   int it = 0;
   for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
     const int s = it & 1;
@@ -548,13 +636,17 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
     radial_rows(a, d_of(s), nvalid, be_s, nullptr);
     mbar_wait(&mbar[s], stage_parity(it));
     __syncthreads();
-    // pre = A[src] + C[dst] + (M.be | Q[bond]);  hid = silu(pre)
-    first_layer(a, tile, s_dst, s_bond, be_s, Mj, nvalid,
-                [&](int r, float p) { tile[r * LD + (tid & 127)] = r < nvalid ? silu_f(p) : 0.f; });
-    __syncthreads();
-    const Map m;
+    // pre = A[src] + C[dst] + (M.be | Q[bond]);  hid = silu(pre) straight into the second layer, per 64-row half
     float acc[AR][AC];
-    gemm64(tile, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      first_layer_half(a, m, h, tile, s_dst, s_bond, be_s, Msm, nvalid, acc);
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) acc[2 * h + ii][j] = silu_f(acc[2 * h + ii][j]);
+      wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
+    }
 #pragma unroll
     for (int i = 0; i < AR; i++)
 #pragma unroll
@@ -562,32 +654,39 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
         const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
         acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
       }
-    __syncthreads();
+    // m = L . G . w_ab: warpgroup 1 forms G . w_ab in its own tile positions, warpgroup 0 multiplies by L in its own
     if (m.branch == 1) {
+      float be[AR][9];
+#pragma unroll
+      for (int i = 0; i < AR; i++) ld9(be_s + m.row(i) * 12, be[i]);
+#pragma unroll
+      for (int j = 0; j < AC; j++) {
+        float wk[9];
+        ld9(wabW + m.col(j) * 12, wk);
+#pragma unroll
+        for (int i = 0; i < AR; i++) acc[i][j] *= dot9(be[i], wk);
+      }
 #pragma unroll
       for (int i = 0; i < AR; i++)
 #pragma unroll
-        for (int j = 0; j < AC; j++) tile[m.row(i) * LD + m.col(j)] = acc[i][j];
+        for (int jj = 0; jj < AC / 2; jj++)
+          st_f2(tile + m.row(i) * LDE + 64 + m.col(2 * jj), acc[i][2 * jj], acc[i][2 * jj + 1]);
     }
     __syncthreads();
     if (m.branch == 0) {
 #pragma unroll
-      for (int i = 0; i < AR; i++) {
-        const int r = m.row(i);
+      for (int i = 0; i < AR; i++)
 #pragma unroll
-        for (int j = 0; j < AC; j++) {
-          const int c = m.col(j);
-          float wab = 0.f;
-#pragma unroll
-          for (int k = 0; k < 9; k++) wab = fmaf(be_s[r * 12 + k], wabW[c * 9 + k], wab);
-          tile[r * LD + c] = acc[i][j] * tile[r * LD + c] * wab;
+        for (int jj = 0; jj < AC / 2; jj++) {
+          float* p = tile + m.row(i) * LDE + m.col(2 * jj);
+          const float2 g = ld_f2(p + 64);
+          st_f2(p, acc[i][2 * jj] * g.x, acc[i][2 * jj + 1] * g.y);
         }
-      }
     }
     __syncthreads();
     {
       const int c = tid & 63, part = tid >> 6;
-      seg_flush(tile, LD, c, part * 32, part * 32 + 32, s_dst, a.agg, D);
+      seg_flush(tile, LDE, c, part * 32, part * 32 + 32, s_dst, a.agg, D);
     }
   }
 }
@@ -606,44 +705,47 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
 // ============================================================================================
 // atom conv: backward (recompute forward in-tile, then hand-derived reverse pass)
 // ============================================================================================
-// Shared memory holds one weight image (64 KB) and two [TM][LD] tiles whose roles alternate: the tile's gathered rows
-// arrive in buffer it & 1, which becomes P (pre-activations, then their adjoints); the other buffer is H (hidden
-// activations, then the second-layer adjoints).  Once g.W2 has read H and the W2^T image, both are refilled by bulk
-// copies -- H with the next tile's A[src] rows, the image with W2 -- which land while this tile's scatter phase runs.
-// The W2^T image is loaded right after the recompute product, under the elementwise reverse.  The weight barrier
-// completes two phases per tile (W2^T, then W2), waited on in that order.
+// Shared memory holds one weight image (64 KB) and two [TM][LDE] tiles whose roles alternate: the tile's gathered rows
+// arrive in buffer it & 1, which becomes P: each thread overwrites its own A[src] values with its pre-activations, and
+// later with their adjoints gpre, which the scatter phase reads row-major.  The other buffer is H: the branches
+// exchange their activations through it.  Both second-layer products take their A operand from registers.  Once g.W2
+// has read the W2^T image and H is no longer read, both are refilled by bulk copies -- H with the next tile's A[src]
+// rows, the image with W2 -- which land while this tile's scatter phase runs.  The W2^T image is loaded right after the
+// recompute product, under the elementwise reverse.  The weight barrier completes two phases per tile (W2^T, then W2),
+// waited on in that order.
 struct AtomSmemBwd {
-  static constexpr int kBuf = 32;               // two [TM][LD] tiles (first 128 B: 2 gather mbarriers + weight mbarrier)
-  static constexpr int kGw = kBuf + 2 * TM * LD;  // dE/dw_ab . W_ab per (row, radial k) [TM][12]
-  static constexpr int kW = kGw + TM * 12;        // wgmma image of W2 or W2^T (2 branches x hi | lo)
-  static constexpr int kBe = kW + 16384;
-  static constexpr int kDbe = kBe + TM * 12;
-  static constexpr int kWab = kDbe + TM * 12;
-  static constexpr int kM = kWab + 576;
-  static constexpr int kB2 = kM + 1152;
+  static constexpr int kBuf = 32;               // two [TM][LDE] tiles (first 128 B: 2 gather mbarriers + weight mbarrier)
+  static constexpr int kW = kBuf + 2 * TM * LDE;  // wgmma image of W2 or W2^T (2 branches x hi | lo, k permuted)
+  static constexpr int kBe = kW + 16384;        // be [TM][12]
+  static constexpr int kDbe = kBe + TM * 12;    // d be / dd [TM][12]
+  static constexpr int kM = kDbe + TM * 12;     // M [128][12]
+  static constexpr int kWab = kM + 128 * 12;    // W_ab [64][12]
+  static constexpr int kB2 = kWab + 64 * 12;
   static constexpr int kD = kB2 + 128;          // [2][TM]
   static constexpr int kIdx = kD + 2 * TM;      // src, dst, bond: [2][TM] each
   static constexpr int kTotal = kIdx + 6 * TM;
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
 static_assert(AtomSmemBwd::bytes <= 232448, "atom-conv backward shared memory");
+static_assert(AtomSmemBwd::kW % 4 == 0 && AtomSmemBwd::kBe % 4 == 0 && AtomSmemBwd::kM % 4 == 0 &&
+                  AtomSmemBwd::kWab % 4 == 0,
+              "16-byte aligned images and pitch-12 rows");
 
 __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
   uint64_t* gbar = reinterpret_cast<uint64_t*>(smem);  // [2]: gather buffers
   uint64_t* wbar = gbar + 2;                            // weight image
-  float* gws = smem + AtomSmemBwd::kGw;
   float* Wsm = smem + AtomSmemBwd::kW;
   float* be_s = smem + AtomSmemBwd::kBe;
   float* dbe_s = smem + AtomSmemBwd::kDbe;
-  float* wabW = smem + AtomSmemBwd::kWab;
   float* Msm = smem + AtomSmemBwd::kM;
+  float* wabW = smem + AtomSmemBwd::kWab;
   float* b2s = smem + AtomSmemBwd::kB2;
 
   const int tid = threadIdx.x;
   const int64_t ntiles = (a.E + TM - 1) / TM, step = gridDim.x;
   const bool useQ = a.Qproj != nullptr;
-  auto buf_of = [&](int s) { return smem + AtomSmemBwd::kBuf + s * TM * LD; };
+  auto buf_of = [&](int s) { return smem + AtomSmemBwd::kBuf + s * TM * LDE; };
   auto d_of = [&](int s) { return smem + AtomSmemBwd::kD + s * TM; };
   auto src_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + s * TM; };
   auto dst_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + (2 + s) * TM; };
@@ -656,18 +758,17 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     fence_barrier_init();
   }
   EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
-  for (int i = tid; i < 576; i += NT) wabW[i] = a.Wabw[i];
-  for (int i = tid; i < 1152; i += NT) Msm[i] = a.M[i];
+  stage_pitch12(Msm, a.M, 128);
+  stage_pitch12(wabW, a.Wabw, 64);
   if (tid < 128) b2s[tid] = a.b2[tid];
-  float Mj[9];
-#pragma unroll
-  for (int k = 0; k < 9; k++) Mj[k] = a.M[(tid & 127) * 9 + k];
   __syncthreads();
   if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
   issue_gather(a, blockIdx.x, nxt, buf_of(0), &gbar[0], src_of(0), dst_of(0), bond_of(0), d_of(0));
   nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid);
   uint32_t wpar = 0;
 
+  const Map m;
+  const int c0 = 64 * m.branch;  // this warpgroup's first-layer columns
   int it = 0;
   for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
     const int s = it & 1;
@@ -678,144 +779,158 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     const int* s_bond = bond_of(s);
     const int64_t e0 = t * TM;
     const int nvalid = (int)min((int64_t)TM, a.E - e0);
-    __syncthreads();  // the previous tile's scatter phase is done with tileH (its P), gws, be_s, dbe_s
+    __syncthreads();  // the previous tile's scatter phase is done with tileH (its P), be_s, dbe_s
     radial_rows(a, d_of(s), nvalid, be_s, dbe_s);
     mbar_wait(&gbar[s], stage_parity(it));
     mbar_wait(wbar, wpar);  // W2
     wpar ^= 1;
     __syncthreads();
-    first_layer(a, tileP, s_dst, s_bond, be_s, Mj, nvalid, [&](int r, float p) {
-      const int j = tid & 127;
-      tileP[r * LD + j] = p;
-      tileH[r * LD + j] = r < nvalid ? silu_f(p) : 0.f;
-    });
-    __syncthreads();
-    const Map m;
+    // recompute: pre (kept in P at the thread's own positions), silu(pre) . W2^T + b2 = u (L) / v (G)
     float acc[AR][AC];
-    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      first_layer_half(a, m, h, tileP, s_dst, s_bond, be_s, Msm, nvalid, acc);
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++) {
+          float* p = tileP + m.row(2 * h + ii) * LDE + c0 + m.col(2 * jj);
+          float& x0 = acc[2 * h + ii][2 * jj];
+          float& x1 = acc[2 * h + ii][2 * jj + 1];
+          st_f2(p, x0, x1);
+          x0 = silu_f(x0);
+          x1 = silu_f(x1);
+        }
+      wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
+    }
 #pragma unroll
     for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];  // u (L) / v (G)
-    __syncthreads();  // hid + the W2 image no longer needed
+      for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
+    __syncthreads();  // the W2 image is no longer needed
     if (tid == 0) bulk_g2s_image(Wsm, a.W2Tcan, 16384 * 4, wbar);
     // exchange activations between the two branches through tileH
 #pragma unroll
     for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const float u = acc[i][j];
-        tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
+      for (int jj = 0; jj < AC / 2; jj++) {
+        const float u0 = acc[i][2 * jj], u1 = acc[i][2 * jj + 1];
+        st_f2(tileH + m.row(i) * LDE + c0 + m.col(2 * jj), m.branch == 0 ? silu_f(u0) : sigm(u0),
+              m.branch == 0 ? silu_f(u1) : sigm(u1));
       }
     __syncthreads();
-    float gw[AR][9];  // branch 0: this thread's columns of sum_c dE/dw_ab[r][c] W_ab[c][k]
+    // elementwise reverse: acc = dE/du (L) / dE/dv (G); branch 0 also sums dE/dw_ab[r][c] W_ab[c][k] over its columns
+    float gwr[9];  // branch 0: the row m.row(lane & 3) of sum_c dE/dw_ab W_ab
 #pragma unroll
-    for (int i = 0; i < AR; i++)
+    for (int h = 0; h < 2; h++) {
+      float gw[2][9];
 #pragma unroll
-      for (int k = 0; k < 9; k++) gw[i][k] = 0.f;
+      for (int ii = 0; ii < 2; ii++)
 #pragma unroll
-    for (int i = 0; i < AR; i++) {
-      const int r = m.row(i);
-      const int dst = s_dst[r];
-      float2 gm2[AC / 2];  // this row's 16 dE/dagg values, loaded before any is used
+        for (int k = 0; k < 9; k++) gw[ii][k] = 0.f;
 #pragma unroll
-      for (int jj = 0; jj < AC / 2; jj++)
-        gm2[jj] = dst >= 0 ? __ldg(reinterpret_cast<const float2*>(&a.gagg[(size_t)dst * D + m.col(2 * jj)]))
-                           : make_float2(0.f, 0.f);
+      for (int ii = 0; ii < 2; ii++) {
+        const int i = 2 * h + ii;
+        const int r = m.row(i);
+        const int dst = s_dst[r];
+        float2 gm2[AC / 2];  // this row's 16 dE/dagg values, loaded before any is used
+        const float* gp = a.gagg + (size_t)max(dst, 0) * D + m.cb;
 #pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const int c = m.col(j);
-        const float u = acc[i][j];
-        const float po = tileH[r * LD + (1 - m.branch) * 64 + c];  // partner activation
-        float g = 0.f;
-        if (dst >= 0) {
-          const float gm = (j & 1) ? gm2[j >> 1].y : gm2[j >> 1].x;
-          float wab = 0.f;
+        for (int jj = 0; jj < AC / 2; jj++)
+          gm2[jj] = dst >= 0 ? __ldg(reinterpret_cast<const float2*>(gp + 8 * jj)) : make_float2(0.f, 0.f);
+        float be[9];
+        ld9(be_s + r * 12, be);
 #pragma unroll
-          for (int k = 0; k < 9; k++) wab = fmaf(be_s[r * 12 + k], wabW[c * 9 + k], wab);
-          if (m.branch == 0) {
-            const float sg = sigm(u);
-            const float oL = u * sg;
-            const float gwv = gm * oL * po;                    // d/d w_ab
+        for (int jj = 0; jj < AC / 2; jj++) {
+          const float2 po2 = ld_f2(tileH + r * LDE + (64 - c0) + m.col(2 * jj));  // partner activations
 #pragma unroll
-            for (int k = 0; k < 9; k++) gw[i][k] = fmaf(gwv, wabW[c * 9 + k], gw[i][k]);
-            g = gm * po * wab * (sg * (1.f + u * (1.f - sg)));  // d/du
-          } else {
-            const float oG = sigm(u);
-            g = gm * po * wab * oG * (1.f - oG);               // d/dv
+          for (int e = 0; e < 2; e++) {
+            const int j = 2 * jj + e;
+            const float u = acc[i][j];
+            const float po = e ? po2.y : po2.x;
+            const float gm = e ? gm2[jj].y : gm2[jj].x;
+            float g = 0.f;
+            if (dst >= 0) {
+              float wk[9];
+              ld9(wabW + m.col(j) * 12, wk);
+              const float wab = dot9(be, wk);
+              if (m.branch == 0) {
+                const float sg = sigm(u);
+                const float oL = u * sg;
+                const float gwv = gm * oL * po;  // d/d w_ab
+#pragma unroll
+                for (int k = 0; k < 9; k++) gw[ii][k] = fmaf(gwv, wk[k], gw[ii][k]);
+                g = gm * po * wab * (sg * (1.f + u * (1.f - sg)));  // d/du
+              } else {
+                const float oG = sigm(u);
+                g = gm * po * wab * oG * (1.f - oG);  // d/dv
+              }
+            }
+            acc[i][j] = g;
           }
         }
-        acc[i][j] = g;
       }
+      quad_reduce_half(gw, h, gwr);
     }
-    if (m.branch == 0) {  // the four lanes l/4 = const of a warp own one row's 64 columns
-#pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int k = 0; k < 9; k++) {
-          float v = gw[i][k];
-          v += __shfl_xor_sync(0xffffffffu, v, 1);
-          v += __shfl_xor_sync(0xffffffffu, v, 2);
-          if ((threadIdx.x & 3) == 0) gws[m.row(i) * 12 + k] = v;
-        }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int j = 0; j < AC; j++) tileH[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
     mbar_wait(wbar, wpar);  // W2^T
     wpar ^= 1;
-    __syncthreads();
-    // ghid = [gu @ W2L, gv @ W2G];  gpre = ghid * dsilu(pre)
-    gemm64(tileH, LD, m.branch * 64, Wsm + m.branch * 8192, acc);
+    // ghid = [gu @ W2L, gv @ W2G];  gpre = ghid * dsilu(pre), into P at the thread's own positions
 #pragma unroll
-    for (int i = 0; i < AR; i++)
+    for (int h = 0; h < 2; h++) {
+      wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
 #pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
-        tileP[idx] = acc[i][j] * dsilu_f(tileP[idx]);
-      }
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++) {
+          float* p = tileP + m.row(2 * h + ii) * LDE + c0 + m.col(2 * jj);
+          const float2 pre = ld_f2(p);
+          float& x0 = acc[2 * h + ii][2 * jj];
+          float& x1 = acc[2 * h + ii][2 * jj + 1];
+          x0 *= dsilu_f(pre.x);
+          x1 *= dsilu_f(pre.y);
+          st_f2(p, x0, x1);
+        }
+    }
     fence_proxy_async_smem();  // this thread's generic accesses of tileH come before its bulk refill
-    __syncthreads();           // tileH and the W2^T image are free
+    __syncthreads();           // tileH and the W2^T image are free; P holds gpre
     if (t + step < ntiles) {
       if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
       issue_gather(a, t + step, nxt, tileH, &gbar[s ^ 1], src_of(s ^ 1), dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
       nxt = edge_row(a, (t + 2 * step) * TM + tid);
     }
-    // ---- scatter phase (reads tileP and this tile's index arrays only) ----
-    {  // d E / d d_e through the radial basis (w_ab weights and, unless a bond row fed by Q, M.be): warpgroup h sums
-       // sum_j gpre[r][j] M[j][k] over j in [64 h, 64 h + 64) for row r = tid & 127, all k at once
-      const int r = tid & 127, h = tid >> 7;
-      float sk[9];
+    // ---- scatter phase (reads P, be_s / dbe_s and this tile's index arrays only) ----
+    {  // d E / d d_e through the radial basis (w_ab weights and, unless a bond row fed by Q, M.be): each warpgroup sums
+       // sum_j gpre[r][j] M[j][k] over its 64 columns from the gpre values in registers
+      float sk[AR][9];
 #pragma unroll
-      for (int k = 0; k < 9; k++) sk[k] = 0.f;
-      const bool viaM = r < nvalid && !(useQ && s_bond[r] >= 0);
-      if (viaM) {
-#pragma unroll 4
-        for (int jq = 0; jq < 16; jq++) {
-          const float4 p = *reinterpret_cast<const float4*>(&tileP[r * LD + 64 * h + 4 * jq]);
-          const float* Mq = Msm + (64 * h + 4 * jq) * 9;
+      for (int i = 0; i < AR; i++)
 #pragma unroll
-          for (int k = 0; k < 9; k++) {
-            float v = sk[k];
-            v = fmaf(p.x, Mq[k], v);
-            v = fmaf(p.y, Mq[9 + k], v);
-            v = fmaf(p.z, Mq[18 + k], v);
-            v = fmaf(p.w, Mq[27 + k], v);
-            sk[k] = v;
-          }
-        }
+        for (int k = 0; k < 9; k++) sk[i][k] = 0.f;
+#pragma unroll
+      for (int j = 0; j < AC; j++) {
+        float mk[9];
+        ld9(Msm + (c0 + m.col(j)) * 12, mk);
+#pragma unroll
+        for (int i = 0; i < AR; i++)
+#pragma unroll
+          for (int k = 0; k < 9; k++) sk[i][k] = fmaf(acc[i][j], mk[k], sk[i][k]);
       }
-      if (h == 1) {
+      float skr[9];
+      quad_reduce_half(reinterpret_cast<const float(&)[2][9]>(sk[0]), 0, skr);
+      quad_reduce_half(reinterpret_cast<const float(&)[2][9]>(sk[2]), 1, skr);
+      const int r = m.row(tid & 3);
+      const bool viaM = r < nvalid && !(useQ && s_bond[r] >= 0);
 #pragma unroll
-        for (int k = 0; k < 9; k++) be_s[r * 12 + k] = sk[k];  // be_s is free until the next tile
+      for (int k = 0; k < 9; k++) skr[k] = viaM ? skr[k] : 0.f;
+      if (m.branch == 1) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) be_s[r * 12 + k] = skr[k];  // be_s is free until the next tile
       }
       __syncthreads();
-      if (h == 0 && r < nvalid) {
+      if (m.branch == 0 && r < nvalid) {
         float part = 0.f;
 #pragma unroll
-        for (int k = 0; k < 9; k++) part = fmaf(gws[r * 12 + k] + (sk[k] + be_s[r * 12 + k]), dbe_s[r * 12 + k], part);
+        for (int k = 0; k < 9; k++) part = fmaf(gwr[k] + (skr[k] + be_s[r * 12 + k]), dbe_s[r * 12 + k], part);
         a.gd[e0 + r] += part;
       }
     }
@@ -824,10 +939,10 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
       if (useQ && a.gQ != nullptr) {
         for (int i = 0; i < 64; i++) {
           const int r = rh + 2 * i;
-          if (r < nvalid && s_bond[r] >= 0) a.gQ[(size_t)s_bond[r] * D2 + j] = tileP[r * LD + j];
+          if (r < nvalid && s_bond[r] >= 0) a.gQ[(size_t)s_bond[r] * D2 + j] = tileP[r * LDE + j];
         }
       }
-      if (a.gA != nullptr) seg_flush(tileP, LD, j, rh * 64, rh * 64 + 64, s_dst, a.gC, D2);
+      if (a.gA != nullptr) seg_flush(tileP, LDE, j, rh * 64, rh * 64 + 64, s_dst, a.gC, D2);
     }
     if (a.gA != nullptr) {  // gA[src] += gpre: a 4-wide reduction per (row, column quad), a warp per row
       const int q = tid & 31, rg = tid >> 5;
@@ -835,7 +950,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
       for (int i = 0; i < TM / 8; i++) {
         const int r = rg + 8 * i;
         if (r < nvalid)
-          red_add_v4(&a.gA[(size_t)s_src[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&tileP[r * LD + 4 * q]));
+          red_add_v4(&a.gA[(size_t)s_src[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&tileP[r * LDE + 4 * q]));
       }
     }
   }
