@@ -279,28 +279,35 @@ static std::vector<float> canon_split(const std::vector<float>& raw, int N, int 
   return o;
 }
 
-// both 64-row branches (L then G) of a stacked [128][64] block as wgmma B operands of the fused kernels:
-// per branch canon_split of B[n][k] = raw[br*64 + n][k] (transposed = false) or raw[br*64 + k][n] (true).
-// permute_k: k slot q of every 8-wide k block holds column 2q and slot q + 4 column 2q + 1 -- the atom-conv kernels
-// pass their wgmma accumulator fragments (columns 2 (l%4), 2 (l%4) + 1 of a block) as the register A fragment (k slots
-// l%4, l%4 + 4) of the next product (kernels.cu: wg_mm64_acc)
-static std::vector<float> second_layer_can(const std::vector<float>& raw128x64, bool transposed, bool permute_k) {
+// raw [N][K] with k permuted inside every 8-wide k block: slot q holds column 2q and slot q + 4 column 2q + 1.  The
+// fused kernels pass A as float2 pairs (columns 2 (l%4), 2 (l%4) + 1 of a block), from their wgmma accumulator
+// fragments or from a shared-memory tile, as the register A fragment (k slots l%4, l%4 + 4) of the product
+// (kernels.cu: wg_mm64_acc, wg_mm64), so every fused-kernel B image is formatted this way.
+static std::vector<float> permute_k8(const std::vector<float>& raw, int N, int K) {
+  std::vector<float> o(raw.size());
+  for (int n = 0; n < N; n++)
+    for (int k = 0; k < K; k++) {
+      const int q = k % 8;
+      o[(size_t)n * K + k] = raw[(size_t)n * K + (k - q) + (q < 4 ? 2 * q : 2 * (q - 4) + 1)];
+    }
+  return o;
+}
+
+// both 64-row branches (L then G) of a stacked [128][64] block as k-permuted wgmma B operands of the fused kernels:
+// per branch canon_split of B[n][k] = raw[br*64 + n][k] (transposed = false) or raw[br*64 + k][n] (true)
+static std::vector<float> second_layer_can(const std::vector<float>& raw128x64, bool transposed) {
   std::vector<float> out;
   for (int br = 0; br < 2; br++) {
     std::vector<float> blk(raw128x64.begin() + (size_t)br * 4096, raw128x64.begin() + (size_t)(br + 1) * 4096);
     if (transposed) blk = transpose(blk, 64, 64);
-    if (permute_k) {
-      const std::vector<float> b = blk;
-      for (int n = 0; n < 64; n++)
-        for (int k = 0; k < 64; k++) {
-          const int q = k % 8;
-          blk[(size_t)n * 64 + k] = b[(size_t)n * 64 + (k - q) + (q < 4 ? 2 * q : 2 * (q - 4) + 1)];
-        }
-    }
-    const auto c = canon_split(blk, 64, 64, 64);
+    const auto c = canon_split(permute_k8(blk, 64, 64), 64, 64, 64);
     out.insert(out.end(), c.begin(), c.end());
   }
   return out;
+}
+// the [128][64] first-layer block W as the k-permuted B operand of gpre . W (K = 128): B[n][k] = W[k][n]
+static std::vector<float> line_reverse_can(const std::vector<float>& raw128x64) {
+  return canon_split(permute_k8(transpose(raw128x64, 128, 64), 64, 128), 64, 128, 128);
 }
 
 static void finalize_weights(b2m_engine* e) {
@@ -386,8 +393,8 @@ static void finalize_weights(b2m_engine* e) {
     put(q + "W1e_raw", W1e);
     put(q + "W1t_raw", W1t);
     put(q + "M", M);
-    put(q + "W2can", second_layer_can(W2, false, true));
-    put(q + "W2Tcan", second_layer_can(W2, true, true));
+    put(q + "W2can", second_layer_can(W2, false));
+    put(q + "W2Tcan", second_layer_can(W2, true));
     put(q + "b2", b2);
     put(q + "Wout_k", transpose(Wout, 64, 64));
     put(q + "Wout_raw", Wout);
@@ -415,26 +422,26 @@ static void finalize_weights(b2m_engine* e) {
     put(q + "W1a_k", transpose(W1a, 128, 64));
     put(q + "W1b_k", transpose(W1b, 128, 64));
     put(q + "W1c_k", transpose(W1c, 128, 64));
-    put(q + "Wgcan", second_layer_can(W1g, false, false));
+    put(q + "Wgcan", second_layer_can(W1g, false));
     put(q + "b1", b1);
     put(q + "W1a_raw", W1a);
     put(q + "W1b_raw", W1b);
     put(q + "W1c_raw", W1c);
-    put(q + "WgTcan", canon_split(transpose(W1g, 128, 64), 64, 128, 128));
-    put(q + "W2can", second_layer_can(W2, false, false));
-    put(q + "W2Tcan", second_layer_can(W2, true, false));
+    put(q + "WgTcan", line_reverse_can(W1g));
+    put(q + "W2can", second_layer_can(W2, false));
+    put(q + "W2Tcan", second_layer_can(W2, true));
     put(q + "b2", b2);
     put(q + "Wout_k", transpose(Wout, 64, 64));
     put(q + "Wout_raw", Wout);
     put(q + "WAa_k", transpose(WAa, 128, 64));
     put(q + "WAb_k", transpose(WAb, 128, 64));
     put(q + "WAc_k", transpose(WAc, 128, 64));
-    put(q + "WAgcan", second_layer_can(WAg, false, false));
+    put(q + "WAgcan", second_layer_can(WAg, false));
     put(q + "bA", bA);
     put(q + "WAa_raw", WAa);
     put(q + "WAb_raw", WAb);
     put(q + "WAc_raw", WAc);
-    put(q + "WAgTcan", canon_split(transpose(WAg, 128, 64), 64, 128, 128));
+    put(q + "WAgTcan", line_reverse_can(WAg));
   }
   const auto& F0 = W(e, "final_layer.layers.0.weight", {D, D});
   const auto& F1 = W(e, "final_layer.layers.1.weight", {D, D});

@@ -107,26 +107,23 @@ struct Map {
   __device__ __forceinline__ int col(int j) const { return 8 * (j >> 1) + cb + (j & 1); }
 };
 
-// d = (accumulate ? d : 0) + At[row0 .. row0+63][acol .. acol+64) . B[0..63][bk .. bk+64)^T on the tensor cores
-// (warpgroup-collective), 3xTF32 (hi.hi + lo.hi + hi.lo, fp32 accumulate).  At: fp32 in shared memory, row pitch lda
-// (A fragments are read into registers: lda % 32 == 4 keeps the 32 lanes on 32 banks); B: canonical K-major
-// [64 n][K k] image in shared memory, tf32 hi plane at b_hi and lo plane at b_lo.
-__device__ __forceinline__ void wg_mm64(const float* At, int lda, int row0, int acol, uint32_t b_hi, uint32_t b_lo,
-                                        int bk, bool accumulate, float (&d)[32]) {
+// d = (accumulate ? d : 0) + A . B[0..63][bk .. bk+64)^T on the tensor cores (warpgroup-collective), 3xTF32 (hi.hi +
+// lo.hi + hi.lo, fp32 accumulate).  x[ks]: this thread's fp32 A fragment of k block ks in the instruction's order
+// (rows 16 w + l/4 and + 8 of the 64-row block, k slots l%4 and l%4 + 4).  B: canonical K-major [64 n][K k] image in
+// shared memory, tf32 hi plane at b_hi and lo plane at b_lo, k permuted inside each block of 8 (slot q <- column 2q,
+// slot q + 4 <- column 2q + 1; engine.cu: permute_k8), so that slots l%4 and l%4 + 4 take A's columns 8 ks + 2 (l%4)
+// and + 1: the pair a thread holds in the accumulator layout, or reads from a tile as one float2.
+__device__ __forceinline__ void wg_mma64(const float (&x)[8][4], uint32_t b_hi, uint32_t b_lo, int bk, bool accumulate,
+                                         float (&d)[32]) {
   constexpr uint32_t LBO = 8 * 128;  // byte step between core matrices along K (N = 64)
-  const int lane = threadIdx.x & 31;
-  const float* p0 = At + (row0 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2)) * lda + acol + (lane & 3);
-  const float* p1 = p0 + 8 * lda;
   uint32_t ah[8][4], al[8][4];
 #pragma unroll
-  for (int ks = 0; ks < 8; ks++) {
-    const float x[4] = {p0[8 * ks], p1[8 * ks], p0[8 * ks + 4], p1[8 * ks + 4]};
+  for (int ks = 0; ks < 8; ks++)
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      ah[ks][q] = tf32_hi_bits(x[q]);
-      al[ks][q] = __float_as_uint(x[q] - __uint_as_float(ah[ks][q]));
+      ah[ks][q] = tf32_hi_bits(x[ks][q]);
+      al[ks][q] = __float_as_uint(x[ks][q] - __uint_as_float(ah[ks][q]));
     }
-  }
   const uint32_t koff = (uint32_t)(bk / 4) * LBO;
   acc_fence(d);
   wgmma_fence();
@@ -141,6 +138,23 @@ __device__ __forceinline__ void wg_mm64(const float* At, int lda, int row0, int 
   wgmma_commit();
   wgmma_wait_all();
   acc_fence(d);
+}
+
+// d = (accumulate ? d : 0) + At[row0 .. row0+63][acol .. acol+64) . B[0..63][bk .. bk+64)^T (wg_mma64).  At: fp32 in
+// shared memory, row pitch lda; each k pair is one float2 read, and lda % 32 == 8 puts the 8 rows x 4 pairs of a
+// half-warp on 32 distinct banks.
+__device__ __forceinline__ void wg_mm64(const float* At, int lda, int row0, int acol, uint32_t b_hi, uint32_t b_lo,
+                                        int bk, bool accumulate, float (&d)[32]) {
+  const int lane = threadIdx.x & 31;
+  const float* p0 = At + (row0 + ((threadIdx.x & 127) >> 5) * 16 + (lane >> 2)) * lda + acol + 2 * (lane & 3);
+  const float* p1 = p0 + 8 * lda;
+  float x[8][4];
+#pragma unroll
+  for (int ks = 0; ks < 8; ks++) {
+    const float2 u = *reinterpret_cast<const float2*>(p0 + 8 * ks), v = *reinterpret_cast<const float2*>(p1 + 8 * ks);
+    x[ks][0] = u.x, x[ks][1] = v.x, x[ks][2] = u.y, x[ks][3] = v.y;
+  }
+  wg_mma64(x, b_hi, b_lo, bk, accumulate, d);
 }
 
 // acc (Map layout) = At[0..127][kofs .. kofs+64) . B^T for this thread's branch; Bcan: the branch's canonical image
@@ -406,7 +420,7 @@ void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats) {
 // (the hidden columns its branch's second layer reads) and the branch's 64 outputs, and a thread owns 4 rows x 16
 // columns of both.  Such a thread touches the tile only at its own positions (row(i), 64 b + col(j)), as float2 pairs
 // (col(2 jj), col(2 jj) + 1); the pitch LDE = 136 (8 mod 32 floats) puts the 8 rows x 4 pairs of a half-warp on 32
-// distinct banks.
+// distinct banks.  The line-graph tiles use the same pitch and layout.
 constexpr int LDE = 136;
 
 struct EdgeRow {
@@ -514,38 +528,19 @@ __device__ __forceinline__ void first_layer_half(const AtomConvArgs& a, const Ma
   }
 }
 
-// acc rows of half h (2h, 2h + 1) = x rows of half h . B^T on the tensor cores (warpgroup-collective), 3xTF32 (hi.hi +
-// lo.hi + hi.lo, fp32 accumulate).  x is in the accumulator layout and is the register A fragment as it stands: in k
-// block ks a thread holds columns 8 ks + 2 (l%4) and + 1, which fill the fragment's k slots l%4 and l%4 + 4.  So B (the
-// branch's canonical image, hi plane of 4096 floats, then lo) has its k index permuted within each block of 8 (slot q
-// <- column 2q, slot q + 4 <- column 2q + 1; engine.cu: second_layer_can).  x and acc may be the same array.
+// acc rows of half h (2h, 2h + 1) = x rows of half h . B^T (wg_mma64).  x is in the accumulator layout and is the
+// register A fragment as it stands: in k block ks a thread holds columns 8 ks + 2 (l%4) and + 1.  Bcan: the branch's
+// k-permuted canonical image (hi plane of 4096 floats, then lo).  x and acc may be the same array.
 __device__ __forceinline__ void wg_mm64_acc(const float (&x)[AR][AC], int h, const float* Bcan, float (&acc)[AR][AC]) {
-  constexpr uint32_t LBO = 8 * 128;  // byte step between core matrices along K (N = 64)
-  const uint32_t b_hi = s_u32(Bcan), b_lo = b_hi + 4096u * 4u;
-  uint32_t ah[8][4], al[8][4];
+  float v[8][4];
 #pragma unroll
   for (int ks = 0; ks < 8; ks++) {
-    const float v[4] = {x[2 * h][2 * ks], x[2 * h + 1][2 * ks], x[2 * h][2 * ks + 1], x[2 * h + 1][2 * ks + 1]};
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      ah[ks][q] = tf32_hi_bits(v[q]);
-      al[ks][q] = __float_as_uint(v[q] - __uint_as_float(ah[ks][q]));
-    }
+    v[ks][0] = x[2 * h][2 * ks], v[ks][1] = x[2 * h + 1][2 * ks];
+    v[ks][2] = x[2 * h][2 * ks + 1], v[ks][3] = x[2 * h + 1][2 * ks + 1];
   }
+  const uint32_t b_hi = s_u32(Bcan);
   float d[32];
-  acc_fence(d);
-  wgmma_fence();
-#pragma unroll
-  for (int ks = 0; ks < 8; ks++) {
-#pragma unroll
-    for (int term = 0; term < 3; term++) {
-      const uint64_t bd = gmma_desc((term == 2 ? b_lo : b_hi) + ks * 2 * LBO, LBO, 128u);
-      wgmma_tf32_n64_rA(d, term == 1 ? al[ks] : ah[ks], bd, (ks > 0 || term > 0) ? 1 : 0);
-    }
-  }
-  wgmma_commit();
-  wgmma_wait_all();
-  acc_fence(d);
+  wg_mma64(v, b_hi, b_hi + 4096u * 4u, 0, false, d);
 #pragma unroll
   for (int q = 0; q < 32; q++) acc[2 * h + ((q >> 1) & 1)][2 * (q >> 2) + (q & 1)] = d[q];
 }
@@ -970,15 +965,20 @@ void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
 // ============================================================================================
 // line-graph kernels: bond conv (HIDDEN) and angle update (!HIDDEN)
 // ============================================================================================
-// Persistent like the atom conv: min(tiles, SMs) CTAs, CTA c takes tiles c, c + grid, ...  Two [TM][LD] buffers
+// Persistent like the atom conv: min(tiles, SMs) CTAs, CTA c takes tiles c, c + grid, ...  Two [TM][LDE] buffers
 // alternate: tile number `it` of a CTA has its Ha[a] rows in buffer it & 1 (P) and its own angle rows in columns
-// 64..127 of the other buffer (Q; pitch LD, so the A fragments of ang.Wg^T read conflict-free).  Each copy completes on
-// the barrier of its tile's stage (hbar / abar [it & 1], parity stage_parity(it)).  One 64 KB weight slot holds the
-// image the next product needs; images that share it are refilled by bulk copies as soon as the product before has
-// read the slot, and waited on (wbar, one phase per fill, in fill order) just before the product that reads them.
+// 64..127 of the other buffer (Q).  Each copy completes on the barrier of its tile's stage (hbar / abar [it & 1], parity
+// stage_parity(it)).  One 64 KB weight slot holds the image the next product needs; images that share it are refilled
+// by bulk copies as soon as the product before has read the slot, and waited on (wbar, one phase per fill, in fill
+// order) just before the product that reads them.
+//
+// Every per-element phase works in the accumulator layout (Map), as in the atom conv: a thread touches the tiles only at
+// its own positions (row(i), 64 b + col(j)), as float2 pairs, and the A operands of the products are either its
+// accumulator fragments (hid . W2^T, g . W2) or float2 pairs of a tile (ang . Wg^T, gpre . Wg; wg_mm64).  All B images
+// are k-permuted (engine.cu: permute_k8).
 struct LineSmem {
-  static constexpr int kBuf = 32;              // two [TM][LD] buffers (first 128 B: hbar[2], abar[2], wbar)
-  static constexpr int kW = kBuf + 2 * TM * LD;  // one weight image (2 branches x hi | lo, or Wg^T hi | lo)
+  static constexpr int kBuf = 32;               // two [TM][LDE] buffers (first 128 B: hbar[2], abar[2], wbar)
+  static constexpr int kW = kBuf + 2 * TM * LDE;  // one weight image (2 branches x hi | lo, or Wg^T hi | lo)
   static constexpr int kB2 = kW + 16384;
   static constexpr int kIdx = kB2 + 128;       // a_in, a_out, a_ctr: [2][TM] each
   static constexpr int kTotal = kIdx + 6 * TM;
@@ -991,7 +991,7 @@ struct LineSm {
   __device__ __forceinline__ uint64_t* hbar() const { return reinterpret_cast<uint64_t*>(smem); }
   __device__ __forceinline__ uint64_t* abar() const { return hbar() + 2; }
   __device__ __forceinline__ uint64_t* wbar() const { return hbar() + 4; }
-  __device__ __forceinline__ float* buf(int s) const { return smem + LineSmem::kBuf + s * TM * LD; }
+  __device__ __forceinline__ float* buf(int s) const { return smem + LineSmem::kBuf + s * TM * LDE; }
   __device__ __forceinline__ float* W() const { return smem + LineSmem::kW; }
   __device__ __forceinline__ float* b2() const { return smem + LineSmem::kB2; }
   __device__ __forceinline__ int* idx(int s, int k) const {  // k: 0 a_in, 1 a_out, 2 a_ctr
@@ -1021,7 +1021,7 @@ __device__ __forceinline__ void line_issue_ha(const LineArgs& a, const LineSm& s
     sm.idx(s, 0)[tid] = x.a;
     sm.idx(s, 1)[tid] = x.b;
     sm.idx(s, 2)[tid] = x.c;
-    if (x.a >= 0) bulk_g2s(buf + tid * LD, a.Ha + (size_t)x.a * D2, 512u, &sm.hbar()[s]);
+    if (x.a >= 0) bulk_g2s(buf + tid * LDE, a.Ha + (size_t)x.a * D2, 512u, &sm.hbar()[s]);
   }
 }
 // the 256 B angle rows of tile t into columns 64..127 of `buf`, completing on abar[s]
@@ -1029,7 +1029,7 @@ __device__ __forceinline__ void line_issue_ang(const LineArgs& a, const LineSm& 
   const int tid = threadIdx.x;
   const int nvalid = (int)min((int64_t)TM, a.A - t * TM);
   if (tid == 0) mbar_expect_tx(&sm.abar()[s], (uint32_t)nvalid * 256u);
-  if (tid < nvalid) bulk_g2s(buf + tid * LD + 64, a.ang + (size_t)(t * TM + tid) * D, 256u, &sm.abar()[s]);
+  if (tid < nvalid) bulk_g2s(buf + tid * LDE + 64, a.ang + (size_t)(t * TM + tid) * D, 256u, &sm.abar()[s]);
 }
 // barriers, b2, the first weight image and the copies of the CTA's first tile (Ha into buffer 0, angles into buffer 1)
 __device__ __forceinline__ AngleIdx line_prologue(const LineArgs& a, const LineSm& sm) {
@@ -1047,31 +1047,37 @@ __device__ __forceinline__ AngleIdx line_prologue(const LineArgs& a, const LineS
   return angle_idx(a, ((int64_t)blockIdx.x + gridDim.x) * TM + tid);
 }
 
-// pre = Ha[a] (in tile P) + ang.Wg^T (acc) + Hb[b] + Xc[c] on this thread's accumulator elements, handed to f(i, j, pre)
-// (rows r >= nvalid: f(i, j, 0)).  A row's 16 Hb and 16 Xc values are loaded as float2 pairs before any is used.
-template <class F>
+// pre = ((Ha[a] + ang.Wg^T) + Hb[b]) + Xc[c] in place of acc (which holds ang.Wg^T), in the accumulator layout: Ha from
+// P at the thread's own positions, a row's 16 Hb and 16 Xc values as float2 loads issued before any is used.  Rows
+// r >= nvalid get 0.
 __device__ __forceinline__ void line_first_layer(const LineArgs& a, const Map& m, const float* P, const int* s_b,
-                                                 const int* s_c, int nvalid, const float (&acc)[AR][AC], F&& f) {
+                                                 const int* s_c, int nvalid, float (&acc)[AR][AC]) {
+  const int c0 = 64 * m.branch + m.cb;
 #pragma unroll
   for (int i = 0; i < AR; i++) {
     const int r = m.row(i);
     const bool ok = r < nvalid;
-    const float* hb = a.Hb + (size_t)(ok ? s_b[r] : 0) * D2 + m.branch * 64;
-    const float* xc = a.Xc + (size_t)(ok ? s_c[r] : 0) * D2 + m.branch * 64;
+    const float* hb = a.Hb + (size_t)(ok ? s_b[r] : 0) * D2 + c0;
+    const float* xc = a.Xc + (size_t)(ok ? s_c[r] : 0) * D2 + c0;
     float2 hv[AC / 2], xv[AC / 2];
 #pragma unroll
     for (int jj = 0; jj < AC / 2; jj++) {
-      hv[jj] = ok ? __ldg(reinterpret_cast<const float2*>(hb + m.col(2 * jj))) : make_float2(0.f, 0.f);
-      xv[jj] = ok ? __ldg(reinterpret_cast<const float2*>(xc + m.col(2 * jj))) : make_float2(0.f, 0.f);
+      hv[jj] = ok ? __ldg(reinterpret_cast<const float2*>(hb + 8 * jj)) : make_float2(0.f, 0.f);
+      xv[jj] = ok ? __ldg(reinterpret_cast<const float2*>(xc + 8 * jj)) : make_float2(0.f, 0.f);
     }
 #pragma unroll
-    for (int j = 0; j < AC; j++) {
-      const int col = m.branch * 64 + m.col(j);
-      float p = 0.f;
-      if (ok) p = P[r * LD + col] + acc[i][j] + ((j & 1) ? hv[j >> 1].y : hv[j >> 1].x) + ((j & 1) ? xv[j >> 1].y : xv[j >> 1].x);
-      f(i, j, p);
+    for (int jj = 0; jj < AC / 2; jj++) {
+      const float2 ha = ok ? ld_f2(P + r * LDE + c0 + 8 * jj) : make_float2(0.f, 0.f);
+      float& x0 = acc[i][2 * jj];
+      float& x1 = acc[i][2 * jj + 1];
+      x0 = ok ? ha.x + x0 + hv[jj].x + xv[jj].x : 0.f;
+      x1 = ok ? ha.y + x1 + hv[jj].y + xv[jj].y : 0.f;
     }
   }
+}
+
+__device__ __forceinline__ void red_add_v2(float* p, float x, float y) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(x), "f"(y) : "memory");
 }
 
 template <bool HIDDEN>
@@ -1100,7 +1106,7 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
     mbar_wait(&sm.abar()[s], stage_parity(it));
     mbar_wait(sm.wbar(), wpar);  // Wg
     if (HIDDEN) wpar ^= 1;       // (!HIDDEN: Wg stays, its only phase is complete)
-    gemm64(Q, LD, 64, sm.W() + m.branch * 8192, acc);
+    gemm64(Q, LDE, 64, sm.W() + m.branch * 8192, acc);
     fence_proxy_async_smem();  // this thread's generic accesses of Q come before its bulk refill
     __syncthreads();           // Q (angle rows, the previous tile's gates) and its index arrays are free; so is Wg
     if (more) {
@@ -1109,19 +1115,17 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
     }
     if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.W2can, 16384 * 4, sm.wbar());
     mbar_wait(&sm.hbar()[s], stage_parity(it));
-    line_first_layer(a, m, P, s_b, s_c, nvalid, acc, [&](int i, int j, float p) {
-      if (HIDDEN) {
-        P[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.row(i) < nvalid ? silu_f(p) : 0.f;
-      } else {
-        acc[i][j] = m.branch == 0 ? silu_f(p) : sigm(p);
-      }
-    });
-    fence_proxy_async_smem();
-    __syncthreads();  // (!HIDDEN: the Ha rows in P have been read, its columns 64..127 are free)
+    line_first_layer(a, m, P, s_b, s_c, nvalid, acc);
+    // HIDDEN: hid = silu(pre) straight into the second layer;  !HIDDEN: pre is the last layer's pre-activation
+#pragma unroll
+    for (int i = 0; i < AR; i++)
+#pragma unroll
+      for (int j = 0; j < AC; j++) acc[i][j] = HIDDEN || m.branch == 0 ? silu_f(acc[i][j]) : sigm(acc[i][j]);
     if (HIDDEN) {
       mbar_wait(sm.wbar(), wpar);  // W2
       wpar ^= 1;
-      gemm64(P, LD, m.branch * 64, sm.W() + m.branch * 8192, acc);
+      wg_mm64_acc(acc, 0, sm.W() + m.branch * 8192, acc);
+      wg_mm64_acc(acc, 1, sm.W() + m.branch * 8192, acc);
 #pragma unroll
       for (int i = 0; i < AR; i++)
 #pragma unroll
@@ -1129,18 +1133,19 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
           const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
           acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
         }
-      fence_proxy_async_smem();
-      __syncthreads();  // columns 64..127 of P are free (and so is W2)
     }
+    fence_proxy_async_smem();  // this thread's generic accesses of P come before its bulk refill
+    __syncthreads();           // the Ha rows in P have been read, its columns 64..127 are free (HIDDEN: and so is W2)
     if (more) {
       line_issue_ang(a, sm, t + step, P, s ^ 1);
       if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.Wgcan, 16384 * 4, sm.wbar());
     }
+    // m = L . G: warpgroup 1 hands G over through columns 0..63 of P, at the positions warpgroup 0 owns as well
     if (m.branch == 1) {
 #pragma unroll
       for (int i = 0; i < AR; i++)
 #pragma unroll
-        for (int j = 0; j < AC; j++) P[m.row(i) * LD + m.col(j)] = acc[i][j];
+        for (int jj = 0; jj < AC / 2; jj++) st_f2(P + m.row(i) * LDE + m.col(2 * jj), acc[i][2 * jj], acc[i][2 * jj + 1]);
     }
     __syncthreads();
     if (m.branch == 0) {
@@ -1149,7 +1154,11 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
         const int r = m.row(i);
         if (HIDDEN) {
 #pragma unroll
-          for (int j = 0; j < AC; j++) P[r * LD + m.col(j)] = acc[i][j] * P[r * LD + m.col(j)];
+          for (int jj = 0; jj < AC / 2; jj++) {
+            float* p = P + r * LDE + m.col(2 * jj);
+            const float2 g = ld_f2(p);
+            st_f2(p, acc[i][2 * jj] * g.x, acc[i][2 * jj + 1] * g.y);
+          }
         } else if (r < nvalid) {  // ang_out = ang + m, the angle rows re-read (L2) as float2 pairs
           const float* ang = a.ang + (size_t)(r0 + r) * D;
           float* out = a.ang_out + (size_t)(r0 + r) * D;
@@ -1159,9 +1168,8 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
 #pragma unroll
           for (int jj = 0; jj < AC / 2; jj++) {
             const int c = m.col(2 * jj);
-            const float2 v = make_float2(av[jj].x + acc[i][2 * jj] * P[r * LD + c],
-                                         av[jj].y + acc[i][2 * jj + 1] * P[r * LD + c + 1]);
-            *reinterpret_cast<float2*>(out + c) = v;
+            const float2 g = ld_f2(P + r * LDE + c);
+            st_f2(out + c, av[jj].x + acc[i][2 * jj] * g.x, av[jj].y + acc[i][2 * jj + 1] * g.y);
           }
         }
       }
@@ -1169,14 +1177,16 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
     if (HIDDEN) {
       __syncthreads();
       const int c = tid & 63, part = tid >> 6;
-      seg_flush(P, LD, c, part * 32, part * 32 + 32, s_b, a.aggB, D);
+      seg_flush(P, LDE, c, part * 32, part * 32 + 32, s_b, a.aggB, D);
     }
   }
 }
 
-// Backward: P (buffer it & 1) holds the tile's Ha rows, then its pre-activations, then their adjoints; H (the other
-// buffer) holds the angle rows, then the hidden activations and the second-layer adjoints.  Once H has been read for the
-// last time (HIDDEN: by g.W2, !HIDDEN: by the elementwise reverse), the next tile's Ha rows are copied into it (H becomes
+// Backward, mirroring the atom conv: P (buffer it & 1) holds the tile's Ha rows, then (HIDDEN) its pre-activations,
+// each thread's over its own Ha values, then their adjoints gpre, which the scatter phase and gpre.Wg read row-major;
+// H (the other buffer) holds the angle rows, then the branch activations the two warpgroups exchange.  Both products of
+// the hidden layer take their A operand from registers.  Once H has been read for the last time (by the elementwise
+// reverse), the next tile's Ha rows are copied into it (H becomes
 // the next tile's P); once the scatter phase and gang += gpre.Wg have read P, the next tile's angle rows go into its
 // columns 64..127 (P becomes the next tile's H).  Weight images through the one slot: HIDDEN Wg -> W2 -> W2^T -> Wg^T
 // per tile, !HIDDEN Wg -> Wg^T.
@@ -1206,38 +1216,42 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
     mbar_wait(&sm.abar()[s], stage_parity(it));
     mbar_wait(sm.wbar(), wpar);  // Wg
     wpar ^= 1;
-    gemm64(H, LD, 64, sm.W() + m.branch * 8192, acc);
+    gemm64(H, LDE, 64, sm.W() + m.branch * 8192, acc);
     __syncthreads();  // both warpgroups have read the angle rows and Wg: H and the slot may be written
     if (tid == 0) bulk_g2s_image(sm.W(), HIDDEN ? a.W2can : a.WgTcan, 16384 * 4, sm.wbar());
     mbar_wait(&sm.hbar()[s], stage_parity(it));
-    line_first_layer(a, m, P, s_b, s_c, nvalid, acc, [&](int i, int j, float p) {
-      if (HIDDEN) {
-        const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
-        P[idx] = p;
-        H[idx] = m.row(i) < nvalid ? silu_f(p) : 0.f;
-      } else {
-        acc[i][j] = p;
-      }
-    });
-    __syncthreads();
+    line_first_layer(a, m, P, s_b, s_c, nvalid, acc);
     if (HIDDEN) {
+      // pre overwrites the thread's own Ha values in P (same thread, same addresses); silu(pre) . W2^T + b2 = u | v
+#pragma unroll
+      for (int i = 0; i < AR; i++)
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++) {
+          float& x0 = acc[i][2 * jj];
+          float& x1 = acc[i][2 * jj + 1];
+          st_f2(P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), x0, x1);
+          x0 = silu_f(x0);
+          x1 = silu_f(x1);
+        }
       mbar_wait(sm.wbar(), wpar);  // W2
       wpar ^= 1;
-      gemm64(H, LD, m.branch * 64, sm.W() + m.branch * 8192, acc);
+      wg_mm64_acc(acc, 0, sm.W() + m.branch * 8192, acc);
+      wg_mm64_acc(acc, 1, sm.W() + m.branch * 8192, acc);
 #pragma unroll
       for (int i = 0; i < AR; i++)
 #pragma unroll
         for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
-      __syncthreads();  // H and W2 have been read
+      __syncthreads();  // W2 has been read
       if (tid == 0) bulk_g2s_image(sm.W(), a.W2Tcan, 16384 * 4, sm.wbar());
     }
-    // acc = pre-activation of the last layer of this GatedMLP (u | v).  Exchange activations.
+    // acc = pre-activation of the last layer of this GatedMLP (u | v).  Exchange activations through H.
 #pragma unroll
     for (int i = 0; i < AR; i++)
 #pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const float u = acc[i][j];
-        H[m.row(i) * LD + m.branch * 64 + m.col(j)] = m.branch == 0 ? silu_f(u) : sigm(u);
+      for (int jj = 0; jj < AC / 2; jj++) {
+        const float u0 = acc[i][2 * jj], u1 = acc[i][2 * jj + 1];
+        st_f2(H + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), m.branch == 0 ? silu_f(u0) : sigm(u0),
+              m.branch == 0 ? silu_f(u1) : sigm(u1));
       }
     __syncthreads();
 #pragma unroll
@@ -1252,9 +1266,9 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
         gm2[jj] = ok ? *reinterpret_cast<const float2*>(gsrc + m.col(2 * jj)) : make_float2(0.f, 0.f);
 #pragma unroll
       for (int j = 0; j < AC; j++) {
-        const int c = m.col(j);
         const float u = acc[i][j];
-        const float po = H[r * LD + (1 - m.branch) * 64 + c];
+        const float2 po2 = ld_f2(H + r * LDE + (1 - m.branch) * 64 + m.col(j & ~1));  // partner activations
+        const float po = (j & 1) ? po2.y : po2.x;
         float g = 0.f;
         if (ok) {
           const float gm = (j & 1) ? gm2[j >> 1].y : gm2[j >> 1].x;
@@ -1269,28 +1283,26 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
         acc[i][j] = g;
       }
     }
-    __syncthreads();
     if (HIDDEN) {
-#pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int j = 0; j < AC; j++) H[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+      // ghid = [gu . W2L, gv . W2G] from the adjoints in registers;  gpre = ghid * dsilu(pre), into P over pre
       mbar_wait(sm.wbar(), wpar);  // W2^T
       wpar ^= 1;
-      __syncthreads();
-      gemm64(H, LD, m.branch * 64, sm.W() + m.branch * 8192, acc);
+      wg_mm64_acc(acc, 0, sm.W() + m.branch * 8192, acc);
+      wg_mm64_acc(acc, 1, sm.W() + m.branch * 8192, acc);
 #pragma unroll
       for (int i = 0; i < AR; i++)
 #pragma unroll
-        for (int j = 0; j < AC; j++) {
-          const int idx = m.row(i) * LD + m.branch * 64 + m.col(j);
-          P[idx] = acc[i][j] * dsilu_f(P[idx]);
+        for (int jj = 0; jj < AC / 2; jj++) {
+          float* p = P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj);
+          const float2 pre = ld_f2(p);
+          st_f2(p, acc[i][2 * jj] * dsilu_f(pre.x), acc[i][2 * jj + 1] * dsilu_f(pre.y));
         }
     } else {
 #pragma unroll
       for (int i = 0; i < AR; i++)
 #pragma unroll
-        for (int j = 0; j < AC; j++) P[m.row(i) * LD + m.branch * 64 + m.col(j)] = acc[i][j];
+        for (int jj = 0; jj < AC / 2; jj++)
+          st_f2(P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), acc[i][2 * jj], acc[i][2 * jj + 1]);
     }
     fence_proxy_async_smem();  // this thread's generic accesses of H come before its bulk refill
     __syncthreads();           // H, its stage's index arrays and (HIDDEN) W2^T are free; P holds gpre
@@ -1302,8 +1314,8 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
     // ---- scatter phase (reads P and this tile's index arrays) ----
     {
       const int j = tid & 127, rh = tid >> 7;
-      seg_flush(P, LD, j, rh * 64, rh * 64 + 64, s_b, a.gHb, D2);
-      seg_flush(P, LD, j, rh * 64, rh * 64 + 64, s_c, a.gXc, D2);
+      seg_flush(P, LDE, j, rh * 64, rh * 64 + 64, s_b, a.gHb, D2);
+      seg_flush(P, LDE, j, rh * 64, rh * 64 + 64, s_c, a.gXc, D2);
     }
     {  // gHa[a] += gpre: a 4-wide reduction per (row, column quad), a warp per row
       const int q = tid & 31, rg = tid >> 5;
@@ -1311,26 +1323,23 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
       for (int i = 0; i < TM / 8; i++) {
         const int r = rg + 8 * i;
         if (r < nvalid)
-          red_add_v4(&a.gHa[(size_t)s_a[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&P[r * LD + 4 * q]));
+          red_add_v4(&a.gHa[(size_t)s_a[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&P[r * LDE + 4 * q]));
       }
     }
-    // gang += gpre @ Wg   (K = 128, N = 64) on the tensor cores: warpgroup w takes rows 64 w .. 64 w + 63
+    // gang += gpre @ Wg   (K = 128, N = 64) on the tensor cores: warpgroup w takes rows 64 w .. 64 w + 63.  Each angle
+    // row belongs to this tile alone, and (!HIDDEN) its upstream reads of gang are behind the barrier above, so the
+    // update is a fire-and-forget reduction: one addition per element, as a load-add-store would do.
     mbar_wait(sm.wbar(), wpar);  // Wg^T
     wpar ^= 1;
     {
       float d[32];
       const uint32_t bh = s_u32(sm.W()), bl = bh + 64u * 128u * 4u;
-      wg_mm64(P, LD, 64 * m.branch, 0, bh, bl, 0, false, d);
-      wg_mm64(P, LD, 64 * m.branch, 64, bh, bl, 64, true, d);
+      wg_mm64(P, LDE, 64 * m.branch, 0, bh, bl, 0, false, d);
+      wg_mm64(P, LDE, 64 * m.branch, 64, bh, bl, 64, true, d);
 #pragma unroll
       for (int q = 0; q < 32; q += 2) {
         const int r = 64 * m.branch + m.rb + 8 * ((q >> 1) & 1), c = 8 * (q >> 2) + m.cb;
-        if (r < nvalid) {
-          float2* gp = reinterpret_cast<float2*>(&a.gang[(size_t)(r0 + r) * D + c]);
-          float2 v = *gp;
-          v.x += d[q], v.y += d[q + 1];
-          *gp = v;
-        }
+        if (r < nvalid) red_add_v2(&a.gang[(size_t)(r0 + r) * D + c], d[q], d[q + 1]);
       }
     }
     fence_proxy_async_smem();  // this thread's generic accesses of P come before its bulk refill

@@ -12,7 +12,6 @@
 namespace b2m {
 
 constexpr int TM = 128;   // rows (edges / angles) per tile
-constexpr int LD = 132;   // smem row pitch of a [TM][128] tile (16B aligned, 4-bank skew)
 constexpr int LDA = 68;   // smem row pitch of a [TM][64] tile
 constexpr int NT = 256;   // threads per block for the fused tile kernels
 
@@ -78,7 +77,8 @@ struct LineArgs {
   const float* Ha;    // [B_loc,128]
   const float* Hb;    // [B_own,128] (+bias folded)
   const float* Xc;    // [n_loc,128]
-  // wgmma B operands (canonical core-matrix images, tf32 hi plane then lo plane; engine.cu canon_split)
+  // wgmma B operands (canonical core-matrix images, tf32 hi plane then lo plane, k permuted inside every 8-wide k block;
+  // engine.cu second_layer_can / line_reverse_can)
   const float* Wgcan;   // per branch [64 n][64 k]: B[n][k] = Wg[br*64 + n][k]  (angle block of the first layer)
   const float* WgTcan;  // [64 n][128 k]: B[n][k] = Wg[k][n]                     (backward: gang += gpre . Wg)
   const float* W2can;   // hidden only, as AtomConvArgs
