@@ -75,12 +75,15 @@ static Nccl g_nccl;
   } while (0)
 
 // ------------------------------------------------------------------------------------------
+// row-GEMM weights as TcW pairs (the projection, then its transpose for the reverse pass); the fused-kernel images and
+// the biases as device pointers
 struct AtomLayerW {
-  float *W1s_k, *W1e_k, *W1t_k, *b1, *W1s_raw, *W1e_raw, *W1t_raw, *M, *W2can, *W2Tcan, *b2, *Wout_k, *Wout_raw;
+  TcW W1s, W1sT, W1e, W1eT, W1t, W1tT, Wout, WoutT;
+  float *b1, *M, *W2can, *W2Tcan, *b2;
 };
 struct BondLayerW {
-  float *W1a_k, *W1b_k, *W1c_k, *Wgcan, *b1, *W1a_raw, *W1b_raw, *W1c_raw, *WgTcan, *W2can, *W2Tcan, *b2, *Wout_k, *Wout_raw;
-  float *WAa_k, *WAb_k, *WAc_k, *WAgcan, *bA, *WAa_raw, *WAb_raw, *WAc_raw, *WAgTcan;
+  TcW W1a, W1aT, W1b, W1bT, W1c, W1cT, Wout, WoutT, WAa, WAaT, WAb, WAbT, WAc, WAcT;
+  float *Wgcan, *WgTcan, *b1, *W2can, *W2Tcan, *b2, *WAgcan, *WAgTcan, *bA;
 };
 
 }  // namespace b2m
@@ -136,8 +139,8 @@ struct b2m_engine {
   std::vector<AtomLayerW> aw;
   std::vector<BondLayerW> bw;
   float *d_emb = nullptr, *d_Wbe = nullptr, *d_Wae = nullptr, *d_Wabw = nullptr, *d_W3bw = nullptr, *d_fa = nullptr;
-  float *d_F0k = nullptr, *d_c0 = nullptr, *d_F0raw = nullptr, *d_F1k = nullptr, *d_c1 = nullptr, *d_F1raw = nullptr,
-        *d_F2 = nullptr, *d_Ws = nullptr;
+  TcW F0, F0T, F1, F1T;  // final MLP 64 -> 64 -> 64 and transposes
+  float *d_c0 = nullptr, *d_c1 = nullptr, *d_F2 = nullptr, *d_Ws = nullptr;
   const double* d_eref = nullptr;  // per-element energy offsets, double like the energy accumulator
   float c2 = 0.f, bs = 0.f;
   RadialParams rp2, rp3;
@@ -201,9 +204,7 @@ struct b2m_engine {
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> gather_ev;
   long long launches_last = 0;
   double last_energy = 0;
-  std::map<const float*, const float*> canon_of;  // FFMA-layout GEMM operand -> canonical wgmma copy
   int num_sms = 132;
-  bool use_tc = true;  // row GEMMs on the wgmma kernels; B2M_LEGACY_FFMA=1 selects the FP32-FFMA GEMM tiles (A/B checks)
   bool debug_no_halo = false;  // B2M_DEBUG_NO_HALO=1: a b2m_set_partition view may run with its exchanges skipped (wrong
                                // numbers, right amount of per-partition work: timing one slab of an N-way split on one GPU)
 };
@@ -310,6 +311,46 @@ static std::vector<float> line_reverse_can(const std::vector<float>& raw128x64) 
   return canon_split(permute_k8(transpose(raw128x64, 128, 64), 64, 128), 64, 128, 128);
 }
 
+// a [K][N] row-major weight (y = x W, K and N multiples of 64) as the wgmma blocks of tc_mm, packed into P: K chunks of
+// kmax (128 or 64; 64 for a remainder), per chunk N blocks of 64, or of 128 when the chunk is 64 deep
+static TcW pack_tc(Packer& P, const std::vector<float>& W, int K, int N, int kmax = 128) {
+  TcW w;
+  w.K = K, w.N = N;
+  for (int k0 = 0; k0 < K;) {
+    const int kc = K - k0 >= kmax ? kmax : 64;
+    for (int n0 = 0; n0 < N;) {
+      const int nc = kc == 64 && N - n0 >= 128 ? 128 : 64;
+      std::vector<float> raw((size_t)nc * kc);  // B[n][k] = W[k0 + k][n0 + n]
+      for (int n = 0; n < nc; n++)
+        for (int k = 0; k < kc; k++) raw[(size_t)n * kc + k] = W[(size_t)(k0 + k) * N + n0 + n];
+      w.blk.push_back({k0, kc, n0, nc, P.add(canon_split(raw, nc, kc, kc))});
+      n0 += nc;
+    }
+    k0 += kc;
+  }
+  return w;
+}
+// the weight and its transpose [N][K] (the reverse pass's product, in K chunks of rev_kmax)
+static void pack_tc2(Packer& P, const std::vector<float>& W, int K, int N, TcW& fwd, TcW& rev, int rev_kmax = 128) {
+  fwd = pack_tc(P, W, K, N);
+  rev = pack_tc(P, transpose(W, K, N), N, K, rev_kmax);
+}
+// out[M][N] (+)= epi(A[M][K] @ W + bias) (+ R, pitch ldr): the K chunks after the first accumulate in place, so bias and R
+// go with the first; epi 1 (SiLU, pre-activation kept in Cpre) needs a single K chunk, epi 2 (times SiLU'(Pre)) is applied
+// by the last one
+static void tc_mm(b2m_engine* e, const float* A, int lda, const TcW& W, float* out, int ldc, int M, bool accum,
+                  const float* bias = nullptr, const float* R = nullptr, int ldr = 0, int epi = 0, float* Cpre = nullptr,
+                  const float* Pre = nullptr, int ldp = 0) {
+  B2M_REQUIRE(epi != 1 || W.blk.back().k0 == 0, B2M_ERR_INVALID, "row GEMM: SiLU epilogue over several K chunks");
+  for (const TcW::Blk& b : W.blk) {
+    const bool first = b.k0 == 0, last = b.k0 + b.kc == W.K;
+    launch_gemm_wg(e->st, A + b.k0, lda, e->wbuf.p + b.off, out + b.n0, ldc, M, b.nc, b.kc,
+                   first && bias ? bias + b.n0 : nullptr, first && R ? R + b.n0 : nullptr, ldr, accum || !first,
+                   epi == 2 && !last ? 0 : epi, Cpre ? Cpre + b.n0 : nullptr, epi == 2 && last ? Pre + b.n0 : nullptr,
+                   ldp, e->num_sms);
+  }
+}
+
 static void finalize_weights(b2m_engine* e) {
   const int nb = e->desc.n_blocks;
   for (auto& kv : e->host_w) {
@@ -324,25 +365,10 @@ static void finalize_weights(b2m_engine* e) {
   e->consumed.clear();
   Packer P;
   std::map<std::string, size_t> off;
-  std::vector<std::string> gemm_names;
-  // every [K][N] row-major GEMM operand also gets a wgmma copy: canonical hi/lo planes of its [N][K] view
-  auto put = [&](const std::string& name, const std::vector<float>& v) {
-    off[name] = P.add(v);
-    const bool is_k = name.size() > 2 && name.substr(name.size() - 2) == "_k";
-    const bool is_raw = name.size() > 4 && name.substr(name.size() - 4) == "_raw";
-    const bool is_f = name == "F0k" || name == "F1k" || name == "F0raw" || name == "F1raw";
-    if (is_k || is_raw || is_f) {
-      int K = 0, N = 0;
-      if (v.size() == 64 * 64) K = 64, N = 64;
-      else if (v.size() == 64 * 128) {
-        // "_k" arrays of the first layers are [64][128]; "_raw" first-layer blocks are [128][64]
-        if (is_raw) K = 128, N = 64; else K = 64, N = 128;
-      }
-      if (K) {
-        off[name + ".can"] = P.add(canon_split(transpose(v, K, N), N, K, K));
-        gemm_names.push_back(name);
-      }
-    }
+  auto put = [&](const std::string& name, const std::vector<float>& v) { off[name] = P.add(v); };
+  // an nn.Linear weight [out][in] as the row GEMM x . W^T (K = in) and its reverse g . W
+  auto linear = [&](const std::vector<float>& w, int out, int in, TcW& fwd, TcW& rev) {
+    pack_tc2(P, transpose(w, out, in), in, out, fwd, rev);
   };
 
   const auto& f2 = W(e, "bond_expansion.frequencies", {NR});
@@ -365,6 +391,7 @@ static void finalize_weights(b2m_engine* e) {
   put("Wabw", W(e, "atom_bond_weights.weight", {D, NR}));
   put("W3bw", W(e, "threebody_bond_weights.weight", {D, NR}));
 
+  e->aw.resize(nb);
   for (int l = 0; l < nb; l++) {
     const std::string p = "atom_graph_layers." + std::to_string(l) + ".conv_layer.";
     const auto W1 = vcat(W(e, p + "node_update_func.layers.layers.0.weight", {D, 3 * D}),
@@ -385,20 +412,18 @@ static void finalize_weights(b2m_engine* e) {
         M[j * 9 + k] = (float)s;
       }
     const std::string q = "a" + std::to_string(l) + ".";
-    put(q + "W1s_k", transpose(W1s, 128, 64));
-    put(q + "W1e_k", transpose(W1e, 128, 64));
-    put(q + "W1t_k", transpose(W1t, 128, 64));
+    AtomLayerW& w = e->aw[l];
+    linear(W1s, 128, 64, w.W1s, w.W1sT);
+    linear(W1e, 128, 64, w.W1e, w.W1eT);
+    linear(W1t, 128, 64, w.W1t, w.W1tT);
+    linear(Wout, 64, 64, w.Wout, w.WoutT);
     put(q + "b1", b1);
-    put(q + "W1s_raw", W1s);
-    put(q + "W1e_raw", W1e);
-    put(q + "W1t_raw", W1t);
     put(q + "M", M);
     put(q + "W2can", second_layer_can(W2, false));
     put(q + "W2Tcan", second_layer_can(W2, true));
     put(q + "b2", b2);
-    put(q + "Wout_k", transpose(Wout, 64, 64));
-    put(q + "Wout_raw", Wout);
   }
+  e->bw.resize(nb - 1);
   for (int l = 0; l < nb - 1; l++) {
     const std::string p = "bond_graph_layers." + std::to_string(l) + ".conv_layer.";
     const auto W1 = vcat(W(e, p + "node_update_func.layers.layers.0.weight", {D, 4 * D}),
@@ -419,37 +444,27 @@ static void finalize_weights(b2m_engine* e) {
     const auto WAa = cols(WA, 128, 256, 0), WAg = cols(WA, 128, 256, 64), WAc = cols(WA, 128, 256, 128),
                WAb = cols(WA, 128, 256, 192);
     const std::string q = "b" + std::to_string(l) + ".";
-    put(q + "W1a_k", transpose(W1a, 128, 64));
-    put(q + "W1b_k", transpose(W1b, 128, 64));
-    put(q + "W1c_k", transpose(W1c, 128, 64));
+    BondLayerW& w = e->bw[l];
+    linear(W1a, 128, 64, w.W1a, w.W1aT);
+    linear(W1b, 128, 64, w.W1b, w.W1bT);
+    linear(W1c, 128, 64, w.W1c, w.W1cT);
+    linear(Wout, 64, 64, w.Wout, w.WoutT);
+    linear(WAa, 128, 64, w.WAa, w.WAaT);
+    linear(WAb, 128, 64, w.WAb, w.WAbT);
+    linear(WAc, 128, 64, w.WAc, w.WAcT);
     put(q + "Wgcan", second_layer_can(W1g, false));
     put(q + "b1", b1);
-    put(q + "W1a_raw", W1a);
-    put(q + "W1b_raw", W1b);
-    put(q + "W1c_raw", W1c);
     put(q + "WgTcan", line_reverse_can(W1g));
     put(q + "W2can", second_layer_can(W2, false));
     put(q + "W2Tcan", second_layer_can(W2, true));
     put(q + "b2", b2);
-    put(q + "Wout_k", transpose(Wout, 64, 64));
-    put(q + "Wout_raw", Wout);
-    put(q + "WAa_k", transpose(WAa, 128, 64));
-    put(q + "WAb_k", transpose(WAb, 128, 64));
-    put(q + "WAc_k", transpose(WAc, 128, 64));
     put(q + "WAgcan", second_layer_can(WAg, false));
     put(q + "bA", bA);
-    put(q + "WAa_raw", WAa);
-    put(q + "WAb_raw", WAb);
-    put(q + "WAc_raw", WAc);
     put(q + "WAgTcan", line_reverse_can(WAg));
   }
-  const auto& F0 = W(e, "final_layer.layers.0.weight", {D, D});
-  const auto& F1 = W(e, "final_layer.layers.1.weight", {D, D});
-  put("F0k", transpose(F0, 64, 64));
-  put("F0raw", F0);
+  linear(W(e, "final_layer.layers.0.weight", {D, D}), 64, 64, e->F0, e->F0T);
   put("c0", W(e, "final_layer.layers.0.bias", {D}));
-  put("F1k", transpose(F1, 64, 64));
-  put("F1raw", F1);
+  linear(W(e, "final_layer.layers.1.weight", {D, D}), 64, 64, e->F1, e->F1T);
   put("c1", W(e, "final_layer.layers.1.bias", {D}));
   put("F2", W(e, "final_layer.layers.2.weight", {1, D}));
   e->c2 = W(e, "final_layer.layers.2.bias", {1})[0];
@@ -472,54 +487,27 @@ static void finalize_weights(b2m_engine* e) {
   B2M_CK(cudaMemcpyAsync(e->wbuf.p, P.host.data(), P.host.size() * sizeof(float), cudaMemcpyHostToDevice, e->st));
   B2M_CK(cudaStreamSynchronize(e->st));
   auto dp = [&](const std::string& n) { return e->wbuf.p + off.at(n); };
-  e->canon_of.clear();
-  for (auto& n : gemm_names) e->canon_of[dp(n)] = dp(n + ".can");
   e->d_fa = dp("fa");
   e->d_emb = dp("emb");
   e->d_Wbe = dp("Wbe");
   e->d_Wae = dp("Wae");
   e->d_Wabw = dp("Wabw");
   e->d_W3bw = dp("W3bw");
-  e->d_F0k = dp("F0k"), e->d_F0raw = dp("F0raw"), e->d_c0 = dp("c0");
-  e->d_F1k = dp("F1k"), e->d_F1raw = dp("F1raw"), e->d_c1 = dp("c1");
-  e->d_F2 = dp("F2"), e->d_Ws = dp("Ws");
+  e->d_c0 = dp("c0"), e->d_c1 = dp("c1"), e->d_F2 = dp("F2"), e->d_Ws = dp("Ws");
   e->d_eref = e->elem_refs.empty() ? nullptr : e->erefbuf.p;
-  e->aw.resize(nb);
   for (int l = 0; l < nb; l++) {
     const std::string q = "a" + std::to_string(l) + ".";
     AtomLayerW& w = e->aw[l];
-    w.W1s_k = dp(q + "W1s_k"), w.W1e_k = dp(q + "W1e_k"), w.W1t_k = dp(q + "W1t_k"), w.b1 = dp(q + "b1");
-    w.W1s_raw = dp(q + "W1s_raw"), w.W1e_raw = dp(q + "W1e_raw"), w.W1t_raw = dp(q + "W1t_raw");
-    w.M = dp(q + "M"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
-    w.Wout_k = dp(q + "Wout_k"), w.Wout_raw = dp(q + "Wout_raw");
+    w.b1 = dp(q + "b1"), w.M = dp(q + "M"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
   }
-  e->bw.resize(nb - 1);
   for (int l = 0; l < nb - 1; l++) {
     const std::string q = "b" + std::to_string(l) + ".";
     BondLayerW& w = e->bw[l];
-    w.W1a_k = dp(q + "W1a_k"), w.W1b_k = dp(q + "W1b_k"), w.W1c_k = dp(q + "W1c_k"), w.Wgcan = dp(q + "Wgcan");
-    w.b1 = dp(q + "b1"), w.W1a_raw = dp(q + "W1a_raw"), w.W1b_raw = dp(q + "W1b_raw"), w.W1c_raw = dp(q + "W1c_raw");
-    w.WgTcan = dp(q + "WgTcan"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
-    w.Wout_k = dp(q + "Wout_k"), w.Wout_raw = dp(q + "Wout_raw");
-    w.WAa_k = dp(q + "WAa_k"), w.WAb_k = dp(q + "WAb_k"), w.WAc_k = dp(q + "WAc_k"), w.WAgcan = dp(q + "WAgcan");
-    w.bA = dp(q + "bA"), w.WAa_raw = dp(q + "WAa_raw"), w.WAb_raw = dp(q + "WAb_raw"), w.WAc_raw = dp(q + "WAc_raw");
-    w.WAgTcan = dp(q + "WAgTcan");
+    w.Wgcan = dp(q + "Wgcan"), w.WgTcan = dp(q + "WgTcan"), w.b1 = dp(q + "b1");
+    w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
+    w.WAgcan = dp(q + "WAgcan"), w.WAgTcan = dp(q + "WAgTcan"), w.bA = dp(q + "bA");
   }
   e->finalized = true;
-}
-
-// node-level GEMM dispatch: wgmma when a canonical copy of B exists, FFMA tile kernel otherwise
-static void gemm(b2m_engine* e, const float* A, int lda, const float* B, float* C, int ldc, int M, int N, int K,
-                 const float* bias, const float* R, int ldr, bool accum) {
-  if (e->use_tc) {
-    auto it = e->canon_of.find(B);
-    if (it != e->canon_of.end()) {
-      launch_gemm_tc(e->st, A, lda, it->second, C, ldc, M, N, K, bias, R, ldr, accum, e->num_sms);
-      return;
-    }
-  }
-  B2M_REQUIRE(!e->use_tc, B2M_ERR_STATE, "wgmma path: GEMM operand without a canonical copy");
-  launch_gemm(e->st, A, lda, B, C, ldc, M, N, K, bias, R, ldr, accum);  // FP32-FFMA tile kernel (legacy path only)
 }
 
 // ------------------------------------------------------------------------------------------
@@ -720,9 +708,9 @@ static void atom_projections(b2m_engine* e, int l) {
   Graph& g = e->g;
   const AtomLayerW& w = e->aw[l];
   const int ps = e->proj_slot(l);
-  gemm(e, e->x[l].p, D, w.W1s_k, e->ApL[ps].p, D2, g.n_loc, D2, D, nullptr, nullptr, 0, false);
-  gemm(e, e->x[l].p, D, w.W1t_k, e->CpL[ps].p, D2, g.n_own, D2, D, w.b1, nullptr, 0, false);
-  if (l > 0) gemm(e, e->h[l].p, D, w.W1e_k, e->QpL[ps].p, D2, g.B_own, D2, D, nullptr, nullptr, 0, false);
+  tc_mm(e, e->x[l].p, D, w.W1s, e->ApL[ps].p, D2, g.n_loc, false);
+  tc_mm(e, e->x[l].p, D, w.W1t, e->CpL[ps].p, D2, g.n_own, false, w.b1);
+  if (l > 0) tc_mm(e, e->h[l].p, D, w.W1e, e->QpL[ps].p, D2, g.B_own, false);
 }
 static void atom_layer_fwd(b2m_engine* e, int l) {
   Graph& g = e->g;
@@ -738,13 +726,13 @@ static void atom_layer_fwd(b2m_engine* e, int l) {
   launch_atomconv_fwd(e->st, a, e->num_sms);
   B2M_CK(cudaEventRecord(e1, e->st));
   e->gather_ev.push_back({e0, e1});
-  gemm(e, e->agg.p, D, w.Wout_k, e->x[l + 1].p, D, g.n_own, D, D, nullptr, e->x[l].p, D, false);
+  tc_mm(e, e->agg.p, D, w.Wout, e->x[l + 1].p, D, g.n_own, false, nullptr, e->x[l].p, D);
 }
 // in: gx = dE/dx[l+1] (owned rows valid, halo rows zero).  out: gx = dE/dx[l] (all local rows)
 static void atom_layer_bwd(b2m_engine* e, int l) {
   Graph& g = e->g;
   const AtomLayerW& w = e->aw[l];
-  gemm(e, e->gx.p, D, w.Wout_raw, e->gagg.p, D, g.n_own, D, D, nullptr, nullptr, 0, false);
+  tc_mm(e, e->gx.p, D, w.WoutT, e->gagg.p, D, g.n_own, false);
   // A / C / Q of this layer are still in their per-layer buffers from the forward: no recompute
   AtomConvArgs a = atom_args(e, l);
   a.gagg = e->gagg.p;
@@ -757,9 +745,9 @@ static void atom_layer_bwd(b2m_engine* e, int l) {
   }
   launch_atomconv_bwd(e->st, a, e->num_sms);
   if (need_gx) {
-    gemm(e, e->gA.p, D2, w.W1s_raw, e->gx.p, D, g.n_loc, D, D2, nullptr, nullptr, 0, true);
-    gemm(e, e->gC.p, D2, w.W1t_raw, e->gx.p, D, g.n_own, D, D2, nullptr, nullptr, 0, true);
-    gemm(e, e->gQ.p, D2, w.W1e_raw, e->gh.p, D, g.B_own, D, D2, nullptr, nullptr, 0, true);
+    tc_mm(e, e->gA.p, D2, w.W1sT, e->gx.p, D, g.n_loc, true);
+    tc_mm(e, e->gC.p, D2, w.W1tT, e->gx.p, D, g.n_own, true);
+    tc_mm(e, e->gQ.p, D2, w.W1eT, e->gh.p, D, g.B_own, true);
   }
 }
 
@@ -783,16 +771,16 @@ static LineArgs line_args(b2m_engine* e, int l, bool hidden) {
 static void line_proj_Ha(b2m_engine* e, int l, bool hidden) {
   const BondLayerW& w = e->bw[l];
   const float* hsrc = hidden ? e->h[l].p : e->h[l + 1].p;
-  gemm(e, hsrc, D, hidden ? w.W1a_k : w.WAa_k, e->Ha.p, D2, e->g.B_loc, D2, D, nullptr, nullptr, 0, false);
+  tc_mm(e, hsrc, D, hidden ? w.W1a : w.WAa, e->Ha.p, D2, e->g.B_loc, false);
 }
 static void line_proj_Hb(b2m_engine* e, int l, bool hidden) {
   const BondLayerW& w = e->bw[l];
   const float* hsrc = hidden ? e->h[l].p : e->h[l + 1].p;
-  gemm(e, hsrc, D, hidden ? w.W1b_k : w.WAb_k, e->Hb.p, D2, e->g.B_own, D2, D, hidden ? w.b1 : w.bA, nullptr, 0, false);
+  tc_mm(e, hsrc, D, hidden ? w.W1b : w.WAb, e->Hb.p, D2, e->g.B_own, false, hidden ? w.b1 : w.bA);
 }
 static void line_proj_Xc(b2m_engine* e, int l, bool hidden) {
   const BondLayerW& w = e->bw[l];
-  gemm(e, e->x[l + 1].p, D, hidden ? w.W1c_k : w.WAc_k, e->Xc.p, D2, e->g.n_loc, D2, D, nullptr, nullptr, 0, false);
+  tc_mm(e, e->x[l + 1].p, D, hidden ? w.W1c : w.WAc, e->Xc.p, D2, e->g.n_loc, false);
 }
 static void line_projections(b2m_engine* e, int l, bool hidden) {
   line_proj_Ha(e, l, hidden), line_proj_Hb(e, l, hidden), line_proj_Xc(e, l, hidden);
@@ -805,9 +793,9 @@ static void line_bwd_common(b2m_engine* e, int l, bool hidden, LineArgs& a) {
   launch_zero_rows(e->st, e->gXc.p, (int64_t)g.n_loc * D2);
   a.gang = e->gang.p, a.gHa = e->gHa.p, a.gHb = e->gHb.p, a.gXc = e->gXc.p;
   launch_line_bwd(e->st, a, hidden, e->num_sms);
-  gemm(e, e->gHa.p, D2, hidden ? w.W1a_raw : w.WAa_raw, e->gh.p, D, g.B_loc, D, D2, nullptr, nullptr, 0, true);
-  gemm(e, e->gHb.p, D2, hidden ? w.W1b_raw : w.WAb_raw, e->gh.p, D, g.B_own, D, D2, nullptr, nullptr, 0, true);
-  gemm(e, e->gXc.p, D2, hidden ? w.W1c_raw : w.WAc_raw, e->gx.p, D, g.n_loc, D, D2, nullptr, nullptr, 0, true);
+  tc_mm(e, e->gHa.p, D2, hidden ? w.W1aT : w.WAaT, e->gh.p, D, g.B_loc, true);
+  tc_mm(e, e->gHb.p, D2, hidden ? w.W1bT : w.WAbT, e->gh.p, D, g.B_own, true);
+  tc_mm(e, e->gXc.p, D2, hidden ? w.W1cT : w.WAcT, e->gx.p, D, g.n_loc, true);
 }
 
 static void forward(b2m_engine* e) {
@@ -828,7 +816,7 @@ static void forward(b2m_engine* e) {
     LineArgs a = line_args(e, l, true);
     a.aggB = e->aggB.p;
     launch_line_fwd(e->st, a, true, e->num_sms);
-    gemm(e, e->aggB.p, D, w.Wout_k, e->upd[l].p, D, g.B_own, D, D, nullptr, nullptr, 0, false);
+    tc_mm(e, e->aggB.p, D, w.Wout, e->upd[l].p, D, g.B_own, false);
     launch_bond_update_fwd(e->st, g.B_own, g.b_vec.p, e->rp3, e->d_W3bw, e->h[l].p, e->upd[l].p, e->h[l + 1].p);
     if (l < nb - 2) {
       // the last block's angle update (and the halo copy of h feeding it) is dead code in the
@@ -847,9 +835,9 @@ static void forward(b2m_engine* e) {
   launch_rowdot(e->st, g.n_own, e->x[nb - 1].p, e->d_Ws, e->bs, e->site.p, nullptr, nullptr, nullptr, 1.f);
   atom_layer_fwd(e, nb - 1);
   // final MLP 64 -> 64 -> 64 -> 1, sum (chgnet.py:422-440); E = std * E + mean (+ element refs) (pes.py:109-113)
-  gemm(e, e->x[nb].p, D, e->d_F0k, e->y1p.p, D, g.n_own, D, D, e->d_c0, nullptr, 0, false);
+  tc_mm(e, e->x[nb].p, D, e->F0, e->y1p.p, D, g.n_own, false, e->d_c0);
   launch_silu(e->st, (int64_t)g.n_own * D, e->y1p.p, e->y1.p);
-  gemm(e, e->y1.p, D, e->d_F1k, e->y2p.p, D, g.n_own, D, D, e->d_c1, nullptr, 0, false);
+  tc_mm(e, e->y1.p, D, e->F1, e->y2p.p, D, g.n_own, false, e->d_c1);
   launch_silu(e->st, (int64_t)g.n_own * D, e->y2p.p, e->y2.p);
   B2M_CK(cudaMemsetAsync(e->scal.p, 0, 16 * sizeof(double), e->st));
   launch_rowdot(e->st, g.n_own, e->y2.p, e->d_F2, e->c2, e->e_atom.p, e->scal.p, g.type.p, e->d_eref,
@@ -870,9 +858,9 @@ static void backward(b2m_engine* e) {
   // readout backward
   launch_readout_seed(e->st, g.n_own, e->y2p.p, e->d_F2, (float)e->desc.data_std, e->gy2.p, g.gid.p,
                       e->hf_n ? e->hf_w.p : nullptr);
-  gemm(e, e->gy2.p, D, e->d_F1raw, e->gy1.p, D, g.n_own, D, D, nullptr, nullptr, 0, false);
+  tc_mm(e, e->gy2.p, D, e->F1T, e->gy1.p, D, g.n_own, false);
   launch_dsilu_mul(e->st, (int64_t)g.n_own * D, e->y1p.p, e->gy1.p);
-  gemm(e, e->gy1.p, D, e->d_F0raw, e->gx.p, D, g.n_own, D, D, nullptr, nullptr, 0, false);
+  tc_mm(e, e->gy1.p, D, e->F0T, e->gx.p, D, g.n_own, false);
   atom_layer_bwd(e, nb - 1);
   for (int l = nb - 2; l >= 0; l--) {
     const BondLayerW& w = e->bw[l];
@@ -884,7 +872,7 @@ static void backward(b2m_engine* e) {
       halo_backward(e, e->gh.p, true);
     }
     launch_bond_update_bwd(e->st, g.B_own, g.b_vec.p, e->rp3, e->d_W3bw, e->gh.p, e->upd[l].p, e->gupd.p, e->gdb.p);
-    gemm(e, e->gupd.p, D, w.Wout_raw, e->gaggB.p, D, g.B_own, D, D, nullptr, nullptr, 0, false);
+    tc_mm(e, e->gupd.p, D, w.WoutT, e->gaggB.p, D, g.B_own, false);
     line_projections(e, l, true);
     LineArgs a = line_args(e, l, true);
     a.gaggB = e->gaggB.p;
@@ -1313,8 +1301,6 @@ static b2m_engine* create_one(const b2m_model_desc* desc, int device, int count)
     B2M_CK(cudaGetDeviceProperties(&prop, e->device));
     if (prop.major != 9 || prop.minor != 0) throw Error(B2M_ERR_CUDA, "libb200mlip is built for sm_90a (H100) only");
     e->num_sms = prop.multiProcessorCount;
-    const char* leg = getenv("B2M_LEGACY_FFMA");
-    e->use_tc = !(leg && leg[0] == '1');
     const char* nh = getenv("B2M_DEBUG_NO_HALO");
     e->debug_no_halo = nh && nh[0] == '1';
     B2M_CK(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));

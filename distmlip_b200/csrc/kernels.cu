@@ -194,85 +194,6 @@ __device__ __forceinline__ void seg_flush(const float* tile, int ld, int col, in
 }
 
 // ============================================================================================
-// generic row GEMM (node-level projections; ~10% of the FLOPs)
-// ============================================================================================
-__global__ void __launch_bounds__(256) k_gemm(const float* __restrict__ A, int lda, const float* __restrict__ B,
-                                              float* __restrict__ C, int ldc, int M, int N, int K,
-                                              const float* __restrict__ bias, const float* __restrict__ R, int ldr,
-                                              int accum) {
-  __shared__ __align__(16) float As[128][36];
-  __shared__ __align__(16) float Bs[32][64];
-  const int tid = threadIdx.x;
-  const int m0 = blockIdx.x * 128, n0 = blockIdx.y * 64;
-  const int rg = tid >> 4, cg = tid & 15;
-  float acc[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; i++)
-    for (int j = 0; j < 4; j++) acc[i][j] = 0.f;
-  for (int k0 = 0; k0 < K; k0 += 32) {
-#pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int idx = tid + 256 * i;
-      const int row = idx >> 3, c4 = idx & 7;
-      const int gm = m0 + row;
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (gm < M) v = *reinterpret_cast<const float4*>(&A[(size_t)gm * lda + k0 + c4 * 4]);
-      *reinterpret_cast<float4*>(&As[row][c4 * 4]) = v;
-    }
-#pragma unroll
-    for (int i = 0; i < 2; i++) {
-      const int idx = tid + 256 * i;
-      const int kr = idx >> 4, c4 = idx & 15;
-      *reinterpret_cast<float4*>(&Bs[kr][c4 * 4]) =
-          *reinterpret_cast<const float4*>(&B[(size_t)(k0 + kr) * N + n0 + c4 * 4]);
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int k = 0; k < 32; k++) {
-      const float4 b = *reinterpret_cast<const float4*>(&Bs[k][cg * 4]);
-#pragma unroll
-      for (int i = 0; i < 8; i++) {
-        const float a = As[rg + 16 * i][k];
-        acc[i][0] = fmaf(a, b.x, acc[i][0]);
-        acc[i][1] = fmaf(a, b.y, acc[i][1]);
-        acc[i][2] = fmaf(a, b.z, acc[i][2]);
-        acc[i][3] = fmaf(a, b.w, acc[i][3]);
-      }
-    }
-    __syncthreads();
-  }
-  const int col = n0 + cg * 4;
-  float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (bias) bv = *reinterpret_cast<const float4*>(&bias[col]);
-#pragma unroll
-  for (int i = 0; i < 8; i++) {
-    const int gm = m0 + rg + 16 * i;
-    if (gm >= M) continue;
-    float4 v = make_float4(acc[i][0] + bv.x, acc[i][1] + bv.y, acc[i][2] + bv.z, acc[i][3] + bv.w);
-    if (R) {
-      const float4 r = *reinterpret_cast<const float4*>(&R[(size_t)gm * ldr + col]);
-      v.x += r.x, v.y += r.y, v.z += r.z, v.w += r.w;
-    }
-    float4* cp = reinterpret_cast<float4*>(&C[(size_t)gm * ldc + col]);
-    if (accum) {
-      const float4 c = *cp;
-      v.x += c.x, v.y += c.y, v.z += c.z, v.w += c.w;
-    }
-    *cp = v;
-  }
-}
-
-void launch_gemm(cudaStream_t st, const float* A, int lda, const float* B, float* C, int ldc, int M, int N, int K,
-                 const float* bias, const float* R, int ldr, bool accum) {
-  if (M <= 0) return;
-  B2M_REQUIRE(K % 32 == 0 && N % 64 == 0, B2M_ERR_INVALID, "gemm shape");
-  dim3 grid(cdiv(M, 128), N / 64);
-  k_gemm<<<grid, 256, 0, st>>>(A, lda, B, C, ldc, M, N, K, bias, R, ldr, accum ? 1 : 0);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
-}
-
-// ============================================================================================
 // small elementwise / init kernels
 // ============================================================================================
 __global__ void k_embed(int n, const int* __restrict__ type, const float* __restrict__ emb, float* __restrict__ x0) {

@@ -22,10 +22,6 @@ struct RadialParams {
   int p;
 };
 
-// -------- generic row GEMM: C[M,N] = (R | accum C | 0) + A[M,K] @ B[K,N] + bias --------
-void launch_gemm(cudaStream_t st, const float* A, int lda, const float* B, float* C, int ldc, int M, int N, int K,
-                 const float* bias, const float* R, int ldr, bool accum);
-
 // -------- elementwise / init --------
 void launch_embed(cudaStream_t st, int n, const int* type, const float* emb, float* x0);
 void launch_bond_init(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp, const float* W /*[64][9]*/,
@@ -142,15 +138,23 @@ void launch_scatter_add_rows(cudaStream_t st, int n, int width, const int* idx, 
 // core-matrix layout (8 rows x 16 B), hi and lo planes (see engine.cu: canon_split()).
 // ---------------------------------------------------------------------------------------------
 namespace b2m {
-// C[M,N] = (R | accum C | 0) + A[M,K] @ B + bias, B given as canonical hi/lo planes of its [N][K] view.
-// (K,N) in {(64,128), (64,64), (128,64)}.
-void launch_gemm_tc(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N,
-                    int K, const float* bias, const float* R, int ldr, bool accum, int num_sms);
-// same kernel with an epilogue (TensorNet edge MLP): epi 1 keeps the pre-activation in Cpre (pitch ldc) and writes
-// SiLU(value) to C; epi 2 multiplies the (accumulated) value by SiLU'(Pre[row][col]) (pitch ldp); epi 0 = plain
-void launch_gemm_tc_epi(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N,
-                        int K, const float* bias, bool accum, int epi, float* Cpre, const float* Pre, int ldp,
-                        int num_sms);
+// C[M,N] = (R | accum C | 0) + A[M,K] @ B + bias, B given as canonical hi/lo planes of its [N][K] view, then the
+// epilogue: epi 1 keeps the value in Cpre (pitch ldc) and writes SiLU(value) to C; epi 2 multiplies the (accumulated)
+// value by SiLU'(Pre[row][col]) (pitch ldp); epi 0 = plain.  (K,N) in {(64,128), (64,64), (128,64)}.
+// The engine calls it only through tc_mm (engine.cu), which splits a larger product into these blocks.
+void launch_gemm_wg(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N, int K,
+                    const float* bias, const float* R, int ldr, bool accum, int epi, float* Cpre, const float* Pre,
+                    int ldp, int num_sms);
+// A [K][N] weight (y = x W) as B operands of launch_gemm_wg: the blocks tc_mm launches, in launch order (engine.cu
+// pack_tc), each the canonical hi/lo image of its [nc][kc] view stored at float offset `off` of the engine's weight buffer
+struct TcW {
+  struct Blk {
+    int k0, kc, n0, nc;
+    size_t off;
+  };
+  int K = 0, N = 0;
+  std::vector<Blk> blk;
+};
 }  // namespace b2m
 
 // ---------------------------------------------------------------------------------------------

@@ -4,7 +4,7 @@
 // engine_mace.inl runs these kernels stage by stage.
 //
 // First generation: the node- and edge-level products (radial MLP, linear_up, the per-l mixes, the product linear) run
-// on the wgmma row GEMM of the other paths (kernels_wg.cu, engine_mace.inl tc_mm); the element-dependent mixes
+// on the wgmma row GEMM of the other paths (kernels_wg.cu, engine.cu tc_mm); the element-dependent mixes
 // (skip_tp) read the element's C x C block per atom; the symmetric contraction is one thread per (atom, channel) that
 // walks the nonzero terms of U, which every channel shares.  Aggregations walk the CSR-by-destination rows (no atomics
 // in the forward); the reverse scatters to sources with atomics.

@@ -11,9 +11,8 @@
 // CSR-by-destination rows (no atomics in the forward); the reverse pass scatters to sources with red.add.
 // First generation of this path.  The edge-level products (edge MLP 32 -> 64 -> 128 -> 192 and the three distance
 // projections) run on the wgmma row GEMM of the CHGNet path (kernels_wg.cu, k_gemm_wg with a
-// SiLU / SiLU' epilogue; engine_tn.inl composes the 192-wide layers from its 64/128 shapes); the node-level products
-// (channel mixes, scalar MLPs, readout) use the FP32-FFMA tile kernel below, which also serves the edge level under
-// B2M_TN_FFMA=1 (A/B checks).  DESIGN.md 8 lists what comes next.
+// SiLU / SiLU' epilogue; engine.cu tc_mm splits the 192-wide layers into its 64/128 shapes); the node-level products
+// (channel mixes, scalar MLPs, readout) use the FP32-FFMA tile kernel below.  DESIGN.md 8 lists what comes next.
 #include <math_constants.h>
 
 #include "atomic_virial.cuh"

@@ -1,5 +1,6 @@
-// kernels_wg.cu -- node-level row GEMMs on the Hopper tensor cores (wgmma, sm_90a): the CHGNet projections and their
-// transposes, and the TensorNet edge MLP (with its SiLU / SiLU' epilogues).
+// kernels_wg.cu -- row GEMMs on the Hopper tensor cores (wgmma, sm_90a): the CHGNet projections and their transposes,
+// the TensorNet edge MLP and distance projection, and the dense MACE products (with SiLU / SiLU' epilogues).  Weights of
+// any [K][N] shape (multiples of 64) are split into this kernel's three block shapes on the host (engine.cu pack_tc, tc_mm).
 //
 //   * 3xTF32 split (hi*hi + lo*hi + hi*lo, fp32 accumulate in registers) keeps fp32-level accuracy;
 //   * a CTA of two warpgroups owns 128-row tiles (persistent over the grid); warpgroup w multiplies rows 64w .. 64w+63
@@ -174,23 +175,17 @@ static void launch_gemm_wg_s(cudaStream_t st, const float* A, int lda, const flo
     throw Error(B2M_ERR_INVALID, "gemm_wg shape");
 }
 
-void launch_gemm_tc_epi(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N,
-                        int K, const float* bias, bool accum, int epi, float* Cpre, const float* Pre, int ldp,
-                        int num_sms) {
+void launch_gemm_wg(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N, int K,
+                    const float* bias, const float* R, int ldr, bool accum, int epi, float* Cpre, const float* Pre,
+                    int ldp, int num_sms) {
   if (M <= 0) return;
   B2M_REQUIRE(epi == 1 ? Cpre != nullptr : (epi == 2 ? Pre != nullptr : epi == 0), B2M_ERR_INVALID, "gemm_wg epilogue");
   if (epi == 1)
-    launch_gemm_wg_s<1>(st, A, lda, Bcan, C, ldc, M, N, K, bias, nullptr, 0, accum, Cpre, Pre, ldp, num_sms);
+    launch_gemm_wg_s<1>(st, A, lda, Bcan, C, ldc, M, N, K, bias, R, ldr, accum, Cpre, Pre, ldp, num_sms);
   else if (epi == 2)
-    launch_gemm_wg_s<2>(st, A, lda, Bcan, C, ldc, M, N, K, bias, nullptr, 0, accum, Cpre, Pre, ldp, num_sms);
+    launch_gemm_wg_s<2>(st, A, lda, Bcan, C, ldc, M, N, K, bias, R, ldr, accum, Cpre, Pre, ldp, num_sms);
   else
-    launch_gemm_wg_s<0>(st, A, lda, Bcan, C, ldc, M, N, K, bias, nullptr, 0, accum, Cpre, Pre, ldp, num_sms);
-}
-
-void launch_gemm_tc(cudaStream_t st, const float* A, int lda, const float* Bcan, float* C, int ldc, int M, int N, int K,
-                    const float* bias, const float* R, int ldr, bool accum, int num_sms) {
-  if (M <= 0) return;
-  launch_gemm_wg_s<0>(st, A, lda, Bcan, C, ldc, M, N, K, bias, R, ldr, accum, nullptr, nullptr, 0, num_sms);
+    launch_gemm_wg_s<0>(st, A, lda, Bcan, C, ldc, M, N, K, bias, R, ldr, accum, Cpre, Pre, ldp, num_sms);
 }
 
 }  // namespace b2m

@@ -85,13 +85,6 @@ void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_sr
                             const int* gid, const MaceRadial& rp, const float* g_eb, const float* gY, float* forces,
                             double* virial, float* atom_vir = nullptr);
 
-// A [K][N] weight (y = x W) as operands of the wgmma row GEMM (kernels_wg.cu): blocks of K x N = 64 x 128, 64 x 64 or
-// 128 x 64 in the order engine_mace.inl's tc_blocks visits them, each the canonical hi/lo image of its [N][K] view
-struct TcW {
-  int K = 0, N = 0;
-  std::vector<const float*> blk;
-};
-
 struct MaceLayerW {
   bool residual = true;
   int Lin = 0, Lout = 0;      // node features 0e (0) or 0e+1o (1) in and out

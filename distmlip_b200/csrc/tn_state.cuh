@@ -7,12 +7,11 @@
 namespace b2m {
 
 struct TnLayerW {
-  const float *W0t, *b0, *W1t, *b1, *W2t, *b2;  // edge MLP num_rbf -> C -> 2C -> 3C, forward operands [K][N]
-  const float *W0r, *W1r, *W2r;                 // raw nn.Linear weights [out][in] (reverse pass; W0r padded to nrp columns)
-  const float *Wt_t[6], *Wt_r[6];               // linears_tensor 0..5: transposed (forward) and raw (reverse)
-  // wgmma operands of the edge MLP (canonical hi/lo planes, see engine.cu canon_split): forward W0 (64->64, rbf columns
-  // padded), W1 (64->128), W2 as three 128->64 column blocks; reverse W2 as three 64->128 K-chunks, W1 (128->64), W0 (64->64)
-  const float *W0c, *W1c, *W2c[3], *W2rc[3], *W1rc, *W0rc;
+  // edge MLP nrp -> C -> 2C -> 3C on the wgmma row GEMM (engine.cu tc_mm), forward and reverse (W0 with zero rows for the
+  // padding rbf columns; W2T in 64-deep K chunks)
+  TcW W0, W0T, W1, W1T, W2, W2T;
+  const float *b0, *b1, *b2;
+  const float *Wt_t[6], *Wt_r[6];  // linears_tensor 0..5: transposed (forward) and raw (reverse)
 };
 struct TnChainW {  // one hidden Linear of a readout chain
   const float *Wt, *Wr, *b;
@@ -23,9 +22,8 @@ struct TnState {
   int units = 64, num_rbf = 32, nblocks = 2, so3 = 0;
   TnRadial rp;
   // ---- weights (device pointers into the engine's weight buffer) ----
-  const float *Wd_t = nullptr, *bd = nullptr, *Wd_r = nullptr;  // three distance projections stacked: [nrp][3C], [3C], [3C][nrp]
-  const float *Wdc_a = nullptr, *Wdc_b = nullptr, *Wdrc[3] = {nullptr, nullptr, nullptr};  // wgmma: 64->128 | 64->64 ; reverse chunks
-  bool tc = true;  // edge-level GEMMs on the wgmma row GEMM (B2M_TN_FFMA=1: the FP32-FFMA tiles, A/B checks)
+  TcW Wd, WdT;                 // three distance projections stacked, nrp -> 3C, and the reverse (64-deep K chunks)
+  const float* bd = nullptr;   // [3C]
   const float *U = nullptr, *V = nullptr;                       // emb2 halves applied to the embedding table: [n_elem][C]
   const float *Wte_t[3] = {nullptr, nullptr, nullptr}, *Wte_r[3] = {nullptr, nullptr, nullptr};
   const float *ln0_g = nullptr, *ln0_b = nullptr;

@@ -308,28 +308,6 @@ def test_axis_permutation_symmetry(eng, model):
     assert np.abs(F2 - F1[:, P]).max() < 2e-6 and np.abs(S2 - S1[P][:, P]).max() < 2e-6
 
 
-# ------------------------------------------------------------------ the two kernel generations agree on the device
-def test_wgmma_and_ffma_row_gemms_agree(model):
-    """default path = row GEMMs on wgmma (3xTF32); B2M_LEGACY_FFMA=1 selects the FP32-FFMA GEMM tiles."""
-    atoms = si_diamond(4, seed=23)
-    old = os.environ.get("B2M_LEGACY_FFMA")
-    try:
-        os.environ["B2M_LEGACY_FFMA"] = "1"
-        e_ffma = engine_from_model(model)
-        os.environ["B2M_LEGACY_FFMA"] = "0"
-        e_tc = engine_from_model(model)
-    finally:
-        if old is None:
-            os.environ.pop("B2M_LEGACY_FFMA", None)
-        else:
-            os.environ["B2M_LEGACY_FFMA"] = old
-    E1, F1, S1 = run_engine(e_ffma, model, atoms)
-    E2, F2, S2 = run_engine(e_tc, model, atoms)
-    assert abs(E1 - E2) / len(atoms) < 1e-7 and np.abs(F1 - F2).max() < 1e-6 and np.abs(S1 - S2).max() < 1e-6
-    e_ffma.close()
-    e_tc.close()
-
-
 @pytest.mark.parametrize("nb", [2, 3])
 def test_other_block_counts(nb):
     """n_blocks is read from the model (chgnet.py:298): the layer loops, the dead last angle update and the
