@@ -1,7 +1,7 @@
 // kernels_mace.cu -- MACE with hidden features C x 0e or C x 0e + C x 1o on the same partitioned CSR graph as the
 // CHGNet and TensorNet paths.  Arithmetic as oracle/mace_ref.py and, for 0e+1o features, tests/mace_eq_ref.py state it
-// (the conventions are written down there once);
-// engine_mace.inl runs these kernels stage by stage.
+// (the conventions are written down there once), and the ZBL pair term and Agnesi transform as tests/mace_zbl_ref.py
+// states them; engine_mace.inl runs these kernels stage by stage.
 //
 // First generation: the node- and edge-level products (radial MLP, linear_up, the per-l mixes, the product linear) run
 // on the wgmma row GEMM of the other paths (kernels_wg.cu, engine.cu tc_mm); the element-dependent mixes
@@ -72,22 +72,49 @@ __device__ __forceinline__ void sh16(T x, T y, T z, T one, int nsh, T* Y) {
   Y[15] = smul(a, x * (xx - smul(3.f, yy)));
 }
 
-// polynomial cutoff and its derivative in d
-__device__ __forceinline__ void poly_cut(float d, const MaceRadial& rp, float& f, float& df) {
-  const float x = d / rp.r_max;
+// mace's polynomial envelope of d / r (exponent p, zero from d = r on) and its derivative in d
+__device__ __forceinline__ void poly_env(float d, float r, int ip, float& f, float& df) {
+  const float x = d / r;
   if (x >= 1.f) {
     f = 0.f, df = 0.f;
     return;
   }
-  const float p = (float)rp.p;
+  const float p = (float)ip;
   const float xp1 = __powf(x, p - 1.f), xp = xp1 * x, xp1p = xp * x, xp2 = xp1p * x;
   f = 1.f - 0.5f * (p + 1.f) * (p + 2.f) * xp + p * (p + 2.f) * xp1p - 0.5f * p * (p + 1.f) * xp2;
   df = (-0.5f * (p + 1.f) * (p + 2.f) * p * xp1 + p * (p + 2.f) * (p + 1.f) * xp - 0.5f * p * (p + 1.f) * (p + 2.f) * xp1p) /
-       rp.r_max;
+       r;
 }
 
+// polynomial cutoff of the radial basis and its derivative in d
+__device__ __forceinline__ void poly_cut(float d, const MaceRadial& rp, float& f, float& df) {
+  poly_env(d, rp.r_max, rp.p, f, df);
+}
+
+// Agnesi transform x = 1 + a s^q / (1 + s^(q - p)), s = d / r0, and dx/dd
+__device__ __forceinline__ void agnesi(float d, float r0, const MaceCore& c, float& x, float& dx) {
+  const float s = d / r0, sq = powf(s, c.aq), sqp = powf(s, c.aq - c.ap), den = 1.f / (1.f + sqp);
+  x = 1.f + c.aa * sq * den;
+  dx = c.aa * (sq / s) * (c.aq + c.ap * sqp) * den * den / r0;
+}
+
+// ZBL energy of one directed edge u -> v, V = 1/2 14.3996 Z_u Z_v / d phi(d / a_uv) env_p(d / (rho'_u + rho'_v)), and dV/dd
+__device__ __forceinline__ void zbl(float d, float4 eu, float4 ev, const MaceCore& c, float& V, float& dV) {
+  float env, denv;
+  poly_env(d, eu.z + ev.z, c.zp, env, denv);
+  const float ia = (eu.y + ev.y) / c.za, t = d * ia;  // 1 / a_uv
+  const float x0 = expf(-3.2f * t), x1 = expf(-0.9423f * t), x2 = expf(-0.4029f * t), x3 = expf(-0.2016f * t);
+  const float phi = c.zc[0] * x0 + c.zc[1] * x1 + c.zc[2] * x2 + c.zc[3] * x3;
+  const float dphi = -ia * (3.2f * c.zc[0] * x0 + 0.9423f * c.zc[1] * x1 + 0.4029f * c.zc[2] * x2 + 0.2016f * c.zc[3] * x3);
+  const float k = 0.5f * 14.3996f * eu.x * ev.x, rd = 1.f / d;
+  V = k * rd * phi * env;
+  dV = k * rd * ((dphi - phi * rd) * env + phi * denv);
+}
+
+template <bool kSpecies>
 __global__ void k_mace_edge_geom(int64_t E, const float4* __restrict__ e_vec, MaceRadial rp, int nsh,
-                                 float* __restrict__ Y, float* __restrict__ eb) {
+                                 float* __restrict__ Y, float* __restrict__ eb, const int* __restrict__ e_src,
+                                 const int* __restrict__ e_dst, const int* __restrict__ type, MaceCore core) {
   const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (e >= E) return;
   const float4 v = e_vec[e];
@@ -98,7 +125,29 @@ __global__ void k_mace_edge_geom(int64_t E, const float4* __restrict__ e_vec, Ma
   for (int k = 0; k < kMaceMaxNsh; k++) Y[e * kMaceMaxNsh + k] = k < nsh ? y[k] : 0.f;
   float f, df;
   poly_cut(d, rp, f, df);
-  for (int n = 0; n < rp.nbp; n++) eb[e * rp.nbp + n] = n < rp.nb ? rp.pref * sinf(rp.w[n] * d) * rd * f : 0.f;
+  float xb = d, rxb = rd;  // the Bessel argument: d, or (kSpecies: Agnesi on) the transformed x; f stays f(d)
+  if constexpr (kSpecies) {
+    float dx;
+    agnesi(d, 0.5f * (core.elem[type[e_src[e]]].w + core.elem[type[e_dst[e]]].w), core, xb, dx);
+    rxb = 1.f / xb;
+  }
+  for (int n = 0; n < rp.nbp; n++) eb[e * rp.nbp + n] = n < rp.nb ? rp.pref * sinf(rp.w[n] * xb) * rxb * f : 0.f;
+}
+
+// one thread per owned atom i: e_lin[i] += sum_{e -> i} V_e in CSR row order, before any readout adds to it
+__global__ void k_mace_zbl(int n_own, const int* __restrict__ row_ptr, const int* __restrict__ e_src,
+                           const float4* __restrict__ e_vec, const int* __restrict__ type, MaceCore core,
+                           float* __restrict__ e_lin) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_own) return;
+  const float4 ev = core.elem[type[i]];
+  float s = 0.f;
+  for (int e = row_ptr[i]; e < row_ptr[i + 1]; e++) {
+    float V, dV;
+    zbl(e_vec[e].w, core.elem[type[e_src[e]]], ev, core, V, dV);
+    s += V;
+  }
+  e_lin[i] += s;
 }
 
 __global__ void k_mace_embed(int n, int C, const int* __restrict__ type, const float* __restrict__ W,
@@ -507,13 +556,15 @@ __device__ __forceinline__ void virial_reduce_mace(const float (&v)[9], double* 
     atomicAdd(&virial[threadIdx.x], s);
   }
 }
-template <bool kAtomic>
+// kSpecies: the ZBL term (core.zbl) and the chain rule through the Agnesi transform (core.agnesi), switched at run time
+template <bool kAtomic, bool kSpecies>
 __global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, const int* __restrict__ e_src,
                                                          const int* __restrict__ e_dst, const float4* __restrict__ e_vec,
                                                          const int* __restrict__ gid, MaceRadial rp,
                                                          const float* __restrict__ g_eb, const float* __restrict__ gY,
                                                          float* __restrict__ forces, double* __restrict__ virial,
-                                                         float* __restrict__ atom_vir) {
+                                                         float* __restrict__ atom_vir, const int* __restrict__ type,
+                                                         MaceCore core) {
   const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   float vir[9];
 #pragma unroll
@@ -525,12 +576,28 @@ __global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, con
     const float x = v.x * rd, y = v.y * rd, z = v.z * rd;
     float f, df;
     poly_cut(d, rp, f, df);
+    float xb = d, rxb = rd, dxb = 1.f;  // Bessel argument, its inverse and d(xb)/dd
+    float4 eu, ev;
+    if constexpr (kSpecies) {
+      eu = core.elem[type[e_src[e]]], ev = core.elem[type[e_dst[e]]];
+      if (core.agnesi) {
+        agnesi(d, 0.5f * (eu.w + ev.w), core, xb, dxb);
+        rxb = 1.f / xb;
+      }
+    }
     float gd = 0.f;
     for (int n = 0; n < rp.nb; n++) {
       float sn, cn;
-      sincosf(rp.w[n] * d, &sn, &cn);  // w_n d reaches num_bessel * pi: the accurate range reduction
-      const float b = rp.pref * sn * rd, db = rp.pref * (rp.w[n] * cn - sn * rd) * rd;
+      sincosf(rp.w[n] * xb, &sn, &cn);  // w_n d reaches num_bessel * pi: the accurate range reduction
+      const float b = rp.pref * sn * rxb, db = rp.pref * (rp.w[n] * cn - sn * rxb) * rxb * dxb;
       gd = fmaf(g_eb[(size_t)e * rp.nbp + n], db * f + b * df, gd);
+    }
+    if constexpr (kSpecies) {
+      if (core.zbl) {
+        float V, dV;
+        zbl(d, eu, ev, core, V, dV);
+        gd = fmaf(core.zscale, dV, gd);
+      }
     }
     Dual Yd[kMaceMaxNsh];
     sh16<Dual>(Dual{x, 1.f, 0.f, 0.f}, Dual{y, 0.f, 1.f, 0.f}, Dual{z, 0.f, 0.f, 1.f}, Dual{1.f, 0.f, 0.f, 0.f}, nsh, Yd);
@@ -569,8 +636,15 @@ __global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, con
 // launchers
 // ---------------------------------------------------------------------------------------------
 void launch_mace_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const MaceRadial& rp, int nsh, float* Y,
-                           float* eb) {
-  MACE_LAUNCH(k_mace_edge_geom, E, 256, st, E, e_vec, rp, nsh, Y, eb);
+                           float* eb, const int* e_src, const int* e_dst, const int* type, const MaceCore& core) {
+  if (core.agnesi)
+    MACE_LAUNCH(k_mace_edge_geom<true>, E, 256, st, E, e_vec, rp, nsh, Y, eb, e_src, e_dst, type, core);
+  else
+    MACE_LAUNCH(k_mace_edge_geom<false>, E, 256, st, E, e_vec, rp, nsh, Y, eb, e_src, e_dst, type, core);
+}
+void launch_mace_zbl(cudaStream_t st, int n_own, const int* row_ptr, const int* e_src, const float4* e_vec,
+                     const int* type, const MaceCore& core, float* e_lin) {
+  MACE_LAUNCH(k_mace_zbl, n_own, 128, st, n_own, row_ptr, e_src, e_vec, type, core, e_lin);
 }
 void launch_mace_embed(cudaStream_t st, int n, int C, const int* type, const float* W, float* h0) {
   MACE_LAUNCH(k_mace_embed, (int64_t)n * C, 256, st, n, C, type, W, h0);
@@ -654,14 +728,20 @@ void launch_mace_symc_eq_bwd(cudaStream_t st, int n_own, int C, int nsh, int Kto
   MACE_LAUNCH(k_mace_symc_eq<true>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, gB, gA);
 }
 void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
-                            const int* gid, const MaceRadial& rp, const float* g_eb, const float* gY, float* forces,
-                            double* virial, float* atom_vir) {
-  if (atom_vir)
-    MACE_LAUNCH(k_mace_edge_final<true>, E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial,
-                atom_vir);
-  else
-    MACE_LAUNCH(k_mace_edge_final<false>, E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial,
-                atom_vir);
+                            const int* gid, const int* type, const MaceRadial& rp, const MaceCore& core,
+                            const float* g_eb, const float* gY, float* forces, double* virial, float* atom_vir) {
+#define MACE_EDGE_FINAL(A, S)                                                                                     \
+  MACE_LAUNCH((k_mace_edge_final<A, S>), E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial, \
+              atom_vir, type, core)
+  const bool sp = core.zbl || core.agnesi;
+  if (atom_vir) {
+    if (sp) MACE_EDGE_FINAL(true, true);
+    else MACE_EDGE_FINAL(true, false);
+  } else {
+    if (sp) MACE_EDGE_FINAL(false, true);
+    else MACE_EDGE_FINAL(false, false);
+  }
+#undef MACE_EDGE_FINAL
 }
 
 }  // namespace b2m

@@ -21,6 +21,18 @@ struct MaceRadial {
   float w[64];  // Bessel frequencies
 };
 
+// ZBL pair repulsion (mace's ZBLBasis) and the Agnesi distance transform (AgnesiTransform), tests/mace_zbl_ref.py; each
+// is on when its state_dict keys are loaded (DESIGN §11.2)
+struct MaceCore {
+  const float4* elem = nullptr;  // [n_elem]: (Z, Z^a_exp, ZBL covalent radius, Agnesi covalent radius)
+  int zbl = 0, agnesi = 0;
+  int zp = 6;                    // ZBL envelope exponent
+  float za = 0.f;                // a_prefactor * 0.529
+  float zc[4] = {0.f, 0.f, 0.f, 0.f};
+  float zscale = 0.f;            // the model's scale: dE/dd of an edge gains scale * dV/dd
+  float aq = 0.f, ap = 0.f, aa = 0.f;  // Agnesi q, p, a
+};
+
 // one term coef * A[i1] A[i2] A[i3] (first nu factors) of the symmetric contraction, weighted by w[z][kg][c], added to
 // output slot o (0: the 0e output; 1 + m: component m of the 1o output; always 0 on layers with scalar output)
 struct MaceTerm {
@@ -40,8 +52,12 @@ __host__ __device__ constexpr int mace_npaths(int max_ell) { return 3 * max_ell 
 __host__ __device__ constexpr int mace_nslots(int max_ell) { return mace_slot_base(max_ell, max_ell + 1); }
 constexpr int kMaceMaxSlots = mace_nslots(3);  // 40
 
+// Y, eb; with the Agnesi transform on, the Bessel argument is x(d, Z_src, Z_dst) (endpoint species type[e_src / e_dst])
 void launch_mace_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const MaceRadial& rp, int nsh, float* Y,
-                           float* eb);
+                           float* eb, const int* e_src, const int* e_dst, const int* type, const MaceCore& core);
+// e_lin[i] += sum of the ZBL energies V_e of the edges e -> i, in CSR row order (no atomics)
+void launch_mace_zbl(cudaStream_t st, int n_own, const int* row_ptr, const int* e_src, const float4* e_vec,
+                     const int* type, const MaceCore& core, float* e_lin);
 void launch_mace_embed(cudaStream_t st, int n, int C, const int* type, const float* W, float* h0);
 void launch_mace_msg(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
                      const float* Y, const float* u, float* A);
@@ -82,8 +98,8 @@ void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const fl
 // gh[i][c] += scale * w[c]  (c < C, rows of pitch ld)
 void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh);
 void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
-                            const int* gid, const MaceRadial& rp, const float* g_eb, const float* gY, float* forces,
-                            double* virial, float* atom_vir = nullptr);
+                            const int* gid, const int* type, const MaceRadial& rp, const MaceCore& core,
+                            const float* g_eb, const float* gY, float* forces, double* virial, float* atom_vir);
 
 struct MaceLayerW {
   bool residual = true;
@@ -110,6 +126,7 @@ struct MaceState {
   std::vector<int> hw;    // row pitch of h[t], t = 0..T: C or 4 C
   double c_act = 1.0, scale = 1.0, shift = 0.0;
   MaceRadial rp{};
+  MaceCore core{};
   std::vector<int> hid;   // radial MLP hidden widths, padded to 64
   int interaction_residual[kMaceMaxLayers] = {0};
   double avg_nb[kMaceMaxLayers] = {0};

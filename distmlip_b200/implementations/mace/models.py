@@ -3,15 +3,18 @@
 `from_existing` takes any object with mace's attribute tree and `state_dict()` (mace itself need not be importable, so
 the model is recognised by structure, not by `isinstance`); `enable_distributed_mode(gpus)` validates the
 configuration and creates the engine (b2m_create_mace).  The arithmetic, with every e3nn / mace convention it relies on,
-is stated in oracle/mace_ref.py (scalar hidden features) and tests/mace_eq_ref.py (0e+1o); the kernels are
-csrc/kernels_mace.cu.
+is stated in oracle/mace_ref.py (scalar hidden features), tests/mace_eq_ref.py (0e+1o) and tests/mace_zbl_ref.py (the
+ZBL pair repulsion and the Agnesi distance transform); the kernels are csrc/kernels_mace.cu.
 
 Supported configuration (anything else raises NotImplementedError in enable_distributed_mode): ScaleShiftMACE with one
 head, hidden_irreps = C x 0e or C x 0e + C x 1o (C a multiple of 32, C <= 128; the shapes of MACE-MP-0 "small" and
 "medium"), max_ell <= 3 (>= 1 with 1o), correlation <= 3, Bessel radial basis
 (num_bessel <= 64) times PolynomialCutoff, a FullyConnectedNet radial MLP (hidden widths <= 64),
 RealAgnosticResidualInteractionBlock or RealAgnosticInteractionBlock per layer, LinearReadoutBlock on every layer but the
-last and NonLinearReadoutBlock (gated SiLU) on the last; no pair repulsion, no distance transform.
+last and NonLinearReadoutBlock (gated SiLU) on the last.  Optional, as in the MACE-MP-0b / MPA-0 / OMAT-0 checkpoints:
+`pair_repulsion` (ZBLBasis, keys pair_repulsion_fn.{c, a_exp, a_prefactor, p, covalent_radii}) and an AgnesiTransform
+`radial_embedding.distance_transform` (keys q, p, a, covalent_radii).  Other transforms and `apply_cutoff = False` are
+refused.
 """
 from __future__ import annotations
 
@@ -26,6 +29,9 @@ SILU_2MOM = 1.6765324703310909
 
 _RESIDUAL = "RealAgnosticResidualInteractionBlock"
 _PLAIN = "RealAgnosticInteractionBlock"
+# mace's ZBLBasis and AgnesiTransform state_dict keys (tests/mace_zbl_ref.py); the engine turns each on when they load
+_ZBL, _ZBL_KEYS = "pair_repulsion_fn.", {"c", "a_exp", "a_prefactor", "p", "covalent_radii"}
+_AGNESI, _AGNESI_KEYS = "radial_embedding.distance_transform.", {"q", "p", "a", "covalent_radii"}
 
 
 def _parse_irreps(text):
@@ -72,12 +78,32 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
         heads = self._attr("heads", None)
         if heads is not None and len(heads) > 1:
             raise NotImplementedError(f"multi-head models are not supported (heads={list(heads)})")
-        if self._attr("pair_repulsion", False) or any(k.startswith("pair_repulsion_fn.") for k in sd):
-            raise NotImplementedError("pair_repulsion (ZBL) is not supported")
+        zbl = {k[len(_ZBL):] for k in sd if k.startswith(_ZBL)}
+        if self._attr("pair_repulsion", False) or zbl:
+            if not zbl:
+                raise NotImplementedError("pair_repulsion = True without pair_repulsion_fn weights is not supported")
+            if zbl != _ZBL_KEYS:
+                odd = sorted(zbl - _ZBL_KEYS) or sorted(_ZBL_KEYS - zbl)
+                raise NotImplementedError(f"pair_repulsion (ZBL): pair_repulsion_fn.{odd[0]} is " +
+                                          ("not a ZBLBasis key" if zbl - _ZBL_KEYS else "missing") +
+                                          f"; the keys must be {sorted(_ZBL_KEYS)}")
+            if sd[_ZBL + "c"].numel() != 4:
+                raise NotImplementedError("pair_repulsion (ZBL): pair_repulsion_fn.c must have 4 coefficients")
         rad = self._attr("radial_embedding")
-        if getattr(rad, "distance_transform", None) is not None or any(".distance_transform." in k for k in sd):
-            raise NotImplementedError("radial distance_transform is not supported")
-        if any(k.startswith("radial_embedding.") and k.split(".")[1] not in ("bessel_fn", "cutoff_fn") for k in sd):
+        dt = getattr(rad, "distance_transform", None)
+        agn = {k[len(_AGNESI):] for k in sd if k.startswith(_AGNESI)}
+        if dt is not None or any(".distance_transform." in k for k in sd):
+            if type(dt).__name__ != "AgnesiTransform":
+                raise NotImplementedError(f"radial distance_transform {type(dt).__name__} is not supported "
+                                          "(only AgnesiTransform)")
+            if agn != _AGNESI_KEYS or any(".distance_transform." in k and not k.startswith(_AGNESI) for k in sd):
+                raise NotImplementedError(f"radial distance_transform (AgnesiTransform): the keys must be "
+                                          f"{sorted(_AGNESI_KEYS)} under {_AGNESI}, not {sorted(agn)}")
+        if getattr(rad, "apply_cutoff", True) is False:
+            raise NotImplementedError("radial_embedding.apply_cutoff = False (the cutoff after the radial MLP) is not "
+                                      "supported")
+        if any(k.startswith("radial_embedding.") and k.split(".")[1] not in ("bessel_fn", "cutoff_fn", "distance_transform")
+               for k in sd):
             raise NotImplementedError("radial_type other than the Bessel basis is not supported")
         if "radial_embedding.bessel_fn.bessel_weights" not in sd:
             raise NotImplementedError("radial_type other than the Bessel basis is not supported")

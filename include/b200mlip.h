@@ -103,7 +103,11 @@ int b2m_create_tensornet(const b2m_tensornet_desc* desc, const int* devices, int
  * tests/mace_eq_ref.py).
  * Supported: one head, C a multiple of 32 with C <= 128, max_ell <= 3, correlation <= 3, Bessel basis x polynomial cutoff,
  * an e3nn FullyConnectedNet radial MLP (hidden widths <= 64), RealAgnostic(Residual)InteractionBlock per layer, linear
- * readouts and a gated non-linear last readout.  Edges are every periodic image closer than r_max (no bond graph).
+ * readouts and a gated non-linear last readout; optionally mace's ZBL pair repulsion (keys pair_repulsion_fn.{c, a_exp,
+ * a_prefactor, p, covalent_radii}) and Agnesi distance transform (radial_embedding.distance_transform.{q, p, a,
+ * covalent_radii}), each turned on by loading its keys (DESIGN.md §11.2; this struct does not change).  A partial key set,
+ * a wrong shape, an atomic number beyond a covalent_radii table or a non-integer ZBL p fails b2m_finalize_weights with
+ * B2M_ERR_INVALID.  Edges are every periodic image closer than r_max (no bond graph).
  * Scale, shift and the atomic energies E0 come from the state_dict: b2m_set_scaling and b2m_set_element_refs return
  * B2M_ERR_INVALID on such a handle, as do b2m_get_sitewise and b2m_set_heat_flux.  b2m_set_atomic / b2m_get_atomic give
  * energies[i] = E0[z_i] + scale * e_i + shift and the per-atom virials. */
