@@ -1648,7 +1648,6 @@ int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9)
 int b2m_set_heat_flux(b2m_handle h, double reach) {
   API_BEGIN
   B2M_REQUIRE(reach >= 0 && std::isfinite(reach), B2M_ERR_INVALID, "heat-flux reach must be >= 0");
-  B2M_REQUIRE(h->kind != 2, B2M_ERR_INVALID, "the heat flux is not implemented for MACE");
   each_member(h, [&](b2m_engine* e) { e->hf_reach = reach; });
   API_END
 }

@@ -498,12 +498,15 @@ __global__ void k_mace_readout_lin(int n_own, int C, int ld, const float* __rest
   if (lane == 0) e_lin[r] += s;
 }
 
-template <bool kAtomic>
+// kWeighted: eps_i (E0, scale and shift included) times wgt[gid[r]] in the energy sum and atom_e (heat flux: cell mask or
+// position seed); e_lin is weighted here, so k_mace_readout_lin and k_mace_zbl stay unweighted
+template <bool kAtomic, bool kWeighted = false>
 __global__ void k_mace_readout_final(int n_own, int C, int H, const float* __restrict__ h, const float* __restrict__ W1,
                                      const float* __restrict__ w2, const float* __restrict__ e_lin,
                                      const int* __restrict__ type, const double* __restrict__ E0, double scale,
                                      double shift, float* __restrict__ pre, double* __restrict__ energy,
-                                     const int* __restrict__ gid, double* __restrict__ atom_e) {
+                                     const int* __restrict__ gid, double* __restrict__ atom_e,
+                                     const float* __restrict__ wgt) {
   const int r = (int)((blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (r >= n_own) return;
   float e = 0.f;
@@ -515,26 +518,34 @@ __global__ void k_mace_readout_final(int n_own, int C, int H, const float* __res
     e = fmaf(silu_f(s), w2[j], e);
   }
   if (lane == 0) {
-    const double eps = E0[type[r]] + scale * ((double)e_lin[r] + (double)e) + shift;
+    double eps = E0[type[r]] + scale * ((double)e_lin[r] + (double)e) + shift;
+    if constexpr (kWeighted) eps *= (double)wgt[gid[r]];
     if constexpr (kAtomic) atom_e[gid[r]] = eps;
     atomicAdd(energy, eps);
   }
 }
 
+// kWeighted: row r's seed times wgt[gid[r]]
+template <bool kWeighted = false>
 __global__ void k_mace_readout_seed(int n_own, int C, int H, const float* __restrict__ pre, const float* __restrict__ W1,
-                                    const float* __restrict__ w2, float scale, float* __restrict__ gh) {
+                                    const float* __restrict__ w2, float scale, float* __restrict__ gh,
+                                    const int* __restrict__ gid, const float* __restrict__ wgt) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= (int64_t)n_own * C) return;
   const int r = (int)(i / C), c = (int)(i % C);
+  if constexpr (kWeighted) scale *= wgt[gid[r]];
   float s = 0.f;
   for (int j = 0; j < H; j++) s = fmaf(W1[(size_t)c * H + j] * w2[j], dsilu_f(pre[(size_t)r * H + j]), s);
   gh[i] = scale * s;
 }
 
+// adjoint of a linear readout; kWeighted: row r's term times wgt[gid[r]]
+template <bool kWeighted = false>
 __global__ void k_mace_add_row(int n_own, int C, int ld, const float* __restrict__ w, float scale,
-                               float* __restrict__ gh) {
+                               float* __restrict__ gh, const int* __restrict__ gid, const float* __restrict__ wgt) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= (int64_t)n_own * C) return;
+  if constexpr (kWeighted) scale *= wgt[gid[i / C]];
   gh[(i / C) * ld + i % C] += scale * w[i % C];
 }
 
@@ -557,14 +568,17 @@ __device__ __forceinline__ void virial_reduce_mace(const float (&v)[9], double* 
   }
 }
 // kSpecies: the ZBL term (core.zbl) and the chain rule through the Agnesi transform (core.agnesi), switched at run time
-template <bool kAtomic, bool kSpecies>
+// kWeighted (with kSpecies): the ZBL term times wgt[gid[dst]], the readout weight of the atom its pair energy belongs to;
+// g_eb and gY carry the weights already (they are adjoints of the weighted readouts)
+template <bool kAtomic, bool kSpecies, bool kWeighted = false>
 __global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, const int* __restrict__ e_src,
                                                          const int* __restrict__ e_dst, const float4* __restrict__ e_vec,
                                                          const int* __restrict__ gid, MaceRadial rp,
                                                          const float* __restrict__ g_eb, const float* __restrict__ gY,
                                                          float* __restrict__ forces, double* __restrict__ virial,
                                                          float* __restrict__ atom_vir, const int* __restrict__ type,
-                                                         MaceCore core) {
+                                                         MaceCore core, const float* __restrict__ wgt) {
+  static_assert(kSpecies || !kWeighted, "only the ZBL term needs the weight");
   const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   float vir[9];
 #pragma unroll
@@ -596,7 +610,9 @@ __global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, con
       if (core.zbl) {
         float V, dV;
         zbl(d, eu, ev, core, V, dV);
-        gd = fmaf(core.zscale, dV, gd);
+        float zs = core.zscale;
+        if constexpr (kWeighted) zs *= wgt[gid[e_dst[e]]];
+        gd = fmaf(zs, dV, gd);
       }
     }
     Dual Yd[kMaceMaxNsh];
@@ -678,20 +694,30 @@ void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, int ld, const fl
 }
 void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
                                const float* e_lin, const int* type, const double* E0, double scale, double shift,
-                               float* pre, double* energy, const int* gid, double* atom_e) {
-  if (atom_e)
-    MACE_LAUNCH(k_mace_readout_final<true>, (int64_t)n_own * 32, 256, st, n_own, C, H, h, W1, w2, e_lin, type, E0, scale,
-                shift, pre, energy, gid, atom_e);
-  else
-    MACE_LAUNCH(k_mace_readout_final<false>, (int64_t)n_own * 32, 256, st, n_own, C, H, h, W1, w2, e_lin, type, E0, scale,
-                shift, pre, energy, gid, atom_e);
+                               float* pre, double* energy, const int* gid, double* atom_e, const float* wgt) {
+#define MACE_READOUT_FINAL(A, W)                                                                                       \
+  MACE_LAUNCH((k_mace_readout_final<A, W>), (int64_t)n_own * 32, 256, st, n_own, C, H, h, W1, w2, e_lin, type, E0, scale, \
+              shift, pre, energy, gid, atom_e, wgt)
+  if (wgt) {
+    if (atom_e) MACE_READOUT_FINAL(true, true);
+    else MACE_READOUT_FINAL(false, true);
+  } else {
+    if (atom_e) MACE_READOUT_FINAL(true, false);
+    else MACE_READOUT_FINAL(false, false);
+  }
+#undef MACE_READOUT_FINAL
 }
 void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const float* pre, const float* W1,
-                              const float* w2, float scale, float* gh) {
-  MACE_LAUNCH(k_mace_readout_seed, (int64_t)n_own * C, 256, st, n_own, C, H, pre, W1, w2, scale, gh);
+                              const float* w2, float scale, float* gh, const int* gid, const float* wgt) {
+  if (wgt)
+    MACE_LAUNCH(k_mace_readout_seed<true>, (int64_t)n_own * C, 256, st, n_own, C, H, pre, W1, w2, scale, gh, gid, wgt);
+  else
+    MACE_LAUNCH(k_mace_readout_seed<false>, (int64_t)n_own * C, 256, st, n_own, C, H, pre, W1, w2, scale, gh, gid, wgt);
 }
-void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh) {
-  MACE_LAUNCH(k_mace_add_row, (int64_t)n_own * C, 256, st, n_own, C, ld, w, scale, gh);
+void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh,
+                         const int* gid, const float* wgt) {
+  if (wgt) MACE_LAUNCH(k_mace_add_row<true>, (int64_t)n_own * C, 256, st, n_own, C, ld, w, scale, gh, gid, wgt);
+  else MACE_LAUNCH(k_mace_add_row<false>, (int64_t)n_own * C, 256, st, n_own, C, ld, w, scale, gh, gid, wgt);
 }
 void launch_mace_msg_eq(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
                         const float* R, const float* Y, const float* u, float* Am) {
@@ -729,17 +755,21 @@ void launch_mace_symc_eq_bwd(cudaStream_t st, int n_own, int C, int nsh, int Kto
 }
 void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
                             const int* gid, const int* type, const MaceRadial& rp, const MaceCore& core,
-                            const float* g_eb, const float* gY, float* forces, double* virial, float* atom_vir) {
-#define MACE_EDGE_FINAL(A, S)                                                                                     \
-  MACE_LAUNCH((k_mace_edge_final<A, S>), E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial, \
-              atom_vir, type, core)
+                            const float* g_eb, const float* gY, float* forces, double* virial, float* atom_vir,
+                            const float* wgt) {
+#define MACE_EDGE_FINAL(A, S, W)                                                                                     \
+  MACE_LAUNCH((k_mace_edge_final<A, S, W>), E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial, \
+              atom_vir, type, core, wgt)
   const bool sp = core.zbl || core.agnesi;
-  if (atom_vir) {
-    if (sp) MACE_EDGE_FINAL(true, true);
-    else MACE_EDGE_FINAL(true, false);
+  if (wgt && core.zbl) {  // without the pair term the weights are all in g_eb and gY
+    if (atom_vir) MACE_EDGE_FINAL(true, true, true);
+    else MACE_EDGE_FINAL(false, true, true);
+  } else if (atom_vir) {
+    if (sp) MACE_EDGE_FINAL(true, true, false);
+    else MACE_EDGE_FINAL(true, false, false);
   } else {
-    if (sp) MACE_EDGE_FINAL(false, true);
-    else MACE_EDGE_FINAL(false, false);
+    if (sp) MACE_EDGE_FINAL(false, true, false);
+    else MACE_EDGE_FINAL(false, false, false);
   }
 #undef MACE_EDGE_FINAL
 }

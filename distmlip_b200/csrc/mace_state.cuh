@@ -88,18 +88,21 @@ void launch_mace_symc_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, 
 // e_lin[i] += h[i][0:C] . w   (linear readouts; w carries 1 / sqrt(C); rows of pitch ld)
 void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, int ld, const float* h, const float* w, float* e_lin);
 // eps_i = E0[z] + scale * (e_lin + act(h W1) . w2) + shift; pre [n][H] kept for the reverse; energy += sum eps
-// atom_e != nullptr: atom_e[gid[i]] = eps_i
+// atom_e != nullptr: atom_e[gid[i]] = eps_i.  wgt != nullptr (heat flux, DESIGN.md §10): eps_i times wgt[gid[i]]
 void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
                                const float* e_lin, const int* type, const double* E0, double scale, double shift,
-                               float* pre, double* energy, const int* gid, double* atom_e);
-// gh[i][c] = scale * sum_j W1[c][j] w2[j] SiLU'(pre[i][j])
+                               float* pre, double* energy, const int* gid, double* atom_e, const float* wgt);
+// gh[i][c] = scale * sum_j W1[c][j] w2[j] SiLU'(pre[i][j])   (wgt != nullptr: times wgt[gid[i]])
 void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const float* pre, const float* W1,
-                              const float* w2, float scale, float* gh);
-// gh[i][c] += scale * w[c]  (c < C, rows of pitch ld)
-void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh);
+                              const float* w2, float scale, float* gh, const int* gid, const float* wgt);
+// gh[i][c] += scale * w[c]  (c < C, rows of pitch ld; wgt != nullptr: times wgt[gid[i]])
+void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh,
+                         const int* gid, const float* wgt);
+// wgt != nullptr: the ZBL term of edge e times wgt[gid[dst(e)]]
 void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
                             const int* gid, const int* type, const MaceRadial& rp, const MaceCore& core,
-                            const float* g_eb, const float* gY, float* forces, double* virial, float* atom_vir);
+                            const float* g_eb, const float* gY, float* forces, double* virial, float* atom_vir,
+                            const float* wgt);
 
 struct MaceLayerW {
   bool residual = true;

@@ -14,7 +14,7 @@ RealAgnosticResidualInteractionBlock or RealAgnosticInteractionBlock per layer, 
 last and NonLinearReadoutBlock (gated SiLU) on the last.  Optional, as in the MACE-MP-0b / MPA-0 / OMAT-0 checkpoints:
 `pair_repulsion` (ZBLBasis, keys pair_repulsion_fn.{c, a_exp, a_prefactor, p, covalent_radii}) and an AgnesiTransform
 `radial_embedding.distance_transform` (keys q, p, a, covalent_radii).  Other transforms and `apply_cutoff = False` are
-refused.
+refused.  `evaluate_heat_flux` adds the Green-Kubo heat flux of the unfolded cell (DESIGN.md §10) to `evaluate`.
 """
 from __future__ import annotations
 
@@ -70,7 +70,10 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
         return super().from_existing(model, dtype)
 
     def heat_flux_reach(self):
-        raise NotImplementedError("the heat flux is not implemented for MACE")
+        """Receptive-field radius (Angstrom) of an atom's energy, num_interactions * r_max (DESIGN.md §10): h[0] depends
+        on the species only, each interaction adds one r_max hop (the readout of layer t sees t + 1 of them), and the
+        ZBL pair term and the Agnesi transform act within one edge."""
+        return len(self._attr("interactions")) * float(self._attr("r_max"))
 
     def _describe(self):
         """b2m_mace_desc fields of the model, or NotImplementedError naming the first unsupported option"""
@@ -252,19 +255,42 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
     def evaluate(self, atoms, forces=True, stress=True, atomic=False):
         """One evaluation on the engine: (energy, forces [n, 3] eV/A, stress [3, 3] GPa, per-atom energies or None,
         per-atom virials [n, 3, 3] eV or None)."""
+        return self._evaluate(atoms, forces, stress, atomic, 0.0, None)
+
+    def evaluate_heat_flux(self, atoms, velocities, reach=None, atomic=False):
+        """`evaluate` (energy, forces and stress always) plus the heat flux (J_pot [3], J_conv [3]) of velocities
+        [n, 3] (DESIGN.md §10), in eV * velocity unit and not divided by the volume: J_conv = sum_i eps_i v_i over the
+        per-atom energies eps_i (E0 and shift included), without the kinetic term.  Every other output is the periodic
+        one.  reach (Angstrom) defaults to heat_flux_reach() and may not be below it; a later `evaluate` goes back to
+        the periodic graph."""
+        need = self.heat_flux_reach()
+        reach = need if reach is None else float(reach)
+        if reach < need:
+            raise ValueError(f"heat_flux_reach={reach} is below the model's receptive field {need}")
+        v = np.asarray(velocities, dtype=np.float64)
+        if v.shape != (len(atoms), 3):
+            raise ValueError(f"velocities must be [{len(atoms)}, 3], not {list(v.shape)}")
+        return self._evaluate(atoms, True, True, atomic, reach, v)
+
+    def _evaluate(self, atoms, forces, stress, atomic, reach, velocities):
         if not self.__dict__.get("dist_enabled"):
             raise RuntimeError("call enable_distributed_mode(gpus) first")
         eng = self._engine
         if bool(atomic) != self.__dict__.get("_atomic_on", False):
             eng.set_atomic(bool(atomic))
             self._atomic_on = bool(atomic)
+        self._set_heat_flux(reach, None)  # before the graph build, which unfolds the cell when reach > 0
         eng.set_structure(np.asarray(atoms.get_positions(wrap=False), dtype=np.float64), np.array(atoms.get_cell()),
                           self._species_of(atoms), np.asarray(atoms.get_pbc(), dtype=np.int32))
-        e, f, s = eng.compute(forces=forces, stress=stress)
+        flux = None
+        if velocities is not None:
+            e, f, s, flux = eng.compute_heat_flux(velocities)
+        else:
+            e, f, s = eng.compute(forces=forces, stress=stress)
         ae = av = None
         if atomic:
             ae, av = eng.atomic(virials=forces or stress)
-        return e, f, s, ae, av
+        return (e, f, s, ae, av) if flux is None else (e, f, s, ae, av, flux)
 
     def dist_forward(self, *args, **kwargs):
         raise NotImplementedError("dist_forward over torch graphs does not exist here; use MACECalculator_Dist")

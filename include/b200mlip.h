@@ -109,8 +109,9 @@ int b2m_create_tensornet(const b2m_tensornet_desc* desc, const int* devices, int
  * a wrong shape, an atomic number beyond a covalent_radii table or a non-integer ZBL p fails b2m_finalize_weights with
  * B2M_ERR_INVALID.  Edges are every periodic image closer than r_max (no bond graph).
  * Scale, shift and the atomic energies E0 come from the state_dict: b2m_set_scaling and b2m_set_element_refs return
- * B2M_ERR_INVALID on such a handle, as do b2m_get_sitewise and b2m_set_heat_flux.  b2m_set_atomic / b2m_get_atomic give
- * energies[i] = E0[z_i] + scale * e_i + shift and the per-atom virials. */
+ * B2M_ERR_INVALID on such a handle, as does b2m_get_sitewise.  b2m_set_atomic / b2m_get_atomic give
+ * energies[i] = E0[z_i] + scale * e_i + shift and the per-atom virials; b2m_compute_heat_flux weights that whole energy
+ * (its J_conv uses it, E0 and shift included). */
 typedef struct {
   int32_t n_elem;                 /* len(atomic_numbers)                                                 */
   int32_t channels;               /* C of hidden_irreps = C x 0e (+ C x 1o)                              */
@@ -173,7 +174,8 @@ int b2m_set_atomic(b2m_handle h, int on);
 int b2m_get_atomic(b2m_handle h, double* energies, float* virials);
 
 /* Heat flux of the model (DESIGN.md "Heat flux"), off by default (reach = 0).  With reach > 0 (Angstrom, at least the
- * model's receptive field: n_blocks * r_cut for CHGNet, (n_blocks + 1) * r_cut for TensorNet) the following
+ * model's receptive field: n_blocks * r_cut for CHGNet, (n_blocks + 1) * r_cut for TensorNet, num_interactions * r_max
+ * for MACE) the following
  * b2m_set_structure calls build the unfolded cell: the natoms cell atoms, then every periodic image within `reach` of
  * them along the periodic axes, evaluated without periodicity with the energy U = sum of the cell atoms' energies.
  * On such a handle b2m_compute (and b2m_compute_resident, b2m_get_results) returns the periodic energy, forces [natoms][3]
