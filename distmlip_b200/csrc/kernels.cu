@@ -176,7 +176,8 @@ __device__ __forceinline__ void stage_w(float* Wsm, const float* __restrict__ g,
   fence_proxy_async_smem();
 }
 
-// running segmented sum over rows [r0, r1) of a smem tile column, flushed with atomics when the key changes
+// running segmented sum over rows [r0, r1) of a smem tile column, flushed with atomics when the key changes (the
+// atom-conv backward's gC sum: a column per thread; the other kernels use scatter_rows below)
 __device__ __forceinline__ void seg_flush(const float* tile, int ld, int col, int r0, int r1, const int* key,
                                           float* __restrict__ out, int width) {
   float sum = 0.f;
@@ -484,6 +485,62 @@ __device__ __forceinline__ void red_add_v4(float* p, float4 v) {
                : "memory");
 }
 
+// one row of a running segmented sum: `sum` collects the rows of key `cur` and is reduced into out[cur] when the key
+// changes; rows with k < 0 contribute nothing.  The lane owns columns col .. col + 3 of out's rows of `width` floats.
+__device__ __forceinline__ void seg_add(float* out, int width, int col, int k, const float4& v, int& cur, float4& sum) {
+  if (k != cur) {
+    if (cur >= 0) red_add_v4(out + (size_t)cur * width + col, sum);
+    cur = k;
+    sum = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  if (k >= 0) sum.x += v.x, sum.y += v.y, sum.z += v.z, sum.w += v.w;
+}
+
+// Scatter phase of a [TM][LDE] tile, columns 0 .. 4 LPR - 1, in one pass: LPR lanes take a row (lane q its columns
+// 4 q .. 4 q + 3, one LDS.128; a row is contiguous, so the loads are conflict-free at any pitch) and a thread walks
+// R = TM LPR / NT consecutive rows.  Its float4 of row r
+//   - is added to gat[gidx[r]]                                                    (gat != nullptr, gidx[r] >= 0),
+//   - goes into one running sum per key array, reduced into out0[key0[.]] / out1[key1[.]] when the key changes and
+//     after the thread's last row                                                 (out != nullptr, key >= 0).
+// Outputs are rows of 4 LPR floats, and every addition to them is one red.v4.  Rows past the end of a partial tile have
+// all indices < 0.  The indices are equal in the lanes that share a row, so with LPR = 32 no branch diverges.  A run of
+// equal keys that crosses the R-row boundary between two threads is reduced in two parts.  Values and indices are
+// loaded eight rows at a time before those rows are walked: the reductions (asm volatile) keep loads in program order.
+template <int LPR>
+__device__ __forceinline__ void scatter_rows(const float* tile, const int* key0, float* out0, const int* key1,
+                                             float* out1, const int* gidx, float* gat) {
+  constexpr int R = TM * LPR / NT, W = 4 * LPR, B = 8;
+  static_assert(R % B == 0 && B % 4 == 0, "batches of B rows, their indices read as int4");
+  const int q = threadIdx.x % LPR, r0 = threadIdx.x / LPR * R;
+  float4 s0 = make_float4(0.f, 0.f, 0.f, 0.f), s1 = s0;
+  int c0 = -1, c1 = -1;
+#pragma unroll
+  for (int b = 0; b < R; b += B) {
+    float4 v[B];
+    int k0[B], k1[B], kg[B];
+#pragma unroll
+    for (int i = 0; i < B; i++) v[i] = *reinterpret_cast<const float4*>(tile + (r0 + b + i) * LDE + 4 * q);
+    auto ld_idx = [&](const int* idx, bool on, int(&k)[B]) {
+#pragma unroll
+      for (int i = 0; i < B; i += 4) {
+        const int4 x = on ? *reinterpret_cast<const int4*>(idx + r0 + b + i) : make_int4(-1, -1, -1, -1);
+        k[i] = x.x, k[i + 1] = x.y, k[i + 2] = x.z, k[i + 3] = x.w;
+      }
+    };
+    ld_idx(key0, out0 != nullptr, k0);
+    ld_idx(key1, out1 != nullptr, k1);
+    ld_idx(gidx, gat != nullptr, kg);
+#pragma unroll
+    for (int i = 0; i < B; i++) {
+      if (kg[i] >= 0) red_add_v4(gat + (size_t)kg[i] * W + 4 * q, v[i]);
+      seg_add(out0, W, 4 * q, k0[i], v[i], c0, s0);
+      seg_add(out1, W, 4 * q, k1[i], v[i], c1, s1);
+    }
+  }
+  if (c0 >= 0) red_add_v4(out0 + (size_t)c0 * W + 4 * q, s0);
+  if (c1 >= 0) red_add_v4(out1 + (size_t)c1 * W + 4 * q, s1);
+}
+
 // ============================================================================================
 // atom conv: forward
 // ============================================================================================
@@ -600,10 +657,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
         }
     }
     __syncthreads();
-    {
-      const int c = tid & 63, part = tid >> 6;
-      seg_flush(tile, LDE, c, part * 32, part * 32 + 32, s_dst, a.agg, D);
-    }
+    scatter_rows<16>(tile, s_dst, a.agg, nullptr, nullptr, nullptr, nullptr);  // agg[dst] += m
   }
 }
 
@@ -1097,8 +1151,7 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
     }
     if (HIDDEN) {
       __syncthreads();
-      const int c = tid & 63, part = tid >> 6;
-      seg_flush(P, LDE, c, part * 32, part * 32 + 32, s_b, a.aggB, D);
+      scatter_rows<16>(P, s_b, a.aggB, nullptr, nullptr, nullptr, nullptr);  // aggB[b] += m
     }
   }
 }
@@ -1233,20 +1286,8 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
     }
     if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.WgTcan, 16384 * 4, sm.wbar());
     // ---- scatter phase (reads P and this tile's index arrays) ----
-    {
-      const int j = tid & 127, rh = tid >> 7;
-      seg_flush(P, LDE, j, rh * 64, rh * 64 + 64, s_b, a.gHb, D2);
-      seg_flush(P, LDE, j, rh * 64, rh * 64 + 64, s_c, a.gXc, D2);
-    }
-    {  // gHa[a] += gpre: a 4-wide reduction per (row, column quad), a warp per row
-      const int q = tid & 31, rg = tid >> 5;
-#pragma unroll 4
-      for (int i = 0; i < TM / 8; i++) {
-        const int r = rg + 8 * i;
-        if (r < nvalid)
-          red_add_v4(&a.gHa[(size_t)s_a[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&P[r * LDE + 4 * q]));
-      }
-    }
+    // gHb[b] += gpre and gXc[c] += gpre (segmented), gHa[a] += gpre: one pass over P
+    scatter_rows<32>(P, s_b, a.gHb, s_c, a.gXc, s_a, a.gHa);
     // gang += gpre @ Wg   (K = 128, N = 64) on the tensor cores: warpgroup w takes rows 64 w .. 64 w + 63.  Each angle
     // row belongs to this tile alone, and (!HIDDEN) its upstream reads of gang are behind the barrier above, so the
     // update is a fire-and-forget reduction: one addition per element, as a load-add-store would do.
