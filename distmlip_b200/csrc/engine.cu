@@ -79,7 +79,7 @@ static Nccl g_nccl;
 // the biases as device pointers
 struct AtomLayerW {
   TcW W1s, W1sT, W1e, W1eT, W1t, W1tT, Wout, WoutT;
-  float *b1, *M, *W2can, *W2Tcan, *b2;
+  float *b1, *radial, *W2can, *W2Tcan, *b2;
 };
 struct BondLayerW {
   TcW W1a, W1aT, W1b, W1bT, W1c, W1cT, Wout, WoutT, WAa, WAaT, WAb, WAbT, WAc, WAcT;
@@ -138,7 +138,7 @@ struct b2m_engine {
   DBuf<float> wbuf;
   std::vector<AtomLayerW> aw;
   std::vector<BondLayerW> bw;
-  float *d_emb = nullptr, *d_Wbe = nullptr, *d_Wae = nullptr, *d_Wabw = nullptr, *d_W3bw = nullptr, *d_fa = nullptr;
+  float *d_emb = nullptr, *d_Wbe = nullptr, *d_Wae = nullptr, *d_W3bw = nullptr, *d_fa = nullptr;
   TcW F0, F0T, F1, F1T;  // final MLP 64 -> 64 -> 64 and transposes
   float *d_c0 = nullptr, *d_c1 = nullptr, *d_F2 = nullptr, *d_Ws = nullptr;
   const double* d_eref = nullptr;  // per-element energy offsets, double like the energy accumulator
@@ -310,6 +310,22 @@ static std::vector<float> second_layer_can(const std::vector<float>& raw128x64, 
 static std::vector<float> line_reverse_can(const std::vector<float>& raw128x64) {
   return canon_split(permute_k8(transpose(raw128x64, 128, 64), 64, 128), 64, 128, 128);
 }
+// the atom conv's radial weights M [128][9] and W_ab [64][9] in the layout of AtomConvArgs::radial: columns 0..7 of each
+// 64-row block as a k-permuted [64 n][8 k] wgmma B image (one k8 block on the tensor cores), column 8 as a side table
+static std::vector<float> radial_can(const std::vector<float>& M, const std::vector<float>& Wab) {
+  auto k8 = [](const std::vector<float>& w, int row0) {
+    std::vector<float> o(64 * 8);
+    for (int n = 0; n < 64; n++)
+      for (int k = 0; k < 8; k++) o[(size_t)n * 8 + k] = w[(size_t)(row0 + n) * NR + k];
+    return canon_split(permute_k8(o, 64, 8), 64, 8, 8);
+  };
+  std::vector<float> out;
+  for (const auto& c : {k8(M, 0), k8(M, 64), k8(Wab, 0)}) out.insert(out.end(), c.begin(), c.end());
+  for (int j = 0; j < 128; j++) out.push_back(M[(size_t)j * NR + 8]);
+  for (int c = 0; c < 64; c++) out.push_back(Wab[(size_t)c * NR + 8]);
+  B2M_REQUIRE(out.size() == ATOM_RAD, B2M_ERR_INVALID, "atom-conv radial block size");
+  return out;
+}
 
 // a [K][N] row-major weight (y = x W, K and N multiples of 64) as the wgmma blocks of tc_mm, packed into P: K chunks of
 // kmax (128 or 64; 64 for a remainder), per chunk N blocks of 64, or of 128 when the chunk is 64 deep
@@ -388,7 +404,7 @@ static void finalize_weights(b2m_engine* e) {
   const auto& Wbe = W(e, "bond_embedding.layers.0.weight", {D, NR});
   put("Wbe", Wbe);
   put("Wae", W(e, "angle_embedding.layers.0.weight", {D, NF}));
-  put("Wabw", W(e, "atom_bond_weights.weight", {D, NR}));
+  const auto& Wabw = W(e, "atom_bond_weights.weight", {D, NR});
   put("W3bw", W(e, "threebody_bond_weights.weight", {D, NR}));
 
   e->aw.resize(nb);
@@ -418,7 +434,7 @@ static void finalize_weights(b2m_engine* e) {
     linear(W1t, 128, 64, w.W1t, w.W1tT);
     linear(Wout, 64, 64, w.Wout, w.WoutT);
     put(q + "b1", b1);
-    put(q + "M", M);
+    put(q + "radial", radial_can(M, Wabw));
     put(q + "W2can", second_layer_can(W2, false));
     put(q + "W2Tcan", second_layer_can(W2, true));
     put(q + "b2", b2);
@@ -491,14 +507,13 @@ static void finalize_weights(b2m_engine* e) {
   e->d_emb = dp("emb");
   e->d_Wbe = dp("Wbe");
   e->d_Wae = dp("Wae");
-  e->d_Wabw = dp("Wabw");
   e->d_W3bw = dp("W3bw");
   e->d_c0 = dp("c0"), e->d_c1 = dp("c1"), e->d_F2 = dp("F2"), e->d_Ws = dp("Ws");
   e->d_eref = e->elem_refs.empty() ? nullptr : e->erefbuf.p;
   for (int l = 0; l < nb; l++) {
     const std::string q = "a" + std::to_string(l) + ".";
     AtomLayerW& w = e->aw[l];
-    w.b1 = dp(q + "b1"), w.M = dp(q + "M"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
+    w.b1 = dp(q + "b1"), w.radial = dp(q + "radial"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
   }
   for (int l = 0; l < nb - 1; l++) {
     const std::string q = "b" + std::to_string(l) + ".";
@@ -700,7 +715,7 @@ static AtomConvArgs atom_args(b2m_engine* e, int l) {
   a.e_src = g.e_src.p, a.e_dst = g.e_dst.p, a.e_bond = g.e_bond.p, a.e_vec = g.e_vec.p;
   const int ps = e->proj_slot(l);
   a.Aproj = e->ApL[ps].p, a.Cproj = e->CpL[ps].p, a.Qproj = l > 0 ? e->QpL[ps].p : nullptr;
-  a.M = w.M, a.W2can = w.W2can, a.W2Tcan = w.W2Tcan, a.b2 = w.b2, a.Wabw = e->d_Wabw;
+  a.radial = w.radial, a.W2can = w.W2can, a.W2Tcan = w.W2Tcan, a.b2 = w.b2;
   a.rp = e->rp2;
   return a;
 }

@@ -112,13 +112,15 @@ struct Map {
 // (rows 16 w + l/4 and + 8 of the 64-row block, k slots l%4 and l%4 + 4).  B: canonical K-major [64 n][K k] image in
 // shared memory, tf32 hi plane at b_hi and lo plane at b_lo, k permuted inside each block of 8 (slot q <- column 2q,
 // slot q + 4 <- column 2q + 1; engine.cu: permute_k8), so that slots l%4 and l%4 + 4 take A's columns 8 ks + 2 (l%4)
-// and + 1: the pair a thread holds in the accumulator layout, or reads from a tile as one float2.
-__device__ __forceinline__ void wg_mma64(const float (&x)[8][4], uint32_t b_hi, uint32_t b_lo, int bk, bool accumulate,
+// and + 1: the pair a thread holds in the accumulator layout, or reads from a tile as one float2.  KB < 8: the first KB
+// k blocks only (the rank-9 radial products take one, K = 8).
+template <int KB>
+__device__ __forceinline__ void wg_mma64(const float (&x)[KB][4], uint32_t b_hi, uint32_t b_lo, int bk, bool accumulate,
                                          float (&d)[32]) {
   constexpr uint32_t LBO = 8 * 128;  // byte step between core matrices along K (N = 64)
-  uint32_t ah[8][4], al[8][4];
+  uint32_t ah[KB][4], al[KB][4];
 #pragma unroll
-  for (int ks = 0; ks < 8; ks++)
+  for (int ks = 0; ks < KB; ks++)
 #pragma unroll
     for (int q = 0; q < 4; q++) {
       ah[ks][q] = tf32_hi_bits(x[ks][q]);
@@ -128,7 +130,7 @@ __device__ __forceinline__ void wg_mma64(const float (&x)[8][4], uint32_t b_hi, 
   acc_fence(d);
   wgmma_fence();
 #pragma unroll
-  for (int ks = 0; ks < 8; ks++) {
+  for (int ks = 0; ks < KB; ks++) {
 #pragma unroll
     for (int term = 0; term < 3; term++) {
       const uint64_t bd = gmma_desc((term == 2 ? b_lo : b_hi) + koff + ks * 2 * LBO, LBO, 128u);
@@ -373,48 +375,47 @@ __device__ __forceinline__ void issue_gather(const AtomConvArgs& a, int64_t t, c
     if (row.src >= 0) bulk_g2s(buf + tid * LDE, a.Aproj + (size_t)row.src * D2, 512u, bar);
   }
 }
-// be_k(d_r) (and d be_k / dd) of the tile's rows, both warpgroups (rows r, radial halves)
-__device__ __forceinline__ void radial_rows(const AtomConvArgs& a, const float* s_d, int nvalid, float* be_s,
-                                            float* dbe_s) {
+// be_k(d_r) (and d be_k / dd) of the tile's rows, both warpgroups (rows r, radial halves): k = 0..7 into be_s [TM][8]
+// (the A operand of the radial products), k = 8 into be8 [TM]
+__device__ __forceinline__ void radial_rows(const AtomConvArgs& a, const float* s_d, int nvalid, float* be_s, float* be8,
+                                            float* dbe_s, float* dbe8) {
   const int r = threadIdx.x & 127, half = threadIdx.x >> 7;
   const float d = s_d[r];
   const int k0 = half ? 5 : 0, k1 = half ? 9 : 5;
   for (int k = k0; k < k1; k++) {
     float be = 0.f, dbe = 0.f;
     if (r < nvalid) rbf_env_k(d, a.rp.freq[k], a.rp, be, dbe);
-    be_s[r * 12 + k] = be;
-    if (dbe_s != nullptr) dbe_s[r * 12 + k] = dbe;
+    *(k < 8 ? be_s + r * 8 + k : be8 + r) = be;
+    if (dbe_s != nullptr) *(k < 8 ? dbe_s + r * 8 + k : dbe8 + r) = dbe;
   }
-}
-// the radial operands live in shared memory at a row pitch of 12 floats (k < 9 used): a row is two float4 and a float
-__device__ __forceinline__ void stage_pitch12(float* dst, const float* __restrict__ src, int rows) {
-  for (int i = threadIdx.x; i < rows * 12; i += NT) {
-    const int r = i / 12, k = i % 12;
-    dst[i] = k < 9 ? src[r * 9 + k] : 0.f;
-  }
-}
-__device__ __forceinline__ void ld9(const float* p, float (&v)[9]) {
-  const float4 x = *reinterpret_cast<const float4*>(p), y = *reinterpret_cast<const float4*>(p + 4);
-  v[0] = x.x, v[1] = x.y, v[2] = x.z, v[3] = x.w, v[4] = y.x, v[5] = y.y, v[6] = y.z, v[7] = y.w, v[8] = p[8];
-}
-__device__ __forceinline__ float dot9(const float (&x)[9], const float (&y)[9]) {
-  float s = 0.f;
-#pragma unroll
-  for (int k = 0; k < 9; k++) s = fmaf(x[k], y[k], s);
-  return s;
 }
 __device__ __forceinline__ float2 ld_f2(const float* p) { return *reinterpret_cast<const float2*>(p); }
 __device__ __forceinline__ void st_f2(float* p, float x, float y) { *reinterpret_cast<float2*>(p) = make_float2(x, y); }
 
+// index into a wg_mma64 result of this thread's element (row(2h + ii), col(j)) of the 64-row half h (Map layout)
+__device__ __forceinline__ constexpr int fq(int ii, int j) { return 4 * (j >> 1) + 2 * ii + (j & 1); }
+
+// d = x[rows of half h][0..7] . B^T on the tensor cores: x is be_s or dbe_s ([TM][8]; a thread's k pair of a row is one
+// float2, conflict-free at pitch 8 within a half-warp), img a [64 n][8 k] image of the radial block (AtomConvArgs).
+// The ninth column is the caller's: d + x_8 B[.][8].
+__device__ __forceinline__ void radial_mma(const Map& m, int h, const float* x_s, const float* img, float (&d)[32]) {
+  const float2 u = ld_f2(x_s + m.row(2 * h) * 8 + m.cb), v = ld_f2(x_s + m.row(2 * h + 1) * 8 + m.cb);
+  const float x[1][4] = {{u.x, v.x, u.y, v.y}};
+  uint32_t b = s_u32(img);
+  asm volatile("" : "+r"(b));  // formed here: descriptors hoisted out of the tile loop would hold registers throughout
+  wg_mma64(x, b, b + 512u * 4u, 0, false, d);
+}
+
 // pre of this thread's rows of 64-row half h (acc[2h], acc[2h + 1], Map layout): A[src] (in the tile) + C[dst] +
-// (Q[bond] | M.be), summed in that order; rows r >= nvalid are 0.  Index work is per row; the C / Q values of both rows
-// (32 float2 loads) are in flight before any is used.  Msm: M as [128][12], be_s: [TM][12].
+// (Q[bond] | be.M^T), summed in that order; rows r >= nvalid are 0.  be.M^T is k = 0..7 on the tensor cores plus
+// be_8 M[.][8].  Index work is per row; the C / Q values of both rows (32 float2 loads) are in flight under the product.
 __device__ __forceinline__ void first_layer_half(const AtomConvArgs& a, const Map& m, int h, const float* tile,
                                                  const int* s_dst, const int* s_bond, const float* be_s,
-                                                 const float* Msm, int nvalid, float (&acc)[AR][AC]) {
+                                                 const float* be8, const float* rad, int nvalid,
+                                                 float (&acc)[AR][AC]) {
   const int c0 = 64 * m.branch + m.cb;
   float2 cv[2][AC / 2], qv[2][AC / 2];
-  float be[2][9];
+  float b8[2];
   bool viaQ[2], ok[2];
 #pragma unroll
   for (int ii = 0; ii < 2; ii++) {
@@ -433,18 +434,19 @@ __device__ __forceinline__ void first_layer_half(const AtomConvArgs& a, const Ma
 #pragma unroll
       for (int jj = 0; jj < AC / 2; jj++) qv[ii][jj] = make_float2(0.f, 0.f);
     }
-    ld9(be_s + r * 12, be[ii]);
+    b8[ii] = be8[r];
   }
+  float d[32];
+  radial_mma(m, h, be_s, rad + ATOM_RAD_M + 1024 * m.branch, d);
 #pragma unroll
   for (int j = 0; j < AC; j++) {
-    float mk[9];
-    ld9(Msm + (64 * m.branch + m.col(j)) * 12, mk);
+    const float m8 = rad[ATOM_RAD_M8 + 64 * m.branch + m.col(j)];
 #pragma unroll
     for (int ii = 0; ii < 2; ii++) {
       const int r = m.row(2 * h + ii);
       const float x = tile[r * LDE + 64 * m.branch + m.col(j)];
       const float2 c2 = cv[ii][j >> 1], q2 = qv[ii][j >> 1];
-      const float t = viaQ[ii] ? ((j & 1) ? q2.y : q2.x) : dot9(be[ii], mk);
+      const float t = viaQ[ii] ? ((j & 1) ? q2.y : q2.x) : fmaf(b8[ii], m8, d[fq(ii, j)]);
       acc[2 * h + ii][j] = ok[ii] ? x + ((j & 1) ? c2.y : c2.x) + t : 0.f;
     }
   }
@@ -467,17 +469,15 @@ __device__ __forceinline__ void wg_mm64_acc(const float (&x)[AR][AC], int h, con
   for (int q = 0; q < 32; q++) acc[2 * h + ((q >> 1) & 1)][2 * (q >> 2) + (q & 1)] = d[q];
 }
 
-// v[ii][k] of the rows of half h (i = 2h + ii) summed over the 4 lanes of a quad (they share rows): lane l takes the sum
-// of row i = l & 3 into out when that row is in half h
-__device__ __forceinline__ void quad_reduce_half(const float (&v)[2][9], int h, float (&out)[9]) {
+// v[i] (row m.row(i)) summed over the 4 lanes of a quad, which share rows: lane l gets the sum of row l & 3
+__device__ __forceinline__ float quad_row_sum(const float (&v)[AR]) {
   const int l = threadIdx.x & 3;
-  const bool b0 = l & 1, mine = (l >> 1) == h;
+  const bool b0 = l & 1, b1 = l & 2;
+  float w[2];
 #pragma unroll
-  for (int k = 0; k < 9; k++) {
-    float w = (b0 ? v[1][k] : v[0][k]) + __shfl_xor_sync(0xffffffffu, b0 ? v[0][k] : v[1][k], 1);
-    w += __shfl_xor_sync(0xffffffffu, w, 2);
-    if (mine) out[k] = w;
-  }
+  for (int h = 0; h < 2; h++)
+    w[h] = (b0 ? v[2 * h + 1] : v[2 * h]) + __shfl_xor_sync(0xffffffffu, b0 ? v[2 * h] : v[2 * h + 1], 1);
+  return (b1 ? w[1] : w[0]) + __shfl_xor_sync(0xffffffffu, b1 ? w[0] : w[1], 2);
 }
 
 __device__ __forceinline__ void red_add_v4(float* p, float4 v) {
@@ -547,27 +547,26 @@ __device__ __forceinline__ void scatter_rows(const float* tile, const int* key0,
 struct AtomSmemFwd {
   static constexpr int kTile = 32;                  // two [TM][LDE] gather buffers (first 128 B: their mbarriers)
   static constexpr int kW = kTile + 2 * TM * LDE;   // wgmma images of W2 (2 branches x hi | lo, k permuted), staged once
-  static constexpr int kBe = kW + 16384;            // be [TM][12]
-  static constexpr int kM = kBe + TM * 12;          // M [128][12]
-  static constexpr int kWab = kM + 128 * 12;        // W_ab [64][12]
-  static constexpr int kB2 = kWab + 64 * 12;
+  static constexpr int kRad = kW + 16384;           // radial block (M, W_ab: AtomConvArgs::radial), staged once
+  static constexpr int kBe = kRad + ATOM_RAD;       // be [TM][8] (k < 8)
+  static constexpr int kBe8 = kBe + TM * 8;         // be [TM] (k = 8)
+  static constexpr int kB2 = kBe8 + TM;
   static constexpr int kD = kB2 + 128;              // [2][TM] per buffer
   static constexpr int kIdx = kD + 2 * TM;          // dst [2][TM], bond [2][TM]
   static constexpr int kTotal = kIdx + 4 * TM;
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
 static_assert(AtomSmemFwd::bytes <= 232448, "atom-conv forward shared memory");
-static_assert(AtomSmemFwd::kW % 4 == 0 && AtomSmemFwd::kBe % 4 == 0 && AtomSmemFwd::kM % 4 == 0 &&
-                  AtomSmemFwd::kWab % 4 == 0,
-              "16-byte aligned images and pitch-12 rows");
+static_assert(AtomSmemFwd::kW % 4 == 0 && AtomSmemFwd::kRad % 4 == 0 && AtomSmemFwd::kBe % 4 == 0,
+              "16-byte aligned images and radial rows");
 
 __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
   uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);  // [2]
   float* Wsm = smem + AtomSmemFwd::kW;
+  float* rad = smem + AtomSmemFwd::kRad;
   float* be_s = smem + AtomSmemFwd::kBe;
-  float* Msm = smem + AtomSmemFwd::kM;
-  float* wabW = smem + AtomSmemFwd::kWab;
+  float* be8 = smem + AtomSmemFwd::kBe8;
   float* b2s = smem + AtomSmemFwd::kB2;
 
   const int tid = threadIdx.x;
@@ -585,8 +584,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
   EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
   // loop-invariant operands, once per CTA
   stage_w(Wsm, a.W2can, 4096);
-  stage_pitch12(Msm, a.M, 128);
-  stage_pitch12(wabW, a.Wabw, 64);
+  stage_w(rad, a.radial, ATOM_RAD / 4);
   if (tid < 128) b2s[tid] = a.b2[tid];
   __syncthreads();
   issue_gather(a, blockIdx.x, nxt, tile_of(0), &mbar[0], nullptr, dst_of(0), bond_of(0), d_of(0));
@@ -606,14 +604,14 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
       issue_gather(a, t + step, nxt, tile_of(s ^ 1), &mbar[s ^ 1], nullptr, dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
       nxt = edge_row(a, (t + 2 * step) * TM + tid);
     }
-    radial_rows(a, d_of(s), nvalid, be_s, nullptr);
+    radial_rows(a, d_of(s), nvalid, be_s, be8, nullptr, nullptr);
     mbar_wait(&mbar[s], stage_parity(it));
     __syncthreads();
-    // pre = A[src] + C[dst] + (M.be | Q[bond]);  hid = silu(pre) straight into the second layer, per 64-row half
+    // pre = A[src] + C[dst] + (be.M^T | Q[bond]);  hid = silu(pre) straight into the second layer, per 64-row half
     float acc[AR][AC];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      first_layer_half(a, m, h, tile, s_dst, s_bond, be_s, Msm, nvalid, acc);
+      first_layer_half(a, m, h, tile, s_dst, s_bond, be_s, be8, rad, nvalid, acc);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++)
 #pragma unroll
@@ -627,17 +625,19 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
         const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
         acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
       }
-    // m = L . G . w_ab: warpgroup 1 forms G . w_ab in its own tile positions, warpgroup 0 multiplies by L in its own
+    // m = L . G . w_ab: warpgroup 1 forms G . w_ab (w_ab = be.W_ab^T on its tensor cores) in its own tile positions,
+    // warpgroup 0 multiplies by L in its own
     if (m.branch == 1) {
-      float be[AR][9];
 #pragma unroll
-      for (int i = 0; i < AR; i++) ld9(be_s + m.row(i) * 12, be[i]);
+      for (int h = 0; h < 2; h++) {
+        float w[32];
+        radial_mma(m, h, be_s, rad + ATOM_RAD_WAB, w);
 #pragma unroll
-      for (int j = 0; j < AC; j++) {
-        float wk[9];
-        ld9(wabW + m.col(j) * 12, wk);
+        for (int ii = 0; ii < 2; ii++) {
+          const float b8 = be8[m.row(2 * h + ii)];
 #pragma unroll
-        for (int i = 0; i < AR; i++) acc[i][j] *= dot9(be[i], wk);
+          for (int j = 0; j < AC; j++) acc[2 * h + ii][j] *= fmaf(b8, rad[ATOM_RAD_WAB8 + m.col(j)], w[fq(ii, j)]);
+        }
       }
 #pragma unroll
       for (int i = 0; i < AR; i++)
@@ -686,30 +686,32 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
 struct AtomSmemBwd {
   static constexpr int kBuf = 32;               // two [TM][LDE] tiles (first 128 B: 2 gather mbarriers + weight mbarrier)
   static constexpr int kW = kBuf + 2 * TM * LDE;  // wgmma image of W2 or W2^T (2 branches x hi | lo, k permuted)
-  static constexpr int kBe = kW + 16384;        // be [TM][12]
-  static constexpr int kDbe = kBe + TM * 12;    // d be / dd [TM][12]
-  static constexpr int kM = kDbe + TM * 12;     // M [128][12]
-  static constexpr int kWab = kM + 128 * 12;    // W_ab [64][12]
-  static constexpr int kB2 = kWab + 64 * 12;
+  static constexpr int kRad = kW + 16384;       // radial block (M, W_ab: AtomConvArgs::radial), staged once
+  static constexpr int kBe = kRad + ATOM_RAD;   // be [TM][8] (k < 8)
+  static constexpr int kDbe = kBe + TM * 8;     // d be / dd [TM][8]
+  static constexpr int kBe8 = kDbe + TM * 8;    // be [TM] (k = 8)
+  static constexpr int kDbe8 = kBe8 + TM;       // d be / dd [TM] (k = 8)
+  static constexpr int kB2 = kDbe8 + TM;
   static constexpr int kD = kB2 + 128;          // [2][TM]
   static constexpr int kIdx = kD + 2 * TM;      // src, dst, bond: [2][TM] each
   static constexpr int kTotal = kIdx + 6 * TM;
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
 static_assert(AtomSmemBwd::bytes <= 232448, "atom-conv backward shared memory");
-static_assert(AtomSmemBwd::kW % 4 == 0 && AtomSmemBwd::kBe % 4 == 0 && AtomSmemBwd::kM % 4 == 0 &&
-                  AtomSmemBwd::kWab % 4 == 0,
-              "16-byte aligned images and pitch-12 rows");
+static_assert(AtomSmemBwd::kW % 4 == 0 && AtomSmemBwd::kRad % 4 == 0 && AtomSmemBwd::kBe % 4 == 0 &&
+                  AtomSmemBwd::kDbe % 4 == 0,
+              "16-byte aligned images and radial rows");
 
 __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
   uint64_t* gbar = reinterpret_cast<uint64_t*>(smem);  // [2]: gather buffers
   uint64_t* wbar = gbar + 2;                            // weight image
   float* Wsm = smem + AtomSmemBwd::kW;
+  float* rad_base = smem + AtomSmemBwd::kRad;
   float* be_s = smem + AtomSmemBwd::kBe;
   float* dbe_s = smem + AtomSmemBwd::kDbe;
-  float* Msm = smem + AtomSmemBwd::kM;
-  float* wabW = smem + AtomSmemBwd::kWab;
+  float* be8 = smem + AtomSmemBwd::kBe8;
+  float* dbe8 = smem + AtomSmemBwd::kDbe8;
   float* b2s = smem + AtomSmemBwd::kB2;
 
   const int tid = threadIdx.x;
@@ -728,8 +730,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     fence_barrier_init();
   }
   EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
-  stage_pitch12(Msm, a.M, 128);
-  stage_pitch12(wabW, a.Wabw, 64);
+  stage_w(rad_base, a.radial, ATOM_RAD / 4);
   if (tid < 128) b2s[tid] = a.b2[tid];
   __syncthreads();
   if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
@@ -741,6 +742,8 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
   const int c0 = 64 * m.branch;  // this warpgroup's first-layer columns
   int it = 0;
   for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
+    float* rad = rad_base;
+    asm volatile("" : "+l"(rad));  // radial addresses formed per tile: hoisted out of the loop they cost 7 registers
     const int s = it & 1;
     float* tileP = buf_of(s);
     float* tileH = buf_of(s ^ 1);
@@ -749,8 +752,8 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     const int* s_bond = bond_of(s);
     const int64_t e0 = t * TM;
     const int nvalid = (int)min((int64_t)TM, a.E - e0);
-    __syncthreads();  // the previous tile's scatter phase is done with tileH (its P), be_s, dbe_s
-    radial_rows(a, d_of(s), nvalid, be_s, dbe_s);
+    __syncthreads();  // the previous tile's scatter phase is done with tileH (its P) and be8
+    radial_rows(a, d_of(s), nvalid, be_s, be8, dbe_s, dbe8);
     mbar_wait(&gbar[s], stage_parity(it));
     mbar_wait(wbar, wpar);  // W2
     wpar ^= 1;
@@ -759,7 +762,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     float acc[AR][AC];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      first_layer_half(a, m, h, tileP, s_dst, s_bond, be_s, Msm, nvalid, acc);
+      first_layer_half(a, m, h, tileP, s_dst, s_bond, be_s, be8, rad, nvalid, acc);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++)
 #pragma unroll
@@ -789,15 +792,13 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
               m.branch == 0 ? silu_f(u1) : sigm(u1));
       }
     __syncthreads();
-    // elementwise reverse: acc = dE/du (L) / dE/dv (G); branch 0 also sums dE/dw_ab[r][c] W_ab[c][k] over its columns
-    float gwr[9];  // branch 0: the row m.row(lane & 3) of sum_c dE/dw_ab W_ab
+    // elementwise reverse: acc = dE/du (L) / dE/dv (G), with w_ab = be.W_ab^T from the tensor cores.  sd[i]: this
+    // thread's share of dE/dd of row m.row(i); branch 0 adds sum_c dE/dw_ab[r][c] (dbe.W_ab^T)[r][c] over its columns.
+    float sd[AR];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      float gw[2][9];
-#pragma unroll
-      for (int ii = 0; ii < 2; ii++)
-#pragma unroll
-        for (int k = 0; k < 9; k++) gw[ii][k] = 0.f;
+      float w[32];  // w_ab, then (branch 0) dE/dw_ab in place
+      radial_mma(m, h, be_s, rad + ATOM_RAD_WAB, w);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++) {
         const int i = 2 * h + ii;
@@ -808,28 +809,24 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++)
           gm2[jj] = dst >= 0 ? __ldg(reinterpret_cast<const float2*>(gp + 8 * jj)) : make_float2(0.f, 0.f);
-        float be[9];
-        ld9(be_s + r * 12, be);
+        const float b8 = be8[r];
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
           const float2 po2 = ld_f2(tileH + r * LDE + (64 - c0) + m.col(2 * jj));  // partner activations
+          const float2 wk2 = ld_f2(rad + ATOM_RAD_WAB8 + m.col(2 * jj));
 #pragma unroll
           for (int e = 0; e < 2; e++) {
             const int j = 2 * jj + e;
             const float u = acc[i][j];
             const float po = e ? po2.y : po2.x;
             const float gm = e ? gm2[jj].y : gm2[jj].x;
-            float g = 0.f;
+            const float wab = fmaf(b8, e ? wk2.y : wk2.x, w[fq(ii, j)]);
+            float g = 0.f, gwv = 0.f;
             if (dst >= 0) {
-              float wk[9];
-              ld9(wabW + m.col(j) * 12, wk);
-              const float wab = dot9(be, wk);
               if (m.branch == 0) {
                 const float sg = sigm(u);
                 const float oL = u * sg;
-                const float gwv = gm * oL * po;  // d/d w_ab
-#pragma unroll
-                for (int k = 0; k < 9; k++) gw[ii][k] = fmaf(gwv, wk[k], gw[ii][k]);
+                gwv = gm * oL * po;  // d/d w_ab
                 g = gm * po * wab * (sg * (1.f + u * (1.f - sg)));  // d/du
               } else {
                 const float oG = sigm(u);
@@ -837,10 +834,22 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
               }
             }
             acc[i][j] = g;
+            w[fq(ii, j)] = gwv;
           }
         }
       }
-      quad_reduce_half(gw, h, gwr);
+      sd[2 * h] = sd[2 * h + 1] = 0.f;
+      if (m.branch == 0) {
+        float dw[32];
+        radial_mma(m, h, dbe_s, rad + ATOM_RAD_WAB, dw);
+#pragma unroll
+        for (int ii = 0; ii < 2; ii++) {
+          const float db8 = dbe8[m.row(2 * h + ii)];
+#pragma unroll
+          for (int j = 0; j < AC; j++)
+            sd[2 * h + ii] = fmaf(w[fq(ii, j)], fmaf(db8, rad[ATOM_RAD_WAB8 + m.col(j)], dw[fq(ii, j)]), sd[2 * h + ii]);
+        }
+      }
     }
     mbar_wait(wbar, wpar);  // W2^T
     wpar ^= 1;
@@ -861,6 +870,27 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
           st_f2(p, x0, x1);
         }
     }
+    // rows fed by M (not bond rows fed by Q) add sum_j gpre[r][j] (dbe.M^T)[r][j] over this warpgroup's columns to sd;
+    // gpre is read back from P, which leaves the accumulators free for the product
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      float dm[32];
+      radial_mma(m, h, dbe_s, rad + ATOM_RAD_M + 1024 * m.branch, dm);
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++) {
+        const int r = m.row(2 * h + ii);
+        const float db8 = dbe8[r];
+        float s = 0.f;
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++) {
+          const float2 g2 = ld_f2(tileP + r * LDE + c0 + m.col(2 * jj));
+          const float2 mk = ld_f2(rad + ATOM_RAD_M8 + c0 + m.col(2 * jj));
+          s = fmaf(g2.x, fmaf(db8, mk.x, dm[fq(ii, 2 * jj)]), s);
+          s = fmaf(g2.y, fmaf(db8, mk.y, dm[fq(ii, 2 * jj + 1)]), s);
+        }
+        if (r < nvalid && !(useQ && s_bond[r] >= 0)) sd[2 * h + ii] += s;
+      }
+    }
     fence_proxy_async_smem();  // this thread's generic accesses of tileH come before its bulk refill
     __syncthreads();           // tileH and the W2^T image are free; P holds gpre
     if (t + step < ntiles) {
@@ -868,41 +898,13 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
       issue_gather(a, t + step, nxt, tileH, &gbar[s ^ 1], src_of(s ^ 1), dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
       nxt = edge_row(a, (t + 2 * step) * TM + tid);
     }
-    // ---- scatter phase (reads P, be_s / dbe_s and this tile's index arrays only) ----
-    {  // d E / d d_e through the radial basis (w_ab weights and, unless a bond row fed by Q, M.be): each warpgroup sums
-       // sum_j gpre[r][j] M[j][k] over its 64 columns from the gpre values in registers
-      float sk[AR][9];
-#pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int k = 0; k < 9; k++) sk[i][k] = 0.f;
-#pragma unroll
-      for (int j = 0; j < AC; j++) {
-        float mk[9];
-        ld9(Msm + (c0 + m.col(j)) * 12, mk);
-#pragma unroll
-        for (int i = 0; i < AR; i++)
-#pragma unroll
-          for (int k = 0; k < 9; k++) sk[i][k] = fmaf(acc[i][j], mk[k], sk[i][k]);
-      }
-      float skr[9];
-      quad_reduce_half(reinterpret_cast<const float(&)[2][9]>(sk[0]), 0, skr);
-      quad_reduce_half(reinterpret_cast<const float(&)[2][9]>(sk[2]), 1, skr);
+    // ---- scatter phase (reads P, be8 and this tile's index arrays only) ----
+    {  // d E / d d_e: sd summed over the 4 lanes of a row, and across the warpgroups through be8
+      const float v = quad_row_sum(sd);
       const int r = m.row(tid & 3);
-      const bool viaM = r < nvalid && !(useQ && s_bond[r] >= 0);
-#pragma unroll
-      for (int k = 0; k < 9; k++) skr[k] = viaM ? skr[k] : 0.f;
-      if (m.branch == 1) {
-#pragma unroll
-        for (int k = 0; k < 9; k++) be_s[r * 12 + k] = skr[k];  // be_s is free until the next tile
-      }
+      if (m.branch == 1) be8[r] = v;  // be8 is free until the next tile
       __syncthreads();
-      if (m.branch == 0 && r < nvalid) {
-        float part = 0.f;
-#pragma unroll
-        for (int k = 0; k < 9; k++) part = fmaf(gwr[k] + (skr[k] + be_s[r * 12 + k]), dbe_s[r * 12 + k], part);
-        a.gd[e0 + r] += part;
-      }
+      if (m.branch == 0 && r < nvalid) a.gd[e0 + r] += v + be8[r];
     }
     {
       const int j = tid & 127, rh = tid >> 7;

@@ -33,6 +33,7 @@ void launch_dsilu_mul(cudaStream_t st, int64_t n, const float* pre, float* g);  
 void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats);
 
 // -------- atom conv (the edge-gather kernel of the headline metric) --------
+constexpr int ATOM_RAD_M = 0, ATOM_RAD_WAB = 2048, ATOM_RAD_M8 = 3072, ATOM_RAD_WAB8 = 3200, ATOM_RAD = 3264;
 struct AtomConvArgs {
   int64_t E;
   const int* e_src;
@@ -42,13 +43,16 @@ struct AtomConvArgs {
   const float* Aproj;  // [n_loc,128]  x @ W1s^T
   const float* Cproj;  // [n_own,128]  x @ W1t^T + b1
   const float* Qproj;  // [B_own,128]  h @ W1e^T   (nullptr for layer 0)
-  const float* M;      // [128][9]     W1e @ W_be
+  // the rank-9 radial products be . M^T (M = W1e @ W_be, [128][9]) and be . W_ab^T (W_ab [64][9]) as one block of
+  // ATOM_RAD floats (engine.cu radial_can): k = 0..7 as k-permuted wgmma B images of one k8 block, tf32 hi plane then
+  // lo plane (M branch 0 at 0, M branch 1 at 1024, W_ab at 2048; each [64 n][8 k]), then column k = 8: M[.][8] at
+  // 3072, W_ab[.][8] at 3200
+  const float* radial;
   // second layers (L then G) as wgmma B operands: per branch the canonical K-major core-matrix image of a [64 n][64 k]
   // matrix, tf32 hi plane then lo plane (8192 floats per branch; engine.cu canon_split)
   const float* W2can;   // B[n][k] = W2[n][k]   (forward: hid . W2^T)
   const float* W2Tcan;  // B[n][k] = W2[k][n]   (backward: g . W2)
   const float* b2;     // [128]
-  const float* Wabw;   // [64][9]
   RadialParams rp;
   // forward
   float* agg;  // [n_own,64] (+=)
