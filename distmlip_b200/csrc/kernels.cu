@@ -178,24 +178,6 @@ __device__ __forceinline__ void stage_w(float* Wsm, const float* __restrict__ g,
   fence_proxy_async_smem();
 }
 
-// running segmented sum over rows [r0, r1) of a smem tile column, flushed with atomics when the key changes (the
-// atom-conv backward's gC sum: a column per thread; the other kernels use scatter_rows below)
-__device__ __forceinline__ void seg_flush(const float* tile, int ld, int col, int r0, int r1, const int* key,
-                                          float* __restrict__ out, int width) {
-  float sum = 0.f;
-  int cur = -1;
-  for (int r = r0; r < r1; r++) {
-    const int k = key[r];
-    if (k != cur) {
-      if (cur >= 0) atomicAdd(&out[(size_t)cur * width + col], sum);
-      cur = k;
-      sum = 0.f;
-    }
-    if (k >= 0) sum += tile[r * ld + col];
-  }
-  if (cur >= 0) atomicAdd(&out[(size_t)cur * width + col], sum);
-}
-
 // ============================================================================================
 // small elementwise / init kernels
 // ============================================================================================
@@ -501,14 +483,16 @@ __device__ __forceinline__ void seg_add(float* out, int width, int col, int k, c
 // R = TM LPR / NT consecutive rows.  Its float4 of row r
 //   - is added to gat[gidx[r]]                                                    (gat != nullptr, gidx[r] >= 0),
 //   - goes into one running sum per key array, reduced into out0[key0[.]] / out1[key1[.]] when the key changes and
-//     after the thread's last row                                                 (out != nullptr, key >= 0).
+//     after the thread's last row                                                 (out != nullptr, key >= 0),
+//   - is stored to sto[sidx[r]]: for rows whose index occurs once in the whole pass (sto != nullptr, sidx[r] >= 0).
 // Outputs are rows of 4 LPR floats, and every addition to them is one red.v4.  Rows past the end of a partial tile have
 // all indices < 0.  The indices are equal in the lanes that share a row, so with LPR = 32 no branch diverges.  A run of
 // equal keys that crosses the R-row boundary between two threads is reduced in two parts.  Values and indices are
 // loaded eight rows at a time before those rows are walked: the reductions (asm volatile) keep loads in program order.
 template <int LPR>
 __device__ __forceinline__ void scatter_rows(const float* tile, const int* key0, float* out0, const int* key1,
-                                             float* out1, const int* gidx, float* gat) {
+                                             float* out1, const int* gidx, float* gat, const int* sidx = nullptr,
+                                             float* sto = nullptr) {
   constexpr int R = TM * LPR / NT, W = 4 * LPR, B = 8;
   static_assert(R % B == 0 && B % 4 == 0, "batches of B rows, their indices read as int4");
   const int q = threadIdx.x % LPR, r0 = threadIdx.x / LPR * R;
@@ -517,7 +501,7 @@ __device__ __forceinline__ void scatter_rows(const float* tile, const int* key0,
 #pragma unroll
   for (int b = 0; b < R; b += B) {
     float4 v[B];
-    int k0[B], k1[B], kg[B];
+    int k0[B], k1[B], kg[B], ks[B];
 #pragma unroll
     for (int i = 0; i < B; i++) v[i] = *reinterpret_cast<const float4*>(tile + (r0 + b + i) * LDE + 4 * q);
     auto ld_idx = [&](const int* idx, bool on, int(&k)[B]) {
@@ -530,8 +514,10 @@ __device__ __forceinline__ void scatter_rows(const float* tile, const int* key0,
     ld_idx(key0, out0 != nullptr, k0);
     ld_idx(key1, out1 != nullptr, k1);
     ld_idx(gidx, gat != nullptr, kg);
+    ld_idx(sidx, sto != nullptr, ks);
 #pragma unroll
     for (int i = 0; i < B; i++) {
+      if (ks[i] >= 0) *reinterpret_cast<float4*>(sto + (size_t)ks[i] * W + 4 * q) = v[i];
       if (kg[i] >= 0) red_add_v4(gat + (size_t)kg[i] * W + 4 * q, v[i]);
       seg_add(out0, W, 4 * q, k0[i], v[i], c0, s0);
       seg_add(out1, W, 4 * q, k1[i], v[i], c1, s1);
@@ -677,12 +663,13 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
 // ============================================================================================
 // Shared memory holds one weight image (64 KB) and two [TM][LDE] tiles whose roles alternate: the tile's gathered rows
 // arrive in buffer it & 1, which becomes P: each thread overwrites its own A[src] values with its pre-activations, and
-// later with their adjoints gpre, which the scatter phase reads row-major.  The other buffer is H: the branches
-// exchange their activations through it.  Both second-layer products take their A operand from registers.  Once g.W2
-// has read the W2^T image and H is no longer read, both are refilled by bulk copies -- H with the next tile's A[src]
-// rows, the image with W2 -- which land while this tile's scatter phase runs.  The W2^T image is loaded right after the
-// recompute product, under the elementwise reverse.  The weight barrier completes two phases per tile (W2^T, then W2),
-// waited on in that order.
+// later with their adjoints gpre, which the scatter phase reads row-major.  The other buffer is H: the recompute parks
+// the second layer's outputs there at the thread's own positions -- u itself (L), oG = sigm(v) (G) -- so that the
+// reverse keeps one 64-row half of accumulators live at a time and reads its own and its partner's values back.  Both
+// second-layer products take their A operand from registers.  Once g.W2 has read the W2^T image and H is no longer
+// read, both are refilled by bulk copies -- H with the next tile's A[src] rows, the image with W2 -- which land while
+// this tile's scatter phase runs.  The W2^T image is loaded right after the recompute, under the first half's
+// elementwise reverse.  The weight barrier completes two phases per tile (W2^T, then W2), waited on in that order.
 struct AtomSmemBwd {
   static constexpr int kBuf = 32;               // two [TM][LDE] tiles (first 128 B: 2 gather mbarriers + weight mbarrier)
   static constexpr int kW = kBuf + 2 * TM * LDE;  // wgmma image of W2 or W2^T (2 branches x hi | lo, k permuted)
@@ -758,7 +745,8 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     mbar_wait(wbar, wpar);  // W2
     wpar ^= 1;
     __syncthreads();
-    // recompute: pre (kept in P at the thread's own positions), silu(pre) . W2^T + b2 = u (L) / v (G)
+    // recompute, per 64-row half: pre (kept in P at the thread's own positions), silu(pre) . W2^T + b2 = u (L) / v (G),
+    // parked in H at the thread's own positions as u (L) and oG = sigm(v) (G).  acc holds one half at a time.
     float acc[AR][AC];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
@@ -775,62 +763,65 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
           x1 = silu_f(x1);
         }
       wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++) {
+          const float u0 = acc[2 * h + ii][2 * jj] + b2s[m.branch * 64 + m.col(2 * jj)];
+          const float u1 = acc[2 * h + ii][2 * jj + 1] + b2s[m.branch * 64 + m.col(2 * jj + 1)];
+          st_f2(tileH + m.row(2 * h + ii) * LDE + c0 + m.col(2 * jj), m.branch == 0 ? u0 : sigm(u0),
+                m.branch == 0 ? u1 : sigm(u1));
+        }
     }
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
-    __syncthreads();  // the W2 image is no longer needed
+    __syncthreads();  // the W2 image is no longer needed; H holds both branches' values
     if (tid == 0) bulk_g2s_image(Wsm, a.W2Tcan, 16384 * 4, wbar);
-    // exchange activations between the two branches through tileH
-#pragma unroll
-    for (int i = 0; i < AR; i++)
-#pragma unroll
-      for (int jj = 0; jj < AC / 2; jj++) {
-        const float u0 = acc[i][2 * jj], u1 = acc[i][2 * jj + 1];
-        st_f2(tileH + m.row(i) * LDE + c0 + m.col(2 * jj), m.branch == 0 ? silu_f(u0) : sigm(u0),
-              m.branch == 0 ? silu_f(u1) : sigm(u1));
-      }
-    __syncthreads();
-    // elementwise reverse: acc = dE/du (L) / dE/dv (G), with w_ab = be.W_ab^T from the tensor cores.  sd[i]: this
-    // thread's share of dE/dd of row m.row(i); branch 0 adds sum_c dE/dw_ab[r][c] (dbe.W_ab^T)[r][c] over its columns.
+    // reverse, per 64-row half.  Elementwise: acc = dE/du (L) / dE/dv (G), from the values parked in H (the partner's
+    // sigm(v) / silu(u) formed from them) and w_ab = be.W_ab^T from the tensor cores.  sd[i]: this thread's share of
+    // dE/dd of row m.row(i); branch 0 adds sum_c dE/dw_ab[r][c] (dbe.W_ab^T)[r][c] over its columns.  Then ghid =
+    // [gu @ W2L, gv @ W2G] and gpre = ghid * dsilu(pre), into P at the thread's own positions; rows fed by M (not bond
+    // rows fed by Q) add sum_j gpre[r][j] (dbe.M^T)[r][j] over this warpgroup's columns to sd.
     float sd[AR];
 #pragma unroll
     for (int h = 0; h < 2; h++) {
+      int dst[2];
+      float2 gm2[2][AC / 2];  // both rows' 16 dE/dagg values, loaded before any is used
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++) {
+        dst[ii] = s_dst[m.row(2 * h + ii)];
+        const float* gp = a.gagg + (size_t)max(dst[ii], 0) * D + m.cb;
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++)
+          gm2[ii][jj] = dst[ii] >= 0 ? __ldg(reinterpret_cast<const float2*>(gp + 8 * jj)) : make_float2(0.f, 0.f);
+      }
       float w[32];  // w_ab, then (branch 0) dE/dw_ab in place
       radial_mma(m, h, be_s, rad + ATOM_RAD_WAB, w);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++) {
         const int i = 2 * h + ii;
         const int r = m.row(i);
-        const int dst = s_dst[r];
-        float2 gm2[AC / 2];  // this row's 16 dE/dagg values, loaded before any is used
-        const float* gp = a.gagg + (size_t)max(dst, 0) * D + m.cb;
-#pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++)
-          gm2[jj] = dst >= 0 ? __ldg(reinterpret_cast<const float2*>(gp + 8 * jj)) : make_float2(0.f, 0.f);
         const float b8 = be8[r];
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
-          const float2 po2 = ld_f2(tileH + r * LDE + (64 - c0) + m.col(2 * jj));  // partner activations
+          const float2 ow2 = ld_f2(tileH + r * LDE + c0 + m.col(2 * jj));         // u (L) / oG (G)
+          const float2 pt2 = ld_f2(tileH + r * LDE + (64 - c0) + m.col(2 * jj));  // the partner's
           const float2 wk2 = ld_f2(rad + ATOM_RAD_WAB8 + m.col(2 * jj));
 #pragma unroll
           for (int e = 0; e < 2; e++) {
             const int j = 2 * jj + e;
-            const float u = acc[i][j];
-            const float po = e ? po2.y : po2.x;
-            const float gm = e ? gm2[jj].y : gm2[jj].x;
+            const float x = e ? ow2.y : ow2.x;
+            const float pt = e ? pt2.y : pt2.x;
+            const float gm = e ? gm2[ii][jj].y : gm2[ii][jj].x;
             const float wab = fmaf(b8, e ? wk2.y : wk2.x, w[fq(ii, j)]);
             float g = 0.f, gwv = 0.f;
-            if (dst >= 0) {
+            if (dst[ii] >= 0) {
               if (m.branch == 0) {
-                const float sg = sigm(u);
-                const float oL = u * sg;
-                gwv = gm * oL * po;  // d/d w_ab
-                g = gm * po * wab * (sg * (1.f + u * (1.f - sg)));  // d/du
+                const float sg = sigm(x);
+                const float oL = x * sg;
+                gwv = gm * oL * pt;  // d/d w_ab
+                g = gm * pt * wab * (sg * (1.f + x * (1.f - sg)));  // d/du
               } else {
-                const float oG = sigm(u);
-                g = gm * po * wab * oG * (1.f - oG);  // d/dv
+                const float oL = silu_f(pt);
+                g = gm * oL * wab * x * (1.f - x);  // d/dv
               }
             }
             acc[i][j] = g;
@@ -850,12 +841,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
             sd[2 * h + ii] = fmaf(w[fq(ii, j)], fmaf(db8, rad[ATOM_RAD_WAB8 + m.col(j)], dw[fq(ii, j)]), sd[2 * h + ii]);
         }
       }
-    }
-    mbar_wait(wbar, wpar);  // W2^T
-    wpar ^= 1;
-    // ghid = [gu @ W2L, gv @ W2G];  gpre = ghid * dsilu(pre), into P at the thread's own positions
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
+      if (h == 0) mbar_wait(wbar, wpar);  // W2^T
       wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++)
@@ -869,11 +855,6 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
           x1 *= dsilu_f(pre.y);
           st_f2(p, x0, x1);
         }
-    }
-    // rows fed by M (not bond rows fed by Q) add sum_j gpre[r][j] (dbe.M^T)[r][j] over this warpgroup's columns to sd;
-    // gpre is read back from P, which leaves the accumulators free for the product
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
       float dm[32];
       radial_mma(m, h, dbe_s, rad + ATOM_RAD_M + 1024 * m.branch, dm);
 #pragma unroll
@@ -883,14 +864,14 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
         float s = 0.f;
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
-          const float2 g2 = ld_f2(tileP + r * LDE + c0 + m.col(2 * jj));
           const float2 mk = ld_f2(rad + ATOM_RAD_M8 + c0 + m.col(2 * jj));
-          s = fmaf(g2.x, fmaf(db8, mk.x, dm[fq(ii, 2 * jj)]), s);
-          s = fmaf(g2.y, fmaf(db8, mk.y, dm[fq(ii, 2 * jj + 1)]), s);
+          s = fmaf(acc[2 * h + ii][2 * jj], fmaf(db8, mk.x, dm[fq(ii, 2 * jj)]), s);
+          s = fmaf(acc[2 * h + ii][2 * jj + 1], fmaf(db8, mk.y, dm[fq(ii, 2 * jj + 1)]), s);
         }
         if (r < nvalid && !(useQ && s_bond[r] >= 0)) sd[2 * h + ii] += s;
       }
     }
+    wpar ^= 1;
     fence_proxy_async_smem();  // this thread's generic accesses of tileH come before its bulk refill
     __syncthreads();           // tileH and the W2^T image are free; P holds gpre
     if (t + step < ntiles) {
@@ -906,25 +887,9 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
       __syncthreads();
       if (m.branch == 0 && r < nvalid) a.gd[e0 + r] += v + be8[r];
     }
-    {
-      const int j = tid & 127, rh = tid >> 7;
-      if (useQ && a.gQ != nullptr) {
-        for (int i = 0; i < 64; i++) {
-          const int r = rh + 2 * i;
-          if (r < nvalid && s_bond[r] >= 0) a.gQ[(size_t)s_bond[r] * D2 + j] = tileP[r * LDE + j];
-        }
-      }
-      if (a.gA != nullptr) seg_flush(tileP, LDE, j, rh * 64, rh * 64 + 64, s_dst, a.gC, D2);
-    }
-    if (a.gA != nullptr) {  // gA[src] += gpre: a 4-wide reduction per (row, column quad), a warp per row
-      const int q = tid & 31, rg = tid >> 5;
-#pragma unroll 4
-      for (int i = 0; i < TM / 8; i++) {
-        const int r = rg + 8 * i;
-        if (r < nvalid)
-          red_add_v4(&a.gA[(size_t)s_src[r] * D2 + 4 * q], *reinterpret_cast<const float4*>(&tileP[r * LDE + 4 * q]));
-      }
-    }
+    // gC[dst] += gpre (segmented), gA[src] += gpre, gQ[bond] = gpre (each bond row occurs once): one pass over P
+    scatter_rows<32>(tileP, s_dst, a.gA != nullptr ? a.gC : nullptr, nullptr, nullptr, s_src, a.gA, s_bond,
+                     useQ ? a.gQ : nullptr);
   }
 }
 
@@ -1160,10 +1125,11 @@ __global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
 
 // Backward, mirroring the atom conv: P (buffer it & 1) holds the tile's Ha rows, then (HIDDEN) its pre-activations,
 // each thread's over its own Ha values, then their adjoints gpre, which the scatter phase and gpre.Wg read row-major;
-// H (the other buffer) holds the angle rows, then the branch activations the two warpgroups exchange.  Both products of
-// the hidden layer take their A operand from registers.  Once H has been read for the last time (by the elementwise
-// reverse), the next tile's Ha rows are copied into it (H becomes
-// the next tile's P); once the scatter phase and gang += gpre.Wg have read P, the next tile's angle rows go into its
+// H (the other buffer) holds the angle rows, then the last layer's outputs parked at each thread's own positions -- u
+// (L), oG = sigm(v) (G) -- so that the reverse keeps one 64-row half of accumulators live at a time and reads its own
+// and its partner's values back.  Both products of the hidden layer take their A operand from registers.  Once H has
+// been read for the last time (by the elementwise reverse), the next tile's Ha rows are copied into it (H becomes the
+// next tile's P); once the scatter phase and gang += gpre.Wg have read P, the next tile's angle rows go into its
 // columns 64..127 (P becomes the next tile's H).  Weight images through the one slot: HIDDEN Wg -> W2 -> W2^T -> Wg^T
 // per tile, !HIDDEN Wg -> Wg^T.
 template <bool HIDDEN>
@@ -1211,75 +1177,85 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
         }
       mbar_wait(sm.wbar(), wpar);  // W2
       wpar ^= 1;
-      wg_mm64_acc(acc, 0, sm.W() + m.branch * 8192, acc);
-      wg_mm64_acc(acc, 1, sm.W() + m.branch * 8192, acc);
-#pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int j = 0; j < AC; j++) acc[i][j] += b2s[m.branch * 64 + m.col(j)];
-      __syncthreads();  // W2 has been read
-      if (tid == 0) bulk_g2s_image(sm.W(), a.W2Tcan, 16384 * 4, sm.wbar());
     }
-    // acc = pre-activation of the last layer of this GatedMLP (u | v).  Exchange activations through H.
+    // the pre-activation of the last layer of this GatedMLP (u | v; HIDDEN: silu(pre) . W2^T + b2, one 64-row half at a
+    // time), parked in H at the thread's own positions as u (L) and oG = sigm(v) (G)
 #pragma unroll
-    for (int i = 0; i < AR; i++)
+    for (int h = 0; h < 2; h++) {
+      if (HIDDEN) wg_mm64_acc(acc, h, sm.W() + m.branch * 8192, acc);
 #pragma unroll
-      for (int jj = 0; jj < AC / 2; jj++) {
-        const float u0 = acc[i][2 * jj], u1 = acc[i][2 * jj + 1];
-        st_f2(H + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), m.branch == 0 ? silu_f(u0) : sigm(u0),
-              m.branch == 0 ? silu_f(u1) : sigm(u1));
-      }
-    __syncthreads();
-#pragma unroll
-    for (int i = 0; i < AR; i++) {
-      const int r = m.row(i);
-      const bool ok = r < nvalid;
-      // this row's 16 upstream gradients, loaded as float2 pairs before any is used
-      const float* gsrc = HIDDEN ? a.gaggB + (size_t)(ok ? s_b[r] : 0) * D : a.gang + (size_t)(r0 + (ok ? r : 0)) * D;
-      float2 gm2[AC / 2];
-#pragma unroll
-      for (int jj = 0; jj < AC / 2; jj++)
-        gm2[jj] = ok ? *reinterpret_cast<const float2*>(gsrc + m.col(2 * jj)) : make_float2(0.f, 0.f);
-#pragma unroll
-      for (int j = 0; j < AC; j++) {
-        const float u = acc[i][j];
-        const float2 po2 = ld_f2(H + r * LDE + (1 - m.branch) * 64 + m.col(j & ~1));  // partner activations
-        const float po = (j & 1) ? po2.y : po2.x;
-        float g = 0.f;
-        if (ok) {
-          const float gm = (j & 1) ? gm2[j >> 1].y : gm2[j >> 1].x;
-          if (m.branch == 0) {
-            const float sg = sigm(u);
-            g = gm * po * (sg * (1.f + u * (1.f - sg)));
-          } else {
-            const float oG = sigm(u);
-            g = gm * po * oG * (1.f - oG);
-          }
-        }
-        acc[i][j] = g;
-      }
-    }
-    if (HIDDEN) {
-      // ghid = [gu . W2L, gv . W2G] from the adjoints in registers;  gpre = ghid * dsilu(pre), into P over pre
-      mbar_wait(sm.wbar(), wpar);  // W2^T
-      wpar ^= 1;
-      wg_mm64_acc(acc, 0, sm.W() + m.branch * 8192, acc);
-      wg_mm64_acc(acc, 1, sm.W() + m.branch * 8192, acc);
-#pragma unroll
-      for (int i = 0; i < AR; i++)
+      for (int ii = 0; ii < 2; ii++)
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
-          float* p = P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj);
-          const float2 pre = ld_f2(p);
-          st_f2(p, acc[i][2 * jj] * dsilu_f(pre.x), acc[i][2 * jj + 1] * dsilu_f(pre.y));
+          const int i = 2 * h + ii;
+          const float u0 = HIDDEN ? acc[i][2 * jj] + b2s[m.branch * 64 + m.col(2 * jj)] : acc[i][2 * jj];
+          const float u1 = HIDDEN ? acc[i][2 * jj + 1] + b2s[m.branch * 64 + m.col(2 * jj + 1)] : acc[i][2 * jj + 1];
+          st_f2(H + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), m.branch == 0 ? u0 : sigm(u0),
+                m.branch == 0 ? u1 : sigm(u1));
         }
-    } else {
+    }
+    __syncthreads();  // H holds both branches' values (HIDDEN: and W2 has been read)
+    if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.W2Tcan, 16384 * 4, sm.wbar());
+    // reverse, per 64-row half: acc = dE/du (L) / dE/dv (G) from the values parked in H (the partner's sigm(v) /
+    // silu(u) formed from them);  HIDDEN: ghid = [gu . W2L, gv . W2G] from the adjoints in registers and gpre = ghid *
+    // dsilu(pre), into P over pre;  !HIDDEN: gpre = acc, into P
 #pragma unroll
-      for (int i = 0; i < AR; i++)
+    for (int h = 0; h < 2; h++) {
+      bool ok[2];
+      float2 gm2[2][AC / 2];  // both rows' 16 upstream gradients, loaded as float2 pairs before any is used
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++) {
+        const int r = m.row(2 * h + ii);
+        ok[ii] = r < nvalid;
+        const float* gsrc =
+            HIDDEN ? a.gaggB + (size_t)(ok[ii] ? s_b[r] : 0) * D : a.gang + (size_t)(r0 + (ok[ii] ? r : 0)) * D;
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++)
-          st_f2(P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), acc[i][2 * jj], acc[i][2 * jj + 1]);
+          gm2[ii][jj] = ok[ii] ? *reinterpret_cast<const float2*>(gsrc + m.col(2 * jj)) : make_float2(0.f, 0.f);
+      }
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++) {
+        const int i = 2 * h + ii;
+        const int r = m.row(i);
+#pragma unroll
+        for (int j = 0; j < AC; j++) {
+          const float2 ow2 = ld_f2(H + r * LDE + m.branch * 64 + m.col(j & ~1));        // u (L) / oG (G)
+          const float2 pt2 = ld_f2(H + r * LDE + (1 - m.branch) * 64 + m.col(j & ~1));  // the partner's
+          const float x = (j & 1) ? ow2.y : ow2.x;
+          const float pt = (j & 1) ? pt2.y : pt2.x;
+          float g = 0.f;
+          if (ok[ii]) {
+            const float gm = (j & 1) ? gm2[ii][j >> 1].y : gm2[ii][j >> 1].x;
+            if (m.branch == 0) {
+              const float sg = sigm(x);
+              g = gm * pt * (sg * (1.f + x * (1.f - sg)));
+            } else {
+              const float oL = silu_f(pt);
+              g = gm * oL * x * (1.f - x);
+            }
+          }
+          acc[i][j] = g;
+        }
+      }
+      if (HIDDEN) {
+        if (h == 0) mbar_wait(sm.wbar(), wpar);  // W2^T
+        wg_mm64_acc(acc, h, sm.W() + m.branch * 8192, acc);
+      }
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++) {
+          const int i = 2 * h + ii;
+          float* p = P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj);
+          if (HIDDEN) {
+            const float2 pre = ld_f2(p);
+            st_f2(p, acc[i][2 * jj] * dsilu_f(pre.x), acc[i][2 * jj + 1] * dsilu_f(pre.y));
+          } else {
+            st_f2(p, acc[i][2 * jj], acc[i][2 * jj + 1]);
+          }
+        }
     }
+    if (HIDDEN) wpar ^= 1;
     fence_proxy_async_smem();  // this thread's generic accesses of H come before its bulk refill
     __syncthreads();           // H, its stage's index arrays and (HIDDEN) W2^T are free; P holds gpre
     if (more) {
