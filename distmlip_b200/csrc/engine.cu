@@ -267,7 +267,7 @@ static float tf32_hi_host(float x) {
 // raw [N][K] row-major (K contiguous == K-major operand) -> canonical no-swizzle core-matrix layout
 // (8 rows x 16 B per core matrix; K-chunk-major then row-group), hi plane followed by lo plane.
 // element (n, k) at ((k/4) * (N/8) + n/8) * 32 + (n%8)*4 + k%4 ;  Kpad >= K pads with zeros.
-static std::vector<float> canon_split(const std::vector<float>& raw, int N, int K, int Kpad) {
+std::vector<float> canon_split(const std::vector<float>& raw, int N, int K, int Kpad) {
   std::vector<float> o((size_t)2 * N * Kpad, 0.f);
   for (int n = 0; n < N; n++)
     for (int k = 0; k < K; k++) {
@@ -284,7 +284,7 @@ static std::vector<float> canon_split(const std::vector<float>& raw, int N, int 
 // fused kernels pass A as float2 pairs (columns 2 (l%4), 2 (l%4) + 1 of a block), from their wgmma accumulator
 // fragments or from a shared-memory tile, as the register A fragment (k slots l%4, l%4 + 4) of the product
 // (kernels.cu: wg_mm64_acc, wg_mm64), so every fused-kernel B image is formatted this way.
-static std::vector<float> permute_k8(const std::vector<float>& raw, int N, int K) {
+std::vector<float> permute_k8(const std::vector<float>& raw, int N, int K) {
   std::vector<float> o(raw.size());
   for (int n = 0; n < N; n++)
     for (int k = 0; k < K; k++) {
@@ -296,7 +296,7 @@ static std::vector<float> permute_k8(const std::vector<float>& raw, int N, int K
 
 // both 64-row branches (L then G) of a stacked [128][64] block as k-permuted wgmma B operands of the fused kernels:
 // per branch canon_split of B[n][k] = raw[br*64 + n][k] (transposed = false) or raw[br*64 + k][n] (true)
-static std::vector<float> second_layer_can(const std::vector<float>& raw128x64, bool transposed) {
+std::vector<float> second_layer_can(const std::vector<float>& raw128x64, bool transposed) {
   std::vector<float> out;
   for (int br = 0; br < 2; br++) {
     std::vector<float> blk(raw128x64.begin() + (size_t)br * 4096, raw128x64.begin() + (size_t)(br + 1) * 4096);
@@ -307,12 +307,12 @@ static std::vector<float> second_layer_can(const std::vector<float>& raw128x64, 
   return out;
 }
 // the [128][64] first-layer block W as the k-permuted B operand of gpre . W (K = 128): B[n][k] = W[k][n]
-static std::vector<float> line_reverse_can(const std::vector<float>& raw128x64) {
+std::vector<float> line_reverse_can(const std::vector<float>& raw128x64) {
   return canon_split(permute_k8(transpose(raw128x64, 128, 64), 64, 128), 64, 128, 128);
 }
 // the atom conv's radial weights M [128][9] and W_ab [64][9] in the layout of AtomConvArgs::radial: columns 0..7 of each
 // 64-row block as a k-permuted [64 n][8 k] wgmma B image (one k8 block on the tensor cores), column 8 as a side table
-static std::vector<float> radial_can(const std::vector<float>& M, const std::vector<float>& Wab) {
+std::vector<float> radial_can(const std::vector<float>& M, const std::vector<float>& Wab) {
   auto k8 = [](const std::vector<float>& w, int row0) {
     std::vector<float> o(64 * 8);
     for (int n = 0; n < 64; n++)

@@ -98,6 +98,18 @@ struct LineArgs {
 void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms);
 void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms);
 
+// -------- host-side weight images of the fused kernels (engine.cu) --------
+// raw [N][K] row-major -> canonical no-swizzle core-matrix layout, tf32 hi plane then lo plane (Kpad >= K: zero pad)
+std::vector<float> canon_split(const std::vector<float>& raw, int N, int K, int Kpad);
+// raw [N][K] with k permuted inside every 8-wide k block (slot q <- column 2q, slot q + 4 <- column 2q + 1)
+std::vector<float> permute_k8(const std::vector<float>& raw, int N, int K);
+// a stacked [128][64] block as the two k-permuted branch images of W2can / Wgcan (transposed: W2Tcan)
+std::vector<float> second_layer_can(const std::vector<float>& raw128x64, bool transposed);
+// a [128][64] first-layer block W as the k-permuted [64 n][128 k] image of gpre . W (WgTcan)
+std::vector<float> line_reverse_can(const std::vector<float>& raw128x64);
+// M [128][9] and W_ab [64][9] as AtomConvArgs::radial (ATOM_RAD floats)
+std::vector<float> radial_can(const std::vector<float>& M, const std::vector<float>& Wab);
+
 // -------- bond update: h' = h + upd * w3b(d_b) --------
 void launch_bond_update_fwd(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp3, const float* W3bw,
                             const float* h, const float* upd, float* hout);
