@@ -7,6 +7,7 @@
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200mlip.h"
@@ -45,6 +46,11 @@ struct DBuf {
   DBuf(DBuf&& o) noexcept : p(o.p), cap(o.cap) {
     o.p = nullptr;
     o.cap = 0;
+  }
+  DBuf& operator=(DBuf&& o) noexcept {  // the buffer held before goes with `o`
+    std::swap(p, o.p);
+    std::swap(cap, o.cap);
+    return *this;
   }
   ~DBuf() {
     if (p) cudaFree(p);

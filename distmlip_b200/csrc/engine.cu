@@ -1,11 +1,7 @@
-// engine.cu -- host orchestration behind the C-ABI (include/b200mlip.h):
-// weight composition, GPU-resident workspace, forward + hand-derived backward schedule, halo exchange
-// between slab neighbours (NCCL point-to-point between processes, peer-memory stores inside a
-// single-process group), and the extern "C" entry points.
-//
-// Schedule mirrors (and is verified stage-by-stage against) oracle/manual_ref.py; the reference
-// control flow it replaces is DistMLIP/implementations/matgl/models/chgnet.py:208-453 (forward)
-// and pes.py:109-145 (scaling, autograd backward, forces, stress).
+// engine.cu -- host orchestration behind the C-ABI (include/b200mlip.h): the frame every model runs in (weight upload,
+// GPU-resident workspace, halo exchange between slab neighbours (NCCL point-to-point between processes, peer-memory
+// stores inside a single-process group), partition sums, heat flux) and the extern "C" entry points.  The models plug in
+// through `Model`: CHGNet (engine_chgnet.inl), TensorNet (engine_tn.inl) and MACE (engine_mace.inl).
 #include <dlfcn.h>
 #include <nccl.h>
 
@@ -14,7 +10,9 @@
 #include <mutex>
 #include <thread>
 #include <cstring>
+#include <functional>
 #include <map>
+#include <memory>
 #include <new>
 #include <set>
 #include <string>
@@ -74,16 +72,65 @@ static Nccl g_nccl;
       throw b2m::Error(B2M_ERR_CUDA, std::string("NCCL error: ") + g_nccl.GetErrorString(r__));   \
   } while (0)
 
-// ------------------------------------------------------------------------------------------
-// row-GEMM weights as TcW pairs (the projection, then its transpose for the reverse pass); the fused-kernel images and
-// the biases as device pointers
-struct AtomLayerW {
-  TcW W1s, W1sT, W1e, W1eT, W1t, W1tT, Wout, WoutT;
-  float *b1, *radial, *W2can, *W2Tcan, *b2;
+struct Packer {
+  std::vector<float> host;
+  std::map<std::string, size_t> off;  // named images (put)
+  float* dev = nullptr;               // their device copy, once uploaded
+  size_t add(const std::vector<float>& v) {
+    size_t o = (host.size() + 63) / 64 * 64;  // 256 B alignment
+    host.resize(o + v.size());
+    memcpy(host.data() + o, v.data(), v.size() * sizeof(float));
+    return o;
+  }
+  void put(const std::string& name, const std::vector<float>& v) { off[name] = add(v); }
+  float* at(const std::string& name) const { return dev + off.at(name); }
 };
-struct BondLayerW {
-  TcW W1a, W1aT, W1b, W1bT, W1c, W1cT, Wout, WoutT, WAa, WAaT, WAb, WAbT, WAc, WAcT;
-  float *Wgcan, *WgTcan, *b1, *W2can, *W2Tcan, *b2, *WAgcan, *WAgTcan, *bA;
+
+struct HaloRows {
+  float* p;
+  int width;  // floats per row
+};
+
+// A model on the engine: CHGNet (engine_chgnet.inl), TensorNet (engine_tn.inl), MACE (engine_mace.inl).  The frame
+// calls it for everything that differs between models; a model is built by its factory (make_*), which checks the
+// description, and owns its weights and its per-structure workspace.
+struct Model {
+  const char* name = "";        // names the configuration in the refusal of an unused state_dict tensor
+  const char* trace = nullptr;  // stage() prefix when the model's B2M_<MODEL>_TRACE=1
+  bool sitewise = false;        // has a site-wise readout (b2m_get_sitewise)
+  bool own_scaling = false;     // carries its own scale, shift and E0 (b2m_set_scaling / b2m_set_element_refs refuse)
+  virtual ~Model() = default;
+  // state_dict -> weight images in P (each tensor read through weight()); after the upload, the device pointers
+  virtual void pack(b2m_engine* e, Packer& P) = 0;
+  virtual void bind(const Packer& P) = 0;
+  virtual void alloc(b2m_engine* e) = 0;  // workspace of the resident graph
+  virtual void release() = 0;             // frees that workspace
+  virtual void forward(b2m_engine* e) = 0;
+  virtual void backward(b2m_engine* e) = 0;
+  virtual HaloRows halo(int l, bool bonds) = 0;  // rows exchanged for layer l: atom rows, or bond rows
+  virtual int halo_width() const = 0;            // widest halo row, sizes the transport buffers
+  // name -> (pointer, rows, cols) for b2m_debug_tensor; false: no such tensor
+  virtual bool debug(b2m_engine* e, const std::string& n, const float*& src, int64_t& r, int64_t& c) = 0;
+};
+
+// per-structure buffers of the frame (b2m_release_workspace replaces them with empty ones)
+struct Bufs {
+  DBuf<float> forces, sendbuf, recvbuf;
+  DBuf<double> scal;   // [0]=energy, [1..9]=virial
+  DBuf<float> precv[2];  // adjoint rows pushed by my neighbours (backward), double-buffered by point parity
+  DBuf<float> ftmp;      // leader: staging of a peer's force array
+  DBuf<float> fsum;      // leader: the group's summed forces (the partitions' own arrays stay untouched)
+  DBuf<float> site, site_full;  // site-wise readout: owned rows, the whole structure
+  // per-atom energies and virials (b2m_set_atomic; DESIGN.md "Per-atom energies and virials"): allocated on the first
+  // evaluation with the flag on, indexed by global atom id like `forces`
+  DBuf<double> atom_e;        // [N]
+  DBuf<float> atom_vir;       // [N][kVirPitch]
+  DBuf<double> aesum, aetmp;  // leader of a group: the summed energies / staging of a peer's array
+  DBuf<float> avsum, avtmp;   // same for the virials
+  DBuf<float> hf_w;       // [N] readout weight of every unfolded atom (heat flux)
+  DBuf<float> hf_G;       // leader: [3][N][3] forces of the three seeded passes
+  DBuf<float> hf_fold;    // leader: folded forces [n][3] or virials [n][kVirPitch]
+  DBuf<double> hf_vel, hf_out;
 };
 
 }  // namespace b2m
@@ -120,9 +167,7 @@ struct GroupSync {
 
 struct b2m_engine {
   b2m_model_desc desc;
-  int kind = 0;                   // 0: CHGNet (b2m_create), 1: TensorNet (b2m_create_tensornet), 2: MACE (b2m_create_mace)
-  b2m::TnState* tn = nullptr;     // TensorNet weights and workspace (kind 1)
-  b2m::MaceState* mace = nullptr;  // MACE weights and workspace (kind 2)
+  std::unique_ptr<b2m::Model> model;
   int device = 0;
   cudaStream_t st = nullptr;
   cudaStream_t cst = nullptr;            // halo traffic of the forward pass (overlaps the projections that do not need it)
@@ -136,14 +181,7 @@ struct b2m_engine {
   DBuf<double> erefbuf;
   bool finalized = false;
   DBuf<float> wbuf;
-  std::vector<AtomLayerW> aw;
-  std::vector<BondLayerW> bw;
-  float *d_emb = nullptr, *d_Wbe = nullptr, *d_Wae = nullptr, *d_W3bw = nullptr, *d_fa = nullptr;
-  TcW F0, F0T, F1, F1T;  // final MLP 64 -> 64 -> 64 and transposes
-  float *d_c0 = nullptr, *d_c1 = nullptr, *d_F2 = nullptr, *d_Ws = nullptr;
   const double* d_eref = nullptr;  // per-element energy offsets, double like the energy accumulator
-  float c2 = 0.f, bs = 0.f;
-  RadialParams rp2, rp3;
   // comm
   int rank = 0, world = 1;
   ncclComm_t comm = nullptr;
@@ -155,9 +193,6 @@ struct b2m_engine {
   GroupSync gsync;                 // leader only
   std::vector<cudaEvent_t> hev;    // one event per halo-exchange point of a run
   int hpoint = 0;
-  DBuf<float> precv[2];            // adjoint rows pushed by my neighbours (backward), double-buffered by point parity
-  DBuf<float> ftmp;                // leader: staging of a peer's force array
-  DBuf<float> fsum;                // leader: the group's summed forces (the partitions' own arrays stay untouched)
   int view = 0;                    // leader: partition addressed by the inspection calls (b2m_set_view)
   // page-locked staging owned by the library: host arrays go through it with a few copy threads (a single-threaded
   // memcpy of 24 MB of positions was the largest host item of an end-to-end step at 1 M atoms)
@@ -165,28 +200,12 @@ struct b2m_engine {
   size_t pin_in_cap = 0;
   void* pin_out = nullptr;  // [N,3] f32 forces
   size_t pin_out_cap = 0;
-  // graph + workspace
+  // resident graph and the per-structure buffers
   Graph g;
   bool have_graph = false;
-  std::vector<DBuf<float>> x, h, ang, upd;
-  bool want_grads = true;
-  // first-layer projections of every atom-conv layer (A = x W1s^T, C = x W1t^T + b1, Q = h W1e^T), one buffer per
-  // layer: the backward gathers the rows the forward wrote instead of re-running three GEMMs per layer
-  // (about 1.1 GB per 100k atoms for the four layers)
-  std::vector<DBuf<float>> ApL, CpL, QpL;
-  static int proj_slot(int l) { return l; }
-  DBuf<float> Ha, Hb, Xc, agg, aggB, y1p, y1, y2p, y2, e_atom, site;
-  DBuf<float> gx, gh, gang, gA, gC, gQ, gHa, gHb, gXc, gagg, gupd, gaggB, gd, gdb, gbvec, gy1, gy2;
-  DBuf<float> forces, sendbuf, recvbuf, site_full;
-  DBuf<double> scal;  // [0]=energy, [1..9]=virial
-  // per-atom energies and virials (b2m_set_atomic; DESIGN.md "Per-atom energies and virials"): allocated on the first
-  // evaluation with the flag on, indexed by global atom id like `forces`
-  bool atomic = false;
+  b2m::Bufs buf;
+  bool atomic = false;      // b2m_set_atomic
   int atomic_last = 0;      // what the last evaluation left in them: 0 nothing, 1 energies, 2 energies and virials
-  DBuf<double> atom_e;      // [N]
-  DBuf<float> atom_vir;     // [N][kVirPitch]
-  DBuf<double> aesum, aetmp;  // leader of a group: the summed energies / staging of a peer's array
-  DBuf<float> avsum, avtmp;   // same for the virials
   // heat flux (b2m_set_heat_flux; DESIGN.md §10): with hf_reach > 0 b2m_set_structure builds the unfolded cell (`uf`) and
   // the graph of it without periodicity; every readout then weights atom j's energy by hf_w[j]
   double hf_reach = 0;
@@ -194,10 +213,6 @@ struct b2m_engine {
   int64_t hf_n = 0;       // cell atoms of the resident unfolded graph; 0: the graph is the structure itself
   int hf_seed = -1;       // weight of the next evaluation: -1 the cell mask (1 / 0), 0..2 the seed (r_j - c)_alpha
   double hf_c[3] = {0, 0, 0};  // cell centre
-  DBuf<float> hf_w;       // [N] readout weight of every unfolded atom
-  DBuf<float> hf_G;       // leader: [3][N][3] forces of the three seeded passes
-  DBuf<float> hf_fold;    // leader: folded forces [n][3] or virials [n][kVirPitch]
-  DBuf<double> hf_vel, hf_out;
   // timings
   cudaEvent_t ev[8] = {nullptr};
   double t_graph = 0, t_fwd = 0, t_bwd = 0, t_gather = 0, t_total = 0;
@@ -214,27 +229,34 @@ namespace b2m {
 // atoms of the structure the caller passed: the graph's atoms, or the cell atoms of an unfolded graph
 static int64_t cell_atoms(const b2m_engine* e) { return e->hf_n ? e->hf_n : e->g.N; }
 
-static const std::vector<float>& W(b2m_engine* e, const std::string& k, std::vector<int64_t> shape) {
+// state_dict tensor k, marked as used; its shape must be `shape`, or with `flat` only hold as many elements
+static const std::vector<float>& weight(b2m_engine* e, const std::string& k, const std::vector<int64_t>& shape,
+                                        const char* shape_err, bool flat = false) {
   auto it = e->host_w.find(k);
   B2M_REQUIRE(it != e->host_w.end(), B2M_ERR_INVALID, "missing weight: " + k);
   e->consumed.insert(k);
-  const auto& sh = e->host_shape[k];
   size_t n = 1;
   for (auto s : shape) n *= (size_t)s;
-  B2M_REQUIRE(it->second.size() == n && sh == shape, B2M_ERR_INVALID,
-              "weight '" + k + "' has an unsupported shape (engine supports dim=64, max_n=9, max_f=4)");
+  B2M_REQUIRE(it->second.size() == n && (flat || e->host_shape[k] == shape), B2M_ERR_INVALID,
+              "weight '" + k + "' has an unsupported shape" + shape_err);
   return it->second;
 }
 
-struct Packer {
-  std::vector<float> host;
-  size_t add(const std::vector<float>& v) {
-    size_t off = (host.size() + 63) / 64 * 64;  // 256 B alignment
-    host.resize(off + v.size());
-    memcpy(host.data() + off, v.data(), v.size() * sizeof(float));
-    return off;
-  }
-};
+// B2M_TN_TRACE=1 / B2M_MACE_TRACE=1: synchronise after every stage of that model and name it on stderr (locating a
+// faulting or hanging kernel)
+static const char* trace_tag(const char* env, const char* tag) {
+  const char* v = getenv(env);
+  return v && v[0] == '1' ? tag : nullptr;
+}
+static void stage(b2m_engine* e, const char* name) {
+  if (!e->model->trace) return;
+  fprintf(stderr, "[%s] %s ...", e->model->trace, name);
+  fflush(stderr);
+  cudaError_t r = cudaStreamSynchronize(e->st);
+  fprintf(stderr, " %s\n", cudaGetErrorString(r));
+  fflush(stderr);
+}
+
 
 // slice columns [c0, c0+64) of a row-major [rows][ncol] matrix -> [rows][64]
 static std::vector<float> cols(const std::vector<float>& m, int rows, int ncol, int c0) {
@@ -368,132 +390,15 @@ static void tc_mm(b2m_engine* e, const float* A, int lda, const TcW& W, float* o
 }
 
 static void finalize_weights(b2m_engine* e) {
-  const int nb = e->desc.n_blocks;
-  for (auto& kv : e->host_w) {
-    const std::string& k = kv.first;
-    bool bad = k.find("atom_graph_layers") != std::string::npos &&
-               (k.find("edge_update_func") != std::string::npos || k.find("weight_func") != std::string::npos);
-    bad = bad || (k.find("bond_graph_layers") != std::string::npos && k.find("weight_func") != std::string::npos);
-    bad = bad || k.find("state_embedding") != std::string::npos || k.find("normalization") != std::string::npos;
-    B2M_REQUIRE(!bad, B2M_ERR_INVALID,
-                "unsupported CHGNet option (bond_update_hidden_dims / layer_bond_weights / state / norm): " + k);
-  }
   e->consumed.clear();
   Packer P;
-  std::map<std::string, size_t> off;
-  auto put = [&](const std::string& name, const std::vector<float>& v) { off[name] = P.add(v); };
-  // an nn.Linear weight [out][in] as the row GEMM x . W^T (K = in) and its reverse g . W
-  auto linear = [&](const std::vector<float>& w, int out, int in, TcW& fwd, TcW& rev) {
-    pack_tc2(P, transpose(w, out, in), in, out, fwd, rev);
-  };
-
-  const auto& f2 = W(e, "bond_expansion.frequencies", {NR});
-  const auto& f3 = W(e, "threebody_bond_expansion.frequencies", {NR});
-  const auto& fa = W(e, "angle_expansion.frequencies", {5});
-  for (int k = 0; k < NR; k++) {
-    e->rp2.freq[k] = f2[k];
-    e->rp3.freq[k] = f3[k];
-  }
-  e->rp2.rc = (float)e->desc.cutoff;
-  e->rp3.rc = (float)e->desc.three_body_cutoff;
-  e->rp2.norm = (float)std::sqrt(2.0 / e->desc.cutoff);
-  e->rp3.norm = (float)std::sqrt(2.0 / e->desc.three_body_cutoff);
-  e->rp2.p = e->rp3.p = e->desc.cutoff_exponent;
-  put("fa", fa);
-  put("emb", W(e, "atom_embedding.weight", {e->desc.n_elem, D}));
-  const auto& Wbe = W(e, "bond_embedding.layers.0.weight", {D, NR});
-  put("Wbe", Wbe);
-  put("Wae", W(e, "angle_embedding.layers.0.weight", {D, NF}));
-  const auto& Wabw = W(e, "atom_bond_weights.weight", {D, NR});
-  put("W3bw", W(e, "threebody_bond_weights.weight", {D, NR}));
-
-  e->aw.resize(nb);
-  for (int l = 0; l < nb; l++) {
-    const std::string p = "atom_graph_layers." + std::to_string(l) + ".conv_layer.";
-    const auto W1 = vcat(W(e, p + "node_update_func.layers.layers.0.weight", {D, 3 * D}),
-                         W(e, p + "node_update_func.gates.layers.0.weight", {D, 3 * D}));  // [128][192]
-    const auto b1 = vcat(W(e, p + "node_update_func.layers.layers.0.bias", {D}),
-                         W(e, p + "node_update_func.gates.layers.0.bias", {D}));
-    const auto W1s = cols(W1, 128, 192, 0), W1e = cols(W1, 128, 192, 64), W1t = cols(W1, 128, 192, 128);
-    const auto W2 = vcat(W(e, p + "node_update_func.layers.layers.1.weight", {D, D}),
-                         W(e, p + "node_update_func.gates.layers.1.weight", {D, D}));
-    const auto b2 = vcat(W(e, p + "node_update_func.layers.layers.1.bias", {D}),
-                         W(e, p + "node_update_func.gates.layers.1.bias", {D}));
-    const auto& Wout = W(e, p + "node_out_func.weight", {D, D});
-    std::vector<float> M(128 * 9);
-    for (int j = 0; j < 128; j++)
-      for (int k = 0; k < 9; k++) {
-        double s = 0;
-        for (int c = 0; c < 64; c++) s += (double)W1e[(size_t)j * 64 + c] * (double)Wbe[(size_t)c * 9 + k];
-        M[j * 9 + k] = (float)s;
-      }
-    const std::string q = "a" + std::to_string(l) + ".";
-    AtomLayerW& w = e->aw[l];
-    linear(W1s, 128, 64, w.W1s, w.W1sT);
-    linear(W1e, 128, 64, w.W1e, w.W1eT);
-    linear(W1t, 128, 64, w.W1t, w.W1tT);
-    linear(Wout, 64, 64, w.Wout, w.WoutT);
-    put(q + "b1", b1);
-    put(q + "radial", radial_can(M, Wabw));
-    put(q + "W2can", second_layer_can(W2, false));
-    put(q + "W2Tcan", second_layer_can(W2, true));
-    put(q + "b2", b2);
-  }
-  e->bw.resize(nb - 1);
-  for (int l = 0; l < nb - 1; l++) {
-    const std::string p = "bond_graph_layers." + std::to_string(l) + ".conv_layer.";
-    const auto W1 = vcat(W(e, p + "node_update_func.layers.layers.0.weight", {D, 4 * D}),
-                         W(e, p + "node_update_func.gates.layers.0.weight", {D, 4 * D}));  // [128][256]
-    const auto b1 = vcat(W(e, p + "node_update_func.layers.layers.0.bias", {D}),
-                         W(e, p + "node_update_func.gates.layers.0.bias", {D}));
-    const auto W1a = cols(W1, 128, 256, 0), W1g = cols(W1, 128, 256, 64), W1c = cols(W1, 128, 256, 128),
-               W1b = cols(W1, 128, 256, 192);
-    const auto W2 = vcat(W(e, p + "node_update_func.layers.layers.1.weight", {D, D}),
-                         W(e, p + "node_update_func.gates.layers.1.weight", {D, D}));
-    const auto b2 = vcat(W(e, p + "node_update_func.layers.layers.1.bias", {D}),
-                         W(e, p + "node_update_func.gates.layers.1.bias", {D}));
-    const auto& Wout = W(e, p + "node_out_func.weight", {D, D});
-    const auto WA = vcat(W(e, p + "edge_update_func.layers.layers.0.weight", {D, 4 * D}),
-                         W(e, p + "edge_update_func.gates.layers.0.weight", {D, 4 * D}));
-    const auto bA = vcat(W(e, p + "edge_update_func.layers.layers.0.bias", {D}),
-                         W(e, p + "edge_update_func.gates.layers.0.bias", {D}));
-    const auto WAa = cols(WA, 128, 256, 0), WAg = cols(WA, 128, 256, 64), WAc = cols(WA, 128, 256, 128),
-               WAb = cols(WA, 128, 256, 192);
-    const std::string q = "b" + std::to_string(l) + ".";
-    BondLayerW& w = e->bw[l];
-    linear(W1a, 128, 64, w.W1a, w.W1aT);
-    linear(W1b, 128, 64, w.W1b, w.W1bT);
-    linear(W1c, 128, 64, w.W1c, w.W1cT);
-    linear(Wout, 64, 64, w.Wout, w.WoutT);
-    linear(WAa, 128, 64, w.WAa, w.WAaT);
-    linear(WAb, 128, 64, w.WAb, w.WAbT);
-    linear(WAc, 128, 64, w.WAc, w.WAcT);
-    put(q + "Wgcan", second_layer_can(W1g, false));
-    put(q + "b1", b1);
-    put(q + "WgTcan", line_reverse_can(W1g));
-    put(q + "W2can", second_layer_can(W2, false));
-    put(q + "W2Tcan", second_layer_can(W2, true));
-    put(q + "b2", b2);
-    put(q + "WAgcan", second_layer_can(WAg, false));
-    put(q + "bA", bA);
-    put(q + "WAgTcan", line_reverse_can(WAg));
-  }
-  linear(W(e, "final_layer.layers.0.weight", {D, D}), 64, 64, e->F0, e->F0T);
-  put("c0", W(e, "final_layer.layers.0.bias", {D}));
-  linear(W(e, "final_layer.layers.1.weight", {D, D}), 64, 64, e->F1, e->F1T);
-  put("c1", W(e, "final_layer.layers.1.bias", {D}));
-  put("F2", W(e, "final_layer.layers.2.weight", {1, D}));
-  e->c2 = W(e, "final_layer.layers.2.bias", {1})[0];
-  put("Ws", W(e, "sitewise_readout.weight", {1, D}));
-  e->bs = W(e, "sitewise_readout.bias", {1})[0];
+  e->model->pack(e, P);
   // every tensor of the state_dict must have been used: an extra bias / normalisation / per-layer weight function of
-  // a non-default CHGNet configuration would otherwise be dropped silently and give wrong energies (ADVICE r1).
-  // bond_bond_weights is part of the default model but feeds only the (absent) bond update of the atom graph.
-  for (auto& kv : e->host_w) {
-    if (e->consumed.count(kv.first) || kv.first == "bond_bond_weights.weight") continue;
-    throw Error(B2M_ERR_INVALID, "state_dict tensor '" + kv.first +
-                                     "' is not used by this engine (unsupported CHGNet configuration; refusing to ignore it)");
-  }
+  // a configuration the engine does not build would otherwise be dropped silently and give wrong energies (ADVICE r1)
+  for (auto& kv : e->host_w)
+    if (!e->consumed.count(kv.first))
+      throw Error(B2M_ERR_INVALID, "state_dict tensor '" + kv.first + "' is not used by this engine (unsupported " +
+                                       e->model->name + " configuration; refusing to ignore it)");
   if (!e->elem_refs.empty()) {
     e->erefbuf.ensure(e->elem_refs.size());
     B2M_CK(cudaMemcpyAsync(e->erefbuf.p, e->elem_refs.data(), e->elem_refs.size() * sizeof(double), cudaMemcpyHostToDevice,
@@ -502,71 +407,28 @@ static void finalize_weights(b2m_engine* e) {
   e->wbuf.ensure(P.host.size() + 64);
   B2M_CK(cudaMemcpyAsync(e->wbuf.p, P.host.data(), P.host.size() * sizeof(float), cudaMemcpyHostToDevice, e->st));
   B2M_CK(cudaStreamSynchronize(e->st));
-  auto dp = [&](const std::string& n) { return e->wbuf.p + off.at(n); };
-  e->d_fa = dp("fa");
-  e->d_emb = dp("emb");
-  e->d_Wbe = dp("Wbe");
-  e->d_Wae = dp("Wae");
-  e->d_W3bw = dp("W3bw");
-  e->d_c0 = dp("c0"), e->d_c1 = dp("c1"), e->d_F2 = dp("F2"), e->d_Ws = dp("Ws");
+  P.dev = e->wbuf.p;
+  e->model->bind(P);
   e->d_eref = e->elem_refs.empty() ? nullptr : e->erefbuf.p;
-  for (int l = 0; l < nb; l++) {
-    const std::string q = "a" + std::to_string(l) + ".";
-    AtomLayerW& w = e->aw[l];
-    w.b1 = dp(q + "b1"), w.radial = dp(q + "radial"), w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
-  }
-  for (int l = 0; l < nb - 1; l++) {
-    const std::string q = "b" + std::to_string(l) + ".";
-    BondLayerW& w = e->bw[l];
-    w.Wgcan = dp(q + "Wgcan"), w.WgTcan = dp(q + "WgTcan"), w.b1 = dp(q + "b1");
-    w.W2can = dp(q + "W2can"), w.W2Tcan = dp(q + "W2Tcan"), w.b2 = dp(q + "b2");
-    w.WAgcan = dp(q + "WAgcan"), w.WAgTcan = dp(q + "WAgTcan"), w.bA = dp(q + "bA");
-  }
   e->finalized = true;
 }
 
 // ------------------------------------------------------------------------------------------
 static void alloc_workspace(b2m_engine* e) {
+  e->model->alloc(e);
   Graph& g = e->g;
-  const int nb = e->desc.n_blocks;
-  const size_t nl = g.n_loc, no = g.n_own, bl = g.B_loc, bo = g.B_own;
-  const size_t A = (size_t)g.A, E = (size_t)g.E;
-  e->x.resize(nb + 1);
-  e->h.resize(nb);
-  e->ang.resize(nb - 1);
-  e->upd.resize(nb - 1);
-  for (auto& b : e->x) b.ensure(nl * D + 64);
-  for (auto& b : e->h) b.ensure(bl * D + 64);
-  const size_t Apad = (A + 127) / 128 * 128;  // whole 128-row tiles
-  for (auto& b : e->ang) b.ensure(Apad * D + 64);
-  for (auto& b : e->upd) b.ensure(bo * D + 64);
-  e->ApL.resize(nb), e->CpL.resize(nb), e->QpL.resize(nb);
-  for (int l = 0; l < nb; l++) {
-    e->ApL[l].ensure(nl * D2 + 64), e->CpL[l].ensure(no * D2 + 64);
-    if (l > 0) e->QpL[l].ensure(bo * D2 + 64);
-  }
-  e->Ha.ensure(bl * D2 + 64), e->Hb.ensure(bo * D2 + 64), e->Xc.ensure(nl * D2 + 64);
-  e->agg.ensure(no * D + 64), e->aggB.ensure(bo * D + 64);
-  e->y1p.ensure(no * D), e->y1.ensure(no * D), e->y2p.ensure(no * D), e->y2.ensure(no * D);
-  e->e_atom.ensure(no), e->site.ensure(no);
-  e->gx.ensure(nl * D + 64), e->gh.ensure(bl * D + 64), e->gang.ensure(Apad * D + 64);
-  e->gA.ensure(nl * D2 + 64), e->gC.ensure(no * D2 + 64), e->gQ.ensure(bo * D2 + 64);
-  e->gHa.ensure(bl * D2 + 64), e->gHb.ensure(bo * D2 + 64), e->gXc.ensure(nl * D2 + 64);
-  e->gagg.ensure(no * D + 64), e->gupd.ensure(bo * D + 64), e->gaggB.ensure(bo * D + 64);
-  e->gd.ensure(E + 64), e->gdb.ensure(bl + 64), e->gbvec.ensure(bl * 3 + 64);
-  e->gy1.ensure(no * D), e->gy2.ensure(no * D);
-  e->forces.ensure((size_t)g.N * 3 + 64);
-  e->site_full.ensure((size_t)g.N + 64);
-  e->scal.ensure(16);
+  Bufs& b = e->buf;
+  b.forces.ensure((size_t)g.N * 3 + 64);
+  b.scal.ensure(16);
+  if (e->model->sitewise) b.site.ensure(g.n_own), b.site_full.ensure((size_t)g.N + 64);
   if (e->world > 1) {
     size_t tot_to = 0, tot_bto = 0;
     for (int q = 0; q < e->world; q++) tot_to += g.n_to[q], tot_bto += g.nb_to[q];
-    size_t m = std::max(tot_to * D, tot_bto * D);
+    const size_t m = std::max(tot_to, tot_bto) * e->model->halo_width();
     if (e->leader != nullptr) {
-      e->precv[0].ensure(m + 64), e->precv[1].ensure(m + 64);
+      b.precv[0].ensure(m + 64), b.precv[1].ensure(m + 64);
     } else {
-      e->sendbuf.ensure(m + 64);
-      e->recvbuf.ensure(m + 64);
+      b.sendbuf.ensure(m + 64), b.recvbuf.ensure(m + 64);
     }
   }
 }
@@ -576,16 +438,6 @@ static void alloc_workspace(b2m_engine* e) {
 // group, direct peer-memory traffic: the sender's pack kernel stores its boundary rows straight into the receiver's halo
 // rows (forward) or copies its halo adjoints into the owner's receive buffer (backward); a CUDA event per exchange point
 // orders the receiver's stream behind the sender's.
-// kind 0: atom rows x[l] | 1: bond rows h[l] | 2: TensorNet atom tensors X[l] (10 x 64 floats per atom)
-//      3: MACE node features h[l] (C floats per atom, 4 C for 0e+1o features)
-static float* halo_buffer(b2m_engine* e, int kind, int l) {
-  if (kind == 3) return e->mace->h[l].p;
-  return kind == 1 ? e->h[l].p : (kind == 2 ? e->tn->X[l].p : e->x[l].p);
-}
-static int halo_width(const b2m_engine* e, int kind, int l) {
-  if (kind == 3) return e->mace->hw[l];
-  return kind == 2 ? 10 * D : D;
-}
 
 static cudaEvent_t next_halo_event(b2m_engine* e) {
   // the events are created in b2m_create: a neighbour's thread reads hev[k] concurrently, so the vector never grows here
@@ -598,12 +450,12 @@ static cudaEvent_t next_halo_event(b2m_engine* e) {
 // that do not read the halo rows (the reference issues its copies on the compute stream, dist.py:344-356):
 //   halo_forward_begin: [compute: producer done] -> [comm stream: pack, send / receive or peer stores]
 //   halo_forward_end  : compute stream waits for the exchange (and, in a group, for the neighbours' stores)
-static void halo_forward_begin(b2m_engine* e, int kind, int l) {
+static void halo_forward_begin(b2m_engine* e, bool bonds, int l) {
   if (e->world <= 1 || e->debug_no_halo) return;
   Graph& g = e->g;
-  const bool bonds = kind == 1;
-  const size_t W = (size_t)halo_width(e, kind, l);
-  float* buf = halo_buffer(e, kind, l);
+  const HaloRows rows = e->model->halo(l, bonds);
+  const size_t W = (size_t)rows.width;
+  float* buf = rows.p;
   const int* nto = bonds ? g.nb_to : g.n_to;
   const int* toff = bonds ? g.bto_off : g.to_off;
   const int* nfrom = bonds ? g.nb_from : g.n_from;
@@ -622,19 +474,19 @@ static void halo_forward_begin(b2m_engine* e, int kind, int l) {
       B2M_REQUIRE(pn == nto[q], B2M_ERR_STATE, "halo sections of two partitions disagree");
       const size_t pbase = bonds ? (size_t)pg.B_own : (size_t)pg.n_own;
       const size_t pfoff = bonds ? (size_t)pg.bfrom_off[e->rank] : (size_t)pg.from_off[e->rank];
-      launch_gather_rows(e->cst, nto[q], (int)W, list + toff[q], buf, halo_buffer(pe, kind, l) + (pbase + pfoff) * W);
+      launch_gather_rows(e->cst, nto[q], (int)W, list + toff[q], buf, pe->model->halo(l, bonds).p + (pbase + pfoff) * W);
     }
     B2M_CK(cudaEventRecord(next_halo_event(e), e->cst));
     return;
   }
   for (int q = 0; q < e->world; q++)
     if (nto[q] > 0)
-      launch_gather_rows(e->cst, nto[q], (int)W, list + toff[q], buf, e->sendbuf.p + (size_t)toff[q] * W);
+      launch_gather_rows(e->cst, nto[q], (int)W, list + toff[q], buf, e->buf.sendbuf.p + (size_t)toff[q] * W);
   NCCL_CK(g_nccl.GroupStart());
   for (int q = 0; q < e->world; q++) {
     if (q == e->rank) continue;
     if (nto[q] > 0)
-      NCCL_CK(g_nccl.Send(e->sendbuf.p + (size_t)toff[q] * W, (size_t)nto[q] * W, ncclFloat32, q, e->comm, e->cst));
+      NCCL_CK(g_nccl.Send(e->buf.sendbuf.p + (size_t)toff[q] * W, (size_t)nto[q] * W, ncclFloat32, q, e->comm, e->cst));
     if (nfrom[q] > 0)
       NCCL_CK(g_nccl.Recv(buf + (base + foff[q]) * W, (size_t)nfrom[q] * W, ncclFloat32, q, e->comm, e->cst));
   }
@@ -673,8 +525,8 @@ static void halo_backward(b2m_engine* e, float* gbuf, bool bonds, int width = D)
       b2m_engine* pe = L->parts[q];
       const size_t ptoff = bonds ? (size_t)pe->g.bto_off[e->rank] : (size_t)pe->g.to_off[e->rank];
       // the owner's receive buffer of this parity was consumed two exchange points ago (see DESIGN.md, group mode)
-      B2M_CK(cudaMemcpyAsync(pe->precv[k & 1].p + ptoff * W, gbuf + (base + foff[q]) * W, (size_t)nfrom[q] * W * sizeof(float),
-                             cudaMemcpyDefault, e->st));
+      B2M_CK(cudaMemcpyAsync(pe->buf.precv[k & 1].p + ptoff * W, gbuf + (base + foff[q]) * W,
+                             (size_t)nfrom[q] * W * sizeof(float), cudaMemcpyDefault, e->st));
     }
     launch_zero_rows(e->st, gbuf + base * W, nhalo * W);
     cudaEvent_t ev = next_halo_event(e);
@@ -685,7 +537,7 @@ static void halo_backward(b2m_engine* e, float* gbuf, bool bonds, int width = D)
       if (q != e->rank) B2M_CK(cudaStreamWaitEvent(e->st, L->parts[q]->hev[k], 0));
     for (int q = 0; q < e->world; q++)
       if (q != e->rank && nto[q] > 0)
-        launch_scatter_add_rows(e->st, nto[q], (int)W, list + toff[q], e->precv[k & 1].p + (size_t)toff[q] * W, gbuf);
+        launch_scatter_add_rows(e->st, nto[q], (int)W, list + toff[q], e->buf.precv[k & 1].p + (size_t)toff[q] * W, gbuf);
     return;
   }
   NCCL_CK(g_nccl.GroupStart());
@@ -694,216 +546,19 @@ static void halo_backward(b2m_engine* e, float* gbuf, bool bonds, int width = D)
     if (nfrom[q] > 0)
       NCCL_CK(g_nccl.Send(gbuf + (base + foff[q]) * W, (size_t)nfrom[q] * W, ncclFloat32, q, e->comm, e->st));
     if (nto[q] > 0)
-      NCCL_CK(g_nccl.Recv(e->recvbuf.p + (size_t)toff[q] * W, (size_t)nto[q] * W, ncclFloat32, q, e->comm, e->st));
+      NCCL_CK(g_nccl.Recv(e->buf.recvbuf.p + (size_t)toff[q] * W, (size_t)nto[q] * W, ncclFloat32, q, e->comm, e->st));
   }
   NCCL_CK(g_nccl.GroupEnd());
   for (int q = 0; q < e->world; q++)
     if (nto[q] > 0)
-      launch_scatter_add_rows(e->st, nto[q], (int)W, list + toff[q], e->recvbuf.p + (size_t)toff[q] * W, gbuf);
+      launch_scatter_add_rows(e->st, nto[q], (int)W, list + toff[q], e->buf.recvbuf.p + (size_t)toff[q] * W, gbuf);
   launch_zero_rows(e->st, gbuf + base * W, nhalo * W);
 }
 
+#include "engine_chgnet.inl"
 #include "engine_tn.inl"
 #include "engine_mace.inl"
 
-static AtomConvArgs atom_args(b2m_engine* e, int l) {
-  Graph& g = e->g;
-  const AtomLayerW& w = e->aw[l];
-  AtomConvArgs a;
-  memset(&a, 0, sizeof a);
-  a.E = g.E;
-  a.e_src = g.e_src.p, a.e_dst = g.e_dst.p, a.e_bond = g.e_bond.p, a.e_vec = g.e_vec.p;
-  const int ps = e->proj_slot(l);
-  a.Aproj = e->ApL[ps].p, a.Cproj = e->CpL[ps].p, a.Qproj = l > 0 ? e->QpL[ps].p : nullptr;
-  a.radial = w.radial, a.W2can = w.W2can, a.W2Tcan = w.W2Tcan, a.b2 = w.b2;
-  a.rp = e->rp2;
-  return a;
-}
-static void atom_projections(b2m_engine* e, int l) {
-  Graph& g = e->g;
-  const AtomLayerW& w = e->aw[l];
-  const int ps = e->proj_slot(l);
-  tc_mm(e, e->x[l].p, D, w.W1s, e->ApL[ps].p, D2, g.n_loc, false);
-  tc_mm(e, e->x[l].p, D, w.W1t, e->CpL[ps].p, D2, g.n_own, false, w.b1);
-  if (l > 0) tc_mm(e, e->h[l].p, D, w.W1e, e->QpL[ps].p, D2, g.B_own, false);
-}
-static void atom_layer_fwd(b2m_engine* e, int l) {
-  Graph& g = e->g;
-  const AtomLayerW& w = e->aw[l];
-  atom_projections(e, l);
-  launch_zero_rows(e->st, e->agg.p, (int64_t)g.n_own * D);
-  AtomConvArgs a = atom_args(e, l);
-  a.agg = e->agg.p;
-  cudaEvent_t e0, e1;
-  B2M_CK(cudaEventCreate(&e0));
-  B2M_CK(cudaEventCreate(&e1));
-  B2M_CK(cudaEventRecord(e0, e->st));
-  launch_atomconv_fwd(e->st, a, e->num_sms);
-  B2M_CK(cudaEventRecord(e1, e->st));
-  e->gather_ev.push_back({e0, e1});
-  tc_mm(e, e->agg.p, D, w.Wout, e->x[l + 1].p, D, g.n_own, false, nullptr, e->x[l].p, D);
-}
-// in: gx = dE/dx[l+1] (owned rows valid, halo rows zero).  out: gx = dE/dx[l] (all local rows)
-static void atom_layer_bwd(b2m_engine* e, int l) {
-  Graph& g = e->g;
-  const AtomLayerW& w = e->aw[l];
-  tc_mm(e, e->gx.p, D, w.WoutT, e->gagg.p, D, g.n_own, false);
-  // A / C / Q of this layer are still in their per-layer buffers from the forward: no recompute
-  AtomConvArgs a = atom_args(e, l);
-  a.gagg = e->gagg.p;
-  a.gd = e->gd.p;
-  const bool need_gx = l > 0;
-  if (need_gx) {
-    launch_zero_rows(e->st, e->gA.p, (int64_t)g.n_loc * D2);
-    launch_zero_rows(e->st, e->gC.p, (int64_t)g.n_own * D2);
-    a.gA = e->gA.p, a.gC = e->gC.p, a.gQ = e->gQ.p;
-  }
-  launch_atomconv_bwd(e->st, a, e->num_sms);
-  if (need_gx) {
-    tc_mm(e, e->gA.p, D2, w.W1sT, e->gx.p, D, g.n_loc, true);
-    tc_mm(e, e->gC.p, D2, w.W1tT, e->gx.p, D, g.n_own, true);
-    tc_mm(e, e->gQ.p, D2, w.W1eT, e->gh.p, D, g.B_own, true);
-  }
-}
-
-static LineArgs line_args(b2m_engine* e, int l, bool hidden) {
-  Graph& g = e->g;
-  const BondLayerW& w = e->bw[l];
-  LineArgs a;
-  memset(&a, 0, sizeof a);
-  a.A = g.A;
-  a.a_in = g.a_in.p, a.a_out = g.a_out.p, a.a_ctr = g.a_ctr.p;
-  a.ang = e->ang[l].p;
-  a.Ha = e->Ha.p, a.Hb = e->Hb.p, a.Xc = e->Xc.p;
-  if (hidden) {
-    a.Wgcan = w.Wgcan, a.WgTcan = w.WgTcan, a.W2can = w.W2can, a.W2Tcan = w.W2Tcan, a.b2 = w.b2;
-  } else {
-    a.Wgcan = w.WAgcan, a.WgTcan = w.WAgTcan;
-  }
-  return a;
-}
-// first-layer projections of the line-graph MLPs: Ha / Hb from the bond features, Xc from the atom features
-static void line_proj_Ha(b2m_engine* e, int l, bool hidden) {
-  const BondLayerW& w = e->bw[l];
-  const float* hsrc = hidden ? e->h[l].p : e->h[l + 1].p;
-  tc_mm(e, hsrc, D, hidden ? w.W1a : w.WAa, e->Ha.p, D2, e->g.B_loc, false);
-}
-static void line_proj_Hb(b2m_engine* e, int l, bool hidden) {
-  const BondLayerW& w = e->bw[l];
-  const float* hsrc = hidden ? e->h[l].p : e->h[l + 1].p;
-  tc_mm(e, hsrc, D, hidden ? w.W1b : w.WAb, e->Hb.p, D2, e->g.B_own, false, hidden ? w.b1 : w.bA);
-}
-static void line_proj_Xc(b2m_engine* e, int l, bool hidden) {
-  const BondLayerW& w = e->bw[l];
-  tc_mm(e, e->x[l + 1].p, D, hidden ? w.W1c : w.WAc, e->Xc.p, D2, e->g.n_loc, false);
-}
-static void line_projections(b2m_engine* e, int l, bool hidden) {
-  line_proj_Ha(e, l, hidden), line_proj_Hb(e, l, hidden), line_proj_Xc(e, l, hidden);
-}
-static void line_bwd_common(b2m_engine* e, int l, bool hidden, LineArgs& a) {
-  Graph& g = e->g;
-  const BondLayerW& w = e->bw[l];
-  launch_zero_rows(e->st, e->gHa.p, (int64_t)g.B_loc * D2);
-  launch_zero_rows(e->st, e->gHb.p, (int64_t)g.B_own * D2);
-  launch_zero_rows(e->st, e->gXc.p, (int64_t)g.n_loc * D2);
-  a.gang = e->gang.p, a.gHa = e->gHa.p, a.gHb = e->gHb.p, a.gXc = e->gXc.p;
-  launch_line_bwd(e->st, a, hidden, e->num_sms);
-  tc_mm(e, e->gHa.p, D2, hidden ? w.W1aT : w.WAaT, e->gh.p, D, g.B_loc, true);
-  tc_mm(e, e->gHb.p, D2, hidden ? w.W1bT : w.WAbT, e->gh.p, D, g.B_own, true);
-  tc_mm(e, e->gXc.p, D2, hidden ? w.W1cT : w.WAcT, e->gx.p, D, g.n_loc, true);
-}
-
-static void forward(b2m_engine* e) {
-  Graph& g = e->g;
-  const int nb = e->desc.n_blocks;
-  launch_embed(e->st, g.n_loc, g.type.p, e->d_emb, e->x[0].p);
-  launch_bond_init(e->st, g.B_loc, g.b_vec.p, e->rp2, e->d_Wbe, e->h[0].p);
-  launch_angle_init(e->st, g.A, g.a_in.p, g.a_out.p, g.b_vec.p, e->d_fa, e->d_Wae, e->ang[0].p);
-  for (int l = 0; l < nb - 1; l++) {
-    atom_layer_fwd(e, l);
-    const BondLayerW& w = e->bw[l];
-    // x^{l+1} halo rows travel while the two projections of the bond features run (they do not read x)
-    halo_forward_begin(e, false, l + 1);
-    line_proj_Ha(e, l, true), line_proj_Hb(e, l, true);
-    halo_forward_end(e);
-    line_proj_Xc(e, l, true);
-    launch_zero_rows(e->st, e->aggB.p, (int64_t)g.B_own * D);
-    LineArgs a = line_args(e, l, true);
-    a.aggB = e->aggB.p;
-    launch_line_fwd(e->st, a, true, e->num_sms);
-    tc_mm(e, e->aggB.p, D, w.Wout, e->upd[l].p, D, g.B_own, false);
-    launch_bond_update_fwd(e->st, g.B_own, g.b_vec.p, e->rp3, e->d_W3bw, e->h[l].p, e->upd[l].p, e->h[l + 1].p);
-    if (l < nb - 2) {
-      // the last block's angle update (and the halo copy of h feeding it) is dead code in the
-      // reference (chgnet.py:353-368 on the last iteration): nothing reads it afterwards.
-      // h^{l+1} halo rows travel while Hb (owned bonds only) and Xc (atoms) are projected; Ha reads the halo rows
-      halo_forward_begin(e, true, l + 1);
-      line_proj_Hb(e, l, false), line_proj_Xc(e, l, false);
-      halo_forward_end(e);
-      line_proj_Ha(e, l, false);
-      LineArgs b = line_args(e, l, false);
-      b.ang_out = e->ang[l + 1].p;
-      launch_line_fwd(e->st, b, false, e->num_sms);
-    }
-  }
-  // site-wise readout after block n-2 (chgnet.py:392-398)
-  launch_rowdot(e->st, g.n_own, e->x[nb - 1].p, e->d_Ws, e->bs, e->site.p, nullptr, nullptr, nullptr, 1.f);
-  atom_layer_fwd(e, nb - 1);
-  // final MLP 64 -> 64 -> 64 -> 1, sum (chgnet.py:422-440); E = std * E + mean (+ element refs) (pes.py:109-113)
-  tc_mm(e, e->x[nb].p, D, e->F0, e->y1p.p, D, g.n_own, false, e->d_c0);
-  launch_silu(e->st, (int64_t)g.n_own * D, e->y1p.p, e->y1.p);
-  tc_mm(e, e->y1.p, D, e->F1, e->y2p.p, D, g.n_own, false, e->d_c1);
-  launch_silu(e->st, (int64_t)g.n_own * D, e->y2p.p, e->y2.p);
-  B2M_CK(cudaMemsetAsync(e->scal.p, 0, 16 * sizeof(double), e->st));
-  launch_rowdot(e->st, g.n_own, e->y2.p, e->d_F2, e->c2, e->e_atom.p, e->scal.p, g.type.p, e->d_eref,
-                (float)e->desc.data_std, g.gid.p, e->atomic ? e->atom_e.p : nullptr, e->desc.data_mean / cell_atoms(e),
-                e->hf_n ? e->hf_w.p : nullptr);
-}
-
-static void backward(b2m_engine* e) {
-  Graph& g = e->g;
-  const int nb = e->desc.n_blocks;
-  launch_zero_rows(e->st, e->gd.p, g.E);
-  launch_zero_rows(e->st, e->gdb.p, g.B_loc);
-  launch_zero_rows(e->st, e->gbvec.p, (int64_t)g.B_loc * 3);
-  launch_zero_rows(e->st, e->gh.p, (int64_t)g.B_loc * D);
-  launch_zero_rows(e->st, e->gang.p, (g.A + 127) / 128 * 128 * D);
-  launch_zero_rows(e->st, e->gx.p, (int64_t)g.n_loc * D);
-  launch_zero_rows(e->st, e->forces.p, g.N * 3);
-  // readout backward
-  launch_readout_seed(e->st, g.n_own, e->y2p.p, e->d_F2, (float)e->desc.data_std, e->gy2.p, g.gid.p,
-                      e->hf_n ? e->hf_w.p : nullptr);
-  tc_mm(e, e->gy2.p, D, e->F1T, e->gy1.p, D, g.n_own, false);
-  launch_dsilu_mul(e->st, (int64_t)g.n_own * D, e->y1p.p, e->gy1.p);
-  tc_mm(e, e->gy1.p, D, e->F0T, e->gx.p, D, g.n_own, false);
-  atom_layer_bwd(e, nb - 1);
-  for (int l = nb - 2; l >= 0; l--) {
-    const BondLayerW& w = e->bw[l];
-    if (l < nb - 2) {
-      // the first-layer projections of the angle update are recomputed (the buffers hold the next layer's)
-      line_projections(e, l, false);
-      LineArgs a = line_args(e, l, false);
-      line_bwd_common(e, l, false, a);
-      halo_backward(e, e->gh.p, true);
-    }
-    launch_bond_update_bwd(e->st, g.B_own, g.b_vec.p, e->rp3, e->d_W3bw, e->gh.p, e->upd[l].p, e->gupd.p, e->gdb.p);
-    tc_mm(e, e->gupd.p, D, w.WoutT, e->gaggB.p, D, g.B_own, false);
-    line_projections(e, l, true);
-    LineArgs a = line_args(e, l, true);
-    a.gaggB = e->gaggB.p;
-    line_bwd_common(e, l, true, a);
-    halo_backward(e, e->gx.p, false);
-    atom_layer_bwd(e, l);
-  }
-  // geometry: h0 = W_be be(d_b), theta/Fourier, then edges -> forces and virial
-  launch_h0_bwd(e->st, g.B_loc, g.b_vec.p, e->rp2, e->d_Wbe, e->gh.p, e->gdb.p);
-  launch_angle_init_bwd(e->st, g.A, g.a_in.p, g.a_out.p, g.b_vec.p, e->d_fa, e->d_Wae, e->gang.p, e->gbvec.p);
-  float* avir = e->atomic ? e->atom_vir.p : nullptr;
-  launch_edge_final(e->st, g.E, g.e_src.p, g.e_dst.p, g.e_bond.p, g.e_vec.p, g.gid.p, e->gd.p, e->gdb.p, e->gbvec.p,
-                    e->forces.p, e->scal.p + 1, avir);
-  launch_halo_bond_final(e->st, g.B_own, g.B_loc, g.b_src_gid.p, g.b_dst.p, g.b_vec.p, g.gid.p, e->gdb.p, e->gbvec.p,
-                         e->forces.p, e->scal.p + 1, avir);
-}
 
 // ------------------------------------------------------------------------------------------
 // heat flux (DESIGN.md §10)
@@ -985,38 +640,31 @@ static void run(b2m_engine* e, bool grads) {
   e->gather_ev.clear();
   const long long l0 = g_launch_count;
   B2M_CK(cudaEventRecord(e->ev[0], e->st));
-  e->want_grads = grads;
   const size_t N = (size_t)e->g.N;
   if (e->atomic) {  // zeroed here, before the readout writes the energies and the backward accumulates the virials
-    e->atom_e.ensure(N + 64);
-    e->atom_e.zero(N, e->st);
+    e->buf.atom_e.ensure(N + 64);
+    e->buf.atom_e.zero(N, e->st);
     if (grads) {
-      e->atom_vir.ensure(N * kVirPitch + 64);
-      e->atom_vir.zero(N * kVirPitch, e->st);
+      e->buf.atom_vir.ensure(N * kVirPitch + 64);
+      e->buf.atom_vir.zero(N * kVirPitch, e->st);
     }
   }
   e->atomic_last = 0;
   if (e->hf_n) {
     LAUNCH_HF(k_hf_weights, e->g.N, e->st, e->g.N, e->hf_n, e->g.cart.p, e->hf_c[0], e->hf_c[1], e->hf_c[2], e->hf_seed,
-              e->hf_w.p);
+              e->buf.hf_w.p);
   }
-  if (e->kind == 1) tn_forward(e);
-  else if (e->kind == 2) mace_forward(e);
-  else forward(e);
+  e->model->forward(e);
   B2M_CK(cudaEventRecord(e->ev[1], e->st));
-  if (grads) {
-    if (e->kind == 1) tn_backward(e);
-    else if (e->kind == 2) mace_backward(e);
-    else backward(e);
-  }
+  if (grads) e->model->backward(e);
   if (e->world > 1 && e->leader == nullptr && !e->debug_no_halo) {
-    NCCL_CK(g_nccl.AllReduce(e->scal.p, e->scal.p, 10, ncclFloat64, ncclSum, e->comm, e->st));
+    NCCL_CK(g_nccl.AllReduce(e->buf.scal.p, e->buf.scal.p, 10, ncclFloat64, ncclSum, e->comm, e->st));
     if (grads)
-      NCCL_CK(g_nccl.AllReduce(e->forces.p, e->forces.p, (size_t)e->g.N * 3, ncclFloat32, ncclSum, e->comm, e->st));
+      NCCL_CK(g_nccl.AllReduce(e->buf.forces.p, e->buf.forces.p, (size_t)e->g.N * 3, ncclFloat32, ncclSum, e->comm, e->st));
     if (e->atomic) {
-      NCCL_CK(g_nccl.AllReduce(e->atom_e.p, e->atom_e.p, N, ncclFloat64, ncclSum, e->comm, e->st));
+      NCCL_CK(g_nccl.AllReduce(e->buf.atom_e.p, e->buf.atom_e.p, N, ncclFloat64, ncclSum, e->comm, e->st));
       if (grads)
-        NCCL_CK(g_nccl.AllReduce(e->atom_vir.p, e->atom_vir.p, N * kVirPitch, ncclFloat32, ncclSum, e->comm, e->st));
+        NCCL_CK(g_nccl.AllReduce(e->buf.atom_vir.p, e->buf.atom_vir.p, N * kVirPitch, ncclFloat32, ncclSum, e->comm, e->st));
     }
   }
   B2M_CK(cudaEventRecord(e->ev[2], e->st));
@@ -1063,14 +711,12 @@ static void ensure_pinned(void*& p, size_t& cap, size_t bytes) {
   cap = bytes + bytes / 8;
 }
 
-__global__ void k_add_inplace(int64_t n, const float* __restrict__ src, float* __restrict__ dst) {
+template <class T>
+__global__ void k_add_inplace(int64_t n, const T* __restrict__ src, T* __restrict__ dst) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i < n) dst[i] += src[i];
 }
-__global__ void k_add_inplace_f64(int64_t n, const double* __restrict__ src, double* __restrict__ dst) {
-  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i < n) dst[i] += src[i];
-}
+
 
 // Runs fn(partition) for every partition of a group, one host thread each (each sets its own device); the first
 // exception wins and releases the others from the rendezvous.
@@ -1119,34 +765,40 @@ static void run_any(b2m_engine* e, bool grads) {
   e->launches_last = launches;
 }
 
+// `arr` [n] summed over the partitions of the group led by L, on L's device: into `sum`, each peer's array staged in `tmp`
+template <class T>
+static const T* part_sum(b2m_engine* L, DBuf<T> Bufs::*arr, DBuf<T>& sum, DBuf<T>& tmp, size_t n) {
+  sum.ensure(n + 64);
+  tmp.ensure(n + 64);
+  B2M_CK(cudaMemcpyAsync(sum.p, (L->buf.*arr).p, n * sizeof(T), cudaMemcpyDeviceToDevice, L->st));
+  for (size_t p = 1; p < L->parts.size(); p++) {
+    B2M_CK(cudaMemcpyAsync(tmp.p, (L->parts[p]->buf.*arr).p, n * sizeof(T), cudaMemcpyDefault, L->st));
+    k_add_inplace<<<cdiv((int64_t)n, 256), 256, 0, L->st>>>((int64_t)n, tmp.p, sum.p);
+    B2M_CK(cudaGetLastError());
+  }
+  return sum.p;
+}
+
 // forces [N][3] of the whole structure on the leader's device: a group sums its partitions' arrays, a multi-process run
 // has all-reduced them in run()
 static const float* summed_forces(b2m_engine* e) {
-  if (e->parts.empty()) return e->forces.p;
-  const size_t n = (size_t)e->g.N * 3;
-  e->ftmp.ensure(n + 64);
-  e->fsum.ensure(n + 64);
-  B2M_CK(cudaMemcpyAsync(e->fsum.p, e->forces.p, n * sizeof(float), cudaMemcpyDeviceToDevice, e->st));
-  for (size_t p = 1; p < e->parts.size(); p++) {
-    B2M_CK(cudaMemcpyAsync(e->ftmp.p, e->parts[p]->forces.p, n * sizeof(float), cudaMemcpyDefault, e->st));
-    k_add_inplace<<<cdiv((int64_t)n, 256), 256, 0, e->st>>>((int64_t)n, e->ftmp.p, e->fsum.p);
-    B2M_CK(cudaGetLastError());
-  }
-  return e->fsum.p;
+  if (e->parts.empty()) return e->buf.forces.p;
+  return part_sum(e, &Bufs::forces, e->buf.fsum, e->buf.ftmp, (size_t)e->g.N * 3);
 }
+
 
 // unfolded graph: rows [N][pitch] of every unfolded atom summed onto their cell atoms -> [n][pitch] (hf_fold)
 static const float* fold_rows(b2m_engine* e, const float* src, int width, int pitch) {
   const int64_t N = e->g.N, n = e->hf_n;
-  e->hf_fold.ensure((size_t)n * pitch + 64);
-  e->hf_fold.zero((size_t)n * pitch, e->st);
-  LAUNCH_HF(k_hf_fold, N * width, e->st, N, e->uf.image_of.p, width, pitch, src, e->hf_fold.p);
-  return e->hf_fold.p;
+  e->buf.hf_fold.ensure((size_t)n * pitch + 64);
+  e->buf.hf_fold.zero((size_t)n * pitch, e->st);
+  LAUNCH_HF(k_hf_fold, N * width, e->st, N, e->uf.image_of.p, width, pitch, src, e->buf.hf_fold.p);
+  return e->buf.hf_fold.p;
 }
 
 static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) {
   double hs[10];
-  B2M_CK(cudaMemcpyAsync(hs, e->scal.p, 10 * sizeof(double), cudaMemcpyDeviceToHost, e->st));
+  B2M_CK(cudaMemcpyAsync(hs, e->buf.scal.p, 10 * sizeof(double), cudaMemcpyDeviceToHost, e->st));
   const float* fsrc = forces ? summed_forces(e) : nullptr;
   if (forces && e->hf_n) fsrc = fold_rows(e, fsrc, 3, 3);  // periodic forces F_i = sum of F~ over i and its images
   const size_t fbytes = (size_t)cell_atoms(e) * 3 * sizeof(float);
@@ -1160,7 +812,7 @@ static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) 
     double ps[10];
     b2m_engine* pe = e->parts[p];
     B2M_CK(cudaSetDevice(pe->device));
-    B2M_CK(cudaMemcpy(ps, pe->scal.p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
+    B2M_CK(cudaMemcpy(ps, pe->buf.scal.p, 10 * sizeof(double), cudaMemcpyDeviceToHost));
     for (int k = 0; k < 10; k++) hs[k] += ps[k];
   }
   if (!e->parts.empty()) B2M_CK(cudaSetDevice(e->device));
@@ -1175,23 +827,11 @@ static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) 
 // multi-process run has all-reduced them in run()
 static void fetch_atomic(b2m_engine* e, double* energies, float* virials) {
   const size_t N = (size_t)cell_atoms(e), NG = (size_t)e->g.N;  // unfolded graph: cell atoms out, all atoms summed
-  const double* esrc = e->atom_e.p;
-  const float* vsrc = e->atom_vir.p;
+  const double* esrc = e->buf.atom_e.p;
+  const float* vsrc = e->buf.atom_vir.p;
   if (!e->parts.empty()) {
-    auto sum = [&](auto& total, auto& tmp, auto member_buf, size_t n, auto add) {
-      total.ensure(n + 64);
-      tmp.ensure(n + 64);
-      B2M_CK(cudaMemcpyAsync(total.p, member_buf(e).p, n * sizeof(*total.p), cudaMemcpyDeviceToDevice, e->st));
-      for (size_t p = 1; p < e->parts.size(); p++) {
-        B2M_CK(cudaMemcpyAsync(tmp.p, member_buf(e->parts[p]).p, n * sizeof(*total.p), cudaMemcpyDefault, e->st));
-        add<<<cdiv((int64_t)n, 256), 256, 0, e->st>>>((int64_t)n, tmp.p, total.p);
-        B2M_CK(cudaGetLastError());
-      }
-      return total.p;
-    };
-    if (energies) esrc = sum(e->aesum, e->aetmp, [](b2m_engine* m) -> DBuf<double>& { return m->atom_e; }, NG, k_add_inplace_f64);
-    if (virials)
-      vsrc = sum(e->avsum, e->avtmp, [](b2m_engine* m) -> DBuf<float>& { return m->atom_vir; }, NG * kVirPitch, k_add_inplace);
+    if (energies) esrc = part_sum(e, &Bufs::atom_e, e->buf.aesum, e->buf.aetmp, NG);
+    if (virials) vsrc = part_sum(e, &Bufs::atom_vir, e->buf.avsum, e->buf.avtmp, NG * kVirPitch);
   }
   // images carry no energy (weight 0); their virial halves belong to the cell atoms they are images of
   if (virials && e->hf_n) vsrc = fold_rows(e, vsrc, 9, kVirPitch);
@@ -1221,11 +861,11 @@ static void heat_flux(b2m_engine* h, const double* vel, double* flux6) {
     for (size_t k = 0; k < members.size(); k++) members[k]->hf_seed = -1, members[k]->atomic = atomic_flag[k];
   };
   try {
-    h->hf_G.ensure((size_t)N * 9 + 64);
+    h->buf.hf_G.ensure((size_t)N * 9 + 64);
     for (int a = 0; a < 3; a++) {
       for (auto* e : members) e->hf_seed = a;
       run_any(h, true);
-      B2M_CK(cudaMemcpyAsync(h->hf_G.p + (size_t)a * N * 3, summed_forces(h), (size_t)N * 3 * sizeof(float),
+      B2M_CK(cudaMemcpyAsync(h->buf.hf_G.p + (size_t)a * N * 3, summed_forces(h), (size_t)N * 3 * sizeof(float),
                              cudaMemcpyDeviceToDevice, h->st));
     }
     // the masked pass also writes the per-atom energies (J_conv) whatever the handle's b2m_set_atomic flag
@@ -1237,28 +877,17 @@ static void heat_flux(b2m_engine* h, const double* vel, double* flux6) {
   }
   restore();
   const float* F = summed_forces(h);
-  const double* eps = h->atom_e.p;
-  if (!h->parts.empty()) {
-    h->aesum.ensure(N + 64);
-    h->aetmp.ensure(N + 64);
-    B2M_CK(cudaMemcpyAsync(h->aesum.p, h->atom_e.p, N * sizeof(double), cudaMemcpyDeviceToDevice, h->st));
-    for (size_t p = 1; p < h->parts.size(); p++) {
-      B2M_CK(cudaMemcpyAsync(h->aetmp.p, h->parts[p]->atom_e.p, N * sizeof(double), cudaMemcpyDefault, h->st));
-      k_add_inplace_f64<<<cdiv(N, 256), 256, 0, h->st>>>(N, h->aetmp.p, h->aesum.p);
-      B2M_CK(cudaGetLastError());
-    }
-    eps = h->aesum.p;
-  }
-  h->hf_vel.ensure((size_t)n * 3 + 64);
-  h->hf_out.ensure(64);
-  B2M_CK(cudaMemcpyAsync(h->hf_vel.p, vel, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->st));
-  h->hf_out.zero(6, h->st);
+  const double* eps = h->parts.empty() ? h->buf.atom_e.p : part_sum(h, &Bufs::atom_e, h->buf.aesum, h->buf.aetmp, N);
+  h->buf.hf_vel.ensure((size_t)n * 3 + 64);
+  h->buf.hf_out.ensure(64);
+  B2M_CK(cudaMemcpyAsync(h->buf.hf_vel.p, vel, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->st));
+  h->buf.hf_out.zero(6, h->st);
   const int grid = std::max(1, std::min(cdiv(N, 256), 4 * h->num_sms));
   k_hf_contract<<<grid, 256, 0, h->st>>>(N, n, h->g.cart.p, h->hf_c[0], h->hf_c[1], h->hf_c[2], h->uf.image_of.p,
-                                         h->hf_vel.p, F, h->hf_G.p, eps, h->hf_out.p);
+                                         h->buf.hf_vel.p, F, h->buf.hf_G.p, eps, h->buf.hf_out.p);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
-  B2M_CK(cudaMemcpyAsync(flux6, h->hf_out.p, 6 * sizeof(double), cudaMemcpyDeviceToHost, h->st));
+  B2M_CK(cudaMemcpyAsync(flux6, h->buf.hf_out.p, 6 * sizeof(double), cudaMemcpyDeviceToHost, h->st));
   B2M_CK(cudaStreamSynchronize(h->st));
 }
 
@@ -1330,41 +959,16 @@ static b2m_engine* create_one(const b2m_model_desc* desc, int device, int count)
   return e;
 }
 
-static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdesc, const int* devices, int ndev,
-                      b2m_handle* out, const b2m_mace_desc* mdesc = nullptr) {
+// make() builds the model of one partition and checks its description; it runs for every partition before any device
+// is touched
+static int create_any(const b2m_model_desc* desc, const int* devices, int ndev, b2m_handle* out,
+                      const std::function<std::unique_ptr<Model>()>& make) {
   if (!desc || !devices || !out) return B2M_ERR_INVALID;
   std::vector<b2m_engine*> made;
   try {
     B2M_REQUIRE(ndev >= 1 && ndev <= MAXP, B2M_ERR_PARTITIONS, "ndev must be in [1,16]");
-    if (mdesc) {
-      B2M_REQUIRE(mdesc->channels >= 32 && mdesc->channels <= 128 && mdesc->channels % 32 == 0, B2M_ERR_INVALID,
-                  "MACE engine supports hidden_irreps = C x 0e (+ C x 1o) with C a multiple of 32, C <= 128");
-      B2M_REQUIRE(mdesc->hidden_max_l == 0 || mdesc->hidden_max_l == 1, B2M_ERR_INVALID,
-                  "MACE engine supports hidden_max_l 0 (C x 0e) or 1 (C x 0e + C x 1o)");
-      B2M_REQUIRE(mdesc->hidden_max_l == 0 || mdesc->max_ell >= 1, B2M_ERR_INVALID,
-                  "0e+1o hidden features need max_ell >= 1");
-      B2M_REQUIRE(mdesc->max_ell >= 0 && mdesc->max_ell <= 3, B2M_ERR_INVALID, "MACE engine supports max_ell <= 3");
-      B2M_REQUIRE(mdesc->correlation >= 1 && mdesc->correlation <= 3, B2M_ERR_INVALID, "MACE engine supports correlation <= 3");
-      B2M_REQUIRE(mdesc->num_interactions >= 1 && mdesc->num_interactions <= kMaceMaxLayers, B2M_ERR_INVALID,
-                  "num_interactions must be in [1,8]");
-      B2M_REQUIRE(mdesc->num_bessel >= 1 && mdesc->num_bessel <= 64, B2M_ERR_INVALID, "num_bessel must be in [1,64]");
-      B2M_REQUIRE(mdesc->mlp_hidden >= 1 && mdesc->mlp_hidden <= 256, B2M_ERR_INVALID, "readout MLP width must be in [1,256]");
-      B2M_REQUIRE(mdesc->num_polynomial_cutoff >= 1 && mdesc->r_max > 0 && mdesc->c_act > 0, B2M_ERR_INVALID,
-                  "r_max, the cutoff exponent and c_act must be positive");
-      for (int t = 0; t < mdesc->num_interactions; t++)
-        B2M_REQUIRE(mdesc->avg_num_neighbors[t] > 0, B2M_ERR_INVALID, "avg_num_neighbors must be positive");
-    } else if (tdesc) {
-      B2M_REQUIRE(tdesc->units == D, B2M_ERR_INVALID, "TensorNet engine supports units = 64");
-      B2M_REQUIRE(tdesc->num_rbf >= 1 && tdesc->num_rbf <= 64, B2M_ERR_INVALID, "num_rbf must be in [1,64]");
-      B2M_REQUIRE(tdesc->n_blocks >= 1 && tdesc->n_blocks <= 16, B2M_ERR_INVALID, "nblocks must be in [1,16]");
-      B2M_REQUIRE(tdesc->cutoff > 0 && tdesc->rbf_width > 0, B2M_ERR_INVALID, "cutoff and rbf width must be positive");
-    } else {
-      B2M_REQUIRE(desc->dim == D && desc->max_n == NR && desc->max_f == 4, B2M_ERR_INVALID,
-                  "engine supports dim=64, max_n=9, max_f=4");
-      B2M_REQUIRE(desc->n_blocks >= 2 && desc->n_blocks <= 16, B2M_ERR_INVALID, "n_blocks must be in [2,16]");
-      B2M_REQUIRE(desc->cutoff > 0 && desc->three_body_cutoff > 0 && desc->three_body_cutoff <= desc->cutoff,
-                  B2M_ERR_INVALID, "bond_r cannot be greater than regular cutoff");
-    }
+    std::vector<std::unique_ptr<Model>> models;
+    for (int p = 0; p < ndev; p++) models.push_back(make());
     int count = 0;
     cudaError_t ce = cudaGetDeviceCount(&count);
     if (ce != cudaSuccess || count <= 0)
@@ -1372,31 +976,7 @@ static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdes
                                     cudaGetErrorString(ce));
     for (int p = 0; p < ndev; p++) {
       made.push_back(create_one(desc, devices[p], count));
-      if (mdesc) {
-        b2m_engine* m = made.back();
-        m->kind = 2;
-        m->mace = new MaceState();
-        MaceState& M = *m->mace;
-        M.Cr = mdesc->channels, M.C = (mdesc->channels + 63) / 64 * 64;
-        M.L1 = mdesc->max_ell + 1, M.nsh = M.L1 * M.L1, M.T = mdesc->num_interactions;
-        M.correlation = mdesc->correlation, M.H = mdesc->mlp_hidden, M.c_act = mdesc->c_act;
-        M.hidden_max_l = mdesc->hidden_max_l;
-        M.hw.assign(M.T + 1, M.C);  // h[t] of 0 < t < T carries 0e+1o when hidden_max_l = 1
-        for (int t = 1; t < M.T; t++) M.hw[t] = M.hidden_max_l ? 4 * M.C : M.C;
-        M.rp.nb = mdesc->num_bessel, M.rp.nbp = 64, M.rp.p = mdesc->num_polynomial_cutoff;
-        M.rp.r_max = (float)mdesc->r_max, M.rp.pref = (float)std::sqrt(2.0 / mdesc->r_max);
-        for (int t = 0; t < M.T; t++)
-          M.interaction_residual[t] = (mdesc->residual_mask >> t) & 1, M.avg_nb[t] = mdesc->avg_num_neighbors[t];
-      } else if (tdesc) {
-        b2m_engine* m = made.back();
-        m->kind = 1;
-        m->tn = new TnState();
-        m->tn->units = tdesc->units, m->tn->num_rbf = tdesc->num_rbf, m->tn->nblocks = tdesc->n_blocks;
-        m->tn->so3 = tdesc->so3 ? 1 : 0;
-        m->tn->rp.nr = tdesc->num_rbf, m->tn->rp.nrp = 64;
-        m->tn->rp.width = (float)tdesc->rbf_width, m->tn->rp.rc = (float)tdesc->cutoff;
-        for (float& v : m->tn->rp.mu) v = 0.f;
-      }
+      made.back()->model = std::move(models[p]);
     }
     b2m_engine* e = made[0];
     if (ndev > 1) {
@@ -1422,11 +1002,7 @@ static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdes
     }
     *out = e;
   } catch (const b2m::Error& ex) {
-    for (auto* m : made) {
-      delete m->tn;
-      delete m->mace;
-      delete m;
-    }
+    for (auto* m : made) delete m;
     g_create_err = ex.what();
     return ex.code;
   }
@@ -1434,7 +1010,7 @@ static int create_any(const b2m_model_desc* desc, const b2m_tensornet_desc* tdes
 }
 
 int b2m_create(const b2m_model_desc* desc, const int* devices, int ndev, b2m_handle* out) {
-  return create_any(desc, nullptr, devices, ndev, out);
+  return create_any(desc, devices, ndev, out, [&] { return make_chgnet(*desc); });
 }
 
 int b2m_create_tensornet(const b2m_tensornet_desc* tdesc, const int* devices, int ndev, b2m_handle* out) {
@@ -1445,7 +1021,7 @@ int b2m_create_tensornet(const b2m_tensornet_desc* tdesc, const int* devices, in
   memset(&d, 0, sizeof d);
   d.n_elem = tdesc->n_elem, d.dim = D, d.max_n = NR, d.max_f = 4, d.n_blocks = tdesc->n_blocks, d.cutoff_exponent = 0;
   d.cutoff = tdesc->cutoff, d.three_body_cutoff = 0.0, d.data_mean = tdesc->data_mean, d.data_std = tdesc->data_std;
-  return create_any(&d, tdesc, devices, ndev, out);
+  return create_any(&d, devices, ndev, out, [&] { return make_tensornet(*tdesc); });
 }
 
 int b2m_create_mace(const b2m_mace_desc* mdesc, const int* devices, int ndev, b2m_handle* out) {
@@ -1456,13 +1032,11 @@ int b2m_create_mace(const b2m_mace_desc* mdesc, const int* devices, int ndev, b2
   memset(&d, 0, sizeof d);
   d.n_elem = mdesc->n_elem, d.dim = D, d.max_n = NR, d.max_f = 4, d.n_blocks = mdesc->num_interactions;
   d.cutoff = mdesc->r_max, d.three_body_cutoff = 0.0, d.data_mean = 0.0, d.data_std = 1.0;
-  return create_any(&d, nullptr, devices, ndev, out, mdesc);
+  return create_any(&d, devices, ndev, out, [&] { return make_mace(*mdesc); });
 }
 
 static void destroy_one(b2m_engine* h) {
   cudaSetDevice(h->device);
-  delete h->tn;  // frees its device buffers
-  delete h->mace;
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
   for (auto& p : h->gather_ev) {
     cudaEventDestroy(p.first);
@@ -1507,7 +1081,7 @@ int b2m_load_weights(b2m_handle h, const char* name, const float* host_ptr, cons
 
 int b2m_set_element_refs(b2m_handle h, const double* offsets, int n) {
   API_BEGIN
-  B2M_REQUIRE(h->kind != 2, B2M_ERR_INVALID, "a MACE model carries its own atomic energies (atomic_energies_fn)");
+  B2M_REQUIRE(!h->model->own_scaling, B2M_ERR_INVALID, "a MACE model carries its own atomic energies (atomic_energies_fn)");
   B2M_REQUIRE(offsets == nullptr || n == 0 || n == h->desc.n_elem, B2M_ERR_INVALID, "element_refs length must equal n_elem");
   each_member(h, [&](b2m_engine* e) {
     if (offsets == nullptr || n == 0) {  // clear: a later Potential without element_refs must not inherit the old offsets
@@ -1523,7 +1097,7 @@ int b2m_set_element_refs(b2m_handle h, const double* offsets, int n) {
 
 int b2m_set_scaling(b2m_handle h, double data_mean, double data_std) {
   API_BEGIN
-  B2M_REQUIRE(h->kind != 2, B2M_ERR_INVALID, "a MACE model carries its own scale and shift (scale_shift)");
+  B2M_REQUIRE(!h->model->own_scaling, B2M_ERR_INVALID, "a MACE model carries its own scale and shift (scale_shift)");
   each_member(h, [&](b2m_engine* e) {
     e->desc.data_mean = data_mean;
     e->desc.data_std = data_std;
@@ -1533,11 +1107,7 @@ int b2m_set_scaling(b2m_handle h, double data_mean, double data_std) {
 
 int b2m_finalize_weights(b2m_handle h) {
   API_BEGIN
-  each_member(h, [&](b2m_engine* e) {
-    if (e->kind == 1) tn_finalize_weights(e);
-    else if (e->kind == 2) mace_finalize_weights(e);
-    else finalize_weights(e);
-  });
+  each_member(h, finalize_weights);
   API_END
 }
 
@@ -1606,16 +1176,14 @@ static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart,
     h->g.build(h->st, h->uf.N, h->uf.cart.p, lattice9, h->uf.species.p, no_pbc, h->desc.cutoff,
                h->desc.three_body_cutoff, tol, h->rank, h->world);
     h->hf_n = natoms;
-    h->hf_w.ensure((size_t)h->uf.N + 64);
+    h->buf.hf_w.ensure((size_t)h->uf.N + 64);
     for (int m = 0; m < 3; m++) h->hf_c[m] = 0.5 * (lattice9[m] + lattice9[3 + m] + lattice9[6 + m]);
   } else {
     h->g.walls_from_min = false;
     h->g.build(h->st, natoms, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff, tol, h->rank,
                h->world);
   }
-  if (h->kind == 1) tn_alloc_workspace(h);
-  else if (h->kind == 2) mace_alloc_workspace(h);
-  else alloc_workspace(h);
+  alloc_workspace(h);
   B2M_CK(cudaEventRecord(h->ev[4], h->st));
   B2M_CK(cudaStreamSynchronize(h->st));
   float ms;
@@ -1699,13 +1267,13 @@ int b2m_get_atomic(b2m_handle h, double* energies, float* virials) {
 int b2m_get_sitewise(b2m_handle h, float* out) {
   API_BEGIN
   B2M_REQUIRE(h->have_graph && out, B2M_ERR_STATE, "no structure");
-  B2M_REQUIRE(h->kind == 0, B2M_ERR_INVALID, "the site-wise readout belongs to CHGNet (TensorNet and MACE have none)");
+  B2M_REQUIRE(h->model->sitewise, B2M_ERR_INVALID, "the site-wise readout belongs to CHGNet (TensorNet and MACE have none)");
   std::vector<float> full(h->g.N, 0.f);
   auto collect = [&](b2m_engine* e) {  // owned rows of one partition -> global order
     Graph& g = e->g;
     std::vector<float> loc(g.n_own);
     std::vector<int> gid(g.n_own);
-    B2M_CK(cudaMemcpyAsync(loc.data(), e->site.p, g.n_own * sizeof(float), cudaMemcpyDeviceToHost, e->st));
+    B2M_CK(cudaMemcpyAsync(loc.data(), e->buf.site.p, g.n_own * sizeof(float), cudaMemcpyDeviceToHost, e->st));
     B2M_CK(cudaMemcpyAsync(gid.data(), g.gid.p, g.n_own * sizeof(int), cudaMemcpyDeviceToHost, e->st));
     B2M_CK(cudaStreamSynchronize(e->st));
     for (int i = 0; i < g.n_own; i++) full[gid[i]] = loc[i];
@@ -1713,9 +1281,9 @@ int b2m_get_sitewise(b2m_handle h, float* out) {
   each_member(h, collect);
   Graph& g = h->g;
   if (h->world > 1 && h->parts.empty()) {
-    B2M_CK(cudaMemcpyAsync(h->site_full.p, full.data(), g.N * sizeof(float), cudaMemcpyHostToDevice, h->st));
-    NCCL_CK(g_nccl.AllReduce(h->site_full.p, h->site_full.p, (size_t)g.N, ncclFloat32, ncclSum, h->comm, h->st));
-    B2M_CK(cudaMemcpyAsync(full.data(), h->site_full.p, g.N * sizeof(float), cudaMemcpyDeviceToHost, h->st));
+    B2M_CK(cudaMemcpyAsync(h->buf.site_full.p, full.data(), g.N * sizeof(float), cudaMemcpyHostToDevice, h->st));
+    NCCL_CK(g_nccl.AllReduce(h->buf.site_full.p, h->buf.site_full.p, (size_t)g.N, ncclFloat32, ncclSum, h->comm, h->st));
+    B2M_CK(cudaMemcpyAsync(full.data(), h->buf.site_full.p, g.N * sizeof(float), cudaMemcpyDeviceToHost, h->st));
     B2M_CK(cudaStreamSynchronize(h->st));
   }
   memcpy(out, full.data(), cell_atoms(h) * sizeof(float));  // unfolded graph: the cell atoms come first
@@ -1758,46 +1326,10 @@ int64_t b2m_get_partition_info(b2m_handle h, int which, int64_t* out, int64_t ca
 int b2m_debug_tensor(b2m_handle h, const char* name, float* out, int64_t cap, int64_t* rows, int64_t* cols) {
   API_BEGIN
   B2M_REQUIRE(h->have_graph && name && out && rows && cols, B2M_ERR_STATE, "no structure");
-  Graph& g = h->g;
   std::string n(name);
   const float* src = nullptr;
   int64_t r = 0, c = D;
-  auto idx = [&](const std::string& pre) { return atoi(n.c_str() + pre.size()); };
-  if (h->kind == 1) {
-    B2M_REQUIRE(tn_debug_lookup(h, n, src, r, c), B2M_ERR_INVALID, "unknown debug tensor: " + n);
-  } else if (h->kind == 2) {
-    B2M_REQUIRE(mace_debug_lookup(h, n, src, r, c), B2M_ERR_INVALID, "unknown debug tensor: " + n);
-  } else if (n[0] == 'x' && isdigit(n[1])) {
-    int l = idx("x");
-    B2M_REQUIRE(l >= 0 && l < (int)h->x.size(), B2M_ERR_INVALID, "bad layer");
-    src = h->x[l].p, r = l == (int)h->x.size() - 1 ? g.n_own : g.n_loc;
-  } else if (n[0] == 'h' && isdigit(n[1])) {
-    int l = idx("h");
-    B2M_REQUIRE(l >= 0 && l < (int)h->h.size(), B2M_ERR_INVALID, "bad layer");
-    src = h->h[l].p, r = g.B_own;
-  } else if (n.rfind("ang", 0) == 0 && isdigit(n[3])) {
-    int l = idx("ang");
-    B2M_REQUIRE(l >= 0 && l < (int)h->ang.size(), B2M_ERR_INVALID, "bad layer");
-    src = h->ang[l].p, r = g.A;
-  } else if (n == "e_atom") {
-    src = h->e_atom.p, r = g.n_own, c = 1;
-  } else if (n == "gd") {
-    src = h->gd.p, r = g.E, c = 1;
-  } else if (n == "gdb") {
-    src = h->gdb.p, r = g.B_loc, c = 1;
-  } else if (n == "gbvec") {
-    src = h->gbvec.p, r = g.B_loc, c = 3;
-  } else if (n == "gx") {
-    src = h->gx.p, r = g.n_loc;
-  } else if (n == "gh") {
-    src = h->gh.p, r = g.B_loc;
-  } else if (n == "gang") {
-    src = h->gang.p, r = g.A;
-  } else if (n == "e_vec") {
-    src = reinterpret_cast<const float*>(g.e_vec.p), r = g.E, c = 4;
-  } else {
-    throw Error(B2M_ERR_INVALID, "unknown debug tensor: " + n);
-  }
+  B2M_REQUIRE(h->model->debug(h, n, src, r, c), B2M_ERR_INVALID, "unknown debug tensor: " + n);
   B2M_REQUIRE(r * c <= cap, B2M_ERR_INVALID, "debug buffer too small");
   B2M_CK(cudaMemcpyAsync(out, src, r * c * sizeof(float), cudaMemcpyDeviceToHost, h->st));
   B2M_CK(cudaStreamSynchronize(h->st));
@@ -1810,25 +1342,12 @@ int b2m_release_workspace(b2m_handle h) {
   each_member(h, [&](b2m_engine* e) {
     B2M_CK(cudaStreamSynchronize(e->st));
     e->have_graph = false;
-    auto drop = [](auto& b) {
-      if (b.p) cudaFree(b.p);
-      b.p = nullptr, b.cap = 0;
-    };
-    for (auto* v : {&e->x, &e->h, &e->ang, &e->upd, &e->ApL, &e->CpL, &e->QpL})
-      for (auto& b : *v) drop(b);
-    for (auto* b : {&e->Ha, &e->Hb, &e->Xc, &e->agg, &e->aggB, &e->y1p, &e->y1, &e->y2p, &e->y2,
-                    &e->e_atom, &e->site, &e->gx, &e->gh, &e->gang, &e->gA, &e->gC, &e->gQ, &e->gHa, &e->gHb, &e->gXc,
-                    &e->gagg, &e->gupd, &e->gaggB, &e->gd, &e->gdb, &e->gbvec, &e->gy1, &e->gy2, &e->forces,
-                    &e->sendbuf, &e->recvbuf, &e->site_full, &e->precv[0], &e->precv[1], &e->ftmp, &e->fsum,
-                    &e->atom_vir, &e->avsum, &e->avtmp, &e->hf_w, &e->hf_G, &e->hf_fold})
-      drop(*b);
-    for (auto* b : {&e->atom_e, &e->aesum, &e->aetmp, &e->hf_vel, &e->hf_out}) drop(*b);
     e->atomic_last = 0;
     e->hf_n = 0;
+    e->buf = Bufs();
+    e->model->release();
     e->uf.~Unfold();
     new (&e->uf) Unfold();
-    tn_release(e);
-    mace_release(e);
     e->g.~Graph();  // the resident graph goes too
     new (&e->g) Graph();
   });
@@ -1843,3 +1362,4 @@ int b2m_last_timings(b2m_handle h, double* out, int n) {
 }
 
 }  // extern "C"
+

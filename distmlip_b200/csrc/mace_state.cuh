@@ -121,7 +121,16 @@ struct MaceLayerW {
   const float* wread = nullptr;                             // linear readout [C] / sqrt(C) (all layers but the last)
 };
 
-struct MaceState {
+// workspace of the resident structure (b2m_release_workspace replaces it with an empty one)
+struct MaceWork {
+  DBuf<float> Y, eb, R, e_lin, pre_out, B, Am, sc;
+  std::vector<DBuf<float>> h, u, A, pre;  // h: T + 1, u / A: T, pre: radial MLP hidden layers
+  DBuf<float> act[2];
+  // reverse
+  DBuf<float> gY, g_eb, gR, gB, gA, gAm, gh, ghn, gu, gact[2];
+};
+
+struct MaceState : MaceWork {
   // C: row pitch of every per-atom array, the model's channel count Cr rounded up to a multiple of 64 (the wgmma GEMM
   // shapes); the padding channels carry zero weights and stay zero
   int C = 128, Cr = 128, L1 = 4, nsh = 16, T = 2, correlation = 3, H = 16;
@@ -139,12 +148,6 @@ struct MaceState {
   const float *W1 = nullptr, *w2 = nullptr;  // non-linear readout: [C][H] / sqrt(C), [H] c_act / sqrt(H)
   const double* E0 = nullptr;
   DBuf<double> e0buf;
-  // workspace
-  DBuf<float> Y, eb, R, e_lin, pre_out, B, Am, sc;
-  std::vector<DBuf<float>> h, u, A, pre;  // h: T + 1, u / A: T, pre: radial MLP hidden layers
-  DBuf<float> act[2];
-  // reverse
-  DBuf<float> gY, g_eb, gR, gB, gA, gAm, gh, ghn, gu, gact[2];
 };
 
 }  // namespace b2m

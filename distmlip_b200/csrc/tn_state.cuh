@@ -18,7 +18,20 @@ struct TnChainW {  // one hidden Linear of a readout chain
   int in, out;
 };
 
-struct TnState {
+// workspace of the resident structure (b2m_release_workspace replaces it with an empty one)
+struct TnWork {
+  DBuf<float> rbf, cut, P, T0, nr0, ln0, st0, s1p, s1, s2p, T0m;
+  DBuf<float> f1, f2;  // [E][C], [E][2C]: activations of the edge MLP (forward), adjoints of its hidden layers (reverse)
+  std::vector<DBuf<float>> X;                                       // nblocks + 1 : [n_loc][10][C]
+  std::vector<DBuf<float>> f1p, f2p, f3p, q, Xh, Y, msg, Pn, dX;    // per layer
+  DBuf<float> inv, str, r, xr, lout, gout, e_atom;
+  std::vector<DBuf<float>> cpre[2], cact[2];
+  // reverse pass
+  DBuf<float> gX, gY, gmsg, gdX, gPn, gf, g_rbf, gC, gvh, gd, gT0m, gT0, gs2p, gs1p, gln0, gnr0, gr, ginv, gxr,
+      gca, gcb;
+};
+
+struct TnState : TnWork {
   int units = 64, num_rbf = 32, nblocks = 2, so3 = 0;
   TnRadial rp;
   // ---- weights (device pointers into the engine's weight buffer) ----
@@ -34,16 +47,6 @@ struct TnState {
   const float* wlast[2] = {nullptr, nullptr};
   float blast[2] = {0.f, 0.f};
   int wlast_in = 64;
-  // ---- workspace ----
-  DBuf<float> rbf, cut, P, T0, nr0, ln0, st0, s1p, s1, s2p, T0m;
-  DBuf<float> f1, f2;  // [E][C], [E][2C]: activations of the edge MLP (forward), adjoints of its hidden layers (reverse)
-  std::vector<DBuf<float>> X;                                       // nblocks + 1 : [n_loc][10][C]
-  std::vector<DBuf<float>> f1p, f2p, f3p, q, Xh, Y, msg, Pn, dX;    // per layer
-  DBuf<float> inv, str, r, xr, lout, gout, e_atom;
-  std::vector<DBuf<float>> cpre[2], cact[2];
-  // reverse pass
-  DBuf<float> gX, gY, gmsg, gdX, gPn, gf, g_rbf, gC, gvh, gd, gT0m, gT0, gs2p, gs1p, gln0, gnr0, gr, ginv, gxr,
-      gca, gcb;
 };
 
 }  // namespace b2m
