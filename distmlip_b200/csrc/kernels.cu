@@ -173,8 +173,9 @@ __device__ __forceinline__ void gemm64(const float* At, int lda, int kofs, const
 }
 
 // weights -> shared memory; the fence makes the generic-proxy stores visible to wgmma after the next barrier
+template <int NTH = NT>
 __device__ __forceinline__ void stage_w(float* Wsm, const float* __restrict__ g, int nfloat4) {
-  for (int i = threadIdx.x; i < nfloat4; i += NT) reinterpret_cast<float4*>(Wsm)[i] = reinterpret_cast<const float4*>(g)[i];
+  for (int i = threadIdx.x; i < nfloat4; i += NTH) reinterpret_cast<float4*>(Wsm)[i] = reinterpret_cast<const float4*>(g)[i];
   fence_proxy_async_smem();
 }
 
@@ -317,14 +318,16 @@ void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats) {
 // ============================================================================================
 // atom conv: shared pieces of the persistent forward and backward
 // ============================================================================================
-// Both kernels run one CTA per SM (grid = min(tiles, SMs)); CTA c takes tiles c, c + grid, c + 2 grid, ...  Every
-// tile's A[src] rows arrive by per-row bulk copies into one of two [TM][LDE] buffers, tile number `it` of the CTA in
-// buffer it & 1 (its mbarrier: stage_parity(it)).  The copies of tile it + 1 are issued while tile it is computed;
-// its index loads one tile earlier still, into registers (EdgeRow).
+// Both kernels are persistent, one CTA per SM.  In the backward (grid = min(128-edge tiles, SMs)) CTA c takes tiles c,
+// c + grid, c + 2 grid, ...; every tile's A[src] rows arrive by per-row bulk copies into one of two [TM][LDE] buffers,
+// tile number `it` of the CTA in buffer it & 1 (its mbarrier: stage_parity(it)).  The copies of tile it + 1 are issued
+// while tile it is computed; its index loads one tile earlier still, into registers (EdgeRow).  The forward splits the
+// work per warpgroup, over 64-edge tiles (below).
 //
-// Every per-element phase works in the accumulator layout (Map): warpgroup b owns first-layer columns 64 b .. 64 b + 63
-// (the hidden columns its branch's second layer reads) and the branch's 64 outputs, and a thread owns 4 rows x 16
-// columns of both.  Such a thread touches the tile only at its own positions (row(i), 64 b + col(j)), as float2 pairs
+// Every per-element phase works in the accumulator layout (Map).  In the backward warpgroup b owns first-layer columns
+// 64 b .. 64 b + 63 (the hidden columns its branch's second layer reads) and the branch's 64 outputs, and a thread owns
+// 4 rows x 16 columns of both; in the forward a thread owns 2 rows x 16 columns of each branch.  Such a thread touches
+// the tile only at its own positions (row(i), 64 b + col(j)), as float2 pairs
 // (col(2 jj), col(2 jj) + 1); the pitch LDE = 136 (8 mod 32 floats) puts the 8 rows x 4 pairs of a half-warp on 32
 // distinct banks.  The line-graph tiles use the same pitch and layout.
 constexpr int LDE = 136;
@@ -333,9 +336,10 @@ struct EdgeRow {
   int src, dst, bond;
   float d;
 };
-__device__ __forceinline__ EdgeRow edge_row(const AtomConvArgs& a, int64_t e) {
+// edge e's indices and distance, for a thread that owns a row of its tile (has_row) and e < E; else an empty row
+__device__ __forceinline__ EdgeRow edge_row(const AtomConvArgs& a, int64_t e, bool has_row) {
   EdgeRow r{-1, -1, -1, 1.f};
-  if (threadIdx.x < TM && e < a.E) {
+  if (has_row && e < a.E) {
     r.src = a.e_src[e];
     r.dst = a.e_dst[e];
     r.bond = a.e_bond[e];
@@ -343,25 +347,27 @@ __device__ __forceinline__ EdgeRow edge_row(const AtomConvArgs& a, int64_t e) {
   }
   return r;
 }
-// threads 0..TM-1 publish their row of tile t (indices, distance) and start its A[src] copy into `buf`; the caller has
-// made sure, with a barrier, that nobody reads `buf` or the index arrays of this stage any more
-__device__ __forceinline__ void issue_gather(const AtomConvArgs& a, int64_t t, const EdgeRow& row, float* buf,
+// the threads with rows lr = 0..ROWS-1 of a ROWS-row tile t publish their row (indices, distance) and start its A[src]
+// copy into `buf`; the caller has made sure, with a barrier, that nobody reads `buf` or the index arrays of this stage
+// any more
+template <int ROWS>
+__device__ __forceinline__ void issue_gather(const AtomConvArgs& a, int64_t t, const EdgeRow& row, int lr, float* buf,
                                              uint64_t* bar, int* s_src, int* s_dst, int* s_bond, float* s_d) {
-  const int tid = threadIdx.x;
-  if (tid == 0) mbar_expect_tx(bar, (uint32_t)min((int64_t)TM, a.E - t * TM) * 512u);
-  if (tid < TM) {
-    if (s_src != nullptr) s_src[tid] = row.src;
-    s_dst[tid] = row.dst;
-    s_bond[tid] = row.bond;
-    s_d[tid] = row.d;
-    if (row.src >= 0) bulk_g2s(buf + tid * LDE, a.Aproj + (size_t)row.src * D2, 512u, bar);
+  if (lr == 0) mbar_expect_tx(bar, (uint32_t)min((int64_t)ROWS, a.E - t * ROWS) * 512u);
+  if (lr < ROWS) {
+    if (s_src != nullptr) s_src[lr] = row.src;
+    s_dst[lr] = row.dst;
+    s_bond[lr] = row.bond;
+    s_d[lr] = row.d;
+    if (row.src >= 0) bulk_g2s(buf + lr * LDE, a.Aproj + (size_t)row.src * D2, 512u, bar);
   }
 }
-// be_k(d_r) (and d be_k / dd) of the tile's rows, both warpgroups (rows r, radial halves): k = 0..7 into be_s [TM][8]
-// (the A operand of the radial products), k = 8 into be8 [TM]
+// be_k(d_r) (and d be_k / dd) of a ROWS-row tile's rows by 2 ROWS threads (rows r, radial halves): k = 0..7 into be_s
+// [ROWS][8] (the A operand of the radial products), k = 8 into be8 [ROWS]
+template <int ROWS>
 __device__ __forceinline__ void radial_rows(const AtomConvArgs& a, const float* s_d, int nvalid, float* be_s, float* be8,
                                             float* dbe_s, float* dbe8) {
-  const int r = threadIdx.x & 127, half = threadIdx.x >> 7;
+  const int r = threadIdx.x % ROWS, half = (threadIdx.x / ROWS) & 1;
   const float d = s_d[r];
   const int k0 = half ? 5 : 0, k1 = half ? 9 : 5;
   for (int k = k0; k < k1; k++) {
@@ -391,10 +397,11 @@ __device__ __forceinline__ void radial_mma(const Map& m, int h, const float* x_s
 // pre of this thread's rows of 64-row half h (acc[2h], acc[2h + 1], Map layout): A[src] (in the tile) + C[dst] +
 // (Q[bond] | be.M^T), summed in that order; rows r >= nvalid are 0.  be.M^T is k = 0..7 on the tensor cores plus
 // be_8 M[.][8].  Index work is per row; the C / Q values of both rows (32 float2 loads) are in flight under the product.
+template <int R>
 __device__ __forceinline__ void first_layer_half(const AtomConvArgs& a, const Map& m, int h, const float* tile,
                                                  const int* s_dst, const int* s_bond, const float* be_s,
                                                  const float* be8, const float* rad, int nvalid,
-                                                 float (&acc)[AR][AC]) {
+                                                 float (&acc)[R][AC]) {
   const int c0 = 64 * m.branch + m.cb;
   float2 cv[2][AC / 2], qv[2][AC / 2];
   float b8[2];
@@ -437,7 +444,8 @@ __device__ __forceinline__ void first_layer_half(const AtomConvArgs& a, const Ma
 // acc rows of half h (2h, 2h + 1) = x rows of half h . B^T (wg_mma64).  x is in the accumulator layout and is the
 // register A fragment as it stands: in k block ks a thread holds columns 8 ks + 2 (l%4) and + 1.  Bcan: the branch's
 // k-permuted canonical image (hi plane of 4096 floats, then lo).  x and acc may be the same array.
-__device__ __forceinline__ void wg_mm64_acc(const float (&x)[AR][AC], int h, const float* Bcan, float (&acc)[AR][AC]) {
+template <int R>
+__device__ __forceinline__ void wg_mm64_acc(const float (&x)[R][AC], int h, const float* Bcan, float (&acc)[R][AC]) {
   float v[8][4];
 #pragma unroll
   for (int ks = 0; ks < 8; ks++) {
@@ -478,9 +486,9 @@ __device__ __forceinline__ void seg_add(float* out, int width, int col, int k, c
   if (k >= 0) sum.x += v.x, sum.y += v.y, sum.z += v.z, sum.w += v.w;
 }
 
-// Scatter phase of a [TM][LDE] tile, columns 0 .. 4 LPR - 1, in one pass: LPR lanes take a row (lane q its columns
-// 4 q .. 4 q + 3, one LDS.128; a row is contiguous, so the loads are conflict-free at any pitch) and a thread walks
-// R = TM LPR / NT consecutive rows.  Its float4 of row r
+// Scatter phase of a [ROWS][LDE] tile by NTH threads (threadIdx.x % NTH), columns 0 .. 4 LPR - 1, in one pass: LPR
+// lanes take a row (lane q its columns 4 q .. 4 q + 3, one LDS.128; a row is contiguous, so the loads are conflict-free
+// at any pitch) and a thread walks R = ROWS LPR / NTH consecutive rows.  Its float4 of row r
 //   - is added to gat[gidx[r]]                                                    (gat != nullptr, gidx[r] >= 0),
 //   - goes into one running sum per key array, reduced into out0[key0[.]] / out1[key1[.]] when the key changes and
 //     after the thread's last row                                                 (out != nullptr, key >= 0),
@@ -489,13 +497,13 @@ __device__ __forceinline__ void seg_add(float* out, int width, int col, int k, c
 // all indices < 0.  The indices are equal in the lanes that share a row, so with LPR = 32 no branch diverges.  A run of
 // equal keys that crosses the R-row boundary between two threads is reduced in two parts.  Values and indices are
 // loaded eight rows at a time before those rows are walked: the reductions (asm volatile) keep loads in program order.
-template <int LPR>
+template <int LPR, int ROWS = TM, int NTH = NT>
 __device__ __forceinline__ void scatter_rows(const float* tile, const int* key0, float* out0, const int* key1,
                                              float* out1, const int* gidx, float* gat, const int* sidx = nullptr,
                                              float* sto = nullptr) {
-  constexpr int R = TM * LPR / NT, W = 4 * LPR, B = 8;
+  constexpr int R = ROWS * LPR / NTH, W = 4 * LPR, B = 8;
   static_assert(R % B == 0 && B % 4 == 0, "batches of B rows, their indices read as int4");
-  const int q = threadIdx.x % LPR, r0 = threadIdx.x / LPR * R;
+  const int t = threadIdx.x % NTH, q = t % LPR, r0 = t / LPR * R;
   float4 s0 = make_float4(0.f, 0.f, 0.f, 0.f), s1 = s0;
   int c0 = -1, c1 = -1;
 #pragma unroll
@@ -530,120 +538,122 @@ __device__ __forceinline__ void scatter_rows(const float* tile, const int* key0,
 // ============================================================================================
 // atom conv: forward
 // ============================================================================================
+// The three warpgroups of a CTA do not wait for each other: warpgroup w of CTA c owns the 64-edge tiles g, g + 3 grid,
+// g + 6 grid, ... (g = 3 c + w) and computes both branches of each, so that some warpgroups' gathers, loads and
+// activations run while another's products are on the tensor cores.  Each warpgroup has its own [TW][LDE] gather buffer
+// (the k-th fill completes phase k of its mbarrier), its own index, distance and be slots, and its own named barrier;
+// the W2 images, the radial block and b2 are staged once per CTA behind the only CTA-wide barrier and are read-only
+// afterwards.  The next tile's gather is issued once the scatter pass is done with the buffer: one buffer per
+// warpgroup is what lets three warpgroups fit next to the W2 image, and the other warpgroups' work covers the wait.  A
+// thread holds rows m.row(0), m.row(1) of the tile and columns m.col(j) of both branches: the layers' 32 outputs L stay
+// in registers while the gates' first layer and product run, and m = L . (G . w_ab) is formed in registers and stored
+// at the thread's own positions (columns 0..63) for the scatter pass.  Three warpgroups of 128 threads leave each
+// thread at most 168 registers.
+constexpr int TW = 64;               // rows of a warpgroup's forward tile
+constexpr int WGF = 3, NTF = 128 * WGF;  // warpgroups and threads of a forward CTA
 struct AtomSmemFwd {
-  static constexpr int kTile = 32;                  // two [TM][LDE] gather buffers (first 128 B: their mbarriers)
-  static constexpr int kW = kTile + 2 * TM * LDE;   // wgmma images of W2 (2 branches x hi | lo, k permuted), staged once
-  static constexpr int kRad = kW + 16384;           // radial block (M, W_ab: AtomConvArgs::radial), staged once
-  static constexpr int kBe = kRad + ATOM_RAD;       // be [TM][8] (k < 8)
-  static constexpr int kBe8 = kBe + TM * 8;         // be [TM] (k = 8)
-  static constexpr int kB2 = kBe8 + TM;
-  static constexpr int kD = kB2 + 128;              // [2][TM] per buffer
-  static constexpr int kIdx = kD + 2 * TM;          // dst [2][TM], bond [2][TM]
-  static constexpr int kTotal = kIdx + 4 * TM;
+  static constexpr int kTile = 32;                   // [WGF][TW][LDE] gather buffers (first 128 B: their mbarriers)
+  static constexpr int kW = kTile + WGF * TW * LDE;  // wgmma images of W2 (2 branches x hi | lo, k permuted), staged once
+  static constexpr int kRad = kW + 16384;            // radial block (M, W_ab: AtomConvArgs::radial), staged once
+  static constexpr int kBe = kRad + ATOM_RAD;        // be [WGF][TW][8] (k < 8)
+  static constexpr int kBe8 = kBe + WGF * TW * 8;    // be [WGF][TW] (k = 8)
+  static constexpr int kB2 = kBe8 + WGF * TW;
+  static constexpr int kD = kB2 + 128;               // d [WGF][TW]
+  static constexpr int kIdx = kD + WGF * TW;         // dst [WGF][TW], then bond [WGF][TW]
+  static constexpr int kTotal = kIdx + 2 * WGF * TW;
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
 static_assert(AtomSmemFwd::bytes <= 232448, "atom-conv forward shared memory");
-static_assert(AtomSmemFwd::kW % 4 == 0 && AtomSmemFwd::kRad % 4 == 0 && AtomSmemFwd::kBe % 4 == 0,
-              "16-byte aligned images and radial rows");
+static_assert(AtomSmemFwd::kW % 4 == 0 && AtomSmemFwd::kRad % 4 == 0 && AtomSmemFwd::kBe % 4 == 0 &&
+                  AtomSmemFwd::kIdx % 4 == 0,
+              "16-byte aligned images, radial rows and index slots");
 
-__global__ void __launch_bounds__(NT, 1) k_atomconv_fwd(const AtomConvArgs a) {
+// barrier of warpgroup w's 128 threads alone (named barrier 1 + w; barrier 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int w) { asm volatile("bar.sync %0, 128;" ::"r"(1 + w) : "memory"); }
+
+__global__ void __launch_bounds__(NTF, 1) k_atomconv_fwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
-  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem);  // [2]
-  float* Wsm = smem + AtomSmemFwd::kW;
-  float* rad = smem + AtomSmemFwd::kRad;
-  float* be_s = smem + AtomSmemFwd::kBe;
-  float* be8 = smem + AtomSmemFwd::kBe8;
-  float* b2s = smem + AtomSmemFwd::kB2;
+  const int tid = threadIdx.x, w = tid >> 7, lr = tid & 127;  // warpgroup; thread lr < TW gathers row lr
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem) + w;      // this warpgroup's gather buffer
+  const float* Wsm = smem + AtomSmemFwd::kW;
+  const float* rad = smem + AtomSmemFwd::kRad;
+  const float* b2s = smem + AtomSmemFwd::kB2;
+  float* tile = smem + AtomSmemFwd::kTile + w * TW * LDE;
+  float* be_s = smem + AtomSmemFwd::kBe + w * TW * 8;
+  float* be8 = smem + AtomSmemFwd::kBe8 + w * TW;
+  float* s_d = smem + AtomSmemFwd::kD + w * TW;
+  int* s_dst = reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + w * TW;
+  int* s_bond = reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + (WGF + w) * TW;
 
-  const int tid = threadIdx.x;
-  const int64_t ntiles = (a.E + TM - 1) / TM, step = gridDim.x;
-  auto tile_of = [&](int s) { return smem + AtomSmemFwd::kTile + s * TM * LDE; };
-  auto d_of = [&](int s) { return smem + AtomSmemFwd::kD + s * TM; };
-  auto dst_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + s * TM; };
-  auto bond_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemFwd::kIdx) + (2 + s) * TM; };
-
+  const int64_t ntiles = (a.E + TW - 1) / TW, first = WGF * (int64_t)blockIdx.x + w, step = WGF * (int64_t)gridDim.x;
   if (tid == 0) {
-    mbar_init(&mbar[0], 1);
-    mbar_init(&mbar[1], 1);
+    for (int i = 0; i < WGF; i++) mbar_init(reinterpret_cast<uint64_t*>(smem) + i, 1);
     fence_barrier_init();
   }
-  EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
+  EdgeRow nxt = edge_row(a, first * TW + lr, lr < TW);
   // loop-invariant operands, once per CTA
-  stage_w(Wsm, a.W2can, 4096);
-  stage_w(rad, a.radial, ATOM_RAD / 4);
-  if (tid < 128) b2s[tid] = a.b2[tid];
+  stage_w<NTF>(smem + AtomSmemFwd::kW, a.W2can, 4096);
+  stage_w<NTF>(smem + AtomSmemFwd::kRad, a.radial, ATOM_RAD / 4);
+  if (tid < 128) smem[AtomSmemFwd::kB2 + tid] = a.b2[tid];
   __syncthreads();
-  issue_gather(a, blockIdx.x, nxt, tile_of(0), &mbar[0], nullptr, dst_of(0), bond_of(0), d_of(0));
-  nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid);
+  if (first < ntiles)  // the last CTA's later warpgroups have no tile when the tile count is not a multiple of WGF
+    issue_gather<TW>(a, first, nxt, lr, tile, mbar, nullptr, s_dst, s_bond, s_d);
+  nxt = edge_row(a, (first + step) * TW + lr, lr < TW);
 
   const Map m;
+  Map mL = m, mG = m;  // the first layer's columns and radial image of each branch
+  mL.branch = 0;
+  mG.branch = 1;
   int it = 0;
-  for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
-    const int s = it & 1;
-    float* tile = tile_of(s);
-    const int* s_dst = dst_of(s);
-    const int* s_bond = bond_of(s);
-    const int nvalid = (int)min((int64_t)TM, a.E - t * TM);
-    fence_proxy_async_smem();  // this thread's generic accesses of the other buffer come before its bulk refill
-    __syncthreads();           // the previous tile is done with the other buffer and be_s
-    if (t + step < ntiles) {
-      issue_gather(a, t + step, nxt, tile_of(s ^ 1), &mbar[s ^ 1], nullptr, dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
-      nxt = edge_row(a, (t + 2 * step) * TM + tid);
-    }
-    radial_rows(a, d_of(s), nvalid, be_s, be8, nullptr, nullptr);
-    mbar_wait(&mbar[s], stage_parity(it));
-    __syncthreads();
-    // pre = A[src] + C[dst] + (be.M^T | Q[bond]);  hid = silu(pre) straight into the second layer, per 64-row half
-    float acc[AR][AC];
+  for (int64_t t = first; t < ntiles; t += step, it++) {
+    const int nvalid = (int)min((int64_t)TW, a.E - t * TW);
+    wg_sync(w);  // the tile's indices and distances are published
+    radial_rows<TW>(a, s_d, nvalid, be_s, be8, nullptr, nullptr);
+    mbar_wait(mbar, (uint32_t)it & 1u);
+    wg_sync(w);
+    // per branch: pre = A[src] + C[dst] + (be.M^T | Q[bond]); silu(pre) straight into the second layer; + b2
+    float L[2][AC];
+    first_layer_half(a, mL, 0, tile, s_dst, s_bond, be_s, be8, rad, nvalid, L);
 #pragma unroll
-    for (int h = 0; h < 2; h++) {
-      first_layer_half(a, m, h, tile, s_dst, s_bond, be_s, be8, rad, nvalid, acc);
+    for (int ii = 0; ii < 2; ii++)
 #pragma unroll
-      for (int ii = 0; ii < 2; ii++)
+      for (int j = 0; j < AC; j++) L[ii][j] = silu_f(L[ii][j]);
+    wg_mm64_acc(L, 0, Wsm, L);
 #pragma unroll
-        for (int j = 0; j < AC; j++) acc[2 * h + ii][j] = silu_f(acc[2 * h + ii][j]);
-      wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
-    }
+    for (int ii = 0; ii < 2; ii++)
 #pragma unroll
-    for (int i = 0; i < AR; i++)
+      for (int j = 0; j < AC; j++) L[ii][j] = silu_f(L[ii][j] + b2s[m.col(j)]);
+    float G[2][AC];
+    first_layer_half(a, mG, 0, tile, s_dst, s_bond, be_s, be8, rad, nvalid, G);
+#pragma unroll
+    for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+      for (int j = 0; j < AC; j++) G[ii][j] = silu_f(G[ii][j]);
+    wg_mm64_acc(G, 0, Wsm + 8192, G);
+    // m = L . (G . w_ab), w_ab = be.W_ab^T on the tensor cores, over the A[src] values of columns 0..63
+    float wab[32];
+    radial_mma(m, 0, be_s, rad + ATOM_RAD_WAB, wab);
+#pragma unroll
+    for (int ii = 0; ii < 2; ii++) {
+      const int r = m.row(ii);
+      const float b8 = be8[r];
+      float mv[AC];
 #pragma unroll
       for (int j = 0; j < AC; j++) {
-        const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
-        acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
-      }
-    // m = L . G . w_ab: warpgroup 1 forms G . w_ab (w_ab = be.W_ab^T on its tensor cores) in its own tile positions,
-    // warpgroup 0 multiplies by L in its own
-    if (m.branch == 1) {
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        float w[32];
-        radial_mma(m, h, be_s, rad + ATOM_RAD_WAB, w);
-#pragma unroll
-        for (int ii = 0; ii < 2; ii++) {
-          const float b8 = be8[m.row(2 * h + ii)];
-#pragma unroll
-          for (int j = 0; j < AC; j++) acc[2 * h + ii][j] *= fmaf(b8, rad[ATOM_RAD_WAB8 + m.col(j)], w[fq(ii, j)]);
-        }
+        const float g = sigm(G[ii][j] + b2s[64 + m.col(j)]) * fmaf(b8, rad[ATOM_RAD_WAB8 + m.col(j)], wab[fq(ii, j)]);
+        mv[j] = L[ii][j] * g;
       }
 #pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++)
-          st_f2(tile + m.row(i) * LDE + 64 + m.col(2 * jj), acc[i][2 * jj], acc[i][2 * jj + 1]);
+      for (int jj = 0; jj < AC / 2; jj++) st_f2(tile + r * LDE + m.col(2 * jj), mv[2 * jj], mv[2 * jj + 1]);
     }
-    __syncthreads();
-    if (m.branch == 0) {
-#pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++) {
-          float* p = tile + m.row(i) * LDE + m.col(2 * jj);
-          const float2 g = ld_f2(p + 64);
-          st_f2(p, acc[i][2 * jj] * g.x, acc[i][2 * jj + 1] * g.y);
-        }
+    wg_sync(w);
+    scatter_rows<16, TW, 128>(tile, s_dst, a.agg, nullptr, nullptr, nullptr, nullptr);  // agg[dst] += m
+    fence_proxy_async_smem();  // this thread's generic accesses of the buffer come before its bulk refill
+    wg_sync(w);                // the warpgroup is done with the buffer, the indices and be_s
+    if (t + step < ntiles) {
+      issue_gather<TW>(a, t + step, nxt, lr, tile, mbar, nullptr, s_dst, s_bond, s_d);
+      nxt = edge_row(a, (t + 2 * step) * TW + lr, lr < TW);
     }
-    __syncthreads();
-    scatter_rows<16>(tile, s_dst, a.agg, nullptr, nullptr, nullptr, nullptr);  // agg[dst] += m
   }
 }
 
@@ -653,7 +663,7 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
   if (auto once_ = attr.first(); once_) {
     B2M_CK(cudaFuncSetAttribute(k_atomconv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AtomSmemFwd::bytes));
   }
-  k_atomconv_fwd<<<std::min(cdiv(a.E, TM), num_sms), NT, AtomSmemFwd::bytes, st>>>(a);
+  k_atomconv_fwd<<<std::min(cdiv(cdiv(a.E, TW), WGF), num_sms), NTF, AtomSmemFwd::bytes, st>>>(a);
   B2M_CK(cudaGetLastError());
   g_launch_count++;
 }
@@ -716,13 +726,13 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     mbar_init(wbar, 1);
     fence_barrier_init();
   }
-  EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid);
+  EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid, threadIdx.x < TM);
   stage_w(rad_base, a.radial, ATOM_RAD / 4);
   if (tid < 128) b2s[tid] = a.b2[tid];
   __syncthreads();
   if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
-  issue_gather(a, blockIdx.x, nxt, buf_of(0), &gbar[0], src_of(0), dst_of(0), bond_of(0), d_of(0));
-  nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid);
+  issue_gather<TM>(a, blockIdx.x, nxt, tid, buf_of(0), &gbar[0], src_of(0), dst_of(0), bond_of(0), d_of(0));
+  nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid, threadIdx.x < TM);
   uint32_t wpar = 0;
 
   const Map m;
@@ -740,7 +750,7 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     const int64_t e0 = t * TM;
     const int nvalid = (int)min((int64_t)TM, a.E - e0);
     __syncthreads();  // the previous tile's scatter phase is done with tileH (its P) and be8
-    radial_rows(a, d_of(s), nvalid, be_s, be8, dbe_s, dbe8);
+    radial_rows<TM>(a, d_of(s), nvalid, be_s, be8, dbe_s, dbe8);
     mbar_wait(&gbar[s], stage_parity(it));
     mbar_wait(wbar, wpar);  // W2
     wpar ^= 1;
@@ -876,8 +886,8 @@ __global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
     __syncthreads();           // tileH and the W2^T image are free; P holds gpre
     if (t + step < ntiles) {
       if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
-      issue_gather(a, t + step, nxt, tileH, &gbar[s ^ 1], src_of(s ^ 1), dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
-      nxt = edge_row(a, (t + 2 * step) * TM + tid);
+      issue_gather<TM>(a, t + step, nxt, tid, tileH, &gbar[s ^ 1], src_of(s ^ 1), dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
+      nxt = edge_row(a, (t + 2 * step) * TM + tid, threadIdx.x < TM);
     }
     // ---- scatter phase (reads P, be8 and this tile's index arrays only) ----
     {  // d E / d d_e: sd summed over the 4 lanes of a row, and across the warpgroups through be8
