@@ -3,6 +3,7 @@
 // contiguous span; the l-resolved atom basis A [nsh][n_own][C] (lm-major, so that the rows of one l form one contiguous
 // [(2l+1) n_own][C] block for the per-l channel mixes); edge quantities [E][...].
 #pragma once
+#include <array>
 #include <vector>
 
 #include "kernels.cuh"
@@ -51,6 +52,14 @@ __host__ __device__ constexpr int mace_slot_base(int max_ell, int l) {
 __host__ __device__ constexpr int mace_npaths(int max_ell) { return 3 * max_ell + 1; }
 __host__ __device__ constexpr int mace_nslots(int max_ell) { return mace_slot_base(max_ell, max_ell + 1); }
 constexpr int kMaceMaxSlots = mace_nslots(3);  // 40
+
+// host side of the weight packing (engine_mace.inl).  The conv_tp paths (l_in, l_sh, l_out) for node features 0e (+ 1o
+// when hidden_l = 1), in the order of tests/mace_eq_ref.py conv_paths (the radial MLP's output blocks)
+std::vector<std::array<int, 3>> mace_conv_paths(int max_ell, int hidden_l);
+// the terms of one U tensor of the symmetric contraction: U [ncomp][nsh]^nu [K] (ncomp 1: contractions.0, output slot 0;
+// 3: contractions.1, slot 1 + m), summed over the permutations of each sorted index tuple, entries <= 1e-6 max |U|
+// dropped, weight rows kg0 + k
+std::vector<MaceTerm> mace_sym_terms(const float* U, int nsh, int nu, int ncomp, int K, int kg0);
 
 // Y, eb; with the Agnesi transform on, the Bessel argument is x(d, Z_src, Z_dst) (endpoint species type[e_src / e_dst])
 void launch_mace_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const MaceRadial& rp, int nsh, float* Y,

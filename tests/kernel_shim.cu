@@ -1,14 +1,17 @@
-// kernel_shim.cu -- test-only C entry points into the shipped CHGNet hot-path launchers of libb200mlip.so.
+// kernel_shim.cu -- test-only C entry points into the shipped CHGNet hot-path launchers and the MACE launchers
+// (mace_state.cuh) of libb200mlip.so.
 //
-// tests/test_gpu_kernel_units.py builds this file into a temporary directory (tests/kernel_units_ref.py: build_shim)
+// tests/test_gpu_kernel_units.py and tests/test_gpu_mace_units.py build this file into a temporary directory (tests/kernel_units_ref.py: build_shim)
 // and calls it through ctypes.  Each entry point fills the launcher's argument struct from device pointers (torch
 // tensors), a stream handle and a num_sms value, calls the launcher, and returns 0 or the b2m::Error code with its
-// message; the weight-image entry points run the engine's own host formatters (engine.cu) on host buffers.  The shim
+// message; the weight-image entry points run the engine's own host formatters (engine.cu) on host buffers, and the MACE
+// host entry points the engine's own conv-path list and symmetric-contraction term builder (engine_mace.inl).  The shim
 // does no arithmetic of its own.
+#include <algorithm>
 #include <cstring>
 #include <exception>
 
-#include "kernels.cuh"
+#include "mace_state.cuh"
 
 namespace {
 int fail(int code, const char* what, char* msg, int msglen) {
@@ -39,6 +42,23 @@ b2m::RadialParams radial_params(const float* freq, float rc, float norm, int p) 
 }
 std::vector<float> host_vec(const float* p, size_t n) { return std::vector<float>(p, p + n); }
 void put(const std::vector<float>& v, float* out) { memcpy(out, v.data(), v.size() * sizeof(float)); }
+// MaceRadial from nb, p, r_max, the prefactor and the nb Bessel frequencies w (host); pitch 64 as the engine sets it
+b2m::MaceRadial mace_radial(int nb, int p, float r_max, float pref, const float* w) {
+  b2m::MaceRadial rp{};
+  rp.nb = nb, rp.nbp = 64, rp.p = p, rp.r_max = r_max, rp.pref = pref;
+  for (int n = 0; n < 64; n++) rp.w[n] = n < nb ? w[n] : 0.f;
+  return rp;
+}
+// MaceCore from the element table (device float4 [n_elem]) and cf = (za, zc[4], zscale, aq, ap, aa) (host)
+b2m::MaceCore mace_core(const float* elem, int zbl, int agnesi, int zp, const float* cf) {
+  b2m::MaceCore c{};
+  c.elem = reinterpret_cast<const float4*>(elem);
+  c.zbl = zbl, c.agnesi = agnesi, c.zp = zp;
+  c.za = cf[0];
+  for (int k = 0; k < 4; k++) c.zc[k] = cf[1 + k];
+  c.zscale = cf[5], c.aq = cf[6], c.ap = cf[7], c.aa = cf[8];
+  return c;
+}
 }  // namespace
 
 extern "C" {
@@ -114,5 +134,121 @@ int shim_radial_can(const float* M, const float* Wab, float* out, char* msg, int
   return guarded(msg, msglen, [&] { put(b2m::radial_can(host_vec(M, 128 * 9), host_vec(Wab, 64 * 9)), out); });
 }
 int shim_atom_rad() { return b2m::ATOM_RAD; }
+
+// ---------------------------------------------------------------------------------------------- MACE (mace_state.cuh)
+int shim_mace_edge_geom(void* st, int64_t E, const float* e_vec, int nb, int p, float r_max, float pref, const float* w,
+                        int nsh, float* Y, float* eb, const int* e_src, const int* e_dst, const int* type,
+                        const float* elem, int zbl, int agnesi, int zp, const float* cf, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_mace_edge_geom((cudaStream_t)st, E, reinterpret_cast<const float4*>(e_vec), mace_radial(nb, p, r_max, pref, w),
+                               nsh, Y, eb, e_src, e_dst, type, mace_core(elem, zbl, agnesi, zp, cf));
+  });
+}
+int shim_mace_zbl(void* st, int n_own, const int* row_ptr, const int* e_src, const float* e_vec, const int* type,
+                  const float* elem, int zbl, int agnesi, int zp, const float* cf, float* e_lin, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_mace_zbl((cudaStream_t)st, n_own, row_ptr, e_src, reinterpret_cast<const float4*>(e_vec), type,
+                         mace_core(elem, zbl, agnesi, zp, cf), e_lin);
+  });
+}
+int shim_mace_embed(void* st, int n, int C, const int* type, const float* W, float* h0, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] { b2m::launch_mace_embed((cudaStream_t)st, n, C, type, W, h0); });
+}
+// bwd = 0: launch_mace_msg (A =); bwd = 1: launch_mace_msg_bwd (gR =, gY +=, gu +=)
+int shim_mace_msg(int bwd, void* st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
+                  const float* Y, const float* u, float* A, const float* gA, float* gR, float* gY, float* gu, char* msg,
+                  int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_mace_msg_bwd((cudaStream_t)st, n_own, C, L1, row_ptr, e_src, R, Y, u, gA, gR, gY, gu);
+    else
+      b2m::launch_mace_msg((cudaStream_t)st, n_own, C, L1, row_ptr, e_src, R, Y, u, A);
+  });
+}
+// bwd = 0: launch_mace_msg_eq (Am =); bwd = 1: launch_mace_msg_eq_bwd (R overwritten with gR, gY +=, gu +=)
+int shim_mace_msg_eq(int bwd, void* st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src, float* R,
+                     const float* Y, const float* u, float* Am, const float* gAm, float* gY, float* gu, char* msg,
+                     int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_mace_msg_eq_bwd((cudaStream_t)st, max_ell, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
+    else
+      b2m::launch_mace_msg_eq((cudaStream_t)st, max_ell, n_own, C, row_ptr, e_src, R, Y, u, Am);
+  });
+}
+int shim_mace_elem_mix(void* st, int n, int C, int L1, int nsh, const int* type, const float* W, const float* in,
+                       float* out, int accum, char* msg, int msglen) {
+  return guarded(msg, msglen,
+                 [&] { b2m::launch_mace_elem_mix((cudaStream_t)st, n, C, L1, nsh, type, W, in, out, accum != 0); });
+}
+int shim_mace_elem_mix_rows(void* st, int n, int C, int ncomp, int ldi, int ldo, const int* type, const float* W,
+                            const float* in, float* out, int accum, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_mace_elem_mix_rows((cudaStream_t)st, n, C, ncomp, ldi, ldo, type, W, in, out, accum != 0);
+  });
+}
+// eq = 0: launch_mace_symc / _bwd; eq = 1: launch_mace_symc_eq / _bwd.  bwd = 0: out = B; bwd = 1: out = gA (gB read)
+int shim_mace_symc(int eq, int bwd, void* st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                   const void* terms, int nterms, const float* w, const float* gB, float* out, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    const auto* tm = static_cast<const b2m::MaceTerm*>(terms);
+    cudaStream_t s = (cudaStream_t)st;
+    if (eq && bwd) b2m::launch_mace_symc_eq_bwd(s, n_own, C, nsh, Ktot, type, A, tm, nterms, w, gB, out);
+    else if (eq) b2m::launch_mace_symc_eq(s, n_own, C, nsh, Ktot, type, A, tm, nterms, w, out);
+    else if (bwd) b2m::launch_mace_symc_bwd(s, n_own, C, nsh, Ktot, type, A, tm, nterms, w, gB, out);
+    else b2m::launch_mace_symc(s, n_own, C, nsh, Ktot, type, A, tm, nterms, w, out);
+  });
+}
+int shim_mace_readout_lin(void* st, int n_own, int C, int ld, const float* h, const float* w, float* e_lin, char* msg,
+                          int msglen) {
+  return guarded(msg, msglen, [&] { b2m::launch_mace_readout_lin((cudaStream_t)st, n_own, C, ld, h, w, e_lin); });
+}
+int shim_mace_readout_final(void* st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
+                            const float* e_lin, const int* type, const double* E0, double scale, double shift, float* pre,
+                            double* energy, const int* gid, double* atom_e, const float* wgt, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_mace_readout_final((cudaStream_t)st, n_own, C, H, h, W1, w2, e_lin, type, E0, scale, shift, pre, energy,
+                                   gid, atom_e, wgt);
+  });
+}
+int shim_mace_readout_seed(void* st, int n_own, int C, int H, const float* pre, const float* W1, const float* w2,
+                           float scale, float* gh, const int* gid, const float* wgt, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_mace_readout_seed((cudaStream_t)st, n_own, C, H, pre, W1, w2, scale, gh, gid, wgt);
+  });
+}
+int shim_mace_add_row(void* st, int n_own, int C, int ld, const float* w, float scale, float* gh, const int* gid,
+                      const float* wgt, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] { b2m::launch_mace_add_row((cudaStream_t)st, n_own, C, ld, w, scale, gh, gid, wgt); });
+}
+int shim_mace_edge_final(void* st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float* e_vec,
+                         const int* gid, const int* type, int nb, int p, float r_max, float pref, const float* w,
+                         const float* elem, int zbl, int agnesi, int zp, const float* cf, const float* g_eb,
+                         const float* gY, float* forces, double* virial, float* atom_vir, const float* wgt, char* msg,
+                         int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_mace_edge_final((cudaStream_t)st, E, nsh, e_src, e_dst, reinterpret_cast<const float4*>(e_vec), gid, type,
+                                mace_radial(nb, p, r_max, pref, w), mace_core(elem, zbl, agnesi, zp, cf), g_eb, gY,
+                                forces, virial, atom_vir, wgt);
+  });
+}
+// host: the engine's conv_tp path list into out [3 * cap] (l_in, l_sh, l_out per path); *n = its length
+int shim_mace_conv_paths(int max_ell, int hidden_l, int* out, int cap, int* n, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    const auto p = b2m::mace_conv_paths(max_ell, hidden_l);
+    *n = (int)p.size();
+    for (int k = 0; k < *n && k < cap; k++)
+      for (int j = 0; j < 3; j++) out[3 * k + j] = p[k][j];
+  });
+}
+// host: the engine's symmetric-contraction terms of one U (host [ncomp][nsh]^nu [K]) into out (MaceTerm [cap]); *n = count
+int shim_mace_sym_terms(const float* U, int nsh, int nu, int ncomp, int K, int kg0, void* out, int cap, int* n,
+                        char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    const auto t = b2m::mace_sym_terms(U, nsh, nu, ncomp, K, kg0);
+    *n = (int)t.size();
+    memcpy(out, t.data(), std::min(t.size(), (size_t)cap) * sizeof(b2m::MaceTerm));
+  });
+}
 
 }  // extern "C"

@@ -95,6 +95,25 @@ class Shim:
         self._call(self.lib.shim_line_reverse_can, _ptr(raw), _ptr(out))
         return out
 
+    def mace_conv_paths(self, max_ell, hidden_l):
+        """engine_mace.inl mace_conv_paths: [(l_in, l_sh, l_out)]"""
+        out, n = (ctypes.c_int * 60)(), ctypes.c_int(0)
+        self._call(self.lib.shim_mace_conv_paths, ctypes.c_int(max_ell), ctypes.c_int(hidden_l), out, ctypes.c_int(20),
+                   ctypes.byref(n))
+        return [tuple(out[3 * k:3 * k + 3]) for k in range(n.value)]
+
+    def mace_sym_terms(self, U, nsh, nu, ncomp, K, kg0):
+        """engine_mace.inl mace_sym_terms on a host U: int32 [n][3] (idx, kg, coef's fp32 bits), the MaceTerm layout"""
+        U = U.float().contiguous()
+        n, cap = ctypes.c_int(0), 4096
+        while True:
+            out = torch.zeros(cap, 3, dtype=torch.int32)
+            self._call(self.lib.shim_mace_sym_terms, _ptr(U), ctypes.c_int(nsh), ctypes.c_int(nu), ctypes.c_int(ncomp),
+                       ctypes.c_int(K), ctypes.c_int(kg0), _ptr(out), ctypes.c_int(cap), ctypes.byref(n))
+            if n.value <= cap:
+                return out[: n.value].clone()
+            cap = n.value
+
     def radial_can(self, M, Wab):
         M, Wab = M.float().contiguous(), Wab.float().contiguous()
         out = torch.empty(self.atom_rad, dtype=torch.float32)
@@ -212,6 +231,31 @@ def tf32(x):
 
 def d64(t):
     return None if t is None else t.detach().to(F64)
+
+
+def check(errs, key, tol, out, ref, what=""):
+    """out (device) against a Mag ref, every element; records the largest normalised error under errs[key]"""
+    import pytest
+
+    err = max_err(out, ref.x, ref.s)
+    errs[key] = max(errs.get(key, 0.0), err)
+    if err > tol:
+        o = out.detach().cpu().double()
+        e = (o - ref.x).abs() / ref.s
+        e = torch.where(torch.isfinite(o), e, torch.full_like(e, float("inf")))
+        idx = torch.nonzero(e > tol)
+        rows = sorted(set(idx[:, 0].tolist())) if idx.ndim == 2 else idx.tolist()
+        pytest.fail(f"{key} {what}: max err {err:.3e} > tol {tol:.1e}; {len(idx)} elements in rows "
+                    f"{rows[:20]} (tiles {sorted(set(r // TM for r in rows))[:20]})")
+
+
+def untouched(name, out, before, rows_hit, what=""):
+    """rows of out that no row of the launch maps to equal their prefill bit for bit"""
+    free = torch.ones(len(before), dtype=torch.bool)
+    free[rows_hit[rows_hit >= 0].long()] = False
+    o = out.detach().cpu()
+    same = (o[free].view(torch.int32) == before[free].view(torch.int32)).all()
+    assert bool(same), f"{name} {what}: rows without contributions changed"
 
 
 def max_err(out, ref, scale):

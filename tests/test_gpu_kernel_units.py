@@ -23,10 +23,6 @@ pytestmark = pytest.mark.gpu
 ERRS = {}
 
 
-def record(key, err):
-    ERRS[key] = max(ERRS.get(key, 0.0), err)
-
-
 @pytest.fixture(scope="module")
 def shim(tmp_path_factory):
     s = R.Shim(R.build_shim(tmp_path_factory.mktemp("kernel_shim")))
@@ -44,26 +40,10 @@ def sms():
 
 
 def check(key, tol, out, ref, what=""):
-    """out (device) against a Mag ref, every element; records the largest normalised error under key."""
-    err = R.max_err(out, ref.x, ref.s)
-    record(key, err)
-    if err > tol:
-        o = out.detach().cpu().double()
-        e = (o - ref.x).abs() / ref.s
-        e = torch.where(torch.isfinite(o), e, torch.full_like(e, float("inf")))
-        idx = torch.nonzero(e > tol)
-        rows = sorted(set(idx[:, 0].tolist())) if idx.ndim == 2 else idx.tolist()
-        pytest.fail(f"{key} {what}: max err {err:.3e} > tol {tol:.1e}; {len(idx)} elements in rows "
-                    f"{rows[:20]} (tiles {sorted(set(r // R.TM for r in rows))[:20]})")
+    R.check(ERRS, key, tol, out, ref, what)
 
 
-def untouched(name, out, before, rows_hit, what=""):
-    """rows of out that no row of the launch maps to equal their prefill bit for bit"""
-    free = torch.ones(len(before), dtype=torch.bool)
-    free[rows_hit[rows_hit >= 0].long()] = False
-    o = out.detach().cpu()
-    same = (o[free].view(torch.int32) == before[free].view(torch.int32)).all()
-    assert bool(same), f"{name} {what}: rows without contributions changed"
+untouched = R.untouched
 
 
 # ------------------------------------------------------------------------------------------------ row GEMM
