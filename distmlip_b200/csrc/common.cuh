@@ -3,10 +3,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
-#include <atomic>
 #include <mutex>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -89,10 +89,34 @@ struct PerDeviceOnce {
   }
 };
 
-extern std::atomic<long long> g_launch_count;  // kernels launched by this library (bench.py gpu_launches); atomic: the
-                                               // partitions of a single-process group are driven by one host thread each
+// Kernels launched by the calling host thread.  Per thread: the partitions of a single-process group run concurrently,
+// one host thread each, and run() counts the launches of its own partition as the change across an evaluation.
+inline thread_local long long g_launch_count = 0;
 
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// kern<<<grid, block, smem, st>>>(args...), checked and counted; an empty grid launches nothing
+template <class... P, class... A>
+void launch(void (*kern)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... args) {
+  if (grid.x == 0 || grid.y == 0 || grid.z == 0) return;
+  kern<<<grid, block, smem, st>>>(std::forward<A>(args)...);
+  B2M_CK(cudaGetLastError());
+  g_launch_count++;
+}
+
+// f(std::bool_constant<b>{}...) for the run-time flags b...: picks a kernel's template instantiation, as in
+//   with_flags([&](auto kAtomic) { launch(k<kAtomic>, ...); }, atom_vir != nullptr);
+template <class F>
+void with_flags(F&& f) {
+  f();
+}
+template <class F, class... B>
+void with_flags(F&& f, bool b, B... rest) {
+  if (b)
+    with_flags([&](auto... c) { f(std::true_type{}, c...); }, rest...);
+  else
+    with_flags([&](auto... c) { f(std::false_type{}, c...); }, rest...);
+}
 
 // ---------------------------------------------------------------- model constants
 constexpr int D = 64;    // feature width (atom = bond = angle)

@@ -21,7 +21,7 @@
 #include <algorithm>
 #include <array>
 
-#include "atomic_virial.cuh"
+#include "final_tail.cuh"
 #include "graph.cuh"
 #include "kernels.cuh"
 #include "mace_state.cuh"
@@ -228,6 +228,12 @@ namespace b2m {
 
 // atoms of the structure the caller passed: the graph's atoms, or the cell atoms of an unfolded graph
 static int64_t cell_atoms(const b2m_engine* e) { return e->hf_n ? e->hf_n : e->g.N; }
+
+// optional outputs of an evaluation and the readout weights, null where they are off: per-atom energies and virials
+// (b2m_set_atomic), and each atom's energy weight (heat flux, DESIGN.md §10)
+static double* atom_e_out(b2m_engine* e) { return e->atomic ? e->buf.atom_e.p : nullptr; }
+static float* atom_vir_out(b2m_engine* e) { return e->atomic ? e->buf.atom_vir.p : nullptr; }
+static const float* readout_wgt(const b2m_engine* e) { return e->hf_n ? e->buf.hf_w.p : nullptr; }
 
 // state_dict tensor k, marked as used; its shape must be `shape`, or with `flat` only hold as many elements
 static const std::vector<float>& weight(b2m_engine* e, const std::string& k, const std::vector<int64_t>& shape,
@@ -562,15 +568,6 @@ static void halo_backward(b2m_engine* e, float* gbuf, bool bonds, int width = D)
 
 // ------------------------------------------------------------------------------------------
 // heat flux (DESIGN.md §10)
-#define LAUNCH_HF(kern, n, st, ...)                              \
-  do {                                                           \
-    if ((n) > 0) {                                               \
-      kern<<<cdiv((n), 256), 256, 0, st>>>(__VA_ARGS__);         \
-      B2M_CK(cudaGetLastError());                                \
-      g_launch_count++;                                          \
-    }                                                            \
-  } while (0)
-
 // readout weight of every unfolded atom: images 0; cell atoms 1 (alpha < 0, the mask) or (r_j - c)_alpha (a seed)
 __global__ void k_hf_weights(int64_t N, int64_t n, const double* __restrict__ cart, double cx, double cy, double cz,
                              int alpha, float* __restrict__ w) {
@@ -611,20 +608,7 @@ __global__ void __launch_bounds__(256) k_hf_contract(int64_t N, int64_t n, const
       if (j < n) acc[3 + a] += eps[j] * v[a];
     }
   }
-  __shared__ double red[6][8];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int k = 0; k < 6; k++) {
-    double x = acc[k];
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-    if (lane == 0) red[k][warp] = x;
-  }
-  __syncthreads();
-  if (threadIdx.x < 6) {
-    double s = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += red[threadIdx.x][w];
-    atomicAdd(&out[threadIdx.x], s);
-  }
+  block_sum_add(acc, out);
 }
 
 static void run(b2m_engine* e, bool grads) {
@@ -651,8 +635,8 @@ static void run(b2m_engine* e, bool grads) {
   }
   e->atomic_last = 0;
   if (e->hf_n) {
-    LAUNCH_HF(k_hf_weights, e->g.N, e->st, e->g.N, e->hf_n, e->g.cart.p, e->hf_c[0], e->hf_c[1], e->hf_c[2], e->hf_seed,
-              e->buf.hf_w.p);
+    launch(k_hf_weights, cdiv(e->g.N, 256), 256, 0, e->st, e->g.N, e->hf_n, e->g.cart.p, e->hf_c[0], e->hf_c[1],
+           e->hf_c[2], e->hf_seed, e->buf.hf_w.p);
   }
   e->model->forward(e);
   B2M_CK(cudaEventRecord(e->ev[1], e->st));
@@ -773,8 +757,7 @@ static const T* part_sum(b2m_engine* L, DBuf<T> Bufs::*arr, DBuf<T>& sum, DBuf<T
   B2M_CK(cudaMemcpyAsync(sum.p, (L->buf.*arr).p, n * sizeof(T), cudaMemcpyDeviceToDevice, L->st));
   for (size_t p = 1; p < L->parts.size(); p++) {
     B2M_CK(cudaMemcpyAsync(tmp.p, (L->parts[p]->buf.*arr).p, n * sizeof(T), cudaMemcpyDefault, L->st));
-    k_add_inplace<<<cdiv((int64_t)n, 256), 256, 0, L->st>>>((int64_t)n, tmp.p, sum.p);
-    B2M_CK(cudaGetLastError());
+    launch(k_add_inplace<T>, cdiv((int64_t)n, 256), 256, 0, L->st, (int64_t)n, tmp.p, sum.p);
   }
   return sum.p;
 }
@@ -792,7 +775,7 @@ static const float* fold_rows(b2m_engine* e, const float* src, int width, int pi
   const int64_t N = e->g.N, n = e->hf_n;
   e->buf.hf_fold.ensure((size_t)n * pitch + 64);
   e->buf.hf_fold.zero((size_t)n * pitch, e->st);
-  LAUNCH_HF(k_hf_fold, N * width, e->st, N, e->uf.image_of.p, width, pitch, src, e->buf.hf_fold.p);
+  launch(k_hf_fold, cdiv(N * width, 256), 256, 0, e->st, N, e->uf.image_of.p, width, pitch, src, e->buf.hf_fold.p);
   return e->buf.hf_fold.p;
 }
 
@@ -883,10 +866,8 @@ static void heat_flux(b2m_engine* h, const double* vel, double* flux6) {
   B2M_CK(cudaMemcpyAsync(h->buf.hf_vel.p, vel, (size_t)n * 3 * sizeof(double), cudaMemcpyHostToDevice, h->st));
   h->buf.hf_out.zero(6, h->st);
   const int grid = std::max(1, std::min(cdiv(N, 256), 4 * h->num_sms));
-  k_hf_contract<<<grid, 256, 0, h->st>>>(N, n, h->g.cart.p, h->hf_c[0], h->hf_c[1], h->hf_c[2], h->uf.image_of.p,
-                                         h->buf.hf_vel.p, F, h->buf.hf_G.p, eps, h->buf.hf_out.p);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_hf_contract, grid, 256, 0, h->st, N, n, h->g.cart.p, h->hf_c[0], h->hf_c[1], h->hf_c[2], h->uf.image_of.p,
+         h->buf.hf_vel.p, F, h->buf.hf_G.p, eps, h->buf.hf_out.p);
   B2M_CK(cudaMemcpyAsync(flux6, h->buf.hf_out.p, 6 * sizeof(double), cudaMemcpyDeviceToHost, h->st));
   B2M_CK(cudaStreamSynchronize(h->st));
 }

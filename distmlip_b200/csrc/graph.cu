@@ -580,14 +580,6 @@ static int read_int(const int* dptr, cudaStream_t st) {
   return v;
 }
 
-#define LAUNCH1D(kern, n, st, ...)                                          \
-  do {                                                                      \
-    if ((n) > 0) {                                                          \
-      kern<<<cdiv((n), 256), 256, 0, st>>>(__VA_ARGS__);                    \
-      B2M_CK(cudaGetLastError());                                           \
-    }                                                                       \
-  } while (0)
-
 void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
                   const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,
                   int rank_, int world_) {
@@ -638,13 +630,12 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     gp.fmin[k] = 0;
     gp.fscale[k] = 0;
   }
-  LAUNCH1D(k_wrap, N, st, N, cart.p, gp, fracw.p, wc.p, corr.p);
+  launch(k_wrap, cdiv(N, 256), 256, 0, st, N, cart.p, gp, fracw.p, wc.p, corr.p);
 
   // ---- min/max (partition axis, walls, non-periodic cell grid) ----
   const int RB = 256;
   red_tmp.ensure(RB * 12);
-  k_minmax<<<RB, 256, 0, st>>>(N, wc.p, fracw.p, red_tmp.p);
-  B2M_CK(cudaGetLastError());
+  launch(k_minmax, RB, 256, 0, st, N, wc.p, fracw.p, red_tmp.p);
   std::vector<double> hred(RB * 12);
   B2M_CK(cudaMemcpyAsync(hred.data(), red_tmp.p, RB * 12 * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2M_CK(cudaStreamSynchronize(st));
@@ -675,7 +666,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     // collision nudge
     for (int iter = 0; iter < 64; iter++) {
       B2M_CK(cudaMemsetAsync(tmp_i0.p, 0, MAXP * sizeof(int), st));
-      LAUNCH1D(k_wall_collisions, N, st, N, fracw.p, wl, tmp_i0.p);
+      launch(k_wall_collisions, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, tmp_i0.p);
       int hits[MAXP];
       B2M_CK(cudaMemcpyAsync(hits, tmp_i0.p, MAXP * sizeof(int), cudaMemcpyDeviceToHost, st));
       B2M_CK(cudaStreamSynchronize(st));
@@ -749,7 +740,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   cell_start.ensure(ncell + 2);
 
   // ---- owner + cell id, sort by cell ----
-  LAUNCH1D(k_owner_cell, N, st, N, fracw.p, wl, gp, owner.p, cell_of.p, tmp_i0.p);
+  launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, gp, owner.p, cell_of.p, tmp_i0.p);
   {
     size_t bytes = 0;
     int bits = 1;
@@ -761,11 +752,11 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     // tmp_i1 = sorted cell ids
     tmp_i2.ensure(std::max<int64_t>(N + 1, ncell + 2));
     B2M_CK(cudaMemsetAsync(tmp_i2.p, 0, (ncell + 1) * sizeof(int), st));
-    LAUNCH1D(k_cell_hist, N, st, N, tmp_i1.p, tmp_i2.p);
+    launch(k_cell_hist, cdiv(N, 256), 256, 0, st, N, tmp_i1.p, tmp_i2.p);
     excl_scan(cub_tmp, tmp_i2.p, cell_start.p, ncell + 1, st);
   }
   // own flags, scan -> local ids
-  LAUNCH1D(k_post_sort, N, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i0.p);
+  launch(k_post_sort, cdiv(N, 256), 256, 0, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i0.p);
   tmp_i3.ensure(N + 1);
   B2M_CK(cudaMemsetAsync(tmp_i0.p + N, 0, sizeof(int), st));
   excl_scan(cub_tmp, tmp_i0.p, tmp_i3.p, N + 1, st);
@@ -777,15 +768,16 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   type.ensure(N);
   loc_sidx.ensure(N);
   to_mask.ensure(n_own);
-  LAUNCH1D(k_assign_owned, N, st, N, s_gid.p, tmp_i0.p, tmp_i3.p, species.p, gid.p, type.p, loc_sidx.p, g2l.p);
+  launch(k_assign_owned, cdiv(N, 256), 256, 0, st, N, s_gid.p, tmp_i0.p, tmp_i3.p, species.p, gid.p, type.p, loc_sidx.p,
+         g2l.p);
 
   // ---- count pass over owned rows ----
   const double r2 = rcut * rcut, rb2 = rbond * rbond;
   row_ptr.ensure(n_own + 2);
   DBuf<int>& cnt_e = tmp_i0;
   DBuf<int>& cnt_b = tmp_i1;
-  LAUNCH1D(k_count, n_own, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p, owner.p, rank, r2, rb2,
-           tol, cnt_e.p, cnt_b.p, to_mask.p);
+  launch(k_count, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p, owner.p,
+         rank, r2, rb2, tol, cnt_e.p, cnt_b.p, to_mask.p);
   B2M_CK(cudaMemsetAsync(cnt_e.p + n_own, 0, sizeof(int), st));
   B2M_CK(cudaMemsetAsync(cnt_b.p + n_own, 0, sizeof(int), st));
   excl_scan(cub_tmp, cnt_e.p, row_ptr.p, n_own + 1, st);
@@ -812,9 +804,9 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   b_edge.ensure(B_own + 1);
   unsigned char* halo_flag = tmp_flag.p;
   B2M_CK(cudaMemsetAsync(halo_flag, 0, N, st));
-  LAUNCH1D(k_fill_owned, n_own, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p, owner.p, rank, r2,
-           rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p, e_bond.p, e_vec.p, b_src_gid.p, b_dst.p,
-           b_img.p, b_edge.p, b_vec.p, halo_flag);
+  launch(k_fill_owned, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p,
+         owner.p, rank, r2, rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p, e_bond.p, e_vec.p,
+         b_src_gid.p, b_dst.p, b_img.p, b_edge.p, b_vec.p, halo_flag);
 
   // ---- halo atoms: grouped by owner, gid ascending ----
   n_halo = 0;
@@ -822,7 +814,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   for (int q = 0; q < MAXP; q++) n_from[q] = n_to[q] = nb_from[q] = nb_to[q] = 0;
   if (world > 1) {
     unsigned char* keys = tmp_flag.p + N;
-    LAUNCH1D(k_halo_keys, N, st, N, halo_flag, owner.p, world, keys, tmp_i0.p);
+    launch(k_halo_keys, cdiv(N, 256), 256, 0, st, N, halo_flag, owner.p, world, keys, tmp_i0.p);
     // sort (key, gid): stable radix sort keeps gid ascending inside each key
     keys_out.ensure(N);
     size_t bytes = 0;
@@ -831,7 +823,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     B2M_CK(cub::DeviceRadixSort::SortPairs(cub_tmp.p, bytes, keys, keys_out.p, tmp_i0.p, tmp_i1.p, (int)N, 0, 8, st));
     // section sizes: histogram of the sorted keys
     B2M_CK(cudaMemsetAsync(tmp_i2.p, 0, (MAXP + 2) * sizeof(int), st));
-    LAUNCH1D(k_key_hist, N, st, N, keys_out.p, tmp_i2.p);
+    launch(k_key_hist, cdiv(N, 256), 256, 0, st, N, keys_out.p, tmp_i2.p);
     int hc[MAXP + 2];
     B2M_CK(cudaMemcpyAsync(hc, tmp_i2.p, (MAXP + 2) * sizeof(int), cudaMemcpyDeviceToHost, st));
     B2M_CK(cudaStreamSynchronize(st));
@@ -843,23 +835,23 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     }
     for (int q = world; q <= MAXP; q++) from_off[q] = off;
     n_halo = off;
-    LAUNCH1D(k_assign_halo, n_halo, st, n_halo, n_own, tmp_i1.p, species.p, sidx_of_gid.p, gid.p, type.p, loc_sidx.p,
-             g2l.p);
+    launch(k_assign_halo, cdiv(n_halo, 256), 256, 0, st, n_halo, n_own, tmp_i1.p, species.p, sidx_of_gid.p, gid.p,
+           type.p, loc_sidx.p, g2l.p);
   }
   n_loc = n_own + n_halo;
-  LAUNCH1D(k_relabel, E, st, E, e_src_gid.p, g2l.p, e_src.p);
+  launch(k_relabel, cdiv(E, 256), 256, 0, st, E, e_src_gid.p, g2l.p, e_src.p);
 
   // ---- halo bonds ----
   B_halo = 0;
   if (n_halo > 0) {
     DBuf<int>& hb_cnt = tmp_i0;
-    LAUNCH1D(k_count, n_halo, st, n_halo, loc_sidx.p + n_own, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p, owner.p,
-             rank, rb2, rb2, tol, (int*)nullptr, hb_cnt.p, (unsigned*)nullptr);
+    launch(k_count, cdiv(n_halo, 256), 256, 0, st, n_halo, loc_sidx.p + n_own, gp, s_gid.p, s_wc.p, cell_start.p,
+           fracw.p, owner.p, rank, rb2, rb2, tol, (int*)nullptr, hb_cnt.p, (unsigned*)nullptr);
     B2M_CK(cudaMemsetAsync(hb_cnt.p + n_halo, 0, sizeof(int), st));
     excl_scan(cub_tmp, hb_cnt.p, tmp_i1.p, n_halo + 1, st);
     B_halo = read_int(tmp_i1.p + n_halo, st);
     // brow_ptr[n_own + h] = B_own + scan[h]
-    LAUNCH1D(k_add_offset, n_halo + 1, st, n_halo + 1, tmp_i1.p, B_own, brow_ptr.p + n_own);
+    launch(k_add_offset, cdiv(n_halo + 1, 256), 256, 0, st, n_halo + 1, tmp_i1.p, B_own, brow_ptr.p + n_own);
   }
   B_loc = B_own + B_halo;
   if ((size_t)B_loc > b_src_gid.cap) {
@@ -884,9 +876,9 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     std::swap(nv.cap, b_vec.cap);
   }
   if (n_halo > 0)
-    LAUNCH1D(k_fill_halo_bonds, n_halo, st, n_halo, n_own, loc_sidx.p + n_own, gp, s_gid.p, s_wc.p, cell_start.p,
-             fracw.p, rb2, tol, brow_ptr.p, b_src_gid.p, b_dst.p, b_img.p, b_vec.p);
-  LAUNCH1D(k_relabel, B_loc, st, (int64_t)B_loc, b_src_gid.p, g2l.p, b_src.p);
+    launch(k_fill_halo_bonds, cdiv(n_halo, 256), 256, 0, st, n_halo, n_own, loc_sidx.p + n_own, gp, s_gid.p, s_wc.p,
+           cell_start.p, fracw.p, rb2, tol, brow_ptr.p, b_src_gid.p, b_dst.p, b_img.p, b_vec.p);
+  launch(k_relabel, cdiv(B_loc, 256), 256, 0, st, (int64_t)B_loc, b_src_gid.p, g2l.p, b_src.p);
   for (int q = 0; q <= MAXP; q++) bfrom_off[q] = 0;
   if (n_halo > 0) {
     // bond halo sections follow the atom halo sections
@@ -914,7 +906,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       to_off[q] = off;
       if (q == rank) continue;
       unsigned char* flag = tmp_flag.p;  // halo_flag no longer needed
-      LAUNCH1D(k_to_flags, N, st, N, owner.p, rank, q, g2l.p, to_mask.p, flag);
+      launch(k_to_flags, cdiv(N, 256), 256, 0, st, N, owner.p, rank, q, g2l.p, to_mask.p, flag);
       size_t bytes = 0;
       cub::CountingInputIterator<int> it(0);
       cub::DeviceSelect::Flagged(nullptr, bytes, it, flag, sel_out.p, nsel.p, (int)N, st);
@@ -922,7 +914,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       B2M_CK(cub::DeviceSelect::Flagged(cub_tmp.p, bytes, it, flag, sel_out.p, nsel.p, (int)N, st));
       int cnt = read_int(nsel.p, st);
       n_to[q] = cnt;
-      if (cnt > 0) LAUNCH1D(k_map_g2l, cnt, st, cnt, sel_out.p, g2l.p, to_list.p + off);
+      if (cnt > 0) launch(k_map_g2l, cdiv(cnt, 256), 256, 0, st, cnt, sel_out.p, g2l.p, to_list.p + off);
       off += cnt;
     }
     for (int q = world; q <= MAXP; q++) to_off[q] = off;
@@ -933,12 +925,13 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       bto_off[q] = boff;
       int cnt = n_to[q];
       if (cnt == 0) continue;
-      LAUNCH1D(k_row_sizes, cnt, st, cnt, to_list.p + to_off[q], brow_ptr.p, tmp_i0.p);
+      launch(k_row_sizes, cdiv(cnt, 256), 256, 0, st, cnt, to_list.p + to_off[q], brow_ptr.p, tmp_i0.p);
       B2M_CK(cudaMemsetAsync(tmp_i0.p + cnt, 0, sizeof(int), st));
       excl_scan(cub_tmp, tmp_i0.p, tmp_i1.p, cnt + 1, st);
       int tot = read_int(tmp_i1.p + cnt, st);
       nb_to[q] = tot;
-      LAUNCH1D(k_expand_rows, cnt, st, cnt, to_list.p + to_off[q], brow_ptr.p, tmp_i1.p, bto_list.p + boff);
+      launch(k_expand_rows, cdiv(cnt, 256), 256, 0, st, cnt, to_list.p + to_off[q], brow_ptr.p, tmp_i1.p,
+             bto_list.p + boff);
       boff += tot;
     }
     for (int q = world; q <= MAXP; q++) bto_off[q] = boff;
@@ -950,14 +943,15 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   {
     DBuf<int>& ocnt = tmp_i0;
     B2M_CK(cudaMemsetAsync(ocnt.p, 0, (n_loc + 1) * sizeof(int), st));
-    LAUNCH1D(k_out_hist, B_own, st, B_own, b_src.p, ocnt.p);
+    launch(k_out_hist, cdiv(B_own, 256), 256, 0, st, B_own, b_src.p, ocnt.p);
     excl_scan(cub_tmp, ocnt.p, out_ptr.p, n_loc + 1, st);
     B2M_CK(cudaMemsetAsync(tmp_i1.p, 0, (n_loc + 1) * sizeof(int), st));
-    LAUNCH1D(k_out_fill, B_own, st, B_own, b_src.p, out_ptr.p, tmp_i1.p, out_list.p);
-    LAUNCH1D(k_out_sort, n_loc, st, n_loc, out_ptr.p, out_list.p);
+    launch(k_out_fill, cdiv(B_own, 256), 256, 0, st, B_own, b_src.p, out_ptr.p, tmp_i1.p, out_list.p);
+    launch(k_out_sort, cdiv(n_loc, 256), 256, 0, st, n_loc, out_ptr.p, out_list.p);
     DBuf<int>& acnt = tmp_i2;
     acnt.ensure(n_loc + 2);
-    LAUNCH1D(k_angle_count, n_loc, st, n_loc, out_ptr.p, out_list.p, brow_ptr.p, b_src_gid.p, b_dst.p, gid.p, acnt.p);
+    launch(k_angle_count, cdiv(n_loc, 256), 256, 0, st, n_loc, out_ptr.p, out_list.p, brow_ptr.p, b_src_gid.p, b_dst.p,
+           gid.p, acnt.p);
     B2M_CK(cudaMemsetAsync(acnt.p + n_loc, 0, sizeof(int), st));
     tmp_i3.ensure(n_loc + 2);
     excl_scan(cub_tmp, acnt.p, tmp_i3.p, n_loc + 1, st);
@@ -965,8 +959,8 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     a_in.ensure(A + 1);
     a_out.ensure(A + 1);
     a_ctr.ensure(A + 1);
-    LAUNCH1D(k_angle_fill, n_loc, st, n_loc, out_ptr.p, out_list.p, brow_ptr.p, b_src_gid.p, b_dst.p, gid.p, tmp_i3.p,
-             a_in.p, a_out.p, a_ctr.p);
+    launch(k_angle_fill, cdiv(n_loc, 256), 256, 0, st, n_loc, out_ptr.p, out_list.p, brow_ptr.p, b_src_gid.p, b_dst.p,
+           gid.p, tmp_i3.p, a_in.p, a_out.p, a_ctr.p);
   }
   B2M_CK(cudaStreamSynchronize(st));
 }
@@ -1087,12 +1081,11 @@ void Unfold::build(cudaStream_t st, int64_t natoms, const double* h_cart, const 
   off.ensure(n + 1);
   B2M_CK(cudaMemcpyAsync(cart0.p, h_cart, 3 * n * sizeof(double), cudaMemcpyDefault, st));
   B2M_CK(cudaMemcpyAsync(species0.p, h_species, n * sizeof(int), cudaMemcpyDefault, st));
-  LAUNCH1D(k_unfold_frac, n, st, n, cart0.p, b, frac0.p);
+  launch(k_unfold_frac, cdiv(n, 256), 256, 0, st, n, cart0.p, b, frac0.p);
   // fractional bounding box of the cell atoms (k_minmax's Cartesian half reads the positions and is not used)
   const int RB = 256;
   red_tmp.ensure(RB * 12);
-  k_minmax<<<RB, 256, 0, st>>>(n, cart0.p, frac0.p, red_tmp.p);
-  B2M_CK(cudaGetLastError());
+  launch(k_minmax, RB, 256, 0, st, n, cart0.p, frac0.p, red_tmp.p);
   std::vector<double> hred(RB * 12);
   B2M_CK(cudaMemcpyAsync(hred.data(), red_tmp.p, RB * 12 * sizeof(double), cudaMemcpyDeviceToHost, st));
   B2M_CK(cudaStreamSynchronize(st));
@@ -1112,7 +1105,7 @@ void Unfold::build(cudaStream_t st, int64_t natoms, const double* h_cart, const 
       B2M_REQUIRE(b.smax[k] - b.smin[k] < 4096, B2M_ERR_INVALID, "heat-flux reach far larger than the cell");
     }
   }
-  LAUNCH1D(k_unfold_count, n, st, n, frac0.p, b, cnt.p);
+  launch(k_unfold_count, cdiv(n, 256), 256, 0, st, n, frac0.p, b, cnt.p);
   B2M_CK(cudaMemsetAsync(cnt.p + n, 0, sizeof(int), st));
   excl_scan(cub_tmp, cnt.p, off.p, n + 1, st);
   const int64_t n_img = read_int(off.p + n, st);
@@ -1121,7 +1114,8 @@ void Unfold::build(cudaStream_t st, int64_t natoms, const double* h_cart, const 
   cart.ensure(3 * N);
   species.ensure(N);
   image_of.ensure(N);
-  LAUNCH1D(k_unfold_fill, n, st, n, cart0.p, species0.p, frac0.p, off.p, b, cart.p, species.p, image_of.p);
+  launch(k_unfold_fill, cdiv(n, 256), 256, 0, st, n, cart0.p, species0.p, frac0.p, off.p, b, cart.p, species.p,
+         image_of.p);
 }
 
 }  // namespace b2m

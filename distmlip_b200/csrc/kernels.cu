@@ -1,15 +1,13 @@
 // kernels.cu -- hand-written sm_90a kernels of the CHGNet hot path (fp32 FFMA math,
 // cp.async.bulk (TMA) row gathers into shared memory, segmented scatter-adds).
 // See kernels.cuh for the formulation; oracle/manual_ref.py is the CPU mirror of every stage.
-#include "atomic_virial.cuh"
+#include "final_tail.cuh"
 #include "kernels.cuh"
 #include "wgmma.cuh"
 
 #include <algorithm>
 
 namespace b2m {
-
-std::atomic<long long> g_launch_count{0};
 
 // ============================================================================================
 // device helpers
@@ -189,10 +187,7 @@ __global__ void k_embed(int n, const int* __restrict__ type, const float* __rest
   reinterpret_cast<float4*>(x0)[(size_t)r * 16 + c4] = reinterpret_cast<const float4*>(emb)[(size_t)type[r] * 16 + c4];
 }
 void launch_embed(cudaStream_t st, int n, const int* type, const float* emb, float* x0) {
-  if (n <= 0) return;
-  k_embed<<<cdiv((int64_t)n * 16, 256), 256, 0, st>>>(n, type, emb, x0);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_embed, cdiv((int64_t)n * 16, 256), 256, 0, st, n, type, emb, x0);
 }
 
 // out[b][c] = sum_k be_k(d_b) W[c][k]     (32 bonds per block)
@@ -219,10 +214,7 @@ __global__ void __launch_bounds__(256) k_bond_init(int nb, const float4* __restr
   }
 }
 void launch_bond_init(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp, const float* W, float* out) {
-  if (nb <= 0) return;
-  k_bond_init<<<cdiv(nb, 32), 256, 0, st>>>(nb, b_vec, rp, W, out);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_bond_init, cdiv(nb, 32), 256, 0, st, nb, b_vec, rp, W, out);
 }
 
 struct AngleGeom {
@@ -285,10 +277,7 @@ __global__ void __launch_bounds__(256) k_angle_init(int64_t na, const int* __res
 }
 void launch_angle_init(cudaStream_t st, int64_t na, const int* a_in, const int* a_out, const float4* b_vec,
                        const float* fa, const float* Wae, float* ang0) {
-  if (na <= 0) return;
-  k_angle_init<<<cdiv(na, 128), 256, 0, st>>>(na, a_in, a_out, b_vec, fa, Wae, ang0);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_angle_init, cdiv(na, 128), 256, 0, st, na, a_in, a_out, b_vec, fa, Wae, ang0);
 }
 
 __global__ void k_silu(int64_t n, const float* __restrict__ pre, float* __restrict__ out) {
@@ -300,16 +289,10 @@ __global__ void k_dsilu_mul(int64_t n, const float* __restrict__ pre, float* __r
   if (i < n) g[i] *= dsilu_f(pre[i]);
 }
 void launch_silu(cudaStream_t st, int64_t n, const float* pre, float* out) {
-  if (n <= 0) return;
-  k_silu<<<cdiv(n, 256), 256, 0, st>>>(n, pre, out);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_silu, cdiv(n, 256), 256, 0, st, n, pre, out);
 }
 void launch_dsilu_mul(cudaStream_t st, int64_t n, const float* pre, float* g) {
-  if (n <= 0) return;
-  k_dsilu_mul<<<cdiv(n, 256), 256, 0, st>>>(n, pre, g);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_dsilu_mul, cdiv(n, 256), 256, 0, st, n, pre, g);
 }
 void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats) {
   if (nfloats > 0) B2M_CK(cudaMemsetAsync(p, 0, nfloats * sizeof(float), st));
@@ -663,9 +646,7 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
   if (auto once_ = attr.first(); once_) {
     B2M_CK(cudaFuncSetAttribute(k_atomconv_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AtomSmemFwd::bytes));
   }
-  k_atomconv_fwd<<<std::min(cdiv(cdiv(a.E, TW), WGF), num_sms), NTF, AtomSmemFwd::bytes, st>>>(a);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_atomconv_fwd, std::min(cdiv(cdiv(a.E, TW), WGF), num_sms), NTF, AtomSmemFwd::bytes, st, a);
 }
 
 // ============================================================================================
@@ -909,9 +890,7 @@ void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
   if (auto once_ = attr.first(); once_) {
     B2M_CK(cudaFuncSetAttribute(k_atomconv_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AtomSmemBwd::bytes));
   }
-  k_atomconv_bwd<<<std::min(cdiv(a.E, TM), num_sms), NT, AtomSmemBwd::bytes, st>>>(a);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_atomconv_bwd, std::min(cdiv(a.E, TM), num_sms), NT, AtomSmemBwd::bytes, st, a);
 }
 
 // ============================================================================================
@@ -1309,12 +1288,7 @@ void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sm
     B2M_CK(cudaFuncSetAttribute(k_line_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
   }
   const int grid = std::min(cdiv(a.A, TM), num_sms);
-  if (hidden)
-    k_line_fwd<true><<<grid, NT, LineSmem::bytes, st>>>(a);
-  else
-    k_line_fwd<false><<<grid, NT, LineSmem::bytes, st>>>(a);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  with_flags([&](auto kHidden) { launch(k_line_fwd<kHidden>, grid, NT, LineSmem::bytes, st, a); }, hidden);
 }
 void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms) {
   if (a.A <= 0) return;
@@ -1324,12 +1298,7 @@ void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sm
     B2M_CK(cudaFuncSetAttribute(k_line_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
   }
   const int grid = std::min(cdiv(a.A, TM), num_sms);
-  if (hidden)
-    k_line_bwd<true><<<grid, NT, LineSmem::bytes, st>>>(a);
-  else
-    k_line_bwd<false><<<grid, NT, LineSmem::bytes, st>>>(a);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  with_flags([&](auto kHidden) { launch(k_line_bwd<kHidden>, grid, NT, LineSmem::bytes, st, a); }, hidden);
 }
 
 // ============================================================================================
@@ -1410,9 +1379,7 @@ static void launch_bond_node(cudaStream_t st, int nb, const float4* b_vec, Radia
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_)
     B2M_CK(cudaFuncSetAttribute(k_bond_node<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBondNodeSmem));
-  k_bond_node<MODE><<<cdiv(nb, BNR), 256, kBondNodeSmem, st>>>(nb, b_vec, rp, W, x0, x1, out, gdb);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_bond_node<MODE>, cdiv(nb, BNR), 256, kBondNodeSmem, st, nb, b_vec, rp, W, x0, x1, out, gdb);
 }
 void launch_bond_update_fwd(cudaStream_t st, int nb, const float4* b_vec, RadialParams rp3, const float* W3bw,
                             const float* h, const float* upd, float* hout) {
@@ -1490,9 +1457,7 @@ void launch_angle_init_bwd(cudaStream_t st, int64_t na, const int* a_in, const i
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_)
     B2M_CK(cudaFuncSetAttribute(k_angle_init_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kAngleBwdSmem));
-  k_angle_init_bwd<<<cdiv(na, ANR), 256, kAngleBwdSmem, st>>>(na, a_in, a_out, b_vec, fa, Wae, gang0, gbvec);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_angle_init_bwd, cdiv(na, ANR), 256, kAngleBwdSmem, st, na, a_in, a_out, b_vec, fa, Wae, gang0, gbvec);
 }
 
 // ============================================================================================
@@ -1520,14 +1485,7 @@ __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__
   if (warp < n && lane == 0) {
     v += bias;
     if (out) out[warp] = v;
-    contrib = (double)scale * (double)v;
-    if (elem_ref) contrib += elem_ref[type[warp]];
-    if constexpr (kWeighted) {
-      const double wt = (double)wgt[gid[warp]];
-      contrib *= wt;
-      mean_per_atom *= wt;
-    }
-    if constexpr (kAtomic) atom_e[gid[warp]] = contrib + mean_per_atom;
+    contrib = readout_energy<kAtomic, kWeighted>(warp, v, scale, type, elem_ref, gid, atom_e, mean_per_atom, wgt);
   }
   if (sum) {
     if (lane == 0) part[threadIdx.x >> 5] = contrib;
@@ -1542,22 +1500,12 @@ __global__ void __launch_bounds__(256) k_rowdot(int n, const float* __restrict__
 void launch_rowdot(cudaStream_t st, int n, const float* X, const float* w, float bias, float* out, double* sum,
                    const int* type, const double* elem_ref, float scale, const int* gid, double* atom_e,
                    double mean_per_atom, const float* wgt) {
-  if (n <= 0) return;
-  const int nb = cdiv((int64_t)n * 32, 256);
-  if (wgt && atom_e)
-    k_rowdot<true, true><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e,
-                                             mean_per_atom, wgt);
-  else if (wgt)
-    k_rowdot<false, true><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e,
-                                              mean_per_atom, wgt);
-  else if (atom_e)
-    k_rowdot<true><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e, mean_per_atom,
-                                       wgt);
-  else
-    k_rowdot<false><<<nb, 256, 0, st>>>(n, X, w, bias, out, sum, type, elem_ref, scale, gid, atom_e, mean_per_atom,
-                                        wgt);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  with_flags(
+      [&](auto kAtomic, auto kWeighted) {
+        launch(k_rowdot<kAtomic, kWeighted>, cdiv((int64_t)n * 32, 256), 256, 0, st, n, X, w, bias, out, sum, type,
+               elem_ref, scale, gid, atom_e, mean_per_atom, wgt);
+      },
+      atom_e != nullptr, wgt != nullptr);
 }
 // kWeighted: row r's seed times wgt[gid[r]]
 template <bool kWeighted = false>
@@ -1570,35 +1518,17 @@ __global__ void k_readout_seed(int n, const float* __restrict__ pre, const float
 }
 void launch_readout_seed(cudaStream_t st, int n, const float* pre, const float* w, float scale, float* g,
                          const int* gid, const float* wgt) {
-  if (n <= 0) return;
-  if (wgt)
-    k_readout_seed<true><<<cdiv((int64_t)n * 64, 256), 256, 0, st>>>(n, pre, w, scale, g, gid, wgt);
-  else
-    k_readout_seed<<<cdiv((int64_t)n * 64, 256), 256, 0, st>>>(n, pre, w, scale, g, gid, wgt);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  with_flags(
+      [&](auto kWeighted) {
+        launch(k_readout_seed<kWeighted>, cdiv((int64_t)n * 64, 256), 256, 0, st, n, pre, w, scale, g, gid, wgt);
+      },
+      wgt != nullptr);
 }
 
 // ============================================================================================
 // final geometry backward: forces and virial
 // ============================================================================================
-__device__ __forceinline__ void virial_reduce(const float (&v)[9], double* __restrict__ virial) {
-  __shared__ float red[9][8];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int k = 0; k < 9; k++) {
-    float x = v[k];
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-    if (lane == 0) red[k][warp] = x;
-  }
-  __syncthreads();
-  if (threadIdx.x < 9) {
-    double s = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += (double)red[threadIdx.x][w];
-    atomicAdd(&virial[threadIdx.x], s);
-  }
-}
-
-// kAtomic: also 1/2 v (x) g into both endpoints' rows of the per-atom virial array (atomic_virial.cuh)
+// kAtomic: also 1/2 v (x) g into both endpoints' rows of the per-atom virial array (final_tail.cuh)
 template <bool kAtomic>
 __global__ void __launch_bounds__(256) k_edge_final(int64_t E, const int* __restrict__ e_src,
                                                     const int* __restrict__ e_dst, const int* __restrict__ e_bond,
@@ -1622,40 +1552,21 @@ __global__ void __launch_bounds__(256) k_edge_final(int64_t E, const int* __rest
     }
     const float s = g / v.w;
     gx += s * v.x, gy += s * v.y, gz += s * v.z;
-    // vec = x_dst + off.L - x_src :  dE/dx_dst += g, dE/dx_src -= g ; F = -dE/dx   (pes.py:122-124)
     const int gdst = gid[e_dst[e]], gsrc = gid[e_src[e]];
-    atomicAdd(&forces[(size_t)gdst * 3], -gx);
-    atomicAdd(&forces[(size_t)gdst * 3 + 1], -gy);
-    atomicAdd(&forces[(size_t)gdst * 3 + 2], -gz);
-    atomicAdd(&forces[(size_t)gsrc * 3], gx);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 1], gy);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 2], gz);
-    // strain_bar[a][b] = sum vec[a] g[b]   (pes.py:140-145)
-    vir[0] = v.x * gx, vir[1] = v.x * gy, vir[2] = v.x * gz;
-    vir[3] = v.y * gx, vir[4] = v.y * gy, vir[5] = v.y * gz;
-    vir[6] = v.z * gx, vir[7] = v.z * gy, vir[8] = v.z * gz;
+    scatter_edge(forces, gsrc, gdst, v, make_float3(gx, gy, gz), vir);
     if constexpr (kAtomic) asrc = gsrc, adst = gdst;
   }
-  if constexpr (kAtomic) {
-    float w[9];
-#pragma unroll
-    for (int k = 0; k < 9; k++) w[k] = 0.5f * vir[k];
-    red_add_edge_virial(atom_vir, asrc, adst, w);
-  }
-  virial_reduce(vir, virial);
+  edge_virial_tail<kAtomic>(atom_vir, asrc, adst, vir, virial);
 }
 void launch_edge_final(cudaStream_t st, int64_t E, const int* e_src, const int* e_dst, const int* e_bond,
                        const float4* e_vec, const int* gid, const float* gd, const float* gdb, const float* gbvec,
                        float* forces, double* virial, float* atom_vir) {
-  if (E <= 0) return;
-  if (atom_vir)
-    k_edge_final<true><<<cdiv(E, 256), 256, 0, st>>>(E, e_src, e_dst, e_bond, e_vec, gid, gd, gdb, gbvec, forces, virial,
-                                                     atom_vir);
-  else
-    k_edge_final<false><<<cdiv(E, 256), 256, 0, st>>>(E, e_src, e_dst, e_bond, e_vec, gid, gd, gdb, gbvec, forces, virial,
-                                                      atom_vir);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  with_flags(
+      [&](auto kAtomic) {
+        launch(k_edge_final<kAtomic>, cdiv(E, 256), 256, 0, st, E, e_src, e_dst, e_bond, e_vec, gid, gd, gdb, gbvec,
+               forces, virial, atom_vir);
+      },
+      atom_vir != nullptr);
 }
 
 // kAtomic: also 1/2 v (x) g of this partition's part of g into both endpoints' per-atom virial rows (the bond's
@@ -1676,15 +1587,7 @@ __global__ void __launch_bounds__(256) k_halo_bond_final(int b0, int b1, const i
     const float gx = gbvec[(size_t)b * 3] + s * v.x, gy = gbvec[(size_t)b * 3 + 1] + s * v.y,
                 gz = gbvec[(size_t)b * 3 + 2] + s * v.z;
     const int gdst = gid[b_dst[b]], gsrc = b_src_gid[b];
-    atomicAdd(&forces[(size_t)gdst * 3], -gx);
-    atomicAdd(&forces[(size_t)gdst * 3 + 1], -gy);
-    atomicAdd(&forces[(size_t)gdst * 3 + 2], -gz);
-    atomicAdd(&forces[(size_t)gsrc * 3], gx);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 1], gy);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 2], gz);
-    vir[0] = v.x * gx, vir[1] = v.x * gy, vir[2] = v.x * gz;
-    vir[3] = v.y * gx, vir[4] = v.y * gy, vir[5] = v.y * gz;
-    vir[6] = v.z * gx, vir[7] = v.z * gy, vir[8] = v.z * gz;
+    scatter_edge(forces, gsrc, gdst, v, make_float3(gx, gy, gz), vir);
     if constexpr (kAtomic) {
       float w[9];
 #pragma unroll
@@ -1693,20 +1596,18 @@ __global__ void __launch_bounds__(256) k_halo_bond_final(int b0, int b1, const i
       red_add_virial(atom_vir, gsrc, w);
     }
   }
-  virial_reduce(vir, virial);
+  block_sum_add(vir, virial);
 }
 void launch_halo_bond_final(cudaStream_t st, int b0, int b1, const int* b_src_gid, const int* b_dst,
                             const float4* b_vec, const int* gid, const float* gdb, const float* gbvec, float* forces,
                             double* virial, float* atom_vir) {
   if (b1 <= b0) return;
-  if (atom_vir)
-    k_halo_bond_final<true><<<cdiv(b1 - b0, 256), 256, 0, st>>>(b0, b1, b_src_gid, b_dst, b_vec, gid, gdb, gbvec,
-                                                                forces, virial, atom_vir);
-  else
-    k_halo_bond_final<false><<<cdiv(b1 - b0, 256), 256, 0, st>>>(b0, b1, b_src_gid, b_dst, b_vec, gid, gdb, gbvec,
-                                                                 forces, virial, atom_vir);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  with_flags(
+      [&](auto kAtomic) {
+        launch(k_halo_bond_final<kAtomic>, cdiv(b1 - b0, 256), 256, 0, st, b0, b1, b_src_gid, b_dst, b_vec, gid, gdb,
+               gbvec, forces, virial, atom_vir);
+      },
+      atom_vir != nullptr);
 }
 
 // ============================================================================================
@@ -1727,18 +1628,12 @@ __global__ void k_scatter_add_rows(int n, int w, const int* __restrict__ idx, co
   dst[(size_t)idx[r] * w + c] += src[i];  // to-lists hold unique rows
 }
 void launch_gather_rows(cudaStream_t st, int n, int width, const int* idx, const float* src, float* dst) {
-  if (n <= 0) return;
   const int w4 = width / 4;
-  k_gather_rows<<<cdiv((int64_t)n * w4, 256), 256, 0, st>>>(n, w4, idx, reinterpret_cast<const float4*>(src),
-                                                            reinterpret_cast<float4*>(dst));
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_gather_rows, cdiv((int64_t)n * w4, 256), 256, 0, st, n, w4, idx, reinterpret_cast<const float4*>(src),
+         reinterpret_cast<float4*>(dst));
 }
 void launch_scatter_add_rows(cudaStream_t st, int n, int width, const int* idx, const float* src, float* dst) {
-  if (n <= 0) return;
-  k_scatter_add_rows<<<cdiv((int64_t)n * width, 256), 256, 0, st>>>(n, width, idx, src, dst);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_scatter_add_rows, cdiv((int64_t)n * width, 256), 256, 0, st, n, width, idx, src, dst);
 }
 
 }  // namespace b2m

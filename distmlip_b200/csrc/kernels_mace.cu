@@ -8,7 +8,7 @@
 // (skip_tp) read the element's C x C block per atom; the symmetric contraction is one thread per (atom, channel) that
 // walks the nonzero terms of U, which every channel shares.  Aggregations walk the CSR-by-destination rows (no atomics
 // in the forward); the reverse scatters to sources with atomics.
-#include "atomic_virial.cuh"
+#include "final_tail.cuh"
 #include "mace_cg.cuh"
 #include "mace_state.cuh"
 
@@ -22,15 +22,6 @@ __device__ __forceinline__ float dsilu_f(float x) {
   const float s = sigm(x);
   return s * (1.f + x * (1.f - s));
 }
-
-#define MACE_LAUNCH(kern, nitems, bs, st, ...)                \
-  do {                                                        \
-    if ((nitems) > 0) {                                       \
-      kern<<<cdiv((nitems), (bs)), (bs), 0, st>>>(__VA_ARGS__); \
-      B2M_CK(cudaGetLastError());                             \
-      g_launch_count++;                                       \
-    }                                                         \
-  } while (0)
 
 // ============================================================================================
 // edge geometry: spherical harmonics (oracle/mace_ref.py sh_basis) and Bessel x polynomial cutoff
@@ -552,21 +543,6 @@ __global__ void k_mace_add_row(int n_own, int C, int ld, const float* __restrict
 // ============================================================================================
 // final geometry reverse: dE/dv from the adjoints of the radial basis (g_eb) and of the harmonics (gY)
 // ============================================================================================
-__device__ __forceinline__ void virial_reduce_mace(const float (&v)[9], double* __restrict__ virial) {
-  __shared__ float red[9][8];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int k = 0; k < 9; k++) {
-    float x = v[k];
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-    if (lane == 0) red[k][warp] = x;
-  }
-  __syncthreads();
-  if (threadIdx.x < 9) {
-    double s = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += (double)red[threadIdx.x][w];
-    atomicAdd(&virial[threadIdx.x], s);
-  }
-}
 // kSpecies: the ZBL term (core.zbl) and the chain rule through the Agnesi transform (core.agnesi), switched at run time
 // kWeighted (with kSpecies): the ZBL term times wgt[gid[dst]], the readout weight of the atom its pair energy belongs to;
 // g_eb and gY carry the weights already (they are adjoints of the weighted readouts)
@@ -622,28 +598,12 @@ __global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, con
       const float gy = gY[(size_t)e * kMaceMaxNsh + m];
       hx = fmaf(gy, Yd[m].x, hx), hy = fmaf(gy, Yd[m].y, hy), hz = fmaf(gy, Yd[m].z, hz);
     }
-    const float pr = hx * x + hy * y + hz * z;
-    const float gx = gd * x + (hx - pr * x) * rd, gyv = gd * y + (hy - pr * y) * rd, gz = gd * z + (hz - pr * z) * rd;
-    // vec = x_dst + off.L - x_src :  dE/dx_dst += g, dE/dx_src -= g ; F = -dE/dx
+    const float3 g = unit_vector_chain(gd, make_float3(x, y, z), rd, make_float3(hx, hy, hz));
     const int gdst = gid[e_dst[e]], gsrc = gid[e_src[e]];
-    atomicAdd(&forces[(size_t)gdst * 3], -gx);
-    atomicAdd(&forces[(size_t)gdst * 3 + 1], -gyv);
-    atomicAdd(&forces[(size_t)gdst * 3 + 2], -gz);
-    atomicAdd(&forces[(size_t)gsrc * 3], gx);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 1], gyv);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 2], gz);
-    vir[0] = v.x * gx, vir[1] = v.x * gyv, vir[2] = v.x * gz;
-    vir[3] = v.y * gx, vir[4] = v.y * gyv, vir[5] = v.y * gz;
-    vir[6] = v.z * gx, vir[7] = v.z * gyv, vir[8] = v.z * gz;
+    scatter_edge(forces, gsrc, gdst, v, g, vir);
     if constexpr (kAtomic) asrc = gsrc, adst = gdst;
   }
-  if constexpr (kAtomic) {
-    float w[9];
-#pragma unroll
-    for (int k = 0; k < 9; k++) w[k] = 0.5f * vir[k];
-    red_add_edge_virial(atom_vir, asrc, adst, w);
-  }
-  virial_reduce_mace(vir, virial);
+  edge_virial_tail<kAtomic>(atom_vir, asrc, adst, vir, virial);
 }
 
 }  // namespace
@@ -653,125 +613,115 @@ __global__ void __launch_bounds__(256) k_mace_edge_final(int64_t E, int nsh, con
 // ---------------------------------------------------------------------------------------------
 void launch_mace_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const MaceRadial& rp, int nsh, float* Y,
                            float* eb, const int* e_src, const int* e_dst, const int* type, const MaceCore& core) {
-  if (core.agnesi)
-    MACE_LAUNCH(k_mace_edge_geom<true>, E, 256, st, E, e_vec, rp, nsh, Y, eb, e_src, e_dst, type, core);
-  else
-    MACE_LAUNCH(k_mace_edge_geom<false>, E, 256, st, E, e_vec, rp, nsh, Y, eb, e_src, e_dst, type, core);
+  with_flags(
+      [&](auto kSpecies) {
+        launch(k_mace_edge_geom<kSpecies>, cdiv(E, 256), 256, 0, st, E, e_vec, rp, nsh, Y, eb, e_src, e_dst, type, core);
+      },
+      core.agnesi != 0);
 }
 void launch_mace_zbl(cudaStream_t st, int n_own, const int* row_ptr, const int* e_src, const float4* e_vec,
                      const int* type, const MaceCore& core, float* e_lin) {
-  MACE_LAUNCH(k_mace_zbl, n_own, 128, st, n_own, row_ptr, e_src, e_vec, type, core, e_lin);
+  launch(k_mace_zbl, cdiv(n_own, 128), 128, 0, st, n_own, row_ptr, e_src, e_vec, type, core, e_lin);
 }
 void launch_mace_embed(cudaStream_t st, int n, int C, const int* type, const float* W, float* h0) {
-  MACE_LAUNCH(k_mace_embed, (int64_t)n * C, 256, st, n, C, type, W, h0);
+  launch(k_mace_embed, cdiv((int64_t)n * C, 256), 256, 0, st, n, C, type, W, h0);
 }
 void launch_mace_msg(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
                      const float* Y, const float* u, float* A) {
-  MACE_LAUNCH(k_mace_msg, (int64_t)n_own * C, 256, st, n_own, C, L1, row_ptr, e_src, R, Y, u, A);
+  launch(k_mace_msg, cdiv((int64_t)n_own * C, 256), 256, 0, st, n_own, C, L1, row_ptr, e_src, R, Y, u, A);
 }
 void launch_mace_msg_bwd(cudaStream_t st, int n_own, int C, int L1, const int* row_ptr, const int* e_src, const float* R,
                          const float* Y, const float* u, const float* gA, float* gR, float* gY, float* gu) {
-  MACE_LAUNCH(k_mace_msg_bwd, (int64_t)n_own * C, 256, st, n_own, C, L1, row_ptr, e_src, R, Y, u, gA, gR, gY, gu);
+  launch(k_mace_msg_bwd, cdiv((int64_t)n_own * C, 256), 256, 0, st, n_own, C, L1, row_ptr, e_src, R, Y, u, gA, gR, gY,
+         gu);
 }
 void launch_mace_elem_mix(cudaStream_t st, int n, int C, int L1, int nsh, const int* type, const float* W,
                           const float* in, float* out, bool accum) {
   if (n <= 0) return;
   B2M_REQUIRE(C <= 128, B2M_ERR_INVALID, "mace elem mix: C <= 128");
-  k_mace_elem_mix<<<n, C, 0, st>>>(n, C, L1, nsh, type, W, in, out, accum ? 1 : 0);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_mace_elem_mix, n, C, 0, st, n, C, L1, nsh, type, W, in, out, accum ? 1 : 0);
 }
 void launch_mace_symc(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
                       const MaceTerm* terms, int nterms, const float* w, float* B) {
-  MACE_LAUNCH(k_mace_symc<false>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, nullptr, B);
+  launch(k_mace_symc<false>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w,
+         nullptr, B);
 }
 void launch_mace_symc_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
                           const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA) {
-  MACE_LAUNCH(k_mace_symc<true>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, gB, gA);
+  launch(k_mace_symc<true>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w,
+         gB, gA);
 }
 void launch_mace_readout_lin(cudaStream_t st, int n_own, int C, int ld, const float* h, const float* w, float* e_lin) {
-  MACE_LAUNCH(k_mace_readout_lin, (int64_t)n_own * 32, 256, st, n_own, C, ld, h, w, e_lin);
+  launch(k_mace_readout_lin, cdiv((int64_t)n_own * 32, 256), 256, 0, st, n_own, C, ld, h, w, e_lin);
 }
 void launch_mace_readout_final(cudaStream_t st, int n_own, int C, int H, const float* h, const float* W1, const float* w2,
                                const float* e_lin, const int* type, const double* E0, double scale, double shift,
                                float* pre, double* energy, const int* gid, double* atom_e, const float* wgt) {
-#define MACE_READOUT_FINAL(A, W)                                                                                       \
-  MACE_LAUNCH((k_mace_readout_final<A, W>), (int64_t)n_own * 32, 256, st, n_own, C, H, h, W1, w2, e_lin, type, E0, scale, \
-              shift, pre, energy, gid, atom_e, wgt)
-  if (wgt) {
-    if (atom_e) MACE_READOUT_FINAL(true, true);
-    else MACE_READOUT_FINAL(false, true);
-  } else {
-    if (atom_e) MACE_READOUT_FINAL(true, false);
-    else MACE_READOUT_FINAL(false, false);
-  }
-#undef MACE_READOUT_FINAL
+  with_flags(
+      [&](auto kAtomic, auto kWeighted) {
+        launch(k_mace_readout_final<kAtomic, kWeighted>, cdiv((int64_t)n_own * 32, 256), 256, 0, st, n_own, C, H, h, W1,
+               w2, e_lin, type, E0, scale, shift, pre, energy, gid, atom_e, wgt);
+      },
+      atom_e != nullptr, wgt != nullptr);
 }
 void launch_mace_readout_seed(cudaStream_t st, int n_own, int C, int H, const float* pre, const float* W1,
                               const float* w2, float scale, float* gh, const int* gid, const float* wgt) {
-  if (wgt)
-    MACE_LAUNCH(k_mace_readout_seed<true>, (int64_t)n_own * C, 256, st, n_own, C, H, pre, W1, w2, scale, gh, gid, wgt);
-  else
-    MACE_LAUNCH(k_mace_readout_seed<false>, (int64_t)n_own * C, 256, st, n_own, C, H, pre, W1, w2, scale, gh, gid, wgt);
+  with_flags(
+      [&](auto kWeighted) {
+        launch(k_mace_readout_seed<kWeighted>, cdiv((int64_t)n_own * C, 256), 256, 0, st, n_own, C, H, pre, W1, w2,
+               scale, gh, gid, wgt);
+      },
+      wgt != nullptr);
 }
 void launch_mace_add_row(cudaStream_t st, int n_own, int C, int ld, const float* w, float scale, float* gh,
                          const int* gid, const float* wgt) {
-  if (wgt) MACE_LAUNCH(k_mace_add_row<true>, (int64_t)n_own * C, 256, st, n_own, C, ld, w, scale, gh, gid, wgt);
-  else MACE_LAUNCH(k_mace_add_row<false>, (int64_t)n_own * C, 256, st, n_own, C, ld, w, scale, gh, gid, wgt);
+  with_flags(
+      [&](auto kWeighted) {
+        launch(k_mace_add_row<kWeighted>, cdiv((int64_t)n_own * C, 256), 256, 0, st, n_own, C, ld, w, scale, gh, gid,
+               wgt);
+      },
+      wgt != nullptr);
 }
 void launch_mace_msg_eq(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
                         const float* R, const float* Y, const float* u, float* Am) {
-  if (max_ell == 1) MACE_LAUNCH(k_mace_msg_eq<1>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, Am);
-  else if (max_ell == 2) MACE_LAUNCH(k_mace_msg_eq<2>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, Am);
-  else if (max_ell == 3) MACE_LAUNCH(k_mace_msg_eq<3>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, Am);
-  else throw Error(B2M_ERR_INVALID, "mace message with 0e+1o features: max_ell must be 1..3");
+  B2M_REQUIRE(max_ell >= 1 && max_ell <= 3, B2M_ERR_INVALID, "mace message with 0e+1o features: max_ell must be 1..3");
+  const auto kern = max_ell == 1 ? k_mace_msg_eq<1> : max_ell == 2 ? k_mace_msg_eq<2> : k_mace_msg_eq<3>;
+  launch(kern, cdiv((int64_t)n_own * C, 256), 256, 0, st, n_own, C, row_ptr, e_src, R, Y, u, Am);
 }
 void launch_mace_msg_eq_bwd(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
                             float* R, const float* Y, const float* u, const float* gAm, float* gY, float* gu) {
-  if (max_ell == 1)
-    MACE_LAUNCH(k_mace_msg_eq_bwd<1>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
-  else if (max_ell == 2)
-    MACE_LAUNCH(k_mace_msg_eq_bwd<2>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
-  else if (max_ell == 3)
-    MACE_LAUNCH(k_mace_msg_eq_bwd<3>, (int64_t)n_own * C, 256, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
-  else throw Error(B2M_ERR_INVALID, "mace message with 0e+1o features: max_ell must be 1..3");
+  B2M_REQUIRE(max_ell >= 1 && max_ell <= 3, B2M_ERR_INVALID, "mace message with 0e+1o features: max_ell must be 1..3");
+  const auto kern = max_ell == 1 ? k_mace_msg_eq_bwd<1> : max_ell == 2 ? k_mace_msg_eq_bwd<2> : k_mace_msg_eq_bwd<3>;
+  launch(kern, cdiv((int64_t)n_own * C, 256), 256, 0, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu);
 }
 void launch_mace_elem_mix_rows(cudaStream_t st, int n, int C, int ncomp, int ldi, int ldo, const int* type,
                                const float* W, const float* in, float* out, bool accum) {
   if (n <= 0) return;
   B2M_REQUIRE(C <= 128 && (ncomp == 1 || ncomp == 4), B2M_ERR_INVALID, "mace elem mix: C <= 128, 1 or 4 components");
-  k_mace_elem_mix_rows<<<n, C, 0, st>>>(n, C, ncomp, ldi, ldo, type, W, in, out, accum ? 1 : 0);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_mace_elem_mix_rows, n, C, 0, st, n, C, ncomp, ldi, ldo, type, W, in, out, accum ? 1 : 0);
 }
 void launch_mace_symc_eq(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
                          const MaceTerm* terms, int nterms, const float* w, float* B) {
-  MACE_LAUNCH(k_mace_symc_eq<false>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, nullptr,
-              B);
+  launch(k_mace_symc_eq<false>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms, nterms,
+         w, nullptr, B);
 }
 void launch_mace_symc_eq_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
                              const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA) {
-  MACE_LAUNCH(k_mace_symc_eq<true>, (int64_t)n_own * C, 128, st, n_own, C, nsh, Ktot, type, A, terms, nterms, w, gB, gA);
+  launch(k_mace_symc_eq<true>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms, nterms,
+         w, gB, gA);
 }
+// kSpecies with the pair term or the Agnesi transform; kWeighted with the pair term and readout weights (without the
+// pair term the weights are all in g_eb and gY)
 void launch_mace_edge_final(cudaStream_t st, int64_t E, int nsh, const int* e_src, const int* e_dst, const float4* e_vec,
                             const int* gid, const int* type, const MaceRadial& rp, const MaceCore& core,
                             const float* g_eb, const float* gY, float* forces, double* virial, float* atom_vir,
                             const float* wgt) {
-#define MACE_EDGE_FINAL(A, S, W)                                                                                     \
-  MACE_LAUNCH((k_mace_edge_final<A, S, W>), E, 256, st, E, nsh, e_src, e_dst, e_vec, gid, rp, g_eb, gY, forces, virial, \
-              atom_vir, type, core, wgt)
-  const bool sp = core.zbl || core.agnesi;
-  if (wgt && core.zbl) {  // without the pair term the weights are all in g_eb and gY
-    if (atom_vir) MACE_EDGE_FINAL(true, true, true);
-    else MACE_EDGE_FINAL(false, true, true);
-  } else if (atom_vir) {
-    if (sp) MACE_EDGE_FINAL(true, true, false);
-    else MACE_EDGE_FINAL(true, false, false);
-  } else {
-    if (sp) MACE_EDGE_FINAL(false, true, false);
-    else MACE_EDGE_FINAL(false, false, false);
-  }
-#undef MACE_EDGE_FINAL
+  with_flags(
+      [&](auto kAtomic, auto kSpecies, auto kWeighted) {
+        launch(k_mace_edge_final<kAtomic, kSpecies || kWeighted, kWeighted>, cdiv(E, 256), 256, 0, st, E, nsh, e_src,
+               e_dst, e_vec, gid, rp, g_eb, gY, forces, virial, atom_vir, type, core, wgt);
+      },
+      atom_vir != nullptr, core.zbl || core.agnesi, wgt != nullptr && core.zbl);
 }
 
 }  // namespace b2m

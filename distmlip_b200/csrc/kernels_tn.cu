@@ -15,7 +15,7 @@
 // (channel mixes, scalar MLPs, readout) use the FP32-FFMA tile kernel below.  DESIGN.md 8 lists what comes next.
 #include <math_constants.h>
 
-#include "atomic_virial.cuh"
+#include "final_tail.cuh"
 #include "kernels.cuh"
 
 namespace b2m {
@@ -102,15 +102,6 @@ __device__ __forceinline__ void scale_bwd10(const float* t, float q, const float
 #pragma unroll
   for (int k = 0; k < 10; k++) gin[k] = gout[k] * rq - s * 2.f * nw_of(k) * t[k];
 }
-
-#define TN_LAUNCH(kern, nitems, st, ...)                                   \
-  do {                                                                     \
-    if ((nitems) > 0) {                                                    \
-      kern<<<cdiv((nitems), 256), 256, 0, st>>>(__VA_ARGS__);              \
-      B2M_CK(cudaGetLastError());                                          \
-      g_launch_count++;                                                    \
-    }                                                                      \
-  } while (0)
 
 // ============================================================================================
 // row GEMM  C[z][M,N] = epi(A[z][M,K] @ B[sel(z)][K,N] + bias)      (FP32 FFMA, 128x64 tile, 8x4 per thread)
@@ -619,15 +610,8 @@ __global__ void k_tn_readout_final(int n, int W, const float* __restrict__ hL, c
   if (lane == 0) {
     const float L = a + bL, Gt = sigm(b + bG);
     lout[r] = L, gout[r] = Gt, e_atom[r] = L * Gt;
-    double ev = (double)scale * (double)(L * Gt);
-    if (eref) ev += eref[type[r]];
-    if constexpr (kWeighted) {
-      const double wt = (double)wgt[gid[r]];
-      ev *= wt;
-      mean_per_atom *= wt;
-    }
-    if constexpr (kAtomic) atom_e[gid[r]] = ev + mean_per_atom;
-    atomicAdd(energy, ev);
+    atomicAdd(energy,
+              readout_energy<kAtomic, kWeighted>(r, L * Gt, scale, type, eref, gid, atom_e, mean_per_atom, wgt));
   }
 }
 // adjoints of the last hidden activations of both chains, already times SiLU'(pre) of that layer
@@ -650,22 +634,7 @@ __global__ void k_tn_readout_seed(int n, int W, const float* __restrict__ lout, 
 // ============================================================================================
 // final geometry reverse: gd = g_rbf . drbf/dd + gC C'(d);  g_vec = gd v^ + (gvh - (gvh.v^) v^) / d
 // ============================================================================================
-__device__ __forceinline__ void virial_reduce_tn(const float (&v)[9], double* __restrict__ virial) {
-  __shared__ float red[9][8];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int k = 0; k < 9; k++) {
-    float x = v[k];
-    for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-    if (lane == 0) red[k][warp] = x;
-  }
-  __syncthreads();
-  if (threadIdx.x < 9) {
-    double s = 0.0;
-    for (int w = 0; w < (int)(blockDim.x >> 5); w++) s += (double)red[threadIdx.x][w];
-    atomicAdd(&virial[threadIdx.x], s);
-  }
-}
-// kAtomic: also 1/2 v (x) g into both endpoints' rows of the per-atom virial array (atomic_virial.cuh)
+// kAtomic: also 1/2 v (x) g into both endpoints' rows of the per-atom virial array (final_tail.cuh)
 template <bool kAtomic>
 __global__ void __launch_bounds__(256) k_tn_edge_final(int64_t E, const int* __restrict__ e_src,
                                                        const int* __restrict__ e_dst, const float4* __restrict__ e_vec,
@@ -689,30 +658,13 @@ __global__ void __launch_bounds__(256) k_tn_edge_final(int64_t E, const int* __r
     }
     if (d <= rp.rc) gd = fmaf(gC[e], -0.5f * CUDART_PI_F / rp.rc * __sinf(CUDART_PI_F * d / rp.rc), gd);
     gd_out[e] = gd;
-    const float x = v.x * rd, y = v.y * rd, z = v.z * rd;
-    const float hx = gvh[3 * e], hy = gvh[3 * e + 1], hz = gvh[3 * e + 2];
-    const float pr = hx * x + hy * y + hz * z;
-    const float gx = gd * x + (hx - pr * x) * rd, gy = gd * y + (hy - pr * y) * rd, gz = gd * z + (hz - pr * z) * rd;
-    // vec = x_dst + off.L - x_src :  dE/dx_dst += g, dE/dx_src -= g ; F = -dE/dx   (pes.py:122-124)
+    const float3 g = unit_vector_chain(gd, make_float3(v.x * rd, v.y * rd, v.z * rd), rd,
+                                       make_float3(gvh[3 * e], gvh[3 * e + 1], gvh[3 * e + 2]));
     const int gdst = gid[e_dst[e]], gsrc = gid[e_src[e]];
-    atomicAdd(&forces[(size_t)gdst * 3], -gx);
-    atomicAdd(&forces[(size_t)gdst * 3 + 1], -gy);
-    atomicAdd(&forces[(size_t)gdst * 3 + 2], -gz);
-    atomicAdd(&forces[(size_t)gsrc * 3], gx);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 1], gy);
-    atomicAdd(&forces[(size_t)gsrc * 3 + 2], gz);
-    vir[0] = v.x * gx, vir[1] = v.x * gy, vir[2] = v.x * gz;  // strain_bar[a][b] = sum vec[a] g[b]  (pes.py:140-145)
-    vir[3] = v.y * gx, vir[4] = v.y * gy, vir[5] = v.y * gz;
-    vir[6] = v.z * gx, vir[7] = v.z * gy, vir[8] = v.z * gz;
+    scatter_edge(forces, gsrc, gdst, v, g, vir);
     if constexpr (kAtomic) asrc = gsrc, adst = gdst;
   }
-  if constexpr (kAtomic) {
-    float w[9];
-#pragma unroll
-    for (int k = 0; k < 9; k++) w[k] = 0.5f * vir[k];
-    red_add_edge_virial(atom_vir, asrc, adst, w);
-  }
-  virial_reduce_tn(vir, virial);
+  edge_virial_tail<kAtomic>(atom_vir, asrc, adst, vir, virial);
 }
 
 }  // namespace
@@ -725,111 +677,105 @@ void launch_tn_gemm(cudaStream_t st, const TnGemm& g, int nz) {
   B2M_REQUIRE(g.K % 32 == 0 && g.N % 64 == 0 && g.lda % 4 == 0 && g.ldc % 4 == 0, B2M_ERR_INVALID, "tn gemm shape");
   B2M_REQUIRE(g.epi == 0 || (nz == 1 && (g.epi == 1 ? g.Cpre != nullptr : g.Pre != nullptr)), B2M_ERR_INVALID,
               "tn gemm epilogue");  // the epilogue pointers carry no z offset
-  dim3 grid(cdiv(g.M, 128), g.N / 64, nz);
-  k_tn_gemm<<<grid, 256, 0, st>>>(g);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_tn_gemm, dim3(cdiv(g.M, 128), g.N / 64, nz), 256, 0, st, g);
 }
 void launch_tn_edge_geom(cudaStream_t st, int64_t E, const float4* e_vec, const TnRadial& rp, float* rbf, float* cut) {
-  TN_LAUNCH(k_tn_edge_geom, E * rp.nrp, st, E, e_vec, rp, rbf, cut);
+  launch(k_tn_edge_geom, cdiv(E * rp.nrp, 256), 256, 0, st, E, e_vec, rp, rbf, cut);
 }
 void launch_tn_embed_agg(cudaStream_t st, int n_own, const int* row_ptr, const int* e_src, const int* type,
                          const float* U, const float* V, const float* P, const float* cut, const float4* e_vec,
                          float* T0, float* nr0) {
-  TN_LAUNCH(k_tn_embed_agg, (int64_t)n_own * TC, st, n_own, row_ptr, e_src, type, U, V, P, cut, e_vec, T0, nr0);
+  launch(k_tn_embed_agg, cdiv((int64_t)n_own * TC, 256), 256, 0, st, n_own, row_ptr, e_src, type, U, V, P, cut, e_vec,
+         T0, nr0);
 }
 void launch_tn_layernorm(cudaStream_t st, int rows, int W, const float* x, const float* gamma, const float* beta,
                          float* y, float* stats) {
-  TN_LAUNCH(k_tn_layernorm, (int64_t)rows * 32, st, rows, W, x, gamma, beta, y, stats);
+  launch(k_tn_layernorm, cdiv((int64_t)rows * 32, 256), 256, 0, st, rows, W, x, gamma, beta, y, stats);
 }
 void launch_tn_layernorm_bwd(cudaStream_t st, int rows, int W, const float* x, const float* stats, const float* gamma,
                              const float* gy, float* gx) {
-  TN_LAUNCH(k_tn_layernorm_bwd, (int64_t)rows * 32, st, rows, W, x, stats, gamma, gy, gx);
+  launch(k_tn_layernorm_bwd, cdiv((int64_t)rows * 32, 256), 256, 0, st, rows, W, x, stats, gamma, gy, gx);
 }
 void launch_tn_embed_out(cudaStream_t st, int n, const float* T0m, const float* s2p, float* X0) {
-  TN_LAUNCH(k_tn_embed_out, (int64_t)n * TC, st, n, T0m, s2p, X0);
+  launch(k_tn_embed_out, cdiv((int64_t)n * TC, 256), 256, 0, st, n, T0m, s2p, X0);
 }
 void launch_tn_embed_out_bwd(cudaStream_t st, int n, const float* T0m, const float* s2p, const float* gX0, float* gT0m,
                              float* gs2p) {
-  TN_LAUNCH(k_tn_embed_out_bwd, (int64_t)n * TC, st, n, T0m, s2p, gX0, gT0m, gs2p);
+  launch(k_tn_embed_out_bwd, cdiv((int64_t)n * TC, 256), 256, 0, st, n, T0m, s2p, gX0, gT0m, gs2p);
 }
 void launch_tn_norm_bwd_add(cudaStream_t st, int n, const float* T0, const float* gnr0, float* gT0) {
-  TN_LAUNCH(k_tn_norm_bwd_add, (int64_t)n * TC, st, n, T0, gnr0, gT0);
+  launch(k_tn_norm_bwd_add, cdiv((int64_t)n * TC, 256), 256, 0, st, n, T0, gnr0, gT0);
 }
 void launch_tn_embed_agg_bwd(cudaStream_t st, int64_t E, const int* e_src, const int* e_dst, const int* type,
                              const float* U, const float* V, const float* P, const float* cut, const float4* e_vec,
                              const float* gT0, float* gP, float* gC, float* gvh) {
-  TN_LAUNCH(k_tn_embed_agg_bwd, E * 32, st, E, e_src, e_dst, type, U, V, P, cut, e_vec, gT0, gP, gC, gvh);
+  launch(k_tn_embed_agg_bwd, cdiv(E * 32, 256), 256, 0, st, E, e_src, e_dst, type, U, V, P, cut, e_vec, gT0, gP, gC,
+         gvh);
 }
 void launch_tn_scale(cudaStream_t st, int n, const float* X, float* Xh, float* q) {
-  TN_LAUNCH(k_tn_scale, (int64_t)n * TC, st, n, X, Xh, q);
+  launch(k_tn_scale, cdiv((int64_t)n * TC, 256), 256, 0, st, n, X, Xh, q);
 }
 void launch_tn_scale_bwd(cudaStream_t st, int n, const float* X, const float* q, float* g) {
-  TN_LAUNCH(k_tn_scale_bwd, (int64_t)n * TC, st, n, X, q, g);
+  launch(k_tn_scale_bwd, cdiv((int64_t)n * TC, 256), 256, 0, st, n, X, q, g);
 }
 void launch_tn_msg(cudaStream_t st, int n_own, const int* row_ptr, const int* e_src, const float* f3p, const float* cut,
                    const float* Y, float* msg) {
-  TN_LAUNCH(k_tn_msg, (int64_t)n_own * TC, st, n_own, row_ptr, e_src, f3p, cut, Y, msg);
+  launch(k_tn_msg, cdiv((int64_t)n_own * TC, 256), 256, 0, st, n_own, row_ptr, e_src, f3p, cut, Y, msg);
 }
 void launch_tn_msg_bwd(cudaStream_t st, int n_own, const int* row_ptr, const int* e_src, const float* f3p,
                        const float* cut, const float* Y, const float* gmsg, float* g3, float* gC, float* gY) {
-  TN_LAUNCH(k_tn_msg_bwd, (int64_t)n_own * TC, st, n_own, row_ptr, e_src, f3p, cut, Y, gmsg, g3, gC, gY);
+  launch(k_tn_msg_bwd, cdiv((int64_t)n_own * TC, 256), 256, 0, st, n_own, row_ptr, e_src, f3p, cut, Y, gmsg, g3, gC,
+         gY);
 }
 void launch_tn_prod(cudaStream_t st, int n, const float* msg, const float* Y, int so3, float* Pn) {
-  TN_LAUNCH(k_tn_prod, (int64_t)n * TC, st, n, msg, Y, so3, Pn);
+  launch(k_tn_prod, cdiv((int64_t)n * TC, 256), 256, 0, st, n, msg, Y, so3, Pn);
 }
 void launch_tn_prod_bwd(cudaStream_t st, int n, const float* msg, const float* Y, int so3, const float* gPn,
                         float* gmsg, float* gY) {
-  TN_LAUNCH(k_tn_prod_bwd, (int64_t)n * TC, st, n, msg, Y, so3, gPn, gmsg, gY);
+  launch(k_tn_prod_bwd, cdiv((int64_t)n * TC, 256), 256, 0, st, n, msg, Y, so3, gPn, gmsg, gY);
 }
 void launch_tn_update(cudaStream_t st, int n, const float* Xh, const float* dX, float* Xn) {
-  TN_LAUNCH(k_tn_update, (int64_t)n * TC, st, n, Xh, dX, Xn);
+  launch(k_tn_update, cdiv((int64_t)n * TC, 256), 256, 0, st, n, Xh, dX, Xn);
 }
 void launch_tn_update_bwd(cudaStream_t st, int n, const float* dX, const float* gXn, float* gdX) {
-  TN_LAUNCH(k_tn_update_bwd, (int64_t)n * TC, st, n, dX, gXn, gdX);
+  launch(k_tn_update_bwd, cdiv((int64_t)n * TC, 256), 256, 0, st, n, dX, gXn, gdX);
 }
 void launch_tn_invariants(cudaStream_t st, int n, const float* X, float* inv) {
-  TN_LAUNCH(k_tn_invariants, (int64_t)n * TC, st, n, X, inv);
+  launch(k_tn_invariants, cdiv((int64_t)n * TC, 256), 256, 0, st, n, X, inv);
 }
 void launch_tn_invariants_bwd(cudaStream_t st, int n, const float* X, const float* ginv, float* gX) {
-  TN_LAUNCH(k_tn_invariants_bwd, (int64_t)n * TC, st, n, X, ginv, gX);
+  launch(k_tn_invariants_bwd, cdiv((int64_t)n * TC, 256), 256, 0, st, n, X, ginv, gX);
 }
 void launch_tn_readout_final(cudaStream_t st, int n, int W, const float* hL, const float* wL, float bL, const float* hG,
                              const float* wG, float bG, const int* type, const double* eref, float scale, float* lout,
                              float* gout, float* e_atom, double* energy, const int* gid, double* atom_e,
                              double mean_per_atom, const float* wgt) {
-  const auto k_weighted_atomic = k_tn_readout_final<true, true>;
-  const auto k_weighted = k_tn_readout_final<false, true>;
-  if (wgt && atom_e)
-    TN_LAUNCH(k_weighted_atomic, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout,
-              e_atom, energy, gid, atom_e, mean_per_atom, wgt);
-  else if (wgt)
-    TN_LAUNCH(k_weighted, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout, e_atom,
-              energy, gid, atom_e, mean_per_atom, wgt);
-  else if (atom_e)
-    TN_LAUNCH(k_tn_readout_final<true>, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout,
-              e_atom, energy, gid, atom_e, mean_per_atom, wgt);
-  else
-    TN_LAUNCH(k_tn_readout_final<false>, (int64_t)n * 32, st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout,
-              gout, e_atom, energy, gid, atom_e, mean_per_atom, wgt);
+  with_flags(
+      [&](auto kAtomic, auto kWeighted) {
+        launch(k_tn_readout_final<kAtomic, kWeighted>, cdiv((int64_t)n * 32, 256), 256, 0, st, n, W, hL, wL, bL, hG, wG,
+               bG, type, eref, scale, lout, gout, e_atom, energy, gid, atom_e, mean_per_atom, wgt);
+      },
+      atom_e != nullptr, wgt != nullptr);
 }
 void launch_tn_readout_seed(cudaStream_t st, int n, int W, const float* lout, const float* gout, float scale,
                             const float* wL, const float* wG, const float* preL, const float* preG, float* gL,
                             float* gG, const int* gid, const float* wgt) {
-  if (wgt)
-    TN_LAUNCH(k_tn_readout_seed<true>, (int64_t)n * W, st, n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG, gid,
-              wgt);
-  else
-    TN_LAUNCH(k_tn_readout_seed, (int64_t)n * W, st, n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG, gid, wgt);
+  with_flags(
+      [&](auto kWeighted) {
+        launch(k_tn_readout_seed<kWeighted>, cdiv((int64_t)n * W, 256), 256, 0, st, n, W, lout, gout, scale, wL, wG,
+               preL, preG, gL, gG, gid, wgt);
+      },
+      wgt != nullptr);
 }
 void launch_tn_edge_final(cudaStream_t st, int64_t E, const int* e_src, const int* e_dst, const float4* e_vec,
                           const int* gid, const TnRadial& rp, const float* g_rbf, const float* gC, const float* gvh,
                           float* gd, float* forces, double* virial, float* atom_vir) {
-  if (atom_vir)
-    TN_LAUNCH(k_tn_edge_final<true>, E, st, E, e_src, e_dst, e_vec, gid, rp, g_rbf, gC, gvh, gd, forces, virial, atom_vir);
-  else
-    TN_LAUNCH(k_tn_edge_final<false>, E, st, E, e_src, e_dst, e_vec, gid, rp, g_rbf, gC, gvh, gd, forces, virial,
-              atom_vir);
+  with_flags(
+      [&](auto kAtomic) {
+        launch(k_tn_edge_final<kAtomic>, cdiv(E, 256), 256, 0, st, E, e_src, e_dst, e_vec, gid, rp, g_rbf, gC, gvh, gd,
+               forces, virial, atom_vir);
+      },
+      atom_vir != nullptr);
 }
 
 }  // namespace b2m

@@ -155,10 +155,8 @@ static void launch_gemm_wg_t(cudaStream_t st, const float* A, int lda, const flo
                   al(A, 16) && al(Bcan, 16) && al(C, 8) && al(bias, 8) && al(R, 8) && al(Cpre, 8) && al(Pre, 8),
               B2M_ERR_INVALID, "gemm_wg operand alignment");
   const int ntiles = (M + 127) / 128;
-  const int grid = std::min(ntiles, per_sm * num_sms);
-  k_gemm_wg<K, N, EPI><<<grid, 256, bytes, st>>>(A, lda, Bcan, C, ldc, M, bias, R, ldr, accum ? 1 : 0, Cpre, Pre, ldp);
-  B2M_CK(cudaGetLastError());
-  g_launch_count++;
+  launch(k_gemm_wg<K, N, EPI>, std::min(ntiles, per_sm * num_sms), 256, bytes, st, A, lda, Bcan, C, ldc, M, bias, R, ldr,
+         accum ? 1 : 0, Cpre, Pre, ldp);
 }
 
 template <int EPI>

@@ -131,3 +131,34 @@ def test_group_triclinic_cell():
     assert abs(E.item() - Eo.item()) / len(atoms) < TOL_E
     assert (F - Fo).abs().max().item() < TOL_F and (S - So).abs().max().item() < TOL_S
     dm._engine.close()
+
+
+def _tensornet_potential(devices):
+    from distmlip_b200.implementations.matgl import Potential_Dist, TensorNet_Dist
+    from tests.test_oracle_tensornet import make_tn
+
+    dm = TensorNet_Dist.from_existing(make_tn(seed=6, scale=1.5))
+    dm.enable_distributed_mode(devices)
+    return dm, Potential_Dist(model=dm)
+
+
+@pytest.mark.parametrize("model", ["chgnet", "tensornet"])
+@pytest.mark.parametrize("devices", [[0], [0, 0]])
+def test_launch_count_is_the_kernels_the_device_ran(model, devices, tmp_path):
+    """counts()["launches"] of an evaluation is the number of kernels it ran; in a group every partition's host thread
+    counts its own launches only, however the partitions' evaluations overlap"""
+    import json
+
+    from torch.profiler import ProfilerActivity, profile
+
+    dm, pot = group_potential(devices) if model == "chgnet" else _tensornet_potential(devices)
+    pot(si_diamond(4, nz=8, seed=2))
+    eng = dm._engine
+    eng.compute_resident(1)
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        eng.compute_resident(1)
+    prof.export_chrome_trace(str(tmp_path / "trace.json"))
+    events = json.loads((tmp_path / "trace.json").read_text())["traceEvents"]
+    kernels = sum(1 for ev in events if ev.get("cat") == "kernel")  # memcpy / memset records are other categories
+    assert kernels > 0 and eng.counts()["launches"] == kernels
+    eng.close()
