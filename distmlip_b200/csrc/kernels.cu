@@ -301,16 +301,13 @@ void launch_zero_rows(cudaStream_t st, float* p, int64_t nfloats) {
 // ============================================================================================
 // atom conv: shared pieces of the persistent forward and backward
 // ============================================================================================
-// Both kernels are persistent, one CTA per SM.  In the backward (grid = min(128-edge tiles, SMs)) CTA c takes tiles c,
-// c + grid, c + 2 grid, ...; every tile's A[src] rows arrive by per-row bulk copies into one of two [TM][LDE] buffers,
-// tile number `it` of the CTA in buffer it & 1 (its mbarrier: stage_parity(it)).  The copies of tile it + 1 are issued
-// while tile it is computed; its index loads one tile earlier still, into registers (EdgeRow).  The forward splits the
-// work per warpgroup, over 64-edge tiles (below).
+// Both kernels are persistent, one CTA per SM, and split the work per warpgroup over 64-edge tiles (below): every
+// tile's A[src] rows arrive by per-row bulk copies into the warpgroup's one [TW][LDE] buffer, issued once the previous
+// tile's scatter pass is done with it; the tile's indices load one tile earlier still, into registers (EdgeRow).
 //
-// Every per-element phase works in the accumulator layout (Map).  In the backward warpgroup b owns first-layer columns
-// 64 b .. 64 b + 63 (the hidden columns its branch's second layer reads) and the branch's 64 outputs, and a thread owns
-// 4 rows x 16 columns of both; in the forward a thread owns 2 rows x 16 columns of each branch.  Such a thread touches
-// the tile only at its own positions (row(i), 64 b + col(j)), as float2 pairs
+// Every per-element phase works in the accumulator layout (Map): a thread owns 2 rows x 16 columns of each branch b,
+// whose first-layer columns are 64 b .. 64 b + 63.  Such a thread touches the tile only at its own positions
+// (row(i), 64 b + col(j)), as float2 pairs
 // (col(2 jj), col(2 jj) + 1); the pitch LDE = 136 (8 mod 32 floats) puts the 8 rows x 4 pairs of a half-warp on 32
 // distinct banks.  The line-graph tiles use the same pitch and layout.
 constexpr int LDE = 136;
@@ -652,235 +649,219 @@ void launch_atomconv_fwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
 // ============================================================================================
 // atom conv: backward (recompute forward in-tile, then hand-derived reverse pass)
 // ============================================================================================
-// Shared memory holds one weight image (64 KB) and two [TM][LDE] tiles whose roles alternate: the tile's gathered rows
-// arrive in buffer it & 1, which becomes P: each thread overwrites its own A[src] values with its pre-activations, and
-// later with their adjoints gpre, which the scatter phase reads row-major.  The other buffer is H: the recompute parks
-// the second layer's outputs there at the thread's own positions -- u itself (L), oG = sigm(v) (G) -- so that the
-// reverse keeps one 64-row half of accumulators live at a time and reads its own and its partner's values back.  Both
-// second-layer products take their A operand from registers.  Once g.W2 has read the W2^T image and H is no longer
-// read, both are refilled by bulk copies -- H with the next tile's A[src] rows, the image with W2 -- which land while
-// this tile's scatter phase runs.  The W2^T image is loaded right after the recompute, under the first half's
-// elementwise reverse.  The weight barrier completes two phases per tile (W2^T, then W2), waited on in that order.
+// Laid out like the forward: the two warpgroups of a CTA do not wait for each other.  Warpgroup w of CTA c owns the
+// 64-edge tiles g, g + 2 grid, g + 4 grid, ... (g = 2 c + w) and computes both branches of each.  Each warpgroup has
+// its own [TW][LDE] buffer P, mbarrier, index, distance, be and d be / dd slots and named barrier.  Both weight images
+// (W2 for the recompute, W2^T for g . W2), the radial block and b2 are staged once per CTA behind the only CTA-wide
+// barrier; one buffer per warpgroup is what lets two warpgroups fit next to 128 KB of images.  The tile's A[src] rows
+// arrive in P; each thread overwrites its own A[src] values with the pre-activations, and later with their adjoints
+// gpre, which the scatter pass reads row-major.  A thread holds rows m.row(0), m.row(1) and columns m.col(j) of both
+// branches, so the second layer's outputs -- u (L) and oG = sigm(v + b2) (G), 32 floats each -- stay in registers
+// through the elementwise reverse, which forms dE/du, dE/dv and dE/dw_ab in place over u, oG and w_ab.  The next
+// tile's gather is issued once the scatter pass is done with P, and the other warpgroup's work covers the wait.
+constexpr int WGB = 2, NTB = 128 * WGB;  // warpgroups and threads of a backward CTA
 struct AtomSmemBwd {
-  static constexpr int kBuf = 32;               // two [TM][LDE] tiles (first 128 B: 2 gather mbarriers + weight mbarrier)
-  static constexpr int kW = kBuf + 2 * TM * LDE;  // wgmma image of W2 or W2^T (2 branches x hi | lo, k permuted)
-  static constexpr int kRad = kW + 16384;       // radial block (M, W_ab: AtomConvArgs::radial), staged once
-  static constexpr int kBe = kRad + ATOM_RAD;   // be [TM][8] (k < 8)
-  static constexpr int kDbe = kBe + TM * 8;     // d be / dd [TM][8]
-  static constexpr int kBe8 = kDbe + TM * 8;    // be [TM] (k = 8)
-  static constexpr int kDbe8 = kBe8 + TM;       // d be / dd [TM] (k = 8)
-  static constexpr int kB2 = kDbe8 + TM;
-  static constexpr int kD = kB2 + 128;          // [2][TM]
-  static constexpr int kIdx = kD + 2 * TM;      // src, dst, bond: [2][TM] each
-  static constexpr int kTotal = kIdx + 6 * TM;
+  static constexpr int kTile = 32;                      // [WGB][TW][LDE] buffers P (first 128 B: their mbarriers)
+  static constexpr int kW = kTile + WGB * TW * LDE;     // wgmma images of W2 (2 branches x hi | lo, k permuted) ...
+  static constexpr int kWT = kW + 16384;                // ... and of W2^T, both staged once
+  static constexpr int kRad = kWT + 16384;              // radial block (M, W_ab: AtomConvArgs::radial), staged once
+  static constexpr int kBe = kRad + ATOM_RAD;           // be [WGB][TW][8] (k < 8)
+  static constexpr int kDbe = kBe + WGB * TW * 8;       // d be / dd [WGB][TW][8]
+  static constexpr int kBe8 = kDbe + WGB * TW * 8;      // be [WGB][TW] (k = 8)
+  static constexpr int kDbe8 = kBe8 + WGB * TW;         // d be / dd [WGB][TW] (k = 8)
+  static constexpr int kB2 = kDbe8 + WGB * TW;
+  static constexpr int kD = kB2 + 128;                  // d [WGB][TW]
+  static constexpr int kIdx = kD + WGB * TW;            // src, dst, bond: [WGB][TW] each
+  static constexpr int kTotal = kIdx + 3 * WGB * TW;
   static constexpr size_t bytes = (size_t)kTotal * 4;
 };
 static_assert(AtomSmemBwd::bytes <= 232448, "atom-conv backward shared memory");
-static_assert(AtomSmemBwd::kW % 4 == 0 && AtomSmemBwd::kRad % 4 == 0 && AtomSmemBwd::kBe % 4 == 0 &&
-                  AtomSmemBwd::kDbe % 4 == 0,
-              "16-byte aligned images and radial rows");
+static_assert(AtomSmemBwd::kW % 4 == 0 && AtomSmemBwd::kWT % 4 == 0 && AtomSmemBwd::kRad % 4 == 0 &&
+                  AtomSmemBwd::kBe % 4 == 0 && AtomSmemBwd::kDbe % 4 == 0 && AtomSmemBwd::kIdx % 4 == 0,
+              "16-byte aligned images, radial rows and index slots");
 
-__global__ void __launch_bounds__(NT, 1) k_atomconv_bwd(const AtomConvArgs a) {
+__global__ void __launch_bounds__(NTB, 1) k_atomconv_bwd(const AtomConvArgs a) {
   extern __shared__ __align__(128) float smem[];
-  uint64_t* gbar = reinterpret_cast<uint64_t*>(smem);  // [2]: gather buffers
-  uint64_t* wbar = gbar + 2;                            // weight image
-  float* Wsm = smem + AtomSmemBwd::kW;
-  float* rad_base = smem + AtomSmemBwd::kRad;
-  float* be_s = smem + AtomSmemBwd::kBe;
-  float* dbe_s = smem + AtomSmemBwd::kDbe;
-  float* be8 = smem + AtomSmemBwd::kBe8;
-  float* dbe8 = smem + AtomSmemBwd::kDbe8;
-  float* b2s = smem + AtomSmemBwd::kB2;
+  const int tid = threadIdx.x, w = tid >> 7, lr = tid & 127;  // warpgroup; thread lr < TW gathers row lr
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem) + w;      // this warpgroup's buffer
+  const float* W2s = smem + AtomSmemBwd::kW;
+  const float* W2Ts = smem + AtomSmemBwd::kWT;
+  const float* rad_base = smem + AtomSmemBwd::kRad;
+  const float* b2s = smem + AtomSmemBwd::kB2;
+  float* P = smem + AtomSmemBwd::kTile + w * TW * LDE;
+  float* be_s = smem + AtomSmemBwd::kBe + w * TW * 8;
+  float* dbe_s = smem + AtomSmemBwd::kDbe + w * TW * 8;
+  float* be8 = smem + AtomSmemBwd::kBe8 + w * TW;
+  float* dbe8 = smem + AtomSmemBwd::kDbe8 + w * TW;
+  float* s_d = smem + AtomSmemBwd::kD + w * TW;
+  int* s_src = reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + w * TW;
+  int* s_dst = reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + (WGB + w) * TW;
+  int* s_bond = reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + (2 * WGB + w) * TW;
 
-  const int tid = threadIdx.x;
-  const int64_t ntiles = (a.E + TM - 1) / TM, step = gridDim.x;
+  const int64_t ntiles = (a.E + TW - 1) / TW, first = WGB * (int64_t)blockIdx.x + w, step = WGB * (int64_t)gridDim.x;
   const bool useQ = a.Qproj != nullptr;
-  auto buf_of = [&](int s) { return smem + AtomSmemBwd::kBuf + s * TM * LDE; };
-  auto d_of = [&](int s) { return smem + AtomSmemBwd::kD + s * TM; };
-  auto src_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + s * TM; };
-  auto dst_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + (2 + s) * TM; };
-  auto bond_of = [&](int s) { return reinterpret_cast<int*>(smem + AtomSmemBwd::kIdx) + (4 + s) * TM; };
-
   if (tid == 0) {
-    mbar_init(&gbar[0], 1);
-    mbar_init(&gbar[1], 1);
-    mbar_init(wbar, 1);
+    for (int i = 0; i < WGB; i++) mbar_init(reinterpret_cast<uint64_t*>(smem) + i, 1);
     fence_barrier_init();
   }
-  EdgeRow nxt = edge_row(a, (int64_t)blockIdx.x * TM + tid, threadIdx.x < TM);
-  stage_w(rad_base, a.radial, ATOM_RAD / 4);
-  if (tid < 128) b2s[tid] = a.b2[tid];
+  EdgeRow nxt = edge_row(a, first * TW + lr, lr < TW);
+  // loop-invariant operands, once per CTA
+  stage_w<NTB>(smem + AtomSmemBwd::kW, a.W2can, 4096);
+  stage_w<NTB>(smem + AtomSmemBwd::kWT, a.W2Tcan, 4096);
+  stage_w<NTB>(smem + AtomSmemBwd::kRad, a.radial, ATOM_RAD / 4);
+  if (tid < 128) smem[AtomSmemBwd::kB2 + tid] = a.b2[tid];
   __syncthreads();
-  if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
-  issue_gather<TM>(a, blockIdx.x, nxt, tid, buf_of(0), &gbar[0], src_of(0), dst_of(0), bond_of(0), d_of(0));
-  nxt = edge_row(a, ((int64_t)blockIdx.x + step) * TM + tid, threadIdx.x < TM);
-  uint32_t wpar = 0;
+  if (first < ntiles)  // the last CTA's second warpgroup has no tile when the tile count is odd
+    issue_gather<TW>(a, first, nxt, lr, P, mbar, s_src, s_dst, s_bond, s_d);
+  nxt = edge_row(a, (first + step) * TW + lr, lr < TW);
 
   const Map m;
-  const int c0 = 64 * m.branch;  // this warpgroup's first-layer columns
+  Map mL = m, mG = m;  // the first layer's columns and radial image of each branch
+  mL.branch = 0;
+  mG.branch = 1;
   int it = 0;
-  for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
-    float* rad = rad_base;
-    asm volatile("" : "+l"(rad));  // radial addresses formed per tile: hoisted out of the loop they cost 7 registers
-    const int s = it & 1;
-    float* tileP = buf_of(s);
-    float* tileH = buf_of(s ^ 1);
-    const int* s_src = src_of(s);
-    const int* s_dst = dst_of(s);
-    const int* s_bond = bond_of(s);
-    const int64_t e0 = t * TM;
-    const int nvalid = (int)min((int64_t)TM, a.E - e0);
-    __syncthreads();  // the previous tile's scatter phase is done with tileH (its P) and be8
-    radial_rows<TM>(a, d_of(s), nvalid, be_s, be8, dbe_s, dbe8);
-    mbar_wait(&gbar[s], stage_parity(it));
-    mbar_wait(wbar, wpar);  // W2
-    wpar ^= 1;
-    __syncthreads();
-    // recompute, per 64-row half: pre (kept in P at the thread's own positions), silu(pre) . W2^T + b2 = u (L) / v (G),
-    // parked in H at the thread's own positions as u (L) and oG = sigm(v) (G).  acc holds one half at a time.
-    float acc[AR][AC];
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      first_layer_half(a, m, h, tileP, s_dst, s_bond, be_s, be8, rad, nvalid, acc);
+  for (int64_t t = first; t < ntiles; t += step, it++) {
+    const float* rad = rad_base;
+    asm volatile("" : "+l"(rad));  // radial addresses formed per tile: hoisted out of the loop they hold registers
+    const int64_t e0 = t * TW;
+    const int nvalid = (int)min((int64_t)TW, a.E - e0);
+    wg_sync(w);  // the tile's indices and distances are published
+    radial_rows<TW>(a, s_d, nvalid, be_s, be8, dbe_s, dbe8);
+    mbar_wait(mbar, (uint32_t)it & 1u);
+    wg_sync(w);
+    // recompute, per branch: pre (kept in P at the thread's own positions), silu(pre) . W2^T + b2 = u (L) / v (G);
+    // L keeps u, G keeps oG = sigm(v)
+    float L[2][AC], G[2][AC];
+    auto recompute = [&](const Map& mb, float(&x)[2][AC]) {
+      first_layer_half(a, mb, 0, P, s_dst, s_bond, be_s, be8, rad, nvalid, x);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++)
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
-          float* p = tileP + m.row(2 * h + ii) * LDE + c0 + m.col(2 * jj);
-          float& x0 = acc[2 * h + ii][2 * jj];
-          float& x1 = acc[2 * h + ii][2 * jj + 1];
-          st_f2(p, x0, x1);
+          float& x0 = x[ii][2 * jj];
+          float& x1 = x[ii][2 * jj + 1];
+          st_f2(P + m.row(ii) * LDE + 64 * mb.branch + m.col(2 * jj), x0, x1);
           x0 = silu_f(x0);
           x1 = silu_f(x1);
         }
-      wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
+      wg_mm64_acc(x, 0, W2s + mb.branch * 8192, x);
+    };
+    recompute(mL, L);
 #pragma unroll
-      for (int ii = 0; ii < 2; ii++)
+    for (int ii = 0; ii < 2; ii++)
 #pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++) {
-          const float u0 = acc[2 * h + ii][2 * jj] + b2s[m.branch * 64 + m.col(2 * jj)];
-          const float u1 = acc[2 * h + ii][2 * jj + 1] + b2s[m.branch * 64 + m.col(2 * jj + 1)];
-          st_f2(tileH + m.row(2 * h + ii) * LDE + c0 + m.col(2 * jj), m.branch == 0 ? u0 : sigm(u0),
-                m.branch == 0 ? u1 : sigm(u1));
-        }
+      for (int j = 0; j < AC; j++) L[ii][j] += b2s[m.col(j)];
+    recompute(mG, G);
+#pragma unroll
+    for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+      for (int j = 0; j < AC; j++) G[ii][j] = sigm(G[ii][j] + b2s[64 + m.col(j)]);
+    // elementwise reverse, in place: L <- dE/du, G <- dE/dv, w <- w_ab = be.W_ab^T (tensor cores) <- dE/dw_ab.  Both
+    // rows' 16 dE/dagg values are loaded before any is used.
+    int dst[2];
+    float2 gm2[2][AC / 2];
+#pragma unroll
+    for (int ii = 0; ii < 2; ii++) {
+      dst[ii] = s_dst[m.row(ii)];
+      const float* gp = a.gagg + (size_t)max(dst[ii], 0) * D + m.cb;
+#pragma unroll
+      for (int jj = 0; jj < AC / 2; jj++)
+        gm2[ii][jj] = dst[ii] >= 0 ? __ldg(reinterpret_cast<const float2*>(gp + 8 * jj)) : make_float2(0.f, 0.f);
     }
-    __syncthreads();  // the W2 image is no longer needed; H holds both branches' values
-    if (tid == 0) bulk_g2s_image(Wsm, a.W2Tcan, 16384 * 4, wbar);
-    // reverse, per 64-row half.  Elementwise: acc = dE/du (L) / dE/dv (G), from the values parked in H (the partner's
-    // sigm(v) / silu(u) formed from them) and w_ab = be.W_ab^T from the tensor cores.  sd[i]: this thread's share of
-    // dE/dd of row m.row(i); branch 0 adds sum_c dE/dw_ab[r][c] (dbe.W_ab^T)[r][c] over its columns.  Then ghid =
-    // [gu @ W2L, gv @ W2G] and gpre = ghid * dsilu(pre), into P at the thread's own positions; rows fed by M (not bond
-    // rows fed by Q) add sum_j gpre[r][j] (dbe.M^T)[r][j] over this warpgroup's columns to sd.
-    float sd[AR];
+    float wv[32];
+    radial_mma(m, 0, be_s, rad + ATOM_RAD_WAB, wv);
 #pragma unroll
-    for (int h = 0; h < 2; h++) {
-      int dst[2];
-      float2 gm2[2][AC / 2];  // both rows' 16 dE/dagg values, loaded before any is used
+    for (int ii = 0; ii < 2; ii++) {
+      const float b8 = be8[m.row(ii)];
 #pragma unroll
-      for (int ii = 0; ii < 2; ii++) {
-        dst[ii] = s_dst[m.row(2 * h + ii)];
-        const float* gp = a.gagg + (size_t)max(dst[ii], 0) * D + m.cb;
+      for (int jj = 0; jj < AC / 2; jj++) {
+        const float2 wk2 = ld_f2(rad + ATOM_RAD_WAB8 + m.col(2 * jj));
 #pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++)
-          gm2[ii][jj] = dst[ii] >= 0 ? __ldg(reinterpret_cast<const float2*>(gp + 8 * jj)) : make_float2(0.f, 0.f);
-      }
-      float w[32];  // w_ab, then (branch 0) dE/dw_ab in place
-      radial_mma(m, h, be_s, rad + ATOM_RAD_WAB, w);
-#pragma unroll
-      for (int ii = 0; ii < 2; ii++) {
-        const int i = 2 * h + ii;
-        const int r = m.row(i);
-        const float b8 = be8[r];
-#pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++) {
-          const float2 ow2 = ld_f2(tileH + r * LDE + c0 + m.col(2 * jj));         // u (L) / oG (G)
-          const float2 pt2 = ld_f2(tileH + r * LDE + (64 - c0) + m.col(2 * jj));  // the partner's
-          const float2 wk2 = ld_f2(rad + ATOM_RAD_WAB8 + m.col(2 * jj));
-#pragma unroll
-          for (int e = 0; e < 2; e++) {
-            const int j = 2 * jj + e;
-            const float x = e ? ow2.y : ow2.x;
-            const float pt = e ? pt2.y : pt2.x;
-            const float gm = e ? gm2[ii][jj].y : gm2[ii][jj].x;
-            const float wab = fmaf(b8, e ? wk2.y : wk2.x, w[fq(ii, j)]);
-            float g = 0.f, gwv = 0.f;
-            if (dst[ii] >= 0) {
-              if (m.branch == 0) {
-                const float sg = sigm(x);
-                const float oL = x * sg;
-                gwv = gm * oL * pt;  // d/d w_ab
-                g = gm * pt * wab * (sg * (1.f + x * (1.f - sg)));  // d/du
-              } else {
-                const float oL = silu_f(pt);
-                g = gm * oL * wab * x * (1.f - x);  // d/dv
-              }
-            }
-            acc[i][j] = g;
-            w[fq(ii, j)] = gwv;
+        for (int e = 0; e < 2; e++) {
+          const int j = 2 * jj + e;
+          const float u = L[ii][j], oG = G[ii][j];
+          const float gm = e ? gm2[ii][jj].y : gm2[ii][jj].x;
+          const float wab = fmaf(b8, e ? wk2.y : wk2.x, wv[fq(ii, j)]);
+          float gu = 0.f, gv = 0.f, gwv = 0.f;
+          if (dst[ii] >= 0) {
+            const float sg = sigm(u);
+            const float oL = u * sg;
+            gwv = gm * oL * oG;                                 // d/d w_ab
+            gu = gm * oG * wab * (sg * (1.f + u * (1.f - sg)));  // d/du
+            gv = gm * oL * wab * oG * (1.f - oG);                // d/dv
           }
+          L[ii][j] = gu;
+          G[ii][j] = gv;
+          wv[fq(ii, j)] = gwv;
         }
       }
-      sd[2 * h] = sd[2 * h + 1] = 0.f;
-      if (m.branch == 0) {
-        float dw[32];
-        radial_mma(m, h, dbe_s, rad + ATOM_RAD_WAB, dw);
+    }
+    // dE/dd of row m.row(ii), one sum per branch over this thread's columns: branch 0 sum_c dE/dw_ab[r][c]
+    // (dbe.W_ab^T)[r][c]; rows fed by M (not bond rows fed by Q) add sum_j gpre[r][j] (dbe.M^T)[r][j] of each branch
+    float sd[AR];  // [2 b + ii]
+    {
+      float dw[32];
+      radial_mma(m, 0, dbe_s, rad + ATOM_RAD_WAB, dw);
 #pragma unroll
-        for (int ii = 0; ii < 2; ii++) {
-          const float db8 = dbe8[m.row(2 * h + ii)];
+      for (int ii = 0; ii < 2; ii++) {
+        const float db8 = dbe8[m.row(ii)];
+        float s = 0.f;
 #pragma unroll
-          for (int j = 0; j < AC; j++)
-            sd[2 * h + ii] = fmaf(w[fq(ii, j)], fmaf(db8, rad[ATOM_RAD_WAB8 + m.col(j)], dw[fq(ii, j)]), sd[2 * h + ii]);
-        }
+        for (int j = 0; j < AC; j++) s = fmaf(wv[fq(ii, j)], fmaf(db8, rad[ATOM_RAD_WAB8 + m.col(j)], dw[fq(ii, j)]), s);
+        sd[ii] = s;
+        sd[2 + ii] = 0.f;
       }
-      if (h == 0) mbar_wait(wbar, wpar);  // W2^T
-      wg_mm64_acc(acc, h, Wsm + m.branch * 8192, acc);
+    }
+    // per branch: gpre = (g . W2) * dsilu(pre), into P at the thread's own positions
+    auto reverse = [&](const Map& mb, float(&x)[2][AC]) {
+      const int c0 = 64 * mb.branch;
+      wg_mm64_acc(x, 0, W2Ts + mb.branch * 8192, x);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++)
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
-          float* p = tileP + m.row(2 * h + ii) * LDE + c0 + m.col(2 * jj);
+          float* p = P + m.row(ii) * LDE + c0 + m.col(2 * jj);
           const float2 pre = ld_f2(p);
-          float& x0 = acc[2 * h + ii][2 * jj];
-          float& x1 = acc[2 * h + ii][2 * jj + 1];
+          float& x0 = x[ii][2 * jj];
+          float& x1 = x[ii][2 * jj + 1];
           x0 *= dsilu_f(pre.x);
           x1 *= dsilu_f(pre.y);
           st_f2(p, x0, x1);
         }
       float dm[32];
-      radial_mma(m, h, dbe_s, rad + ATOM_RAD_M + 1024 * m.branch, dm);
+      radial_mma(m, 0, dbe_s, rad + ATOM_RAD_M + 1024 * mb.branch, dm);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++) {
-        const int r = m.row(2 * h + ii);
+        const int r = m.row(ii);
         const float db8 = dbe8[r];
         float s = 0.f;
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
           const float2 mk = ld_f2(rad + ATOM_RAD_M8 + c0 + m.col(2 * jj));
-          s = fmaf(acc[2 * h + ii][2 * jj], fmaf(db8, mk.x, dm[fq(ii, 2 * jj)]), s);
-          s = fmaf(acc[2 * h + ii][2 * jj + 1], fmaf(db8, mk.y, dm[fq(ii, 2 * jj + 1)]), s);
+          s = fmaf(x[ii][2 * jj], fmaf(db8, mk.x, dm[fq(ii, 2 * jj)]), s);
+          s = fmaf(x[ii][2 * jj + 1], fmaf(db8, mk.y, dm[fq(ii, 2 * jj + 1)]), s);
         }
-        if (r < nvalid && !(useQ && s_bond[r] >= 0)) sd[2 * h + ii] += s;
+        if (r < nvalid && !(useQ && s_bond[r] >= 0)) sd[2 * mb.branch + ii] += s;
       }
-    }
-    wpar ^= 1;
-    fence_proxy_async_smem();  // this thread's generic accesses of tileH come before its bulk refill
-    __syncthreads();           // tileH and the W2^T image are free; P holds gpre
-    if (t + step < ntiles) {
-      if (tid == 0) bulk_g2s_image(Wsm, a.W2can, 16384 * 4, wbar);
-      issue_gather<TM>(a, t + step, nxt, tid, tileH, &gbar[s ^ 1], src_of(s ^ 1), dst_of(s ^ 1), bond_of(s ^ 1), d_of(s ^ 1));
-      nxt = edge_row(a, (t + 2 * step) * TM + tid, threadIdx.x < TM);
-    }
-    // ---- scatter phase (reads P, be8 and this tile's index arrays only) ----
-    {  // d E / d d_e: sd summed over the 4 lanes of a row, and across the warpgroups through be8
+    };
+    reverse(mL, L);
+    reverse(mG, G);
+    {  // quad_row_sum: lane l gets branch l >> 1's sum of row m.row(l & 1); then branch 0's + branch 1's
       const float v = quad_row_sum(sd);
-      const int r = m.row(tid & 3);
-      if (m.branch == 1) be8[r] = v;  // be8 is free until the next tile
-      __syncthreads();
-      if (m.branch == 0 && r < nvalid) a.gd[e0 + r] += v + be8[r];
+      const float v1 = __shfl_xor_sync(0xffffffffu, v, 2);
+      const int r = m.row(tid & 1);
+      if ((tid & 2) == 0 && r < nvalid) a.gd[e0 + r] += v + v1;
     }
+    wg_sync(w);  // P holds the tile's gpre
     // gC[dst] += gpre (segmented), gA[src] += gpre, gQ[bond] = gpre (each bond row occurs once): one pass over P
-    scatter_rows<32>(tileP, s_dst, a.gA != nullptr ? a.gC : nullptr, nullptr, nullptr, s_src, a.gA, s_bond,
-                     useQ ? a.gQ : nullptr);
+    scatter_rows<32, TW, 128>(P, s_dst, a.gA != nullptr ? a.gC : nullptr, nullptr, nullptr, s_src, a.gA, s_bond,
+                              useQ ? a.gQ : nullptr);
+    fence_proxy_async_smem();  // this thread's generic accesses of the buffer come before its bulk refill
+    wg_sync(w);                // the warpgroup is done with the buffer, the indices and the radial slots
+    if (t + step < ntiles) {
+      issue_gather<TW>(a, t + step, nxt, lr, P, mbar, s_src, s_dst, s_bond, s_d);
+      nxt = edge_row(a, (t + 2 * step) * TW + lr, lr < TW);
+    }
   }
 }
 
@@ -890,7 +871,7 @@ void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
   if (auto once_ = attr.first(); once_) {
     B2M_CK(cudaFuncSetAttribute(k_atomconv_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)AtomSmemBwd::bytes));
   }
-  launch(k_atomconv_bwd, std::min(cdiv(a.E, TM), num_sms), NT, AtomSmemBwd::bytes, st, a);
+  launch(k_atomconv_bwd, std::min(cdiv(cdiv(a.E, TW), WGB), num_sms), NTB, AtomSmemBwd::bytes, st, a);
 }
 
 // ============================================================================================
