@@ -1,10 +1,10 @@
-// kernel_shim.cu -- test-only C entry points into the shipped CHGNet hot-path launchers and the MACE launchers
-// (mace_state.cuh) of libb200mlip.so.
+// kernel_shim.cu -- test-only C entry points into the shipped CHGNet hot-path launchers, the MACE launchers
+// (mace_state.cuh) and the TensorNet launchers (kernels.cuh) of libb200mlip.so.
 //
-// tests/test_gpu_kernel_units.py and tests/test_gpu_mace_units.py build this file into a temporary directory (tests/kernel_units_ref.py: build_shim)
-// and calls it through ctypes.  Each entry point fills the launcher's argument struct from device pointers (torch
-// tensors), a stream handle and a num_sms value, calls the launcher, and returns 0 or the b2m::Error code with its
-// message; the weight-image entry points run the engine's own host formatters (engine.cu) on host buffers, and the MACE
+// tests/test_gpu_kernel_units.py, tests/test_gpu_mace_units.py and tests/test_gpu_tn_units.py build this file into a
+// temporary directory (tests/kernel_units_ref.py: build_shim) and call it through ctypes.  Each entry point fills the
+// launcher's argument struct from device pointers (torch tensors), a stream handle and a num_sms value, calls the
+// launcher, and returns 0 or the b2m::Error code with its message; the weight-image entry points run the engine's own host formatters (engine.cu) on host buffers, and the MACE
 // host entry points the engine's own conv-path list and symmetric-contraction term builder (engine_mace.inl).  The shim
 // does no arithmetic of its own.
 #include <algorithm>
@@ -58,6 +58,13 @@ b2m::MaceCore mace_core(const float* elem, int zbl, int agnesi, int zp, const fl
   for (int k = 0; k < 4; k++) c.zc[k] = cf[1 + k];
   c.zscale = cf[5], c.aq = cf[6], c.ap = cf[7], c.aa = cf[8];
   return c;
+}
+// TnRadial from nr, the row pitch nrp, width, rc and the nr centres mu (host); centres past nr are 0 as the engine sets them
+b2m::TnRadial tn_radial(int nr, int nrp, float width, float rc, const float* mu) {
+  b2m::TnRadial rp{};
+  rp.nr = nr, rp.nrp = nrp, rp.width = width, rp.rc = rc;
+  for (int k = 0; k < 64; k++) rp.mu[k] = k < nr ? mu[k] : 0.f;
+  return rp;
 }
 }  // namespace
 
@@ -248,6 +255,139 @@ int shim_mace_sym_terms(const float* U, int nsh, int nu, int ncomp, int K, int k
     const auto t = b2m::mace_sym_terms(U, nsh, nu, ncomp, K, kg0);
     *n = (int)t.size();
     memcpy(out, t.data(), std::min(t.size(), (size_t)cap) * sizeof(b2m::MaceTerm));
+  });
+}
+
+// ---------------------------------------------------------------------------------------------- TensorNet (kernels.cuh)
+int shim_tn_gemm(void* st, const float* A, int lda, int64_t zA, const float* B0, const float* B1, const float* B2,
+                 int bsel, float* C, int ldc, int64_t zC, float* Cpre, const float* Pre, int ldp, const float* bias, int M,
+                 int N, int K, int accum, int epi, int nz, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::TnGemm g;
+    g.A = A, g.lda = lda, g.zA = zA, g.B0 = B0, g.B1 = B1, g.B2 = B2, g.bsel = bsel;
+    g.C = C, g.ldc = ldc, g.zC = zC, g.Cpre = Cpre, g.Pre = Pre, g.ldp = ldp, g.bias = bias;
+    g.M = M, g.N = N, g.K = K, g.accum = accum, g.epi = epi;
+    b2m::launch_tn_gemm((cudaStream_t)st, g, nz);
+  });
+}
+int shim_tn_edge_geom(void* st, int64_t E, const float* e_vec, int nr, int nrp, float width, float rc, const float* mu,
+                      float* rbf, float* cut, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_tn_edge_geom((cudaStream_t)st, E, reinterpret_cast<const float4*>(e_vec),
+                             tn_radial(nr, nrp, width, rc, mu), rbf, cut);
+  });
+}
+// bwd = 0: launch_tn_embed_agg (T0 =, nr0 =) over n_own rows; bwd = 1: launch_tn_embed_agg_bwd over E edges
+// (gP =, gC +=, gvh =)
+int shim_tn_embed_agg(void* st, int bwd, int n_own, int64_t E, const int* row_ptr, const int* e_src, const int* e_dst,
+                      const int* type, const float* U, const float* V, const float* P, const float* cut,
+                      const float* e_vec, float* T0, float* nr0, const float* gT0, float* gP, float* gC, float* gvh,
+                      char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    const auto* ev = reinterpret_cast<const float4*>(e_vec);
+    if (bwd)
+      b2m::launch_tn_embed_agg_bwd((cudaStream_t)st, E, e_src, e_dst, type, U, V, P, cut, ev, gT0, gP, gC, gvh);
+    else
+      b2m::launch_tn_embed_agg((cudaStream_t)st, n_own, row_ptr, e_src, type, U, V, P, cut, ev, T0, nr0);
+  });
+}
+// bwd = 0: y =, stats =; bwd = 1: gx = (gy and stats read)
+int shim_tn_layernorm(void* st, int bwd, int rows, int W, const float* x, const float* gamma, const float* beta,
+                      float* y, float* stats, const float* gy, float* gx, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_tn_layernorm_bwd((cudaStream_t)st, rows, W, x, stats, gamma, gy, gx);
+    else
+      b2m::launch_tn_layernorm((cudaStream_t)st, rows, W, x, gamma, beta, y, stats);
+  });
+}
+// bwd = 0: X0 =; bwd = 1: gT0m =, gs2p =
+int shim_tn_embed_out(void* st, int bwd, int n, const float* T0m, const float* s2p, float* X0, const float* gX0,
+                      float* gT0m, float* gs2p, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_tn_embed_out_bwd((cudaStream_t)st, n, T0m, s2p, gX0, gT0m, gs2p);
+    else
+      b2m::launch_tn_embed_out((cudaStream_t)st, n, T0m, s2p, X0);
+  });
+}
+int shim_tn_norm_bwd_add(void* st, int n, const float* T0, const float* gnr0, float* gT0, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] { b2m::launch_tn_norm_bwd_add((cudaStream_t)st, n, T0, gnr0, gT0); });
+}
+// bwd = 0: Xh =, q =; bwd = 1: g overwritten with the adjoint of X (q read)
+int shim_tn_scale(void* st, int bwd, int n, const float* X, float* Xh, float* q, float* g, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_tn_scale_bwd((cudaStream_t)st, n, X, q, g);
+    else
+      b2m::launch_tn_scale((cudaStream_t)st, n, X, Xh, q);
+  });
+}
+// bwd = 0: msg =; bwd = 1: g3 =, gC +=, gY += (red.add into source rows)
+int shim_tn_msg(void* st, int bwd, int n_own, const int* row_ptr, const int* e_src, const float* f3p, const float* cut,
+                const float* Y, float* out, const float* gmsg, float* g3, float* gC, float* gY, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_tn_msg_bwd((cudaStream_t)st, n_own, row_ptr, e_src, f3p, cut, Y, gmsg, g3, gC, gY);
+    else
+      b2m::launch_tn_msg((cudaStream_t)st, n_own, row_ptr, e_src, f3p, cut, Y, out);
+  });
+}
+// bwd = 0: Pn =; bwd = 1: gmsg =, gY =
+int shim_tn_prod(void* st, int bwd, int n, const float* m, const float* Y, int so3, float* Pn, const float* gPn,
+                 float* gmsg, float* gY, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_tn_prod_bwd((cudaStream_t)st, n, m, Y, so3, gPn, gmsg, gY);
+    else
+      b2m::launch_tn_prod((cudaStream_t)st, n, m, Y, so3, Pn);
+  });
+}
+// bwd = 0: Xn =; bwd = 1: gdX = (Xh unused)
+int shim_tn_update(void* st, int bwd, int n, const float* Xh, const float* dX, float* Xn, const float* gXn, float* gdX,
+                   char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_tn_update_bwd((cudaStream_t)st, n, dX, gXn, gdX);
+    else
+      b2m::launch_tn_update((cudaStream_t)st, n, Xh, dX, Xn);
+  });
+}
+// bwd = 0: inv =; bwd = 1: gX =
+int shim_tn_invariants(void* st, int bwd, int n, const float* X, float* inv, const float* ginv, float* gX, char* msg,
+                       int msglen) {
+  return guarded(msg, msglen, [&] {
+    if (bwd)
+      b2m::launch_tn_invariants_bwd((cudaStream_t)st, n, X, ginv, gX);
+    else
+      b2m::launch_tn_invariants((cudaStream_t)st, n, X, inv);
+  });
+}
+// atom_e and wgt null or not pick the instantiation; eref may be null
+int shim_tn_readout_final(void* st, int n, int W, const float* hL, const float* wL, float bL, const float* hG,
+                          const float* wG, float bG, const int* type, const double* eref, float scale, float* lout,
+                          float* gout, float* e_atom, double* energy, const int* gid, double* atom_e,
+                          double mean_per_atom, const float* wgt, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_tn_readout_final((cudaStream_t)st, n, W, hL, wL, bL, hG, wG, bG, type, eref, scale, lout, gout, e_atom,
+                                 energy, gid, atom_e, mean_per_atom, wgt);
+  });
+}
+int shim_tn_readout_seed(void* st, int n, int W, const float* lout, const float* gout, float scale, const float* wL,
+                         const float* wG, const float* preL, const float* preG, float* gL, float* gG, const int* gid,
+                         const float* wgt, char* msg, int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_tn_readout_seed((cudaStream_t)st, n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG, gid, wgt);
+  });
+}
+// gd =, forces +=, virial +=, atom_vir += (null: the plain instantiation)
+int shim_tn_edge_final(void* st, int64_t E, const int* e_src, const int* e_dst, const float* e_vec, const int* gid,
+                       int nr, int nrp, float width, float rc, const float* mu, const float* g_rbf, const float* gC,
+                       const float* gvh, float* gd, float* forces, double* virial, float* atom_vir, char* msg,
+                       int msglen) {
+  return guarded(msg, msglen, [&] {
+    b2m::launch_tn_edge_final((cudaStream_t)st, E, e_src, e_dst, reinterpret_cast<const float4*>(e_vec), gid,
+                              tn_radial(nr, nrp, width, rc, mu), g_rbf, gC, gvh, gd, forces, virial, atom_vir);
   });
 }
 

@@ -141,6 +141,94 @@ class Shim:
                    _ptr(dev.get("gA")), _ptr(dev.get("gC")), _ptr(dev.get("gQ")), _ptr(dev.get("gd")),
                    ctypes.c_int(num_sms))
 
+    # -------- TensorNet launchers (shim_tn_*(stream, ...)): tensors as pointers (None: null), int as c_int, float as
+    # c_float; c_int64 / c_double given explicitly
+    def _tn(self, entry, *args):
+        def conv(x):
+            if x is None or isinstance(x, (ctypes.c_int64, ctypes.c_double, ctypes.c_void_p)):
+                return x
+            if isinstance(x, torch.Tensor):
+                return ctypes.c_void_p(x.data_ptr())
+            if isinstance(x, (bool, int)):
+                return ctypes.c_int(int(x))
+            return ctypes.c_float(x)
+        st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        self._call(getattr(self.lib, "shim_tn_" + entry), *[conv(x) for x in (st,) + args])
+
+    def tn_gemm(self, A, lda, B0, C, ldc, M, N, K, zA=0, B1=None, B2=None, bsel=False, zC=0, Cpre=None, Pre=None,
+                ldp=0, bias=None, accum=False, epi=0, nz=1):
+        self._tn("gemm", A, lda, ctypes.c_int64(zA), B0, B1, B2, bsel, C, ldc, ctypes.c_int64(zC), Cpre, Pre, ldp, bias,
+                 M, N, K, accum, epi, nz)
+
+    def tn_edge_geom(self, E, e_vec, nr, nrp, width, rc, mu, rbf, cut):
+        self._tn("edge_geom", ctypes.c_int64(E), e_vec, nr, nrp, width, rc, mu, rbf, cut)
+
+    def tn_embed_agg(self, n_own, row_ptr, e_src, type_, U, V, P, cut, e_vec, T0, nr0):
+        self._tn("embed_agg", 0, n_own, ctypes.c_int64(0), row_ptr, e_src, None, type_, U, V, P, cut, e_vec, T0, nr0,
+                 None, None, None, None)
+
+    def tn_embed_agg_bwd(self, E, e_src, e_dst, type_, U, V, P, cut, e_vec, gT0, gP, gC, gvh):
+        self._tn("embed_agg", 1, 0, ctypes.c_int64(E), None, e_src, e_dst, type_, U, V, P, cut, e_vec, None, None, gT0,
+                 gP, gC, gvh)
+
+    def tn_layernorm(self, rows, W, x, gamma, beta, y, stats):
+        self._tn("layernorm", 0, rows, W, x, gamma, beta, y, stats, None, None)
+
+    def tn_layernorm_bwd(self, rows, W, x, stats, gamma, gy, gx):
+        self._tn("layernorm", 1, rows, W, x, gamma, None, None, stats, gy, gx)
+
+    def tn_embed_out(self, n, T0m, s2p, X0):
+        self._tn("embed_out", 0, n, T0m, s2p, X0, None, None, None)
+
+    def tn_embed_out_bwd(self, n, T0m, s2p, gX0, gT0m, gs2p):
+        self._tn("embed_out", 1, n, T0m, s2p, None, gX0, gT0m, gs2p)
+
+    def tn_norm_bwd_add(self, n, T0, gnr0, gT0):
+        self._tn("norm_bwd_add", n, T0, gnr0, gT0)
+
+    def tn_scale(self, n, X, Xh, q):
+        self._tn("scale", 0, n, X, Xh, q, None)
+
+    def tn_scale_bwd(self, n, X, q, g):
+        self._tn("scale", 1, n, X, None, q, g)
+
+    def tn_msg(self, n_own, row_ptr, e_src, f3p, cut, Y, out):
+        self._tn("msg", 0, n_own, row_ptr, e_src, f3p, cut, Y, out, None, None, None, None)
+
+    def tn_msg_bwd(self, n_own, row_ptr, e_src, f3p, cut, Y, gmsg, g3, gC, gY):
+        self._tn("msg", 1, n_own, row_ptr, e_src, f3p, cut, Y, None, gmsg, g3, gC, gY)
+
+    def tn_prod(self, n, m, Y, so3, Pn):
+        self._tn("prod", 0, n, m, Y, so3, Pn, None, None, None)
+
+    def tn_prod_bwd(self, n, m, Y, so3, gPn, gmsg, gY):
+        self._tn("prod", 1, n, m, Y, so3, None, gPn, gmsg, gY)
+
+    def tn_update(self, n, Xh, dX, Xn):
+        self._tn("update", 0, n, Xh, dX, Xn, None, None)
+
+    def tn_update_bwd(self, n, dX, gXn, gdX):
+        self._tn("update", 1, n, None, dX, None, gXn, gdX)
+
+    def tn_invariants(self, n, X, inv):
+        self._tn("invariants", 0, n, X, inv, None, None)
+
+    def tn_invariants_bwd(self, n, X, ginv, gX):
+        self._tn("invariants", 1, n, X, None, ginv, gX)
+
+    def tn_readout_final(self, n, W, hL, wL, bL, hG, wG, bG, type_, eref, scale, lout, gout, e_atom, energy, gid,
+                         atom_e=None, mean_per_atom=0.0, wgt=None):
+        self._tn("readout_final", n, W, hL, wL, bL, hG, wG, bG, type_, eref, scale, lout, gout, e_atom, energy, gid,
+                 atom_e, ctypes.c_double(mean_per_atom), wgt)
+
+    def tn_readout_seed(self, n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG, gid, wgt=None):
+        self._tn("readout_seed", n, W, lout, gout, scale, wL, wG, preL, preG, gL, gG, gid, wgt)
+
+    def tn_edge_final(self, E, e_src, e_dst, e_vec, gid, nr, nrp, width, rc, mu, g_rbf, gC, gvh, gd, forces, virial,
+                      atom_vir=None):
+        self._tn("edge_final", ctypes.c_int64(E), e_src, e_dst, e_vec, gid, nr, nrp, width, rc, mu, g_rbf, gC, gvh, gd,
+                 forces, virial, atom_vir)
+
     def line(self, bwd, hidden, c, dev, num_sms):
         self._call(self.lib.shim_line, ctypes.c_int(int(bwd)), ctypes.c_int(int(hidden)),
                    ctypes.c_void_p(torch.cuda.current_stream().cuda_stream), ctypes.c_int64(c["A"]),
