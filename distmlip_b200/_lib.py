@@ -45,6 +45,7 @@ class MaceDesc(C.Structure):
         ("num_interactions", C.c_int32), ("num_bessel", C.c_int32), ("num_polynomial_cutoff", C.c_int32),
         ("mlp_hidden", C.c_int32), ("residual_mask", C.c_int32), ("hidden_max_l", C.c_int32),
         ("r_max", C.c_double), ("c_act", C.c_double), ("avg_num_neighbors", C.c_double * 8),
+        ("hidden_mul", C.c_int32 * 4),
     ]
 
 

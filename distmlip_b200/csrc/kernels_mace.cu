@@ -1,6 +1,7 @@
-// kernels_mace.cu -- MACE with hidden features C x 0e or C x 0e + C x 1o on the same partitioned CSR graph as the
-// CHGNet and TensorNet paths.  Arithmetic as oracle/mace_ref.py and, for 0e+1o features, tests/mace_eq_ref.py state it
-// (the conventions are written down there once), and the ZBL pair term and Agnesi transform as tests/mace_zbl_ref.py
+// kernels_mace.cu -- MACE with hidden features C x 0e, C x 0e + C x 1o or C x 0e + C x 1o + C x 2e on the same
+// partitioned CSR graph as the CHGNet and TensorNet paths.  Arithmetic as oracle/mace_ref.py and, for 0e+1o features,
+// tests/mace_eq_ref.py and, for 0e+1o+2e, tests/mace_l2_ref.py state it (the conventions are written down there once),
+// and the ZBL pair term and Agnesi transform as tests/mace_zbl_ref.py
 // states them; engine_mace.inl runs these kernels stage by stage.
 //
 // First generation: the node- and edge-level products (radial MLP, linear_up, the per-l mixes, the product linear) run
@@ -8,8 +9,11 @@
 // (skip_tp) read the element's C x C block per atom; the symmetric contraction is one thread per (atom, channel) that
 // walks the nonzero terms of U, which every channel shares.  Aggregations walk the CSR-by-destination rows (no atomics
 // in the forward); the reverse scatters to sources with atomics.
+#include <utility>
+
 #include "final_tail.cuh"
 #include "mace_cg.cuh"
+#include "mace_cg_l2.cuh"
 #include "mace_state.cuh"
 
 namespace b2m {
@@ -301,7 +305,7 @@ __global__ void __launch_bounds__(256) k_mace_msg_eq(int n_own, int C, const int
                                                      const int* __restrict__ e_src, const float* __restrict__ R,
                                                      const float* __restrict__ Y, const float* __restrict__ u,
                                                      float* __restrict__ Am) {
-  constexpr int NP = mace_npaths(kL), NS = mace_nslots(kL), NSH = (kL + 1) * (kL + 1);
+  constexpr int NP = mace_npaths(kL, 1), NS = mace_nslots(kL, 1), NSH = (kL + 1) * (kL + 1);
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= (int64_t)n_own * C) return;
   const int t = (int)(i / C), c = (int)(i % C);
@@ -326,8 +330,8 @@ __global__ void __launch_bounds__(256) k_mace_msg_eq(int n_own, int C, const int
   int s = 0;
 #pragma unroll
   for (int l = 0; l <= kL; l++) {
-    const int np = mace_np_l(kL, l);
-    float* blk = Am + (size_t)mace_slot_base(kL, l) * n_own * C;
+    const int np = mace_np_l(kL, l, 1);
+    float* blk = Am + (size_t)mace_slot_base(kL, l, 1) * n_own * C;
 #pragma unroll
     for (int m = 0; m < 2 * l + 1; m++)
 #pragma unroll
@@ -343,7 +347,7 @@ __global__ void __launch_bounds__(256) k_mace_msg_eq_bwd(int n_own, int C, const
                                                          const float* __restrict__ Y, const float* __restrict__ u,
                                                          const float* __restrict__ gAm, float* __restrict__ gY,
                                                          float* __restrict__ gu) {
-  constexpr int NP = mace_npaths(kL), NS = mace_nslots(kL), NSH = (kL + 1) * (kL + 1);
+  constexpr int NP = mace_npaths(kL, 1), NS = mace_nslots(kL, 1), NSH = (kL + 1) * (kL + 1);
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= (int64_t)n_own * C) return;  // n_own * C is a multiple of 32: whole warps leave together
   const int t = (int)(i / C), c = (int)(i % C), lane = threadIdx.x & 31;
@@ -352,8 +356,8 @@ __global__ void __launch_bounds__(256) k_mace_msg_eq_bwd(int n_own, int C, const
     int s = 0;
 #pragma unroll
     for (int l = 0; l <= kL; l++) {
-      const int np = mace_np_l(kL, l);
-      const float* blk = gAm + (size_t)mace_slot_base(kL, l) * n_own * C;
+      const int np = mace_np_l(kL, l, 1);
+      const float* blk = gAm + (size_t)mace_slot_base(kL, l, 1) * n_own * C;
 #pragma unroll
       for (int m = 0; m < 2 * l + 1; m++)
 #pragma unroll
@@ -397,41 +401,67 @@ __global__ void __launch_bounds__(256) k_mace_msg_eq_bwd(int n_own, int C, const
   }
 }
 
-// out[i][m][:] (+)= in[i][m][:] @ W[type[i]][l(m)], m < ncomp (1 or 4), rows of pitch ldi / ldo: one block of C threads
-// per row, each weight element read once per row and applied to the components of its l
+// out[i][m][:] (+)= in[i][m][:] @ W[type[i]][l(m)], m < ncomp (1 or 4; k2e: 9), rows of pitch ldi / ldo: one block of C
+// threads per row, each weight element read once per row and applied to the components of its l
+template <bool k2e>
 __global__ void k_mace_elem_mix_rows(int n, int C, int ncomp, int ldi, int ldo, const int* __restrict__ type,
                                      const float* __restrict__ W, const float* __restrict__ in, float* __restrict__ out,
                                      int accum) {
-  __shared__ float x[4][128];
+  __shared__ float x[k2e ? 9 : 4][128];
   const int i = blockIdx.x, c2 = threadIdx.x;
-  const int z = type[i], Lw = ncomp == 4 ? 2 : 1;
-  for (int m = 0; m < ncomp; m++) x[m][c2] = in[(size_t)i * ldi + m * C + c2];
-  __syncthreads();
-  const float* W0 = W + (size_t)z * Lw * C * C + c2;
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-  if (ncomp == 4) {
-    const float* W1 = W0 + (size_t)C * C;
+  if constexpr (k2e) {
+    const int z = type[i];
+    for (int m = 0; m < 9; m++) x[m][c2] = in[(size_t)i * ldi + m * C + c2];
+    __syncthreads();
+    const float* W0 = W + (size_t)z * 3 * C * C + c2;
+    const float *W1 = W0 + (size_t)C * C, *W2 = W1 + (size_t)C * C;
+    float a[9];
+#pragma unroll
+    for (int m = 0; m < 9; m++) a[m] = 0.f;
     for (int c = 0; c < C; c++) {
-      const float w0 = W0[(size_t)c * C], w1 = W1[(size_t)c * C];
-      a0 = fmaf(w0, x[0][c], a0), a1 = fmaf(w1, x[1][c], a1), a2 = fmaf(w1, x[2][c], a2), a3 = fmaf(w1, x[3][c], a3);
+      const float w0 = W0[(size_t)c * C], w1 = W1[(size_t)c * C], w2 = W2[(size_t)c * C];
+      a[0] = fmaf(w0, x[0][c], a[0]);
+#pragma unroll
+      for (int m = 1; m < 4; m++) a[m] = fmaf(w1, x[m][c], a[m]);
+#pragma unroll
+      for (int m = 4; m < 9; m++) a[m] = fmaf(w2, x[m][c], a[m]);
+    }
+#pragma unroll
+    for (int m = 0; m < 9; m++) {
+      float* o = out + (size_t)i * ldo + m * C + c2;
+      *o = accum ? *o + a[m] : a[m];
     }
   } else {
-    for (int c = 0; c < C; c++) a0 = fmaf(W0[(size_t)c * C], x[0][c], a0);
-  }
-  const float a[4] = {a0, a1, a2, a3};
-  for (int m = 0; m < ncomp; m++) {
-    float* o = out + (size_t)i * ldo + m * C + c2;
-    *o = accum ? *o + a[m] : a[m];
+    const int z = type[i], Lw = ncomp == 4 ? 2 : 1;
+    for (int m = 0; m < ncomp; m++) x[m][c2] = in[(size_t)i * ldi + m * C + c2];
+    __syncthreads();
+    const float* W0 = W + (size_t)z * Lw * C * C + c2;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    if (ncomp == 4) {
+      const float* W1 = W0 + (size_t)C * C;
+      for (int c = 0; c < C; c++) {
+        const float w0 = W0[(size_t)c * C], w1 = W1[(size_t)c * C];
+        a0 = fmaf(w0, x[0][c], a0), a1 = fmaf(w1, x[1][c], a1), a2 = fmaf(w1, x[2][c], a2), a3 = fmaf(w1, x[3][c], a3);
+      }
+    } else {
+      for (int c = 0; c < C; c++) a0 = fmaf(W0[(size_t)c * C], x[0][c], a0);
+    }
+    const float a[4] = {a0, a1, a2, a3};
+    for (int m = 0; m < ncomp; m++) {
+      float* o = out + (size_t)i * ldo + m * C + c2;
+      *o = accum ? *o + a[m] : a[m];
+    }
   }
 }
 
-// symmetric contraction with a 1o output: as k_mace_symc, with the term's output slot o (MaceTerm) selecting one of four
-// accumulators (forward) or upstream adjoints (reverse); B / gB [4][n_own][C]
-template <bool kBwd>
+// symmetric contraction with a 1o (kNo = 4) or 1o and 2e (kNo = 9) output: as k_mace_symc, with the term's output
+// slot o (MaceTerm) selecting one of kNo accumulators (forward) or upstream adjoints (reverse); B / gB [kNo][n_own][C]
+template <bool kBwd, int kNo>
 __global__ void __launch_bounds__(128) k_mace_symc_eq(int n_own, int C, int nsh, int Ktot, const int* __restrict__ type,
                                                       const float* __restrict__ A, const MaceTerm* __restrict__ terms,
                                                       int nterms, const float* __restrict__ w,
                                                       const float* __restrict__ gB, float* __restrict__ out) {
+  static_assert(kNo == 4 || kNo == 9, "output slots of a 0e+1o or 0e+1o+2e product");
   __shared__ float a[kMaceMaxNsh][128];
   __shared__ float ga[kBwd ? kMaceMaxNsh : 1][128];
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
@@ -444,23 +474,40 @@ __global__ void __launch_bounds__(128) k_mace_symc_eq(int n_own, int C, int nsh,
     if constexpr (kBwd) ga[k][tid] = 0.f;
   }
   const float* wz = w + (size_t)type[t] * Ktot * C + c;
-  float g[4] = {0.f, 0.f, 0.f, 0.f};
+  float g[kNo];
+#pragma unroll
+  for (int o = 0; o < kNo; o++) g[o] = 0.f;
   if constexpr (kBwd) {
 #pragma unroll
-    for (int o = 0; o < 4; o++) g[o] = gB[o * plane + i];
+    for (int o = 0; o < kNo; o++) g[o] = gB[o * plane + i];
   }
-  float acc[4] = {0.f, 0.f, 0.f, 0.f};
+  float acc[kNo];
+#pragma unroll
+  for (int o = 0; o < kNo; o++) acc[o] = 0.f;
   for (int j = 0; j < nterms; j++) {
     const MaceTerm tm = terms[j];
-    const int nu = (tm.idx >> 24) & 3, o = (tm.idx >> 28) & 3;
+    // slots 0..3 keep bits 28..29 (bit 31 stays clear); slot 8 sets bit 31, hence the unsigned field for kNo = 9
+    const int nu = (tm.idx >> 24) & 3, o = kNo == 4 ? (tm.idx >> 28) & 3 : (int)((uint32_t)tm.idx >> 28);
     const int i1 = tm.idx & 255, i2 = (tm.idx >> 8) & 255, i3 = (tm.idx >> 16) & 255;
     const float cw = tm.coef * wz[(size_t)tm.kg * C];
     const float a1 = a[i1][tid], a2 = nu >= 2 ? a[i2][tid] : 1.f, a3 = nu >= 3 ? a[i3][tid] : 1.f;
     if constexpr (!kBwd) {
       const float v = cw * (a1 * a2 * a3);  // the same o for the whole warp: the selects do not diverge
-      acc[0] += o == 0 ? v : 0.f, acc[1] += o == 1 ? v : 0.f, acc[2] += o == 2 ? v : 0.f, acc[3] += o == 3 ? v : 0.f;
+      if constexpr (kNo == 4) {
+        acc[0] += o == 0 ? v : 0.f, acc[1] += o == 1 ? v : 0.f, acc[2] += o == 2 ? v : 0.f, acc[3] += o == 3 ? v : 0.f;
+      } else {
+#pragma unroll
+        for (int k = 0; k < kNo; k++) acc[k] += o == k ? v : 0.f;
+      }
     } else {
-      const float s = cw * (o == 0 ? g[0] : o == 1 ? g[1] : o == 2 ? g[2] : g[3]);
+      float go = g[kNo - 1];
+      if constexpr (kNo == 4) {
+        go = o == 0 ? g[0] : o == 1 ? g[1] : o == 2 ? g[2] : g[3];
+      } else {
+#pragma unroll
+        for (int k = kNo - 2; k >= 0; k--) go = o == k ? g[k] : go;
+      }
+      const float s = cw * go;
       ga[i1][tid] += s * a2 * a3;
       if (nu >= 2) ga[i2][tid] += s * a1 * a3;
       if (nu >= 3) ga[i3][tid] += s * a1 * a2;
@@ -468,11 +515,135 @@ __global__ void __launch_bounds__(128) k_mace_symc_eq(int n_own, int C, int nsh,
   }
   if constexpr (!kBwd) {
 #pragma unroll
-    for (int o = 0; o < 4; o++) out[o * plane + i] = acc[o];
+    for (int o = 0; o < kNo; o++) out[o * plane + i] = acc[o];
   } else {
 #pragma unroll
     for (int k = 0; k < kMaceMaxNsh; k++)
       if (k < nsh) out[k * plane + i] = ga[k][tid];
+  }
+}
+
+// ============================================================================================
+// 0e+1o+2e node features (layers t >= 1 of a model with hidden_irreps C x 0e + C x 1o + C x 2e)
+// ============================================================================================
+#define MACE_CG_L2_EXPAND(L, X) \
+  if constexpr ((L) == 2) { MACE_CG_L2_2(X) } else { MACE_CG_L2_3(X) }
+
+// the slots [S0, S0 + NS) of output l kLo and the paths [P0, P0 + NPL) that reach it, and which u / Y components those
+// paths read (bit masks, from the coupling list)
+template <int kL, int kLo>
+struct MaceL2Group {
+  static constexpr int NP = mace_npaths(kL, 2), NPL = mace_np_l(kL, kLo, 2), P0 = mace_path_base(kL, kLo, 2);
+  static constexpr int S0 = mace_slot_base(kL, kLo, 2), NS = (2 * kLo + 1) * NPL, NSH = (kL + 1) * (kL + 1);
+  static constexpr uint32_t mask(bool y) {
+    uint32_t m = 0;
+#define MACE_X(p, iu, iy, s, cf) \
+  if ((s) >= S0 && (s) < S0 + NS) m |= 1u << (y ? (iy) : (iu));
+    MACE_CG_L2_EXPAND(kL, MACE_X)
+#undef MACE_X
+    return m;
+  }
+  static constexpr uint32_t UM = mask(false), YM = mask(true);
+};
+
+// Am[slot(l_out = kLo, m, j)] = sum_{e -> t} R[e][p] sum CG u[src][l_in m1] Y[e][l_sh m2] over the paths p of that l_out:
+// one launch per l_out (all 71 slots of max_ell 3 in one thread would not fit the register file with the edge operands;
+// DESIGN.md §11.3), one thread per (atom, channel), no atomics
+template <int kL, int kLo>
+__global__ void __launch_bounds__(256) k_mace_msg_l2(int n_own, int C, const int* __restrict__ row_ptr,
+                                                     const int* __restrict__ e_src, const float* __restrict__ R,
+                                                     const float* __restrict__ Y, const float* __restrict__ u,
+                                                     float* __restrict__ Am) {
+  using G = MaceL2Group<kL, kLo>;
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;
+  const int t = (int)(i / C), c = (int)(i % C);
+  float acc[G::NS];
+#pragma unroll
+  for (int k = 0; k < G::NS; k++) acc[k] = 0.f;
+  for (int e = row_ptr[t]; e < row_ptr[t + 1]; e++) {
+    const float* us = u + (size_t)e_src[e] * 9 * C + c;
+    float uu[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) uu[k] = (G::UM >> k) & 1 ? us[k * C] : 0.f;
+    const float* re = R + (size_t)e * G::NP * C + c;
+    float r[G::NP];
+#pragma unroll
+    for (int p = 0; p < G::NP; p++) r[p] = p >= G::P0 && p < G::P0 + G::NPL ? re[p * C] : 0.f;
+    const float* ye = Y + (size_t)e * kMaceMaxNsh;
+    float y[G::NSH];
+#pragma unroll
+    for (int k = 0; k < G::NSH; k++) y[k] = (G::YM >> k) & 1 ? ye[k] : 0.f;
+#define MACE_X(p, iu, iy, s, cf) \
+  if constexpr ((s) >= G::S0 && (s) < G::S0 + G::NS) acc[(s) - G::S0] = fmaf((cf) * r[p], uu[iu] * y[iy], acc[(s) - G::S0]);
+    MACE_CG_L2_EXPAND(kL, MACE_X)
+#undef MACE_X
+  }
+  float* blk = Am + (size_t)G::S0 * n_own * C;
+#pragma unroll
+  for (int m = 0; m < 2 * kLo + 1; m++)
+#pragma unroll
+    for (int j = 0; j < G::NPL; j++) blk[(((size_t)m * n_own + t) * G::NPL + j) * C + c] = acc[m * G::NPL + j];
+}
+
+// reverse of k_mace_msg_l2 for output l kLo: gR over R in place for the paths of that l_out (the thread of (dst, c) is
+// the only reader and writer of R[e][p][c], and no other launch touches those paths), gY[e][k] += the warp's 32 channels
+// (one atomic per warp), gu[src][9][c] += (atomics)
+template <int kL, int kLo>
+__global__ void __launch_bounds__(256) k_mace_msg_l2_bwd(int n_own, int C, const int* __restrict__ row_ptr,
+                                                         const int* __restrict__ e_src, float* __restrict__ R,
+                                                         const float* __restrict__ Y, const float* __restrict__ u,
+                                                         const float* __restrict__ gAm, float* __restrict__ gY,
+                                                         float* __restrict__ gu) {
+  using G = MaceL2Group<kL, kLo>;
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n_own * C) return;  // n_own * C is a multiple of 32: whole warps leave together
+  const int t = (int)(i / C), c = (int)(i % C), lane = threadIdx.x & 31;
+  float ga[G::NS];
+  {
+    const float* blk = gAm + (size_t)G::S0 * n_own * C;
+#pragma unroll
+    for (int m = 0; m < 2 * kLo + 1; m++)
+#pragma unroll
+      for (int j = 0; j < G::NPL; j++) ga[m * G::NPL + j] = blk[(((size_t)m * n_own + t) * G::NPL + j) * C + c];
+  }
+  for (int e = row_ptr[t]; e < row_ptr[t + 1]; e++) {
+    const int src = e_src[e];
+    const float* us = u + (size_t)src * 9 * C + c;
+    float uu[9], g9[9];
+#pragma unroll
+    for (int k = 0; k < 9; k++) uu[k] = (G::UM >> k) & 1 ? us[k * C] : 0.f, g9[k] = 0.f;
+    float* re = R + (size_t)e * G::NP * C + c;
+    float r[G::NP], gr[G::NP];
+#pragma unroll
+    for (int p = 0; p < G::NP; p++) r[p] = p >= G::P0 && p < G::P0 + G::NPL ? re[p * C] : 0.f, gr[p] = 0.f;
+    const float* ye = Y + (size_t)e * kMaceMaxNsh;
+    float y[G::NSH], gy[G::NSH];
+#pragma unroll
+    for (int k = 0; k < G::NSH; k++) y[k] = (G::YM >> k) & 1 ? ye[k] : 0.f, gy[k] = 0.f;
+#define MACE_X(p, iu, iy, s, cf)                    \
+  if constexpr ((s) >= G::S0 && (s) < G::S0 + G::NS) { \
+    const float g = (cf) * ga[(s) - G::S0];         \
+    gr[p] = fmaf(g, uu[iu] * y[iy], gr[p]);         \
+    const float gq = g * r[p];                      \
+    g9[iu] = fmaf(gq, y[iy], g9[iu]);               \
+    gy[iy] = fmaf(gq, uu[iu], gy[iy]);              \
+  }
+    MACE_CG_L2_EXPAND(kL, MACE_X)
+#undef MACE_X
+#pragma unroll
+    for (int p = G::P0; p < G::P0 + G::NPL; p++) re[p * C] = gr[p];
+#pragma unroll
+    for (int k = 1; k < G::NSH; k++) {  // Y[0] = 1 carries no gradient
+      if (!((G::YM >> k) & 1)) continue;
+      float v = gy[k];
+      for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+      if (lane == 0) atomicAdd(&gY[(size_t)e * kMaceMaxNsh + k], v);
+    }
+    float* gs = gu + (size_t)src * 9 * C + c;
+#pragma unroll
+    for (int k = 0; k < 9; k++)
+      if ((G::UM >> k) & 1) atomicAdd(gs + k * C, g9[k]);
   }
 }
 
@@ -697,18 +868,64 @@ void launch_mace_msg_eq_bwd(cudaStream_t st, int max_ell, int n_own, int C, cons
 void launch_mace_elem_mix_rows(cudaStream_t st, int n, int C, int ncomp, int ldi, int ldo, const int* type,
                                const float* W, const float* in, float* out, bool accum) {
   if (n <= 0) return;
-  B2M_REQUIRE(C <= 128 && (ncomp == 1 || ncomp == 4), B2M_ERR_INVALID, "mace elem mix: C <= 128, 1 or 4 components");
-  launch(k_mace_elem_mix_rows, n, C, 0, st, n, C, ncomp, ldi, ldo, type, W, in, out, accum ? 1 : 0);
+  B2M_REQUIRE(C <= 128 && (ncomp == 1 || ncomp == 4 || ncomp == 9), B2M_ERR_INVALID,
+              "mace elem mix: C <= 128, 1, 4 or 9 components");
+  const auto kern = ncomp == 9 ? k_mace_elem_mix_rows<true> : k_mace_elem_mix_rows<false>;
+  launch(kern, n, C, 0, st, n, C, ncomp, ldi, ldo, type, W, in, out, accum ? 1 : 0);
 }
 void launch_mace_symc_eq(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
                          const MaceTerm* terms, int nterms, const float* w, float* B) {
-  launch(k_mace_symc_eq<false>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms, nterms,
-         w, nullptr, B);
+  launch(k_mace_symc_eq<false, 4>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms,
+         nterms, w, nullptr, B);
 }
 void launch_mace_symc_eq_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
                              const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA) {
-  launch(k_mace_symc_eq<true>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms, nterms,
-         w, gB, gA);
+  launch(k_mace_symc_eq<true, 4>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms,
+         nterms, w, gB, gA);
+}
+void launch_mace_symc_l2(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                         const MaceTerm* terms, int nterms, const float* w, float* B) {
+  launch(k_mace_symc_eq<false, 9>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms,
+         nterms, w, nullptr, B);
+}
+void launch_mace_symc_l2_bwd(cudaStream_t st, int n_own, int C, int nsh, int Ktot, const int* type, const float* A,
+                             const MaceTerm* terms, int nterms, const float* w, const float* gB, float* gA) {
+  launch(k_mace_symc_eq<true, 9>, cdiv((int64_t)n_own * C, 128), 128, 0, st, n_own, C, nsh, Ktot, type, A, terms,
+         nterms, w, gB, gA);
+}
+// one launch per output l of the 0e+1o+2e message (kernel<kL, 0>, .., kernel<kL, kL>)
+template <int kL, bool kBwd, int... kLo>
+static void msg_l2_groups(std::integer_sequence<int, kLo...>, cudaStream_t st, int n_own, int C, const int* row_ptr,
+                          const int* e_src, float* R, const float* Y, const float* u, float* Am, const float* gAm,
+                          float* gY, float* gu) {
+  const int grid = cdiv((int64_t)n_own * C, 256);
+  if constexpr (kBwd)
+    (launch(k_mace_msg_l2_bwd<kL, kLo>, grid, 256, 0, st, n_own, C, row_ptr, e_src, R, Y, u, gAm, gY, gu), ...);
+  else
+    (launch(k_mace_msg_l2<kL, kLo>, grid, 256, 0, st, n_own, C, row_ptr, e_src, R, Y, u, Am), ...);
+}
+void launch_mace_msg_l2(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
+                        const float* R, const float* Y, const float* u, float* Am) {
+  B2M_REQUIRE(max_ell == 2 || max_ell == 3, B2M_ERR_INVALID,
+              "mace message with 0e+1o+2e features: max_ell must be 2 or 3");
+  float* Rm = const_cast<float*>(R);  // read only in the forward
+  if (max_ell == 2)
+    msg_l2_groups<2, false>(std::make_integer_sequence<int, 3>{}, st, n_own, C, row_ptr, e_src, Rm, Y, u, Am, nullptr,
+                            nullptr, nullptr);
+  else
+    msg_l2_groups<3, false>(std::make_integer_sequence<int, 4>{}, st, n_own, C, row_ptr, e_src, Rm, Y, u, Am, nullptr,
+                            nullptr, nullptr);
+}
+void launch_mace_msg_l2_bwd(cudaStream_t st, int max_ell, int n_own, int C, const int* row_ptr, const int* e_src,
+                            float* R, const float* Y, const float* u, const float* gAm, float* gY, float* gu) {
+  B2M_REQUIRE(max_ell == 2 || max_ell == 3, B2M_ERR_INVALID,
+              "mace message with 0e+1o+2e features: max_ell must be 2 or 3");
+  if (max_ell == 2)
+    msg_l2_groups<2, true>(std::make_integer_sequence<int, 3>{}, st, n_own, C, row_ptr, e_src, R, Y, u, nullptr, gAm, gY,
+                           gu);
+  else
+    msg_l2_groups<3, true>(std::make_integer_sequence<int, 4>{}, st, n_own, C, row_ptr, e_src, R, Y, u, nullptr, gAm, gY,
+                           gu);
 }
 // kSpecies with the pair term or the Agnesi transform; kWeighted with the pair term and readout weights (without the
 // pair term the weights are all in g_eb and gY)

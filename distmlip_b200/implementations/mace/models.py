@@ -1,14 +1,16 @@
-"""ScaleShiftMACE_Dist -- a mace `ScaleShiftMACE` with hidden features C x 0e or C x 0e + C x 1o on the sm_90a engine.
+"""ScaleShiftMACE_Dist -- a mace `ScaleShiftMACE` with hidden features C x 0e, C x 0e + C x 1o or C x 0e + C x 1o + C x 2e
+on the sm_90a engine.
 
 `from_existing` takes any object with mace's attribute tree and `state_dict()` (mace itself need not be importable, so
 the model is recognised by structure, not by `isinstance`); `enable_distributed_mode(gpus)` validates the
 configuration and creates the engine (b2m_create_mace).  The arithmetic, with every e3nn / mace convention it relies on,
-is stated in oracle/mace_ref.py (scalar hidden features), tests/mace_eq_ref.py (0e+1o) and tests/mace_zbl_ref.py (the
-ZBL pair repulsion and the Agnesi distance transform); the kernels are csrc/kernels_mace.cu.
+is stated in oracle/mace_ref.py (scalar hidden features), tests/mace_eq_ref.py (0e+1o), tests/mace_l2_ref.py (0e+1o+2e)
+and tests/mace_zbl_ref.py (the ZBL pair repulsion and the Agnesi distance transform); the kernels are
+csrc/kernels_mace.cu.
 
 Supported configuration (anything else raises NotImplementedError in enable_distributed_mode): ScaleShiftMACE with one
-head, hidden_irreps = C x 0e or C x 0e + C x 1o (C a multiple of 32, C <= 128; the shapes of MACE-MP-0 "small" and
-"medium"), max_ell <= 3 (>= 1 with 1o), correlation <= 3, Bessel radial basis
+head, hidden_irreps = C x 0e, C x 0e + C x 1o or C x 0e + C x 1o + C x 2e (C a multiple of 32, C <= 128; the shapes of
+MACE-MP-0 "small", "medium" and "large"), max_ell <= 3 (>= 1 with 1o, >= 2 with 2e), correlation <= 3, Bessel radial basis
 (num_bessel <= 64) times PolynomialCutoff, a FullyConnectedNet radial MLP (hidden widths <= 64),
 RealAgnosticResidualInteractionBlock or RealAgnosticInteractionBlock per layer, LinearReadoutBlock on every layer but the
 last and NonLinearReadoutBlock (gated SiLU) on the last.  Optional, as in the MACE-MP-0b / MPA-0 / OMAT-0 checkpoints:
@@ -162,78 +164,102 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
             num_bessel=int(sd["radial_embedding.bessel_fn.bessel_weights"].numel()),
             num_polynomial_cutoff=int(round(float(sd["radial_embedding.cutoff_fn.p"]))),
             mlp_hidden=H, residual_mask=residual, hidden_max_l=hidden_l, r_max=float(sd["r_max"]), c_act=c_act,
-            avg_num_neighbors=(_lib.C.c_double * 8)(*avg))
+            avg_num_neighbors=(_lib.C.c_double * 8)(*avg),
+            hidden_mul=(_lib.C.c_int32 * 4)(*[C if l <= hidden_l else 0 for l in range(4)]))
 
     @staticmethod
     def _hidden_l(sd, inters, C, T, n_elem, nsh, max_ell, correlation):
-        """0 for hidden_irreps C x 0e, 1 for C x 0e + C x 1o, from the interactions' `hidden_irreps` when they carry it
-        and from the state_dict shapes, each checked against what conv_tp's path rule predicts per layer"""
-        hl = 0
+        """0 for hidden_irreps C x 0e, 1 for C x 0e + C x 1o, 2 for C x 0e + C x 1o + C x 2e, from the interactions'
+        `hidden_irreps` when they carry it and from the state_dict shapes (contractions.1 / .2, linear_up, the radial
+        MLP's n_paths C outputs, interactions.t.linear, products.t.linear, weights_max), each checked against what
+        conv_tp's path rule predicts per layer"""
+        hl = None
         irreps = getattr(inters[0], "hidden_irreps", None) if inters else None
         if irreps is not None:
             ir = _parse_irreps(irreps)
-            if any(l > 1 for _, l, _ in ir):
-                raise NotImplementedError(f"hidden_irreps = {irreps}: equivariant hidden features with l > 1 "
-                                          "(MACE-MP-0 'large') are not supported")
+            if any(l > 2 for _, l, _ in ir):
+                raise NotImplementedError(f"hidden_irreps = {irreps}: hidden l = 3 and above (beyond MACE-MP-0 'large', "
+                                          "l > 2) are not supported")
             if len({m for m, _, _ in ir}) > 1:
                 raise NotImplementedError(f"hidden_irreps = {irreps}: unequal multiplicities across l are not supported")
-            if [(l, p) for _, l, p in ir] not in ([(0, "e")], [(0, "e"), (1, "o")]):
-                raise NotImplementedError(f"hidden_irreps = {irreps}: equivariant hidden features other than 0e and 0e+1o "
-                                          "(parity: only 1o) are not supported")
+            shapes = ([(0, "e")], [(0, "e"), (1, "o")], [(0, "e"), (1, "o"), (2, "e")])
+            if [(l, p) for _, l, p in ir] not in shapes:
+                raise NotImplementedError(f"hidden_irreps = {irreps}: equivariant hidden features other than 0e, 0e+1o "
+                                          "and 0e+1o+2e (parity: only 1o and 2e) are not supported")
             hl = len(ir) - 1
         pre = "products.{}.symmetric_contractions.contractions.{}."
         if any(k.startswith("products.") and ".symmetric_contractions.contractions." in k and
-               int(k.split(".")[4]) >= 2 for k in sd):
-            raise NotImplementedError("equivariant hidden features with l > 1 (a third contraction) are not supported")
+               int(k.split(".")[4]) >= 3 for k in sd):
+            raise NotImplementedError("equivariant hidden features with hidden l = 3 and above (a fourth contraction, "
+                                      "l > 2) are not supported")
         has1 = [any(k.startswith(pre.format(t, 1)) for k in sd) for t in range(T)]
-        if any(has1):
-            for t in range(T):
-                u1 = sd.get(pre.format(t, 1) + "U_matrix_1")
-                if has1[t] and (u1 is None or u1.dim() != 3):
-                    raise NotImplementedError(f"equivariant hidden features: products.{t} has contractions.1 without a "
-                                              "[3, nsh, K] U_matrix_1 (malformed state_dict)")
-                if u1 is not None and u1.shape[0] != 3:
-                    raise NotImplementedError(f"equivariant hidden features: contractions.1 of products.{t} gives "
-                                              f"{u1.shape[0]} components; only 1o (3) is supported (l > 1 is not)")
-            if irreps is not None and hl == 0:
-                raise NotImplementedError("equivariant hidden features: contractions.1 on a C x 0e model")
-            hl = 1
+        has2 = [any(k.startswith(pre.format(t, 2)) for k in sd) for t in range(T)]
+        for t in range(T):
+            u1 = sd.get(pre.format(t, 1) + "U_matrix_1")
+            if has1[t] and (u1 is None or u1.dim() != 3):
+                raise NotImplementedError(f"equivariant hidden features: products.{t} has contractions.1 without a "
+                                          "[3, nsh, K] U_matrix_1 (malformed state_dict)")
+            if u1 is not None and u1.shape[0] != 3:
+                raise NotImplementedError(f"equivariant hidden features: contractions.1 of products.{t} gives "
+                                          f"{u1.shape[0]} components; only 1o (3) is supported (l > 1 is not)")
+            u2 = sd.get(pre.format(t, 2) + "U_matrix_1")
+            if has2[t] and (u2 is None or u2.dim() != 3 or u2.shape[0] != 5):
+                raise NotImplementedError(f"hidden l > 1 (2e): products.{t} has contractions.2 without a [5, nsh, K] "
+                                          "U_matrix_1 (only 2e is supported)")
+        sd_hl = 2 if any(has2) else 1 if any(has1) else 0
+        if (sd_hl if hl is None else hl) == 2 and max_ell < 2:
+            raise NotImplementedError(f"hidden l > 1 (2e) needs max_ell >= 2, not max_ell = {max_ell}")
+        if hl is None:
+            hl = sd_hl
+        elif hl != sd_hl and 2 in (hl, sd_hl):
+            raise NotImplementedError(f"hidden l > 1 (2e): hidden_irreps = {irreps} but the state_dict has " +
+                                      ("no contractions.2" if hl == 2 else "contractions.2") + " (inconsistent model)")
+        elif hl == 0 and sd_hl == 1:
+            raise NotImplementedError("equivariant hidden features: contractions.1 on a C x 0e model")
         if hl and max_ell < 1:
             raise NotImplementedError("equivariant hidden features need max_ell >= 1")
+        what = {0: f"{C}x0e", 1: f"{C}x0e+{C}x1o", 2: f"{C}x0e+{C}x1o+{C}x2e"}[hl]
+        l2 = " (hidden l > 1 (2e))" if hl == 2 else ""
         for t in range(T):
-            lin, lout = int(hl and t > 0), int(hl and t < T - 1)
+            lin, lout = (hl if t > 0 else 0), (hl if t < T - 1 else 0)
             npaths = len(conv_paths(max_ell, lin))
             up = int(sd[f"interactions.{t}.linear_up.weight"].numel())
             if up != (1 + lin) * C * C:
                 c1 = round(max(up - C * C, 0) ** 0.5)
-                if lin and c1 * c1 == up - C * C:
+                if lin == 1 and c1 * c1 == up - C * C:
                     raise NotImplementedError(f"interactions.{t}.linear_up maps {C}x0e+{c1}x1o: unequal multiplicities "
                                               "across l are not supported")
                 raise NotImplementedError(f"interactions.{t}.linear_up has {up} weights, {(1 + lin) * C * C} expected for "
-                                          f"hidden_irreps {C}x0e" + (f"+{C}x1o" if hl else "") + " (equivariant hidden "
-                                          "features other than 0e+1o are not supported)")
+                                          f"hidden_irreps {what}{l2} (equivariant hidden features other than 0e+1o and "
+                                          "0e+1o+2e, or unequal multiplicities across l, are not supported)")
             last = max((k for k in sd if k.startswith(f"interactions.{t}.conv_tp_weights.layer")),
                        key=lambda k: int(k.split(".")[3][5:]))
             if int(sd[last].shape[1]) != npaths * C:
-                raise NotImplementedError(f"{last} has {int(sd[last].shape[1])} outputs, {npaths} paths x {C} expected: "
-                                          "equivariant hidden features other than 0e+1o (parity: only 1o) are not supported")
+                raise NotImplementedError(f"{last} has {int(sd[last].shape[1])} outputs, {npaths} paths x {C} expected"
+                                          f"{l2}: equivariant hidden features other than 0e+1o and 0e+1o+2e (parity: "
+                                          "only 1o and 2e) are not supported")
             if int(sd[f"interactions.{t}.linear.weight"].numel()) != npaths * C * C:
                 raise NotImplementedError(f"interactions.{t}.linear does not match the {npaths} conv_tp paths of "
-                                          "0e" + ("+1o" if lin else "") + " node features")
+                                          "0e" + ("+1o" if lin else "") + ("+2e" if lin == 2 else "") +
+                                          f" node features{l2}")
             if int(sd[f"products.{t}.linear.weight"].numel()) != (1 + lout) * C * C:
                 raise NotImplementedError(f"products.{t}.linear has {int(sd[f'products.{t}.linear.weight'].numel())} "
-                                          f"weights, {(1 + lout) * C * C} expected (unequal multiplicities across l or "
-                                          "l > 1 are not supported)")
+                                          f"weights, {(1 + lout) * C * C} expected{l2} (unequal multiplicities across l "
+                                          "or hidden l > 2 are not supported)")
             if has1[t] != bool(lout):
                 raise NotImplementedError(f"equivariant hidden features: products.{t} " +
                                           ("lacks" if lout else "has") + " contractions.1 (only the last layer is 0e)")
-            if lout:
-                w = sd.get(pre.format(t, 1) + "weights_max")
+            if has2[t] != (lout == 2):
+                raise NotImplementedError(f"hidden l > 1 (2e): products.{t} " + ("lacks" if lout == 2 else "has") +
+                                          " contractions.2 (only the last layer is 0e)")
+            for ci in range(1, lout + 1):
+                w = sd.get(pre.format(t, ci) + "weights_max")
                 if w is None or w.dim() != 3 or int(w.shape[0]) != n_elem or int(w.shape[2]) != C:
-                    raise NotImplementedError(f"products.{t} contractions.1 weights_max is not [{n_elem}, K, {C}] "
-                                              "(unequal multiplicities across l are not supported)")
-                if sum(1 for k in sd if k.startswith(pre.format(t, 1) + "U_matrix_")) != correlation:
-                    raise NotImplementedError(f"products.{t}: contractions.1 and contractions.0 differ in correlation")
+                    raise NotImplementedError(f"products.{t} contractions.{ci} weights_max is not [{n_elem}, K, {C}]" +
+                                              (l2 if ci == 2 else "") + " (unequal multiplicities across l are not "
+                                              "supported)")
+                if sum(1 for k in sd if k.startswith(pre.format(t, ci) + "U_matrix_")) != correlation:
+                    raise NotImplementedError(f"products.{t}: contractions.{ci} and contractions.0 differ in correlation")
         return hl
 
     def enable_distributed_mode(self, gpus):

@@ -98,9 +98,11 @@ typedef struct {
 int b2m_create_tensornet(const b2m_tensornet_desc* desc, const int* devices, int ndev, b2m_handle* out);
 
 /* MACE (DESIGN.md §11): the same handle type and calls, for a mace ScaleShiftMACE with hidden features C x 0e
- * (hidden_max_l = 0, MACE-MP-0 "small") or C x 0e + C x 1o (hidden_max_l = 1, MACE-MP-0 "medium"; then max_ell >= 1),
- * loaded key by key from its state_dict (arithmetic and conventions: oracle/mace_ref.py and, for 0e+1o,
- * tests/mace_eq_ref.py).
+ * (hidden_max_l = 0, MACE-MP-0 "small"), C x 0e + C x 1o (hidden_max_l = 1, MACE-MP-0 "medium"; then max_ell >= 1) or
+ * C x 0e + C x 1o + C x 2e (hidden_max_l = 2, MACE-MP-0 "large"; then max_ell >= 2), loaded key by key from its
+ * state_dict (arithmetic and conventions: oracle/mace_ref.py and, for 0e+1o and 0e+1o+2e, tests/mace_eq_ref.py and
+ * tests/mace_l2_ref.py).  hidden_mul must be channels for every l <= hidden_max_l and 0 above (unequal multiplicities
+ * are not supported); a contradiction fails b2m_create_mace with B2M_ERR_INVALID.
  * Supported: one head, C a multiple of 32 with C <= 128, max_ell <= 3, correlation <= 3, Bessel basis x polynomial cutoff,
  * an e3nn FullyConnectedNet radial MLP (hidden widths <= 64), RealAgnostic(Residual)InteractionBlock per layer, linear
  * readouts and a gated non-linear last readout; optionally mace's ZBL pair repulsion (keys pair_repulsion_fn.{c, a_exp,
@@ -114,7 +116,7 @@ int b2m_create_tensornet(const b2m_tensornet_desc* desc, const int* devices, int
  * (its J_conv uses it, E0 and shift included). */
 typedef struct {
   int32_t n_elem;                 /* len(atomic_numbers)                                                 */
-  int32_t channels;               /* C of hidden_irreps = C x 0e (+ C x 1o)                              */
+  int32_t channels;               /* C of hidden_irreps = C x 0e (+ C x 1o (+ C x 2e))                   */
   int32_t max_ell;                /* edge spherical harmonics 0..max_ell                                 */
   int32_t correlation;            /* symmetric-contraction order                                         */
   int32_t num_interactions;       /* <= 8                                                                */
@@ -122,10 +124,11 @@ typedef struct {
   int32_t num_polynomial_cutoff;  /* PolynomialCutoff exponent p                                         */
   int32_t mlp_hidden;             /* width of the non-linear readout                                     */
   int32_t residual_mask;          /* bit t: interactions.t is a RealAgnosticResidualInteractionBlock     */
-  int32_t hidden_max_l;           /* 0: hidden_irreps C x 0e; 1: C x 0e + C x 1o (other values invalid)  */
+  int32_t hidden_max_l;           /* 0: C x 0e; 1: C x 0e + C x 1o; 2: + C x 2e (other values invalid)    */
   double r_max;                   /* cutoff (Angstrom)                                                   */
   double c_act;                   /* e3nn normalize2mom(SiLU) constant of the radial MLP and the readout */
   double avg_num_neighbors[8];    /* per interaction                                                     */
+  int32_t hidden_mul[4];          /* multiplicity of each hidden l, as e3nn's Irreps has it              */
 } b2m_mace_desc;
 int b2m_create_mace(const b2m_mace_desc* desc, const int* devices, int ndev, b2m_handle* out);
 
