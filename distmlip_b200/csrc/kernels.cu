@@ -421,22 +421,34 @@ __device__ __forceinline__ void first_layer_half(const AtomConvArgs& a, const Ma
   }
 }
 
-// acc rows of half h (2h, 2h + 1) = x rows of half h . B^T (wg_mma64).  x is in the accumulator layout and is the
-// register A fragment as it stands: in k block ks a thread holds columns 8 ks + 2 (l%4) and + 1.  Bcan: the branch's
-// k-permuted canonical image (hi plane of 4096 floats, then lo).  x and acc may be the same array.
+// x rows of half h (2h, 2h + 1) in the accumulator layout as the register A fragment of wg_mma64: in k block ks a
+// thread holds columns 8 ks + 2 (l%4) and + 1, the k pair its slots take in the k-permuted images
 template <int R>
-__device__ __forceinline__ void wg_mm64_acc(const float (&x)[R][AC], int h, const float* Bcan, float (&acc)[R][AC]) {
-  float v[8][4];
+__device__ __forceinline__ void acc_frag(const float (&x)[R][AC], int h, float (&v)[8][4]) {
 #pragma unroll
   for (int ks = 0; ks < 8; ks++) {
     v[ks][0] = x[2 * h][2 * ks], v[ks][1] = x[2 * h + 1][2 * ks];
     v[ks][2] = x[2 * h][2 * ks + 1], v[ks][3] = x[2 * h + 1][2 * ks + 1];
   }
+}
+// a wg_mma64 result d as rows 2h, 2h + 1 of acc (accumulator layout)
+template <int R>
+__device__ __forceinline__ void frag_acc(const float (&d)[32], int h, float (&acc)[R][AC]) {
+#pragma unroll
+  for (int q = 0; q < 32; q++) acc[2 * h + ((q >> 1) & 1)][2 * (q >> 2) + (q & 1)] = d[q];
+}
+
+// acc rows of half h (2h, 2h + 1) = x rows of half h . B^T (wg_mma64).  x is in the accumulator layout and is the
+// register A fragment as it stands (acc_frag).  Bcan: the branch's k-permuted canonical image (hi plane of 4096
+// floats, then lo).  x and acc may be the same array.
+template <int R>
+__device__ __forceinline__ void wg_mm64_acc(const float (&x)[R][AC], int h, const float* Bcan, float (&acc)[R][AC]) {
+  float v[8][4];
+  acc_frag(x, h, v);
   const uint32_t b_hi = s_u32(Bcan);
   float d[32];
   wg_mma64(v, b_hi, b_hi + 4096u * 4u, 0, false, d);
-#pragma unroll
-  for (int q = 0; q < 32; q++) acc[2 * h + ((q >> 1) & 1)][2 * (q >> 2) + (q & 1)] = d[q];
+  frag_acc(d, h, acc);
 }
 
 // v[i] (row m.row(i)) summed over the 4 lanes of a quad, which share rows: lane l gets the sum of row l & 3
@@ -877,9 +889,11 @@ void launch_atomconv_bwd(cudaStream_t st, const AtomConvArgs& a, int num_sms) {
 // ============================================================================================
 // line-graph kernels: bond conv (HIDDEN) and angle update (!HIDDEN)
 // ============================================================================================
-// Persistent like the atom conv: min(tiles, SMs) CTAs, CTA c takes tiles c, c + grid, ...  Two [TM][LDE] buffers
-// alternate: tile number `it` of a CTA has its Ha[a] rows in buffer it & 1 (P) and its own angle rows in columns
-// 64..127 of the other buffer (Q).  Each copy completes on the barrier of its tile's stage (hbar / abar [it & 1], parity
+// The forward and the angle-update backward run in independent warpgroups over 64-angle tiles (LineSmemWg, below).
+// The bond-conv backward's four weight images do not fit in a CTA next to one buffer per warpgroup, so it keeps the
+// layout described here (LineSmem, LineSm, line_prologue).  Persistent like the atom conv: min(tiles, SMs) CTAs, CTA c
+// takes 128-angle tiles c, c + grid, ...  Two [TM][LDE] buffers alternate: tile number `it` of a CTA has its Ha[a]
+// rows in buffer it & 1 (P) and its own angle rows in columns 64..127 of the other buffer (Q).  Each copy completes on the barrier of its tile's stage (hbar / abar [it & 1], parity
 // stage_parity(it)).  One 64 KB weight slot holds the image the next product needs; images that share it are refilled
 // by bulk copies as soon as the product before has read the slot, and waited on (wbar, one phase per fill, in fill
 // order) just before the product that reads them.
@@ -914,15 +928,17 @@ struct LineSm {
 struct AngleIdx {
   int a, b, c;
 };
-__device__ __forceinline__ AngleIdx angle_idx(const LineArgs& a, int64_t r) {
+// angle r's indices, for a thread that owns a row of its tile (has_row) and r < A; else an empty row
+__device__ __forceinline__ AngleIdx angle_row(const LineArgs& a, int64_t r, bool has_row) {
   AngleIdx x{-1, -1, -1};
-  if (threadIdx.x < TM && r < a.A) {
+  if (has_row && r < a.A) {
     x.a = a.a_in[r];
     x.b = a.a_out[r];
     x.c = a.a_ctr[r];
   }
   return x;
 }
+__device__ __forceinline__ AngleIdx angle_idx(const LineArgs& a, int64_t r) { return angle_row(a, r, threadIdx.x < TM); }
 // threads 0..TM-1 publish their row of tile t into stage s's index arrays and start its Ha[a] copy into `buf`; the
 // caller has made sure, with a proxy fence and a barrier, that nobody reads `buf` or those arrays any more
 __device__ __forceinline__ void line_issue_ha(const LineArgs& a, const LineSm& sm, int64_t t, const AngleIdx& x,
@@ -961,12 +977,13 @@ __device__ __forceinline__ AngleIdx line_prologue(const LineArgs& a, const LineS
 
 // pre = ((Ha[a] + ang.Wg^T) + Hb[b]) + Xc[c] in place of acc (which holds ang.Wg^T), in the accumulator layout: Ha from
 // P at the thread's own positions, a row's 16 Hb and 16 Xc values as float2 loads issued before any is used.  Rows
-// r >= nvalid get 0.
+// r >= nvalid get 0.  R = AR: the four rows of a 128-row tile; R = 2: the two of a 64-row tile.
+template <int R>
 __device__ __forceinline__ void line_first_layer(const LineArgs& a, const Map& m, const float* P, const int* s_b,
-                                                 const int* s_c, int nvalid, float (&acc)[AR][AC]) {
+                                                 const int* s_c, int nvalid, float (&acc)[R][AC]) {
   const int c0 = 64 * m.branch + m.cb;
 #pragma unroll
-  for (int i = 0; i < AR; i++) {
+  for (int i = 0; i < R; i++) {
     const int r = m.row(i);
     const bool ok = r < nvalid;
     const float* hb = a.Hb + (size_t)(ok ? s_b[r] : 0) * D2 + c0;
@@ -992,118 +1009,232 @@ __device__ __forceinline__ void red_add_v2(float* p, float x, float y) {
   asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(x), "f"(y) : "memory");
 }
 
+// ---- the forward and the angle-update backward: independent warpgroups ----
+// Laid out like the atom conv: the warpgroups of a CTA do not wait for each other.  Warpgroup w of CTA c owns the
+// 64-angle tiles g, g + WG grid, g + 2 WG grid, ... (g = WG c + w, grid = min(ceil(tiles / WG), SMs)) and computes both
+// branches of each.  Each warpgroup has its own [TW][LDE] buffer for the tile's Ha[a] rows (per-row bulk copies; the
+// k-th fill completes phase k of its mbarrier), its own a_in / a_out / a_ctr slots and its own named barrier; the
+// weight images (and b2) are staged once per CTA behind the only CTA-wide barrier and are read-only afterwards.  The
+// next tile's indices load one tile ahead into registers, and its Ha copy is issued as soon as the warpgroup is done
+// with the buffer.  The angle rows need no stage: with the k-permuted images a thread's k pair of an angle row is one
+// float2 of that row, so they go from global memory straight into the register A fragments of ang . Wg^T
+// (line_ang_frag), and both branches' products share one tf32 split of them (wg_mma64_pair).
+template <int WG, int NIMG>
+struct LineSmemWg {
+  static constexpr int kBuf = 32;                  // [WG][TW][LDE] buffers (first 128 B: their mbarriers)
+  static constexpr int kW = kBuf + WG * TW * LDE;  // NIMG wgmma images of 16384 floats, staged once
+  static constexpr int kB2 = kW + NIMG * 16384;
+  static constexpr int kIdx = kB2 + 128;           // a_in, a_out, a_ctr: [WG][TW] each
+  static constexpr int kTotal = kIdx + 3 * WG * TW;
+  static constexpr size_t bytes = (size_t)kTotal * 4;
+  static_assert(bytes <= 232448, "line-graph shared memory");
+  static_assert(kW % 32 == 0 && kIdx % 4 == 0, "128-byte aligned images, 16-byte aligned index slots");
+};
+// forward: HIDDEN (bond conv) keeps Wg and W2 resident next to two buffers; !HIDDEN (angle update) has only Wg, and
+// three buffers fit next to it (three warpgroups, at most 168 registers per thread)
 template <bool HIDDEN>
-__global__ void __launch_bounds__(NT, 1) k_line_fwd(const LineArgs a) {
-  extern __shared__ __align__(128) float smem[];
-  const LineSm sm{smem};
-  const float* b2s = sm.b2();
-  const int tid = threadIdx.x;
-  const int64_t ntiles = (a.A + TM - 1) / TM, step = gridDim.x;
-  AngleIdx nxt = line_prologue(a, sm);
-  uint32_t wpar = 0;
+struct LineFwd {
+  static constexpr int WG = HIDDEN ? 2 : 3;
+  using Smem = LineSmemWg<WG, HIDDEN ? 2 : 1>;
+};
+// angle-update backward: Wg (recompute) and Wg^T (gang += gpre . Wg) resident, two warpgroups
+constexpr int LBWG = 2;
+using LineBwdSmem = LineSmemWg<LBWG, 2>;
 
+// the threads with rows lr = 0..TW-1 of 64-angle tile t publish their row's indices and start its Ha[a] copy into
+// `buf`, completing on `bar`; the caller has made sure, with a proxy fence and a barrier, that nobody reads `buf` or
+// the index slots any more
+__device__ __forceinline__ void line_issue_ha_wg(const LineArgs& a, int64_t t, const AngleIdx& x, int lr, float* buf,
+                                                 uint64_t* bar, int* s_a, int* s_b, int* s_c) {
+  if (lr == 0) mbar_expect_tx(bar, (uint32_t)min((int64_t)TW, a.A - t * TW) * 512u);
+  if (lr < TW) {
+    s_a[lr] = x.a;
+    s_b[lr] = x.b;
+    s_c[lr] = x.c;
+    if (x.a >= 0) bulk_g2s(buf + lr * LDE, a.Ha + (size_t)x.a * D2, 512u, bar);
+  }
+}
+// this thread's A fragment of ang . Wg^T for the 64-angle tile at row r0 (wg_mma64): rows m.row(0), m.row(1), and of
+// each the k pair 8 ks + cb, + 1 as one float2; rows r >= nvalid are 0
+__device__ __forceinline__ void line_ang_frag(const LineArgs& a, const Map& m, int64_t r0, int nvalid, float (&x)[8][4]) {
+  float2 u[2][8];
+#pragma unroll
+  for (int ii = 0; ii < 2; ii++) {
+    const int r = m.row(ii);
+    const bool ok = r < nvalid;
+    const float* p = a.ang + (size_t)(r0 + (ok ? r : 0)) * D + m.cb;
+#pragma unroll
+    for (int ks = 0; ks < 8; ks++) u[ii][ks] = ok ? __ldg(reinterpret_cast<const float2*>(p + 8 * ks)) : make_float2(0.f, 0.f);
+  }
+#pragma unroll
+  for (int ks = 0; ks < 8; ks++) x[ks][0] = u[0][ks].x, x[ks][1] = u[1][ks].x, x[ks][2] = u[0][ks].y, x[ks][3] = u[1][ks].y;
+}
+// L / G (rows 0, 1 of a 64-row tile, accumulator layout) = x . B^T for the two branch images of Bcan (hi plane of
+// 4096 floats, then lo, per branch): wg_mma64 twice, with one tf32 split of x and one commit
+__device__ __forceinline__ void wg_mma64_pair(const float (&x)[8][4], const float* Bcan, float (&L)[2][AC],
+                                              float (&G)[2][AC]) {
+  constexpr uint32_t LBO = 8 * 128;
+  uint32_t ah[8][4], al[8][4];
+#pragma unroll
+  for (int ks = 0; ks < 8; ks++)
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      ah[ks][q] = tf32_hi_bits(x[ks][q]);
+      al[ks][q] = __float_as_uint(x[ks][q] - __uint_as_float(ah[ks][q]));
+    }
+  float dL[32], dG[32];
+  auto mma = [&](float(&d)[32], uint32_t b_hi) {
+#pragma unroll
+    for (int ks = 0; ks < 8; ks++)
+#pragma unroll
+      for (int term = 0; term < 3; term++) {
+        const uint64_t bd = gmma_desc((term == 2 ? b_hi + 4096u * 4u : b_hi) + ks * 2 * LBO, LBO, 128u);
+        wgmma_tf32_n64_rA(d, term == 1 ? al[ks] : ah[ks], bd, (ks > 0 || term > 0) ? 1 : 0);
+      }
+  };
+  const uint32_t b = s_u32(Bcan);
+  acc_fence(dL);
+  acc_fence(dG);
+  wgmma_fence();
+  mma(dL, b);
+  mma(dG, b + 8192u * 4u);
+  wgmma_commit();
+  wgmma_wait_all();
+  acc_fence(dL);
+  acc_fence(dG);
+  frag_acc(dL, 0, L);
+  frag_acc(dG, 0, G);
+}
+
+// Forward.  Per tile: ang . Wg^T of both branches (registers) while the Ha rows land; pre = ((Ha + ang.Wg^T) + Hb) +
+// Xc of both branches (line_first_layer).  !HIDDEN: the buffer is free from here on, so the next tile's Ha copy is
+// issued before ang_out = ang + silu(pre_L) sigm(pre_G) is formed in registers and stored.  HIDDEN: silu(pre) . W2^T
+// + b2 per branch (register A operands), m = silu(u) sigm(v) in registers, stored over the thread's own Ha values of
+// columns 0..63, and aggB[b] += m in one scatter pass over the warpgroup's 64 rows; then the next tile's copy.
+template <bool HIDDEN>
+__global__ void __launch_bounds__(128 * LineFwd<HIDDEN>::WG, 1) k_line_fwd(const LineArgs a) {
+  using S = typename LineFwd<HIDDEN>::Smem;
+  constexpr int WG = LineFwd<HIDDEN>::WG;
+  extern __shared__ __align__(128) float smem[];
+  const int tid = threadIdx.x, w = tid >> 7, lr = tid & 127;  // warpgroup; thread lr < TW copies row lr
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem) + w;      // this warpgroup's buffer
+  const float* Wg = smem + S::kW;
+  const float* W2 = smem + S::kW + 16384;  // HIDDEN
+  const float* b2s = smem + S::kB2;        // HIDDEN
+  float* P = smem + S::kBuf + w * TW * LDE;
+  int* s_a = reinterpret_cast<int*>(smem + S::kIdx) + w * TW;
+  int* s_b = reinterpret_cast<int*>(smem + S::kIdx) + (WG + w) * TW;
+  int* s_c = reinterpret_cast<int*>(smem + S::kIdx) + (2 * WG + w) * TW;
+
+  // tile numbers in 32 bits (up to 2^37 angles): the three-warpgroup forward has no register to spare
+  const int ntiles = (int)((a.A + TW - 1) / TW), first = WG * blockIdx.x + w, step = WG * gridDim.x;
+  if (tid == 0) {
+    for (int i = 0; i < WG; i++) mbar_init(reinterpret_cast<uint64_t*>(smem) + i, 1);
+    fence_barrier_init();
+  }
+  AngleIdx nxt = angle_row(a, (int64_t)first * TW + lr, lr < TW);
+  // loop-invariant operands, once per CTA
+  stage_w<128 * WG>(smem + S::kW, a.Wgcan, 4096);
+  if (HIDDEN) {
+    stage_w<128 * WG>(smem + S::kW + 16384, a.W2can, 4096);
+    if (tid < 128) smem[S::kB2 + tid] = a.b2[tid];
+  }
+  __syncthreads();
+  if (first < ntiles)  // the last CTA's later warpgroups have no tile when the tile count is not a multiple of WG
+    line_issue_ha_wg(a, first, nxt, lr, P, mbar, s_a, s_b, s_c);
+  nxt = angle_row(a, (int64_t)(first + step) * TW + lr, lr < TW);
+
+  const Map m;
+  Map mL = m, mG = m;  // the first layer's columns of each branch
+  mL.branch = 0;
+  mG.branch = 1;
   int it = 0;
-  for (int64_t t = blockIdx.x; t < ntiles; t += step, it++) {
-    const int s = it & 1;
-    float* P = sm.buf(s);
-    float* Q = sm.buf(s ^ 1);
-    const int* s_b = sm.idx(s, 1);
-    const int* s_c = sm.idx(s, 2);
-    const int64_t r0 = t * TM;
-    const int nvalid = (int)min((int64_t)TM, a.A - r0);
-    const bool more = t + step < ntiles;
-    const Map m;
-    float acc[AR][AC];
-    // ang . Wg^T (angle rows in Q)
-    mbar_wait(&sm.abar()[s], stage_parity(it));
-    mbar_wait(sm.wbar(), wpar);  // Wg
-    if (HIDDEN) wpar ^= 1;       // (!HIDDEN: Wg stays, its only phase is complete)
-    gemm64(Q, LDE, 64, sm.W() + m.branch * 8192, acc);
-    fence_proxy_async_smem();  // this thread's generic accesses of Q come before its bulk refill
-    __syncthreads();           // Q (angle rows, the previous tile's gates) and its index arrays are free; so is Wg
-    if (more) {
-      line_issue_ha(a, sm, t + step, nxt, Q, s ^ 1);
-      nxt = angle_idx(a, (t + 2 * step) * TM + tid);
+  for (int t = first; t < ntiles; t += step, it++) {
+    int64_t r0 = (int64_t)t * TW;
+    asm volatile("" : "+l"(r0));  // row addresses formed per tile: carried across tiles they hold registers
+    const int nvalid = (int)min((int64_t)TW, a.A - r0);
+    float L[2][AC], G[2][AC];
+    {
+      float x[8][4];
+      line_ang_frag(a, m, r0, nvalid, x);
+      wg_sync(w);  // the tile's indices are published
+      wg_mma64_pair(x, Wg, L, G);
     }
-    if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.W2can, 16384 * 4, sm.wbar());
-    mbar_wait(&sm.hbar()[s], stage_parity(it));
-    line_first_layer(a, m, P, s_b, s_c, nvalid, acc);
-    // HIDDEN: hid = silu(pre) straight into the second layer;  !HIDDEN: pre is the last layer's pre-activation
+    mbar_wait(mbar, (uint32_t)it & 1u);
+    line_first_layer(a, mL, P, s_b, s_c, nvalid, L);
+    line_first_layer(a, mG, P, s_b, s_c, nvalid, G);
+    if constexpr (!HIDDEN) {
+      fence_proxy_async_smem();  // this thread's generic accesses of the buffer come before its bulk refill
+      wg_sync(w);                // the warpgroup is done with the buffer and the indices
+      if (t + step < ntiles) {
+        line_issue_ha_wg(a, t + step, nxt, lr, P, mbar, s_a, s_b, s_c);
+        nxt = angle_row(a, ((int64_t)t + 2 * step) * TW + lr, lr < TW);
+      }
+      // ang_out = ang + silu(pre_L) sigm(pre_G), the angle rows re-read (L2) as float2 pairs
 #pragma unroll
-    for (int i = 0; i < AR; i++)
+      for (int ii = 0; ii < 2; ii++) {
+        const int r = m.row(ii);
+        if (r >= nvalid) continue;
+        const float* ang = a.ang + (size_t)(r0 + r) * D;
+        float* out = a.ang_out + (size_t)(r0 + r) * D;
+        float2 av[AC / 2];
 #pragma unroll
-      for (int j = 0; j < AC; j++) acc[i][j] = HIDDEN || m.branch == 0 ? silu_f(acc[i][j]) : sigm(acc[i][j]);
-    if (HIDDEN) {
-      mbar_wait(sm.wbar(), wpar);  // W2
-      wpar ^= 1;
-      wg_mm64_acc(acc, 0, sm.W() + m.branch * 8192, acc);
-      wg_mm64_acc(acc, 1, sm.W() + m.branch * 8192, acc);
+        for (int jj = 0; jj < AC / 2; jj++) av[jj] = __ldg(reinterpret_cast<const float2*>(ang + m.col(2 * jj)));
 #pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int j = 0; j < AC; j++) {
-          const float u = acc[i][j] + b2s[m.branch * 64 + m.col(j)];
-          acc[i][j] = m.branch == 0 ? silu_f(u) : sigm(u);
-        }
-    }
-    fence_proxy_async_smem();  // this thread's generic accesses of P come before its bulk refill
-    __syncthreads();           // the Ha rows in P have been read, its columns 64..127 are free (HIDDEN: and so is W2)
-    if (more) {
-      line_issue_ang(a, sm, t + step, P, s ^ 1);
-      if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.Wgcan, 16384 * 4, sm.wbar());
-    }
-    // m = L . G: warpgroup 1 hands G over through columns 0..63 of P, at the positions warpgroup 0 owns as well
-    if (m.branch == 1) {
-#pragma unroll
-      for (int i = 0; i < AR; i++)
-#pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++) st_f2(P + m.row(i) * LDE + m.col(2 * jj), acc[i][2 * jj], acc[i][2 * jj + 1]);
-    }
-    __syncthreads();
-    if (m.branch == 0) {
-#pragma unroll
-      for (int i = 0; i < AR; i++) {
-        const int r = m.row(i);
-        if (HIDDEN) {
-#pragma unroll
-          for (int jj = 0; jj < AC / 2; jj++) {
-            float* p = P + r * LDE + m.col(2 * jj);
-            const float2 g = ld_f2(p);
-            st_f2(p, acc[i][2 * jj] * g.x, acc[i][2 * jj + 1] * g.y);
-          }
-        } else if (r < nvalid) {  // ang_out = ang + m, the angle rows re-read (L2) as float2 pairs
-          const float* ang = a.ang + (size_t)(r0 + r) * D;
-          float* out = a.ang_out + (size_t)(r0 + r) * D;
-          float2 av[AC / 2];
-#pragma unroll
-          for (int jj = 0; jj < AC / 2; jj++) av[jj] = __ldg(reinterpret_cast<const float2*>(ang + m.col(2 * jj)));
-#pragma unroll
-          for (int jj = 0; jj < AC / 2; jj++) {
-            const int c = m.col(2 * jj);
-            const float2 g = ld_f2(P + r * LDE + c);
-            st_f2(out + c, av[jj].x + acc[i][2 * jj] * g.x, av[jj].y + acc[i][2 * jj + 1] * g.y);
-          }
+        for (int jj = 0; jj < AC / 2; jj++) {
+          const float l0 = silu_f(L[ii][2 * jj]), l1 = silu_f(L[ii][2 * jj + 1]);
+          const float g0 = sigm(G[ii][2 * jj]), g1 = sigm(G[ii][2 * jj + 1]);
+          st_f2(out + m.col(2 * jj), av[jj].x + l0 * g0, av[jj].y + l1 * g1);
         }
       }
-    }
-    if (HIDDEN) {
-      __syncthreads();
-      scatter_rows<16>(P, s_b, a.aggB, nullptr, nullptr, nullptr, nullptr);  // aggB[b] += m
+    } else {
+      // hid = silu(pre) straight into the second layer; u (L) and v (G) + b2
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) L[ii][j] = silu_f(L[ii][j]);
+      wg_mm64_acc(L, 0, W2, L);
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) L[ii][j] = silu_f(L[ii][j] + b2s[m.col(j)]);
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int j = 0; j < AC; j++) G[ii][j] = silu_f(G[ii][j]);
+      wg_mm64_acc(G, 0, W2 + 8192, G);
+      // m = silu(u) sigm(v), over the thread's own Ha values of columns 0..63
+#pragma unroll
+      for (int ii = 0; ii < 2; ii++)
+#pragma unroll
+        for (int jj = 0; jj < AC / 2; jj++) {
+          const float g0 = sigm(G[ii][2 * jj] + b2s[64 + m.col(2 * jj)]);
+          const float g1 = sigm(G[ii][2 * jj + 1] + b2s[64 + m.col(2 * jj + 1)]);
+          st_f2(P + m.row(ii) * LDE + m.col(2 * jj), L[ii][2 * jj] * g0, L[ii][2 * jj + 1] * g1);
+        }
+      wg_sync(w);
+      scatter_rows<16, TW, 128>(P, s_b, a.aggB, nullptr, nullptr, nullptr, nullptr);  // aggB[b] += m
+      fence_proxy_async_smem();  // this thread's generic accesses of the buffer come before its bulk refill
+      wg_sync(w);                // the warpgroup is done with the buffer and the indices
+      if (t + step < ntiles) {
+        line_issue_ha_wg(a, t + step, nxt, lr, P, mbar, s_a, s_b, s_c);
+        nxt = angle_row(a, ((int64_t)t + 2 * step) * TW + lr, lr < TW);
+      }
     }
   }
 }
 
-// Backward, mirroring the atom conv: P (buffer it & 1) holds the tile's Ha rows, then (HIDDEN) its pre-activations,
-// each thread's over its own Ha values, then their adjoints gpre, which the scatter phase and gpre.Wg read row-major;
-// H (the other buffer) holds the angle rows, then the last layer's outputs parked at each thread's own positions -- u
-// (L), oG = sigm(v) (G) -- so that the reverse keeps one 64-row half of accumulators live at a time and reads its own
-// and its partner's values back.  Both products of the hidden layer take their A operand from registers.  Once H has
-// been read for the last time (by the elementwise reverse), the next tile's Ha rows are copied into it (H becomes the
-// next tile's P); once the scatter phase and gang += gpre.Wg have read P, the next tile's angle rows go into its
-// columns 64..127 (P becomes the next tile's H).  Weight images through the one slot: HIDDEN Wg -> W2 -> W2^T -> Wg^T
-// per tile, !HIDDEN Wg -> Wg^T.
-template <bool HIDDEN>
-__global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
+// Bond-conv backward (HIDDEN), in the 128-angle layout (LineSmem): its four weight images (Wg, W2, W2^T, Wg^T) do not
+// fit next to one buffer per warpgroup, so they take turns in the one slot.  P (buffer it & 1) holds the tile's Ha rows,
+// then its pre-activations, each thread's over its own Ha values, then their adjoints gpre, which the scatter phase and
+// gpre.Wg read row-major; H (the other buffer) holds the angle rows, then the last layer's outputs parked at each
+// thread's own positions -- u (L), oG = sigm(v) (G) -- so that the reverse keeps one 64-row half of accumulators live
+// at a time and reads its own and its partner's values back.  Both products of the hidden layer take their A operand
+// from registers.  Once H has been read for the last time (by the elementwise reverse), the next tile's Ha rows are
+// copied into it (H becomes the next tile's P); once the scatter phase and gang += gpre.Wg have read P, the next
+// tile's angle rows go into its columns 64..127 (P becomes the next tile's H).  Weight images through the one slot: Wg
+// -> W2 -> W2^T -> Wg^T per tile.
+__device__ __forceinline__ void line_bwd_bond(const LineArgs& a) {
   extern __shared__ __align__(128) float smem[];
   const LineSm sm{smem};
   const float* b2s = sm.b2();
@@ -1130,45 +1261,43 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
     wpar ^= 1;
     gemm64(H, LDE, 64, sm.W() + m.branch * 8192, acc);
     __syncthreads();  // both warpgroups have read the angle rows and Wg: H and the slot may be written
-    if (tid == 0) bulk_g2s_image(sm.W(), HIDDEN ? a.W2can : a.WgTcan, 16384 * 4, sm.wbar());
+    if (tid == 0) bulk_g2s_image(sm.W(), a.W2can, 16384 * 4, sm.wbar());
     mbar_wait(&sm.hbar()[s], stage_parity(it));
     line_first_layer(a, m, P, s_b, s_c, nvalid, acc);
-    if (HIDDEN) {
-      // pre overwrites the thread's own Ha values in P (same thread, same addresses); silu(pre) . W2^T + b2 = u | v
+    // pre overwrites the thread's own Ha values in P (same thread, same addresses); silu(pre) . W2^T + b2 = u | v
 #pragma unroll
-      for (int i = 0; i < AR; i++)
+    for (int i = 0; i < AR; i++)
 #pragma unroll
-        for (int jj = 0; jj < AC / 2; jj++) {
-          float& x0 = acc[i][2 * jj];
-          float& x1 = acc[i][2 * jj + 1];
-          st_f2(P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), x0, x1);
-          x0 = silu_f(x0);
-          x1 = silu_f(x1);
-        }
-      mbar_wait(sm.wbar(), wpar);  // W2
-      wpar ^= 1;
-    }
-    // the pre-activation of the last layer of this GatedMLP (u | v; HIDDEN: silu(pre) . W2^T + b2, one 64-row half at a
+      for (int jj = 0; jj < AC / 2; jj++) {
+        float& x0 = acc[i][2 * jj];
+        float& x1 = acc[i][2 * jj + 1];
+        st_f2(P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), x0, x1);
+        x0 = silu_f(x0);
+        x1 = silu_f(x1);
+      }
+    mbar_wait(sm.wbar(), wpar);  // W2
+    wpar ^= 1;
+    // the pre-activation of the last layer of this GatedMLP (u | v = silu(pre) . W2^T + b2, one 64-row half at a
     // time), parked in H at the thread's own positions as u (L) and oG = sigm(v) (G)
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      if (HIDDEN) wg_mm64_acc(acc, h, sm.W() + m.branch * 8192, acc);
+      wg_mm64_acc(acc, h, sm.W() + m.branch * 8192, acc);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++)
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
           const int i = 2 * h + ii;
-          const float u0 = HIDDEN ? acc[i][2 * jj] + b2s[m.branch * 64 + m.col(2 * jj)] : acc[i][2 * jj];
-          const float u1 = HIDDEN ? acc[i][2 * jj + 1] + b2s[m.branch * 64 + m.col(2 * jj + 1)] : acc[i][2 * jj + 1];
+          const float u0 = acc[i][2 * jj] + b2s[m.branch * 64 + m.col(2 * jj)];
+          const float u1 = acc[i][2 * jj + 1] + b2s[m.branch * 64 + m.col(2 * jj + 1)];
           st_f2(H + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj), m.branch == 0 ? u0 : sigm(u0),
                 m.branch == 0 ? u1 : sigm(u1));
         }
     }
-    __syncthreads();  // H holds both branches' values (HIDDEN: and W2 has been read)
-    if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.W2Tcan, 16384 * 4, sm.wbar());
+    __syncthreads();  // H holds both branches' values and W2 has been read
+    if (tid == 0) bulk_g2s_image(sm.W(), a.W2Tcan, 16384 * 4, sm.wbar());
     // reverse, per 64-row half: acc = dE/du (L) / dE/dv (G) from the values parked in H (the partner's sigm(v) /
-    // silu(u) formed from them);  HIDDEN: ghid = [gu . W2L, gv . W2G] from the adjoints in registers and gpre = ghid *
-    // dsilu(pre), into P over pre;  !HIDDEN: gpre = acc, into P
+    // silu(u) formed from them); ghid = [gu . W2L, gv . W2G] from the adjoints in registers and gpre = ghid *
+    // dsilu(pre), into P over pre
 #pragma unroll
     for (int h = 0; h < 2; h++) {
       bool ok[2];
@@ -1177,8 +1306,7 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
       for (int ii = 0; ii < 2; ii++) {
         const int r = m.row(2 * h + ii);
         ok[ii] = r < nvalid;
-        const float* gsrc =
-            HIDDEN ? a.gaggB + (size_t)(ok[ii] ? s_b[r] : 0) * D : a.gang + (size_t)(r0 + (ok[ii] ? r : 0)) * D;
+        const float* gsrc = a.gaggB + (size_t)(ok[ii] ? s_b[r] : 0) * D;
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++)
           gm2[ii][jj] = ok[ii] ? *reinterpret_cast<const float2*>(gsrc + m.col(2 * jj)) : make_float2(0.f, 0.f);
@@ -1207,38 +1335,32 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
           acc[i][j] = g;
         }
       }
-      if (HIDDEN) {
-        if (h == 0) mbar_wait(sm.wbar(), wpar);  // W2^T
-        wg_mm64_acc(acc, h, sm.W() + m.branch * 8192, acc);
-      }
+      if (h == 0) mbar_wait(sm.wbar(), wpar);  // W2^T
+      wg_mm64_acc(acc, h, sm.W() + m.branch * 8192, acc);
 #pragma unroll
       for (int ii = 0; ii < 2; ii++)
 #pragma unroll
         for (int jj = 0; jj < AC / 2; jj++) {
           const int i = 2 * h + ii;
           float* p = P + m.row(i) * LDE + m.branch * 64 + m.col(2 * jj);
-          if (HIDDEN) {
-            const float2 pre = ld_f2(p);
-            st_f2(p, acc[i][2 * jj] * dsilu_f(pre.x), acc[i][2 * jj + 1] * dsilu_f(pre.y));
-          } else {
-            st_f2(p, acc[i][2 * jj], acc[i][2 * jj + 1]);
-          }
+          const float2 pre = ld_f2(p);
+          st_f2(p, acc[i][2 * jj] * dsilu_f(pre.x), acc[i][2 * jj + 1] * dsilu_f(pre.y));
         }
     }
-    if (HIDDEN) wpar ^= 1;
+    wpar ^= 1;
     fence_proxy_async_smem();  // this thread's generic accesses of H come before its bulk refill
-    __syncthreads();           // H, its stage's index arrays and (HIDDEN) W2^T are free; P holds gpre
+    __syncthreads();           // H, its stage's index arrays and W2^T are free; P holds gpre
     if (more) {
       line_issue_ha(a, sm, t + step, nxt, H, s ^ 1);
       nxt = angle_idx(a, (t + 2 * step) * TM + tid);
     }
-    if (HIDDEN && tid == 0) bulk_g2s_image(sm.W(), a.WgTcan, 16384 * 4, sm.wbar());
+    if (tid == 0) bulk_g2s_image(sm.W(), a.WgTcan, 16384 * 4, sm.wbar());
     // ---- scatter phase (reads P and this tile's index arrays) ----
     // gHb[b] += gpre and gXc[c] += gpre (segmented), gHa[a] += gpre: one pass over P
     scatter_rows<32>(P, s_b, a.gHb, s_c, a.gXc, s_a, a.gHa);
     // gang += gpre @ Wg   (K = 128, N = 64) on the tensor cores: warpgroup w takes rows 64 w .. 64 w + 63.  Each angle
-    // row belongs to this tile alone, and (!HIDDEN) its upstream reads of gang are behind the barrier above, so the
-    // update is a fire-and-forget reduction: one addition per element, as a load-add-store would do.
+    // row belongs to this tile alone, so the update is a fire-and-forget reduction: one addition per element, as a
+    // load-add-store would do.
     mbar_wait(sm.wbar(), wpar);  // Wg^T
     wpar ^= 1;
     {
@@ -1261,25 +1383,156 @@ __global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
   }
 }
 
+// Angle-update backward (!HIDDEN), in the warpgroup layout of the forward with Wg and Wg^T resident.  Per tile: pre of
+// both branches as in the forward (u = pre_L, v = pre_G); the elementwise reverse in registers, with oG = sigm(v) and g
+// the tile's own rows of gang (loaded at the top of the tile with the angle rows): gpre_L = dE/du = g oG dsilu(u),
+// gpre_G = dE/dv = g silu(u) oG (1 - oG), stored over the thread's own Ha values; gHb[b] += gpre and gXc[c] += gpre
+// (segmented) and gHa[a] += gpre in one scatter pass over the warpgroup's 64 rows; the next tile's copy; then, while it
+// flies, gang += gpre . Wg (K = 128) with gpre as the register A operand, one K half per branch.  The thread that adds
+// into a gang element has read its upstream value at the top of the tile, so the update is a fire-and-forget
+// reduction: one addition per element, as a load-add-store would do.
+__device__ __forceinline__ void line_bwd_angle(const LineArgs& a) {
+  using S = LineBwdSmem;
+  constexpr int WG = LBWG;
+  extern __shared__ __align__(128) float smem[];
+  const int tid = threadIdx.x, w = tid >> 7, lr = tid & 127;  // warpgroup; thread lr < TW copies row lr
+  uint64_t* mbar = reinterpret_cast<uint64_t*>(smem) + w;      // this warpgroup's buffer
+  const float* Wg = smem + S::kW;
+  const float* WgT = smem + S::kW + 16384;
+  float* P = smem + S::kBuf + w * TW * LDE;
+  int* s_a = reinterpret_cast<int*>(smem + S::kIdx) + w * TW;
+  int* s_b = reinterpret_cast<int*>(smem + S::kIdx) + (WG + w) * TW;
+  int* s_c = reinterpret_cast<int*>(smem + S::kIdx) + (2 * WG + w) * TW;
+
+  // tile numbers in 32 bits (up to 2^37 angles): the three-warpgroup forward has no register to spare
+  const int ntiles = (int)((a.A + TW - 1) / TW), first = WG * blockIdx.x + w, step = WG * gridDim.x;
+  if (tid == 0) {
+    for (int i = 0; i < WG; i++) mbar_init(reinterpret_cast<uint64_t*>(smem) + i, 1);
+    fence_barrier_init();
+  }
+  AngleIdx nxt = angle_row(a, (int64_t)first * TW + lr, lr < TW);
+  // loop-invariant operands, once per CTA
+  stage_w<128 * WG>(smem + S::kW, a.Wgcan, 4096);
+  stage_w<128 * WG>(smem + S::kW + 16384, a.WgTcan, 4096);
+  __syncthreads();
+  if (first < ntiles)  // the last CTA's second warpgroup has no tile when the tile count is odd
+    line_issue_ha_wg(a, first, nxt, lr, P, mbar, s_a, s_b, s_c);
+  nxt = angle_row(a, (int64_t)(first + step) * TW + lr, lr < TW);
+
+  const Map m;
+  Map mL = m, mG = m;  // the first layer's columns of each branch
+  mL.branch = 0;
+  mG.branch = 1;
+  int it = 0;
+  for (int t = first; t < ntiles; t += step, it++) {
+    int64_t r0 = (int64_t)t * TW;
+    asm volatile("" : "+l"(r0));  // row addresses formed per tile: carried across tiles they hold registers
+    const int nvalid = (int)min((int64_t)TW, a.A - r0);
+    // the upstream gradients (both rows' 16 gang pairs) load with the angle rows, before anything waits
+    bool ok[2];
+    float2 gm2[2][AC / 2];
+#pragma unroll
+    for (int ii = 0; ii < 2; ii++) {
+      const int r = m.row(ii);
+      ok[ii] = r < nvalid;
+      const float* gsrc = a.gang + (size_t)(r0 + (ok[ii] ? r : 0)) * D;
+#pragma unroll
+      for (int jj = 0; jj < AC / 2; jj++)
+        gm2[ii][jj] = ok[ii] ? *reinterpret_cast<const float2*>(gsrc + m.col(2 * jj)) : make_float2(0.f, 0.f);
+    }
+    float L[2][AC], G[2][AC];
+    {
+      float x[8][4];
+      line_ang_frag(a, m, r0, nvalid, x);
+      wg_sync(w);  // the tile's indices are published
+      wg_mma64_pair(x, Wg, L, G);
+    }
+    mbar_wait(mbar, (uint32_t)it & 1u);
+    line_first_layer(a, mL, P, s_b, s_c, nvalid, L);
+    line_first_layer(a, mG, P, s_b, s_c, nvalid, G);
+    // elementwise reverse, in place: L <- gpre_L, G <- gpre_G
+#pragma unroll
+    for (int ii = 0; ii < 2; ii++) {
+#pragma unroll
+      for (int j = 0; j < AC; j++) {
+        const float u = L[ii][j], oG = sigm(G[ii][j]);
+        float gu = 0.f, gv = 0.f;
+        if (ok[ii]) {
+          const float gm = (j & 1) ? gm2[ii][j >> 1].y : gm2[ii][j >> 1].x;
+          const float sg = sigm(u);
+          gu = gm * oG * (sg * (1.f + u * (1.f - sg)));
+          gv = gm * silu_f(u) * oG * (1.f - oG);
+        }
+        L[ii][j] = gu;
+        G[ii][j] = gv;
+      }
+#pragma unroll
+      for (int jj = 0; jj < AC / 2; jj++) {
+        st_f2(P + m.row(ii) * LDE + m.col(2 * jj), L[ii][2 * jj], L[ii][2 * jj + 1]);
+        st_f2(P + m.row(ii) * LDE + 64 + m.col(2 * jj), G[ii][2 * jj], G[ii][2 * jj + 1]);
+      }
+    }
+    wg_sync(w);  // P holds the tile's gpre
+    scatter_rows<32, TW, 128>(P, s_b, a.gHb, s_c, a.gXc, s_a, a.gHa);
+    fence_proxy_async_smem();  // this thread's generic accesses of the buffer come before its bulk refill
+    wg_sync(w);                // the warpgroup is done with the buffer and the indices
+    if (t + step < ntiles) {
+      line_issue_ha_wg(a, t + step, nxt, lr, P, mbar, s_a, s_b, s_c);
+      nxt = angle_row(a, ((int64_t)t + 2 * step) * TW + lr, lr < TW);
+    }
+    // gang += gpre . Wg   (K = 128, N = 64) on the tensor cores, from the registers while the next tile's copy flies
+    {
+      float v[8][4], d[32];
+      const uint32_t bh = s_u32(WgT), bl = bh + 64u * 128u * 4u;
+      acc_frag(L, 0, v);
+      wg_mma64(v, bh, bl, 0, false, d);
+      acc_frag(G, 0, v);
+      wg_mma64(v, bh, bl, 64, true, d);
+#pragma unroll
+      for (int q = 0; q < 32; q += 2) {
+        const int r = m.rb + 8 * ((q >> 1) & 1), c = 8 * (q >> 2) + m.cb;
+        if (r < nvalid) red_add_v2(&a.gang[(size_t)(r0 + r) * D + c], d[q], d[q + 1]);
+      }
+    }
+  }
+}
+
+static_assert(128 * LBWG == NT, "both backward kernels run 256-thread CTAs");
+template <bool HIDDEN>
+__global__ void __launch_bounds__(NT, 1) k_line_bwd(const LineArgs a) {
+  if constexpr (HIDDEN)
+    line_bwd_bond(a);
+  else
+    line_bwd_angle(a);
+}
+
 void launch_line_fwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms) {
   if (a.A <= 0) return;
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_) {
-    B2M_CK(cudaFuncSetAttribute(k_line_fwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
-    B2M_CK(cudaFuncSetAttribute(k_line_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
+    B2M_CK(cudaFuncSetAttribute(k_line_fwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)LineFwd<true>::Smem::bytes));
+    B2M_CK(cudaFuncSetAttribute(k_line_fwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)LineFwd<false>::Smem::bytes));
   }
-  const int grid = std::min(cdiv(a.A, TM), num_sms);
-  with_flags([&](auto kHidden) { launch(k_line_fwd<kHidden>, grid, NT, LineSmem::bytes, st, a); }, hidden);
+  with_flags(
+      [&](auto kHidden) {
+        using F = LineFwd<decltype(kHidden)::value>;
+        launch(k_line_fwd<kHidden>, std::min(cdiv(cdiv(a.A, TW), F::WG), num_sms), 128 * F::WG, F::Smem::bytes, st, a);
+      },
+      hidden);
 }
 void launch_line_bwd(cudaStream_t st, const LineArgs& a, bool hidden, int num_sms) {
   if (a.A <= 0) return;
   static PerDeviceOnce attr;
   if (auto once_ = attr.first(); once_) {
     B2M_CK(cudaFuncSetAttribute(k_line_bwd<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
-    B2M_CK(cudaFuncSetAttribute(k_line_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineSmem::bytes));
+    B2M_CK(cudaFuncSetAttribute(k_line_bwd<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LineBwdSmem::bytes));
   }
-  const int grid = std::min(cdiv(a.A, TM), num_sms);
-  with_flags([&](auto kHidden) { launch(k_line_bwd<kHidden>, grid, NT, LineSmem::bytes, st, a); }, hidden);
+  if (hidden)
+    launch(k_line_bwd<true>, std::min(cdiv(a.A, TM), num_sms), NT, LineSmem::bytes, st, a);
+  else
+    launch(k_line_bwd<false>, std::min(cdiv(cdiv(a.A, TW), LBWG), num_sms), NT, LineBwdSmem::bytes, st, a);
 }
 
 // ============================================================================================
