@@ -19,7 +19,10 @@ SYMBOLS = [
     "b2m_compute_resident", "b2m_get_results", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
     "b2m_debug_tensor", "b2m_last_timings", "b2m_release_workspace", "b2m_set_view", "b2m_create_tensornet",
     "b2m_set_atomic", "b2m_get_atomic", "b2m_set_heat_flux", "b2m_compute_heat_flux", "b2m_create_mace",
+    "b2m_set_partition_policy",
 ]
+
+PARTITION_EQUAL, PARTITION_BALANCED = 0, 1
 
 
 class ModelDesc(C.Structure):
@@ -83,6 +86,7 @@ def load_library():
     lib.b2m_comm_unique_id.argtypes = [C.c_char_p]
     lib.b2m_comm_init.argtypes = [vp, C.c_char_p, i32, i32]
     lib.b2m_set_partition.argtypes = [vp, i32, i32]
+    lib.b2m_set_partition_policy.argtypes = [vp, i32]
     lib.b2m_set_structure.argtypes = [vp, i64, P(dbl), P(dbl), P(C.c_int32), P(C.c_int), dbl]
     lib.b2m_compute.argtypes = [vp, i32, i32, P(dbl), P(C.c_float), P(C.c_float)]
     lib.b2m_compute_resident.argtypes = [vp, i32, i32, i32, P(dbl), P(C.c_float)]
@@ -193,6 +197,11 @@ class Engine:
     def set_partition(self, rank: int, world: int):
         self._ck(self.lib.b2m_set_partition(self.h, rank, world))
         self.rank, self.world = rank, world
+
+    def set_partition_policy(self, policy: int):
+        """PARTITION_EQUAL (default: the reference's equally spaced slab walls) or PARTITION_BALANCED (walls at the
+        quantiles of the atoms' edge + angle work); takes effect at the next set_structure, on every partition"""
+        self._ck(self.lib.b2m_set_partition_policy(self.h, int(policy)))
 
     # ---- structure / compute ----
     def set_structure(self, cart, lattice, species, pbc, tol=1e-8):

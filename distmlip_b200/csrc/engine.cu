@@ -194,6 +194,7 @@ struct b2m_engine {
   std::vector<cudaEvent_t> hev;    // one event per halo-exchange point of a run
   int hpoint = 0;
   int view = 0;                    // leader: partition addressed by the inspection calls (b2m_set_view)
+  int partition_policy = B2M_PARTITION_EQUAL;  // b2m_set_partition_policy, applied at the next graph build
   // page-locked staging owned by the library: host arrays go through it with a few copy threads (a single-threaded
   // memcpy of 24 MB of positions was the largest host item of an end-to-end step at 1 M atoms)
   void* pin_in = nullptr;   // [N,3] f64 positions followed by [N] i32 species
@@ -1134,6 +1135,14 @@ int b2m_set_partition(b2m_handle h, int rank, int world) {
   API_END
 }
 
+int b2m_set_partition_policy(b2m_handle h, int policy) {
+  API_BEGIN
+  B2M_REQUIRE(policy == B2M_PARTITION_EQUAL || policy == B2M_PARTITION_BALANCED, B2M_ERR_INVALID,
+              "partition policy must be B2M_PARTITION_EQUAL (0) or B2M_PARTITION_BALANCED (1)");
+  each_member(h, [&](b2m_engine* e) { e->partition_policy = policy; });
+  API_END
+}
+
 static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart, const double* lattice9,
                               const int32_t* species, const int* pbc3, double tol) {
   h->have_graph = false;
@@ -1149,6 +1158,7 @@ static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart,
   B2M_CK(cudaEventRecord(h->ev[3], h->st));
   h->atomic_last = 0;  // per-atom results of an earlier structure are gone
   h->hf_n = 0, h->hf_seed = -1;
+  h->g.balanced = h->partition_policy == B2M_PARTITION_BALANCED;
   if (h->hf_reach > 0) {
     // heat flux: the unfolded cell, built on the device, is the graph's input; no periodicity
     h->uf.build(h->st, natoms, cart, species, lattice9, pbc3, h->hf_reach);

@@ -15,6 +15,8 @@
 //   * bond nodes: owned = bonds whose dst is owned; halo = every bond whose dst is a halo atom
 //     ............................................................. :497-653
 //   * line graph (s->d) -> (d->x), x != s by atom index, centre d . :703-751
+// Not in the reference: the balanced partition policy (Graph::balanced, DESIGN.md §4.1) places the walls at the
+// quantiles of the atoms' edge + angle work, slabs at least 2 (r_cut + r_bond) wide across the walls.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -153,6 +155,52 @@ __global__ void k_owner_cell(int64_t n, const double* __restrict__ fracw, Walls 
   int cz = cell_coord(fracw[3 * i + 2], 2, gp);
   cell_of[i] = (cx * gp.nc[1] + cy) * gp.nc[2] + cz;
   iota[i] = (int)i;
+}
+
+// balanced partition: work of the atom at sorted (cell-order) index i, keyed by its wrapped fractional coordinate along
+// the partition axis.  w = incoming edges + angles centred on the atom (nb (nb - 1) bond pairs; 0 without a bond graph)
+__global__ void k_work_keys(int64_t n, const int* __restrict__ s_gid, const double* __restrict__ fracw, int axis,
+                            const int* __restrict__ cnt_e, const int* __restrict__ cnt_b, double* __restrict__ key,
+                            long long* __restrict__ w) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const long long nb = cnt_b[i];
+  key[i] = fracw[3 * (int64_t)s_gid[i] + axis];
+  w[i] = (long long)cnt_e[i] + nb * (nb - 1);
+}
+
+// balanced partition, wall k + 1 of `world`: the atoms sorted by coordinate x[] with the inclusive prefix S[] of their
+// work; i = first atom with S[i] * world >= (k + 1) * S[n-1].  gap[2k], gap[2k+1] = x[i] and the next larger coordinate
+// (the wall goes half-way); when x[i] is the largest coordinate, the gap below it.
+__global__ void k_balanced_gaps(int nw, int64_t n, int world, const double* __restrict__ x,
+                                const long long* __restrict__ S, double* __restrict__ gap) {
+  const int k = threadIdx.x;
+  if (k >= nw) return;
+  const long long target = (long long)(k + 1) * S[n - 1];
+  int64_t lo = 0, hi = n - 1;  // S[n-1] * world >= target always
+  while (lo < hi) {
+    const int64_t m = (lo + hi) / 2;
+    if (S[m] * world >= target) hi = m;
+    else lo = m + 1;
+  }
+  const double xi = x[lo];
+  int64_t a = lo, b = n;  // first index with x > xi
+  while (a < b) {
+    const int64_t m = (a + b) / 2;
+    if (x[m] > xi) b = m;
+    else a = m + 1;
+  }
+  if (a < n) {
+    gap[2 * k] = xi, gap[2 * k + 1] = x[a];
+    return;
+  }
+  a = 0, b = lo;  // first index with x >= xi
+  while (a < b) {
+    const int64_t m = (a + b) / 2;
+    if (x[m] < xi) a = m + 1;
+    else b = m;
+  }
+  gap[2 * k] = a > 0 ? x[a - 1] : xi, gap[2 * k + 1] = xi;
 }
 
 __global__ void k_cell_hist(int64_t n, const int* __restrict__ cell_sorted, int* __restrict__ cnt) {
@@ -650,51 +698,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       mx[k] = std::max(mx[k], hred[b * 12 + 6 + k]);
     }
 
-  Walls wl;
-  wl.nw = world - 1;
-  wl.axis = 0;
-  if (world > 1) {
-    // create_partition (:1370-1456)
-    double diffs[3] = {mx[0] - mn[0], mx[1] - mn[1], mx[2] - mn[2]};
-    int longest = 0;
-    for (int i = 1; i < 3; i++)
-      if (diffs[i] > diffs[longest]) longest = i;
-    double fmn = mn[3 + longest], fmx = mx[3 + longest];
-    double flen = fmx - fmn;
-    wl.axis = longest;
-    for (int i = 1; i < world; i++) wl.w[i - 1] = (i * (flen / world)) + kEpsilon + fmn;
-    // collision nudge
-    for (int iter = 0; iter < 64; iter++) {
-      B2M_CK(cudaMemsetAsync(tmp_i0.p, 0, MAXP * sizeof(int), st));
-      launch(k_wall_collisions, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, tmp_i0.p);
-      int hits[MAXP];
-      B2M_CK(cudaMemcpyAsync(hits, tmp_i0.p, MAXP * sizeof(int), cudaMemcpyDeviceToHost, st));
-      B2M_CK(cudaStreamSynchronize(st));
-      bool any = false;
-      for (int k = 0; k < wl.nw; k++)
-        if (hits[k]) {
-          wl.w[k] += kEpsilon;
-          any = true;
-        }
-      if (!any) break;
-    }
-    // check_partition_size (:1512-1529): lattice *column* of the axis, width = walls[0] * |col|
-    double col[3] = {lat[longest], lat[longest + 3], lat[longest + 6]};
-    double width = (wl.w[0] - (walls_from_min ? fmn : 0.0)) * sqrt(col[0] * col[0] + col[1] * col[1] + col[2] * col[2]);
-    double need = 2 * (rcut + rbond);
-    if (width <= need) {
-      char buf[256];
-      snprintf(buf, sizeof buf,
-               "Partition walls are too close together: slab width %.4f <= 2*(atom_cutoff+bond_cutoff) = %.4f; "
-               "reduce the number of partitions",
-               width, need);
-      throw Error(B2M_ERR_SLAB_WIDTH, buf);
-    }
-  }
-  axis = wl.axis;
-  for (int k = 0; k < MAXP; k++) walls[k] = k < wl.nw ? wl.w[k] : 0.0;
-
-  // ---- global cell grid (cell edge >= r_cut where the cell allows it) ----
+  // ---- global cell grid (cell edge >= r_cut where the cell allows it); it does not depend on the walls ----
   {
     // perpendicular height along lattice vector k = 1 / |column k of inv|
     for (int k = 0; k < 3; k++) {
@@ -738,10 +742,9 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   }
   const int ncell = gp.nc[0] * gp.nc[1] * gp.nc[2];
   cell_start.ensure(ncell + 2);
-
-  // ---- owner + cell id, sort by cell ----
-  launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, gp, owner.p, cell_of.p, tmp_i0.p);
-  {
+  tmp_i2.ensure(std::max<int64_t>(N + 1, ncell + 2));
+  // atoms sorted by cell (s_gid), cell_start; cell_of and the iota in tmp_i0 from k_owner_cell
+  auto sort_by_cell = [&] {
     size_t bytes = 0;
     int bits = 1;
     while ((1 << bits) < ncell + 1) bits++;
@@ -750,11 +753,114 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     B2M_CK(cub::DeviceRadixSort::SortPairs(cub_tmp.p, bytes, cell_of.p, tmp_i1.p, tmp_i0.p, s_gid.p, (int)N, 0,
                                            bits, st));
     // tmp_i1 = sorted cell ids
-    tmp_i2.ensure(std::max<int64_t>(N + 1, ncell + 2));
     B2M_CK(cudaMemsetAsync(tmp_i2.p, 0, (ncell + 1) * sizeof(int), st));
     launch(k_cell_hist, cdiv(N, 256), 256, 0, st, N, tmp_i1.p, tmp_i2.p);
     excl_scan(cub_tmp, tmp_i2.p, cell_start.p, ncell + 1, st);
+  };
+  const double r2 = rcut * rcut, rb2 = rbond * rbond;
+
+  Walls wl;
+  wl.nw = world - 1;
+  wl.axis = 0;
+  if (world > 1) {
+    // create_partition (:1370-1456)
+    double diffs[3] = {mx[0] - mn[0], mx[1] - mn[1], mx[2] - mn[2]};
+    int longest = 0;
+    for (int i = 1; i < 3; i++)
+      if (diffs[i] > diffs[longest]) longest = i;
+    double fmn = mn[3 + longest], fmx = mx[3 + longest];
+    double flen = fmx - fmn;
+    wl.axis = longest;
+    if (!balanced) {
+      for (int i = 1; i < world; i++) wl.w[i - 1] = (i * (flen / world)) + kEpsilon + fmn;
+    } else {
+      // balanced (DESIGN.md §4.1): the work of every atom from a count pass over all of them (cell ids do not depend
+      // on the walls, so the cell list is built first), then walls at the work quantiles
+      Walls none = wl;
+      none.nw = 0;
+      launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, none, gp, owner.p, cell_of.p, tmp_i0.p);
+      sort_by_cell();
+      tmp_i3.ensure(N + 1);
+      launch(k_post_sort, cdiv(N, 256), 256, 0, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i3.p);
+      // tmp_i0 still holds the iota: every sorted index is a centre
+      launch(k_count, cdiv(N, 256), 256, 0, st, (int)N, tmp_i0.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p, owner.p,
+             rank, r2, rb2, tol, tmp_i1.p, tmp_i2.p, (unsigned*)nullptr);
+      bal_x.ensure(2 * N);
+      bal_w.ensure(2 * N);
+      double *x_in = bal_x.p, *x_s = bal_x.p + N;
+      long long *w_in = bal_w.p, *w_s = bal_w.p + N;
+      launch(k_work_keys, cdiv(N, 256), 256, 0, st, N, s_gid.p, fracw.p, longest, tmp_i1.p, tmp_i2.p, x_in, w_in);
+      size_t bytes = 0;
+      cub::DeviceRadixSort::SortPairs(nullptr, bytes, x_in, x_s, w_in, w_s, (int)N, 0, 64, st);
+      cub_tmp.ensure(bytes + 16);
+      B2M_CK(cub::DeviceRadixSort::SortPairs(cub_tmp.p, bytes, x_in, x_s, w_in, w_s, (int)N, 0, 64, st));
+      bytes = 0;
+      cub::DeviceScan::InclusiveSum(nullptr, bytes, w_s, w_in, (int)N, st);
+      cub_tmp.ensure(bytes + 16);
+      B2M_CK(cub::DeviceScan::InclusiveSum(cub_tmp.p, bytes, w_s, w_in, (int)N, st));
+      launch(k_balanced_gaps, 1, 32, 0, st, wl.nw, N, world, x_s, w_in, red_tmp.p);
+      double gap[2 * MAXP];
+      B2M_CK(cudaMemcpyAsync(gap, red_tmp.p, 2 * wl.nw * sizeof(double), cudaMemcpyDeviceToHost, st));
+      B2M_CK(cudaStreamSynchronize(st));
+      for (int k = 0; k < wl.nw; k++) wl.w[k] = 0.5 * (gap[2 * k] + gap[2 * k + 1]);
+      // minimum slab width delta = need / h, h the cell's height across the partition axis (stricter than the lattice
+      // column for a tilted cell); forward then backward pass against the end bounds
+      const double need = 2 * (rcut + rbond);
+      const double h = 1.0 / sqrt(inv[longest] * inv[longest] + inv[3 + longest] * inv[3 + longest] +
+                                  inv[6 + longest] * inv[6 + longest]);
+      const double delta = need / h;
+      const bool from_min = walls_from_min || !pbc[longest];
+      const double lo = from_min ? fmn : 0.0, hi = from_min ? fmx : 1.0;
+      for (int k = 0; k < wl.nw; k++) wl.w[k] = std::max(wl.w[k], (k ? wl.w[k - 1] : lo) + delta);
+      for (int k = wl.nw - 1; k >= 0; k--) wl.w[k] = std::min(wl.w[k], (k + 1 < wl.nw ? wl.w[k + 1] : hi) - delta);
+      for (int k = 0; k <= wl.nw; k++) {
+        const double width = (k < wl.nw ? wl.w[k] : hi) - (k ? wl.w[k - 1] : lo);
+        if (width < delta * (1 - 1e-12)) {  // slack for the rounding of the two passes
+          char buf[256];
+          snprintf(buf, sizeof buf,
+                   "Balanced partition: slab %d is %.4f A wide across the walls < 2*(atom_cutoff+bond_cutoff) = %.4f; "
+                   "reduce the number of partitions",
+                   k, width * h, need);
+          throw Error(B2M_ERR_SLAB_WIDTH, buf);
+        }
+      }
+    }
+    // collision nudge
+    for (int iter = 0; iter < 64; iter++) {
+      B2M_CK(cudaMemsetAsync(tmp_i0.p, 0, MAXP * sizeof(int), st));
+      launch(k_wall_collisions, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, tmp_i0.p);
+      int hits[MAXP];
+      B2M_CK(cudaMemcpyAsync(hits, tmp_i0.p, MAXP * sizeof(int), cudaMemcpyDeviceToHost, st));
+      B2M_CK(cudaStreamSynchronize(st));
+      bool any = false;
+      for (int k = 0; k < wl.nw; k++)
+        if (hits[k]) {
+          wl.w[k] += kEpsilon;
+          any = true;
+        }
+      if (!any) break;
+    }
+    if (!balanced) {
+      // check_partition_size (:1512-1529): lattice *column* of the axis, width = walls[0] * |col|
+      double col[3] = {lat[longest], lat[longest + 3], lat[longest + 6]};
+      double width = (wl.w[0] - (walls_from_min ? fmn : 0.0)) * sqrt(col[0] * col[0] + col[1] * col[1] + col[2] * col[2]);
+      double need = 2 * (rcut + rbond);
+      if (width <= need) {
+        char buf[256];
+        snprintf(buf, sizeof buf,
+                 "Partition walls are too close together: slab width %.4f <= 2*(atom_cutoff+bond_cutoff) = %.4f; "
+                 "reduce the number of partitions",
+                 width, need);
+        throw Error(B2M_ERR_SLAB_WIDTH, buf);
+      }
+    }
   }
+  axis = wl.axis;
+  for (int k = 0; k < MAXP; k++) walls[k] = k < wl.nw ? wl.w[k] : 0.0;
+
+  // ---- owner + cell id, sort by cell (a balanced partition sorted the atoms by cell before placing its walls) ----
+  launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, gp, owner.p, cell_of.p, tmp_i0.p);
+  if (!(balanced && world > 1)) sort_by_cell();
   // own flags, scan -> local ids
   launch(k_post_sort, cdiv(N, 256), 256, 0, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i0.p);
   tmp_i3.ensure(N + 1);
@@ -772,7 +878,6 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
          g2l.p);
 
   // ---- count pass over owned rows ----
-  const double r2 = rcut * rcut, rb2 = rbond * rbond;
   row_ptr.ensure(n_own + 2);
   DBuf<int>& cnt_e = tmp_i0;
   DBuf<int>& cnt_b = tmp_i1;

@@ -78,6 +78,11 @@ struct Graph {
   // unfolded (heat-flux) structures: slab walls are measured from the lowest fractional coordinate, not from 0, because
   // the periodic images put atoms below 0 along the partition axis
   bool walls_from_min = false;
+  // partition policy (b2m_set_partition_policy): false = the reference's equally spaced walls, true = walls at the
+  // quantiles of the atoms' work (edges + angles), so that every slab holds about the same share of it (DESIGN.md §4.1)
+  bool balanced = false;
+  DBuf<double> bal_x;     // [2N] coordinates along the axis, then sorted
+  DBuf<long long> bal_w;  // [2N] work per atom, then sorted; its inclusive prefix overwrites the first half
 
   void build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
              const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,

@@ -50,9 +50,10 @@ class MACECalculator_Dist(_Calculator):
             props += ("heat_flux", "heat_flux_potential")
         self.implemented_properties = props
 
-    def enable_distributed_mode(self, gpus):
+    def enable_distributed_mode(self, gpus, balance=False):
+        """`balance`: work-balanced slab walls for every model (ScaleShiftMACE_Dist.enable_distributed_mode)"""
         for m in self.models:
-            m.enable_distributed_mode(gpus)
+            m.enable_distributed_mode(gpus, balance)
         self.dist_enabled = True
 
     def calculate(self, atoms=None, properties=None, system_changes=None):

@@ -262,9 +262,10 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
                     raise NotImplementedError(f"products.{t}: contractions.{ci} and contractions.0 differ in correlation")
         return hl
 
-    def enable_distributed_mode(self, gpus):
+    def enable_distributed_mode(self, gpus, balance=False):
         """mace.py / models.py of the reference: `gpus` are CUDA ordinals, one per partition (a single-process group
-        when one process gets several, one rank per GPU under torchrun, a replica for a single GPU)."""
+        when one process gets several, one rank per GPU under torchrun, a replica for a single GPU).  `balance`: place
+        the slab walls so that every partition holds about the same number of edges (DESIGN.md §4.1)."""
         desc = self._describe()
         gpus, rank, world, group = self._process_layout(gpus)
         from distmlip_b200.structures import Z_OF
@@ -274,7 +275,7 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
         self.__dict__["_e0"] = self._state_dict["atomic_energies_fn.atomic_energies"].double().numpy().reshape(-1)
         eng = _lib.Engine(n_elem=desc.n_elem, n_blocks=desc.num_interactions, cutoff=desc.r_max, mace=desc,
                           device=[int(g) for g in gpus] if group else int(gpus[rank]))
-        self._attach_engine(eng, gpus, rank, world, group)
+        self._attach_engine(eng, gpus, rank, world, group, balance)
         eng.finalize()
         self._engine_finalized = True
 

@@ -1,6 +1,6 @@
 """Shared machinery of the engine-backed `*_Dist` model wrappers (CHGNet_Dist, TensorNet_Dist): the reference's
 `from_existing` shallow copy (chgnet.py:551-560, tensornet.py:206-217), the process layout behind
-`enable_distributed_mode(gpus)`, species lookup, weight finalisation and the `potential_forward_dist` seam."""
+`enable_distributed_mode(gpus, balance=False)`, species lookup, weight finalisation and the `potential_forward_dist` seam."""
 from __future__ import annotations
 
 import numpy as np
@@ -71,9 +71,12 @@ class EngineBackedModel:
                     f"(len(gpus) == world) or a single GPU")
         return gpus, rank, world, group
 
-    def _attach_engine(self, eng, gpus, rank, world, group):
+    def _attach_engine(self, eng, gpus, rank, world, group, balance=False):
+        """`balance`: slab walls at the quantiles of the atoms' edge + angle work instead of equally spaced (DESIGN.md
+        §4.1); under torchrun every rank must pass the same value, since each computes the walls on its own"""
         self.gpus = ["cuda:" + str(g) for g in gpus]
         eng.load_state_dict(self._state_dict)
+        eng.set_partition_policy(_lib.PARTITION_BALANCED if balance else _lib.PARTITION_EQUAL)
         if group:
             rank, world = 0, 1  # one host process: results need no cross-process reduction
         elif world > 1:

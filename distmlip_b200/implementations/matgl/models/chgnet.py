@@ -36,8 +36,9 @@ class CHGNet_Dist(EngineBackedModel):
         nb, rc, rb = int(self._attr("n_blocks")), float(self._attr("cutoff")), float(self._attr("three_body_cutoff"))
         return max(nb * rc, rc + (nb - 1) * rb)
 
-    def enable_distributed_mode(self, gpus):
-        """chgnet.py:455-549. `gpus`: CUDA ordinals, one per partition."""
+    def enable_distributed_mode(self, gpus, balance=False):
+        """chgnet.py:455-549. `gpus`: CUDA ordinals, one per partition.  `balance`: place the slab walls so that every
+        partition holds about the same number of edges and angles (DESIGN.md §4.1) instead of equally spaced."""
         gpus, rank, world, group = self._process_layout(gpus)
         sd = self._state_dict
         dim = int(sd["atom_embedding.weight"].shape[1])
@@ -62,4 +63,4 @@ class CHGNet_Dist(EngineBackedModel):
             three_body_cutoff=float(self._attr("three_body_cutoff")),
             cutoff_exponent=int(self._attr("cutoff_exponent")),
             device=[int(g) for g in gpus] if group else int(gpus[rank]))
-        self._attach_engine(eng, gpus, rank, world, group)
+        self._attach_engine(eng, gpus, rank, world, group, balance)

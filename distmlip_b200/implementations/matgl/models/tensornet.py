@@ -31,8 +31,9 @@ class TensorNet_Dist(EngineBackedModel):
         nblocks = len({int(k.split(".")[1]) for k in self._state_dict if k.startswith("layers.")})
         return (nblocks + 1) * float(self._attr("cutoff"))
 
-    def enable_distributed_mode(self, gpus):
-        """tensornet.py:163-204. `gpus`: CUDA ordinals, one per partition."""
+    def enable_distributed_mode(self, gpus, balance=False):
+        """tensornet.py:163-204. `gpus`: CUDA ordinals, one per partition.  `balance`: place the slab walls so that
+        every partition holds about the same number of edges (DESIGN.md §4.1) instead of equally spaced."""
         gpus, rank, world, group = self._process_layout(gpus)
         sd = self._state_dict
         if self._attr("is_intensive", False):
@@ -63,4 +64,4 @@ class TensorNet_Dist(EngineBackedModel):
             tensornet=dict(units=units, num_rbf=int(sd["bond_expansion.rbf.centers"].shape[0]),
                            so3=group_name == "SO(3)", rbf_width=float(width)),
             device=[int(g) for g in gpus] if group else int(gpus[rank]))
-        self._attach_engine(eng, gpus, rank, world, group)
+        self._attach_engine(eng, gpus, rank, world, group, balance)

@@ -23,6 +23,9 @@
  *        GPU (ndev > 1: peer-memory halo stores ordered by CUDA events, one host thread per
  *        partition) or one process per GPU with NCCL point-to-point halo exchange between slab
  *        neighbours.
+ *   b2m_set_partition_policy
+ *        no counterpart: the reference always places its slab walls equally spaced in fractional coordinate
+ *        (subgraph_creation_utils.c:1370-1456); the balanced policy places them at the quantiles of the atoms' work.
  *   b2m_get_partition_info
  *        the 19-tuple returned by get_subgraphs_fast (subgraph_creation_fast.c:403-422), in
  *        canonical (set) form, for parity tests.
@@ -147,6 +150,23 @@ int b2m_comm_init(b2m_handle h, const char* id128, int rank, int world);
 /* Graph-only view of partition `rank` of `world` without a communicator (parity tests of the
  * partitioner on one GPU).  b2m_compute refuses to run in this state when world > 1. */
 int b2m_set_partition(b2m_handle h, int rank, int world);
+
+/* Where the world - 1 slab walls go (DESIGN.md §4, §4.1).  Axis: the longest Cartesian extent of the wrapped
+ * coordinates, for both policies.
+ *   B2M_PARTITION_EQUAL (default): the reference's walls, equally spaced in fractional coordinate between the lowest and
+ *     highest atom; fails with B2M_ERR_SLAB_WIDTH when the first slab is not wider than 2 (r_cut + r_bond) along the
+ *     lattice column of the axis.
+ *   B2M_PARTITION_BALANCED: every slab owns about the same work w_i = deg_i + nb_i (nb_i - 1) (deg_i: edges into atom
+ *     i, nb_i: bonds into it; the second term is 0 without a bond graph).  Wall k goes half-way between the two
+ *     distinct coordinates where the prefix of the work, atoms sorted along the axis, first reaches k W / world; then
+ *     every slab is widened to at least 2 (r_cut + r_bond) across the walls (the cell's height, not the lattice column),
+ *     or the build fails with B2M_ERR_SLAB_WIDTH naming the slab.  Every partition and every rank computes the same
+ *     walls from the same coordinates: nothing is exchanged.
+ * The policy holds for every partition of a single-process group and takes effect at the next b2m_set_structure (the
+ * unfolded heat-flux cell included).  Any other value: B2M_ERR_INVALID. */
+#define B2M_PARTITION_EQUAL 0
+#define B2M_PARTITION_BALANCED 1
+int b2m_set_partition_policy(b2m_handle h, int policy);
 
 /* Graph build (neighbour list, slab partition, halo sections, bond graph, angles) on the GPU.
  * cart: [natoms,3] f64 Cartesian (unwrapped ok); lattice9: row vectors; species: index into
