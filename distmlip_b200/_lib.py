@@ -19,7 +19,7 @@ SYMBOLS = [
     "b2m_compute_resident", "b2m_get_results", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
     "b2m_debug_tensor", "b2m_last_timings", "b2m_release_workspace", "b2m_set_view", "b2m_create_tensornet",
     "b2m_set_atomic", "b2m_get_atomic", "b2m_set_heat_flux", "b2m_compute_heat_flux", "b2m_create_mace",
-    "b2m_set_partition_policy",
+    "b2m_set_partition_policy", "b2m_set_structures", "b2m_compute_batch",
 ]
 
 PARTITION_EQUAL, PARTITION_BALANCED = 0, 1
@@ -88,7 +88,9 @@ def load_library():
     lib.b2m_set_partition.argtypes = [vp, i32, i32]
     lib.b2m_set_partition_policy.argtypes = [vp, i32]
     lib.b2m_set_structure.argtypes = [vp, i64, P(dbl), P(dbl), P(C.c_int32), P(C.c_int), dbl]
+    lib.b2m_set_structures.argtypes = [vp, i32, P(i64), P(dbl), P(dbl), P(C.c_int32), P(C.c_int), dbl]
     lib.b2m_compute.argtypes = [vp, i32, i32, P(dbl), P(C.c_float), P(C.c_float)]
+    lib.b2m_compute_batch.argtypes = [vp, i32, i32, P(dbl), P(C.c_float), P(C.c_float)]
     lib.b2m_compute_resident.argtypes = [vp, i32, i32, i32, P(dbl), P(C.c_float)]
     lib.b2m_get_results.argtypes = [vp, P(dbl), P(C.c_float), P(C.c_float)]
     lib.b2m_get_sitewise.argtypes = [vp, P(C.c_float)]
@@ -148,6 +150,7 @@ class Engine:
         if rc != 0:
             raise B2MError(rc, (self.lib.b2m_last_error(None) or b"").decode())
         self.natoms = 0
+        self.batch_natoms = np.zeros(0, dtype=np.int64)
         self.rank, self.world = 0, len(devs)
         self.group = len(devs) > 1
 
@@ -217,6 +220,37 @@ class Engine:
             self.h, self.natoms, cart.ctypes.data_as(C.POINTER(C.c_double)),
             lattice.ctypes.data_as(C.POINTER(C.c_double)), species.ctypes.data_as(C.POINTER(C.c_int32)),
             pbc.ctypes.data_as(C.POINTER(C.c_int)), float(tol)))
+
+    def set_structures(self, natoms, cart, lattices, species, pbc, tol=1e-8):
+        """a batch of independent structures (b2m_set_structures): natoms [S] atoms per structure, positions [sum, 3]
+        and species [sum] concatenated in structure order, lattices [S, 3, 3] (row vectors), pbc [S, 3]"""
+        natoms = np.ascontiguousarray(natoms, dtype=np.int64).reshape(-1)
+        cart = np.ascontiguousarray(cart, dtype=np.float64)
+        species = np.ascontiguousarray(species, dtype=np.int32)
+        lattices = np.ascontiguousarray(lattices, dtype=np.float64).reshape(len(natoms), 9)
+        pbc = np.ascontiguousarray(pbc, dtype=np.int32).reshape(len(natoms), 3)
+        if len(natoms) and (len(cart) != int(natoms.sum()) or len(species) != len(cart)):
+            raise ValueError(f"positions [{len(cart)}] and species [{len(species)}] must hold sum(natoms) = "
+                             f"{int(natoms.sum())} atoms")
+        self.natoms = len(cart)
+        self.batch_natoms = natoms
+        self._ck(self.lib.b2m_set_structures(
+            self.h, len(natoms), natoms.ctypes.data_as(C.POINTER(C.c_int64)),
+            cart.ctypes.data_as(C.POINTER(C.c_double)), lattices.ctypes.data_as(C.POINTER(C.c_double)),
+            species.ctypes.data_as(C.POINTER(C.c_int32)), pbc.ctypes.data_as(C.POINTER(C.c_int)), float(tol)))
+
+    def compute_batch(self, forces=True, stress=True):
+        """evaluates the resident batch: (energies [S] f64, forces [sum natoms, 3] f32 or None, stress [S, 3, 3] f32
+        GPa or None), each what compute() returns for that structure alone"""
+        S = len(self.batch_natoms)
+        e = np.empty(S, dtype=np.float64)
+        f = np.empty((self.natoms, 3), dtype=np.float32) if forces else None
+        s = np.empty((S, 9), dtype=np.float32) if stress else None
+        self._ck(self.lib.b2m_compute_batch(
+            self.h, int(bool(forces)), int(bool(stress)), e.ctypes.data_as(C.POINTER(C.c_double)),
+            f.ctypes.data_as(C.POINTER(C.c_float)) if f is not None else None,
+            s.ctypes.data_as(C.POINTER(C.c_float)) if s is not None else None))
+        return e, f, (s.reshape(S, 3, 3) if s is not None else None)
 
     def compute(self, forces=True, stress=True, out_forces=None, out_stress=None):
         e = C.c_double()

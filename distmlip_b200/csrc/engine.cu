@@ -131,6 +131,7 @@ struct Bufs {
   DBuf<float> hf_G;       // leader: [3][N][3] forces of the three seeded passes
   DBuf<float> hf_fold;    // leader: folded forces [n][3] or virials [n][kVirPitch]
   DBuf<double> hf_vel, hf_out;
+  DBuf<double> bsum;      // batch: [S][10] energy and virial of every structure
 };
 
 }  // namespace b2m
@@ -230,10 +231,17 @@ namespace b2m {
 // atoms of the structure the caller passed: the graph's atoms, or the cell atoms of an unfolded graph
 static int64_t cell_atoms(const b2m_engine* e) { return e->hf_n ? e->hf_n : e->g.N; }
 
+// a batch of structures is resident (b2m_set_structures, DESIGN.md §12)
+static bool batched(const b2m_engine* e) { return e->have_graph && e->g.S > 0; }
+
 // optional outputs of an evaluation and the readout weights, null where they are off: per-atom energies and virials
-// (b2m_set_atomic), and each atom's energy weight (heat flux, DESIGN.md §10)
-static double* atom_e_out(b2m_engine* e) { return e->atomic ? e->buf.atom_e.p : nullptr; }
-static float* atom_vir_out(b2m_engine* e) { return e->atomic ? e->buf.atom_vir.p : nullptr; }
+// (b2m_set_atomic; always on for a batch, whose per-structure sums are taken from them), and each atom's energy weight
+// (heat flux, DESIGN.md §10)
+static bool per_atom_on(const b2m_engine* e) { return e->atomic || batched(e); }
+static double* atom_e_out(b2m_engine* e) { return per_atom_on(e) ? e->buf.atom_e.p : nullptr; }
+static float* atom_vir_out(b2m_engine* e) { return per_atom_on(e) ? e->buf.atom_vir.p : nullptr; }
+// data_mean's share of each per-atom energy in the readout; a batch adds each structure's share in k_batch_sums
+static double mean_per_atom(const b2m_engine* e) { return batched(e) ? 0.0 : e->desc.data_mean / cell_atoms(e); }
 static const float* readout_wgt(const b2m_engine* e) { return e->hf_n ? e->buf.hf_w.p : nullptr; }
 
 // state_dict tensor k, marked as used; its shape must be `shape`, or with `flat` only hold as many elements
@@ -626,7 +634,7 @@ static void run(b2m_engine* e, bool grads) {
   const long long l0 = g_launch_count;
   B2M_CK(cudaEventRecord(e->ev[0], e->st));
   const size_t N = (size_t)e->g.N;
-  if (e->atomic) {  // zeroed here, before the readout writes the energies and the backward accumulates the virials
+  if (per_atom_on(e)) {  // zeroed here, before the readout writes the energies and the backward accumulates the virials
     e->buf.atom_e.ensure(N + 64);
     e->buf.atom_e.zero(N, e->st);
     if (grads) {
@@ -655,7 +663,7 @@ static void run(b2m_engine* e, bool grads) {
   B2M_CK(cudaEventRecord(e->ev[2], e->st));
   B2M_CK(cudaStreamSynchronize(e->st));
   e->launches_last = g_launch_count - l0;
-  e->atomic_last = e->atomic ? (grads ? 2 : 1) : 0;
+  e->atomic_last = per_atom_on(e) ? (grads ? 2 : 1) : 0;
   float ms;
   B2M_CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]));
   e->t_fwd = ms;
@@ -829,6 +837,41 @@ static void fetch_atomic(b2m_engine* e, double* energies, float* virials) {
   if (virials) {
     const float* w = static_cast<const float*>(e->pin_out);
     for (size_t i = 0; i < N; i++) memcpy(virials + i * 9, w + i * kVirPitch, 9 * sizeof(float));
+  }
+}
+
+// Batch (DESIGN.md §12): block s sums the per-atom energies and virials (f32 summed in f64; null: energies only) of
+// structure s, the atoms off[s] .. off[s + 1] - 1, into out[s][0] and out[s][1..9] (zeroed before), and adds data_mean's
+// per-atom share data_mean / n_s to each of its per-atom energies, as a single evaluation of the structure has them
+__global__ void __launch_bounds__(256) k_batch_sums(const int64_t* __restrict__ off, double data_mean,
+                                                    double* __restrict__ atom_e, const float* __restrict__ atom_vir,
+                                                    double* __restrict__ out) {
+  const int64_t b = off[blockIdx.x], end = off[blockIdx.x + 1];
+  const double m = data_mean / (end - b);
+  double acc[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  for (int64_t i = b + threadIdx.x; i < end; i += blockDim.x) {
+    acc[0] += atom_e[i];
+    atom_e[i] += m;
+    if (atom_vir)
+      for (int k = 0; k < 9; k++) acc[1 + k] += (double)atom_vir[i * kVirPitch + k];
+  }
+  block_sum_add(acc, out + 10 * blockIdx.x);
+}
+
+// energies [S], forces [N][3] and stress9 [S][9] of the batch just evaluated (any may be null); one launch for any S
+static void fetch_batch(b2m_engine* e, bool grads, double* energies, float* forces, float* stress9) {
+  const Graph& g = e->g;
+  e->buf.bsum.ensure((size_t)g.S * 10 + 64);
+  e->buf.bsum.zero((size_t)g.S * 10, e->st);
+  launch(k_batch_sums, g.S, 256, 0, e->st, g.b_doff.p, e->desc.data_mean, e->buf.atom_e.p,
+         grads ? (const float*)e->buf.atom_vir.p : nullptr, e->buf.bsum.p);
+  std::vector<double> hs((size_t)g.S * 10);
+  B2M_CK(cudaMemcpyAsync(hs.data(), e->buf.bsum.p, hs.size() * sizeof(double), cudaMemcpyDeviceToHost, e->st));
+  fetch(e, nullptr, forces, nullptr);  // forces, and the stream synchronised
+  for (int s = 0; s < g.S; s++) {
+    if (energies) energies[s] = hs[10 * s] + e->desc.data_mean;
+    if (stress9)
+      for (int k = 0; k < 9; k++) stress9[9 * s + k] = (float)(hs[10 * s + 1 + k] / g.b_volume[s] * 160.21766208);
   }
 }
 
@@ -1143,8 +1186,10 @@ int b2m_set_partition_policy(b2m_handle h, int policy) {
   API_END
 }
 
+// natoms atoms of one structure, or (nstruct > 0) the concatenated atoms of nstruct structures with counts[s] atoms each
 static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart, const double* lattice9,
-                              const int32_t* species, const int* pbc3, double tol) {
+                              const int32_t* species, const int* pbc3, double tol, int nstruct = 0,
+                              const int64_t* counts = nullptr) {
   h->have_graph = false;
   // positions and species through the library's page-locked staging (asynchronous upload inside the build)
   if (natoms > 0 && natoms < (1LL << 31) / 4) {
@@ -1159,7 +1204,11 @@ static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart,
   h->atomic_last = 0;  // per-atom results of an earlier structure are gone
   h->hf_n = 0, h->hf_seed = -1;
   h->g.balanced = h->partition_policy == B2M_PARTITION_BALANCED;
-  if (h->hf_reach > 0) {
+  if (nstruct > 0) {
+    h->g.walls_from_min = false;
+    h->g.build_batch(h->st, nstruct, counts, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff,
+                     tol);
+  } else if (h->hf_reach > 0) {
     // heat flux: the unfolded cell, built on the device, is the graph's input; no periodicity
     h->uf.build(h->st, natoms, cart, species, lattice9, pbc3, h->hf_reach);
     const int no_pbc[3] = {0, 0, 0};
@@ -1196,8 +1245,41 @@ int b2m_set_structure(b2m_handle h, int64_t natoms, const double* cart, const do
   API_END
 }
 
+int b2m_set_structures(b2m_handle h, int32_t nstruct, const int64_t* natoms, const double* cart,
+                       const double* lattice9, const int32_t* species, const int* pbc3, double tol) {
+  API_BEGIN
+  B2M_REQUIRE(h->parts.empty() && h->world == 1, B2M_ERR_INVALID,
+              "a batch runs on one partition: not on a single-process group (ndev > 1) or a rank of a multi-process job");
+  B2M_REQUIRE(h->hf_reach == 0, B2M_ERR_STATE, "a batch has no heat flux (b2m_set_heat_flux(h, 0) first)");
+  B2M_REQUIRE(nstruct >= 1, B2M_ERR_INVALID, "a batch needs at least one structure");
+  B2M_REQUIRE(natoms && cart && lattice9 && species && pbc3, B2M_ERR_INVALID, "null structure argument");
+  int64_t total = 0;
+  for (int s = 0; s < nstruct; s++) {
+    B2M_REQUIRE(natoms[s] > 0, B2M_ERR_INVALID, "structure " + std::to_string(s) + ": no atoms");
+    total += natoms[s];
+  }
+  set_structure_one(h, total, cart, lattice9, species, pbc3, tol, nstruct, natoms);
+  API_END
+}
+
+int b2m_compute_batch(b2m_handle h, int want_forces, int want_stress, double* energies, float* forces, float* stress9) {
+  API_BEGIN
+  B2M_REQUIRE(batched(h), B2M_ERR_STATE, "no batch is resident (b2m_set_structures first)");
+  const bool grads = want_forces || want_stress;
+  run(h, grads);
+  fetch_batch(h, grads, energies, want_forces ? forces : nullptr, want_stress ? stress9 : nullptr);
+  API_END
+}
+
+// the single-structure results (one energy, one stress) of b2m_compute and its relatives do not exist for a batch
+static void refuse_batch(b2m_engine* h) {
+  B2M_REQUIRE(!batched(h), B2M_ERR_STATE,
+              "a batch is resident: b2m_compute_batch evaluates it, b2m_set_structure goes back to one structure");
+}
+
 int b2m_compute(b2m_handle h, int want_forces, int want_stress, double* energy, float* forces, float* stress9) {
   API_BEGIN
+  refuse_batch(h);
   run_any(h, want_forces || want_stress);
   fetch(h, energy, want_forces ? forces : nullptr, want_stress ? stress9 : nullptr);
   API_END
@@ -1206,6 +1288,7 @@ int b2m_compute(b2m_handle h, int want_forces, int want_stress, double* energy, 
 int b2m_compute_resident(b2m_handle h, int want_forces, int want_stress, int reps, double* energy, float* ms) {
   API_BEGIN
   B2M_REQUIRE(reps >= 1, B2M_ERR_INVALID, "reps >= 1");
+  refuse_batch(h);
   for (int r = 0; r < reps; r++) run_any(h, want_forces || want_stress);
   fetch(h, energy, nullptr, nullptr);
   if (ms) *ms = (float)h->t_total;
@@ -1215,6 +1298,7 @@ int b2m_compute_resident(b2m_handle h, int want_forces, int want_stress, int rep
 int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9) {
   API_BEGIN
   B2M_REQUIRE(h->have_graph, B2M_ERR_STATE, "no structure");
+  refuse_batch(h);
   fetch(h, energy, forces, stress9);
   API_END
 }
@@ -1230,6 +1314,7 @@ int b2m_compute_heat_flux(b2m_handle h, const double* vel, double* energy, float
                           double* flux6) {
   API_BEGIN
   B2M_REQUIRE(vel && flux6, B2M_ERR_INVALID, "velocities and flux6 are required");
+  refuse_batch(h);
   B2M_REQUIRE(h->hf_reach > 0, B2M_ERR_STATE, "heat flux is off (b2m_set_heat_flux(h, reach > 0) first)");
   B2M_REQUIRE(h->have_graph && h->hf_n > 0, B2M_ERR_STATE,
               "the resident structure is not unfolded (b2m_set_structure after b2m_set_heat_flux)");

@@ -29,18 +29,9 @@ namespace b2m {
 
 static constexpr double kEpsilon = 1e-10;  // subgraph_creation_utils.c:9
 
-struct GridParams {
-  double lat[9];
-  double inv[9];
-  int nc[3], reach[3], pbc[3];
-  double fmin[3], fscale[3];
-};
-
 // ---------------------------------------------------------------------------------------------
-__global__ void k_wrap(int64_t n, const double* __restrict__ cart, GridParams gp,
-                       double* __restrict__ fracw, double* __restrict__ wc, int* __restrict__ corr) {
-  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
+__device__ __forceinline__ void wrap_atom(int64_t i, const double* __restrict__ cart, const GridParams& gp,
+                                          double* __restrict__ fracw, double* __restrict__ wc, int* __restrict__ corr) {
   double x = cart[3 * i], y = cart[3 * i + 1], z = cart[3 * i + 2];
   double f[3];
   // frac = cart @ inv  (fpis.c:198-207, plain triple loop: no FMA contraction)
@@ -71,6 +62,22 @@ __global__ void k_wrap(int64_t n, const double* __restrict__ cart, GridParams gp
     s = __dadd_rn(s, __dmul_rn(w[2], gp.lat[2 * 3 + m]));
     wc[3 * i + m] = s;
   }
+}
+
+__global__ void k_wrap(int64_t n, const double* __restrict__ cart, GridParams gp,
+                       double* __restrict__ fracw, double* __restrict__ wc, int* __restrict__ corr) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  wrap_atom(i, cart, gp, fracw, wc, corr);
+}
+
+// batch: atom i in the lattice of its structure sid[i]
+__global__ void k_wrap_batch(int64_t n, const double* __restrict__ cart, const GridParams* __restrict__ gps,
+                             const int* __restrict__ sid, double* __restrict__ fracw, double* __restrict__ wc,
+                             int* __restrict__ corr) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  wrap_atom(i, cart, gps[sid[i]], fracw, wc, corr);
 }
 
 // per-block min/max of wc[.,0..2] and fracw[.,0..2]; out[block][12]
@@ -111,6 +118,46 @@ __global__ void k_minmax(int64_t n, const double* __restrict__ wc, const double*
       out[blockIdx.x * 12 + 6 + k] = smax[k][0];
     }
 }
+
+// batch: k_minmax with block s over the atoms off[s] .. off[s + 1] - 1 of structure s; out[s][12]
+__global__ void k_minmax_batch(const int64_t* __restrict__ off, const double* __restrict__ wc,
+                               const double* __restrict__ fracw, double* __restrict__ out) {
+  __shared__ double smin[6][256], smax[6][256];
+  double mn[6], mx[6];
+  for (int k = 0; k < 6; k++) {
+    mn[k] = 1e300;
+    mx[k] = -1e300;
+  }
+  for (int64_t i = off[blockIdx.x] + threadIdx.x; i < off[blockIdx.x + 1]; i += blockDim.x) {
+    for (int k = 0; k < 3; k++) {
+      double a = wc[3 * i + k], b = fracw[3 * i + k];
+      mn[k] = fmin(mn[k], a);
+      mx[k] = fmax(mx[k], a);
+      mn[3 + k] = fmin(mn[3 + k], b);
+      mx[3 + k] = fmax(mx[3 + k], b);
+    }
+  }
+  for (int k = 0; k < 6; k++) {
+    smin[k][threadIdx.x] = mn[k];
+    smax[k][threadIdx.x] = mx[k];
+  }
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) {
+      for (int k = 0; k < 6; k++) {
+        smin[k][threadIdx.x] = fmin(smin[k][threadIdx.x], smin[k][threadIdx.x + s]);
+        smax[k][threadIdx.x] = fmax(smax[k][threadIdx.x], smax[k][threadIdx.x + s]);
+      }
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0)
+    for (int k = 0; k < 6; k++) {
+      out[blockIdx.x * 12 + k] = smin[k][0];
+      out[blockIdx.x * 12 + 6 + k] = smax[k][0];
+    }
+}
+
 
 struct Walls {
   double w[MAXP];
@@ -154,6 +201,22 @@ __global__ void k_owner_cell(int64_t n, const double* __restrict__ fracw, Walls 
   int cy = cell_coord(fracw[3 * i + 1], 1, gp);
   int cz = cell_coord(fracw[3 * i + 2], 2, gp);
   cell_of[i] = (cx * gp.nc[1] + cy) * gp.nc[2] + cz;
+  iota[i] = (int)i;
+}
+
+// batch (one partition): owner 0, cell id = the structure's first cell + its cell in the structure's grid
+__global__ void k_owner_cell_batch(int64_t n, const double* __restrict__ fracw, const int* __restrict__ sid,
+                                   const GridParams* __restrict__ gps, const int* __restrict__ cell_off,
+                                   unsigned char* __restrict__ owner, int* __restrict__ cell_of, int* __restrict__ iota) {
+  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int s = sid[i];
+  const GridParams& gp = gps[s];
+  owner[i] = 0;
+  int cx = cell_coord(fracw[3 * i + 0], 0, gp);
+  int cy = cell_coord(fracw[3 * i + 1], 1, gp);
+  int cz = cell_coord(fracw[3 * i + 2], 2, gp);
+  cell_of[i] = cell_off[s] + (cx * gp.nc[1] + cy) * gp.nc[2] + cz;
   iota[i] = (int)i;
 }
 
@@ -314,17 +377,15 @@ __device__ __forceinline__ void traverse(int ci, const GridParams& gp, const int
   }
 }
 
-// count edges / bonds per centre; centres given by sorted index list
-__global__ void k_count(int ncent, const int* __restrict__ cent_sidx, GridParams gp,
-                        const int* __restrict__ s_gid, const double* __restrict__ s_wc,
-                        const int* __restrict__ cell_start, const double* __restrict__ fracw,
-                        const unsigned char* __restrict__ owner, int rank, double r2, double rb2, double tol,
-                        int* __restrict__ cnt_e, int* __restrict__ cnt_b, unsigned* __restrict__ to_mask) {
-  int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= ncent) return;
+// count edges / bonds of the centre t at sorted index ci
+__device__ __forceinline__ void count_row(int t, int ci, const GridParams& gp, const int* __restrict__ s_gid,
+                                          const double* __restrict__ s_wc, const int* __restrict__ cell_start,
+                                          const double* __restrict__ fracw, const unsigned char* __restrict__ owner,
+                                          int rank, double r2, double rb2, double tol, int* __restrict__ cnt_e,
+                                          int* __restrict__ cnt_b, unsigned* __restrict__ to_mask) {
   int ne = 0, nb = 0;
   unsigned mask = 0;
-  traverse(cent_sidx[t], gp, s_gid, s_wc, cell_start, fracw, r2, tol,
+  traverse(ci, gp, s_gid, s_wc, cell_start, fracw, r2, tol,
            [&](int, int gj, double, double, double, double d2, int, int, int) {
              ne++;
              if (d2 < rb2 + tol) nb++;
@@ -336,20 +397,43 @@ __global__ void k_count(int ncent, const int* __restrict__ cent_sidx, GridParams
   if (to_mask) to_mask[t] = mask;
 }
 
-// fill owned rows
-__global__ void k_fill_owned(int n_own, const int* __restrict__ cent_sidx, GridParams gp,
-                             const int* __restrict__ s_gid, const double* __restrict__ s_wc,
-                             const int* __restrict__ cell_start, const double* __restrict__ fracw,
-                             const unsigned char* __restrict__ owner, int rank, double r2, double rb2, double tol,
-                             const int* __restrict__ row_ptr, const int* __restrict__ brow_ptr,
-                             int* __restrict__ e_src_gid, int* __restrict__ e_dst, int* __restrict__ e_img,
-                             int* __restrict__ e_bond, float4* __restrict__ e_vec, int* __restrict__ b_src_gid,
-                             int* __restrict__ b_dst, int* __restrict__ b_img, int* __restrict__ b_edge,
-                             float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
+// count edges / bonds per centre; centres given by sorted index list
+__global__ void k_count(int ncent, const int* __restrict__ cent_sidx, GridParams gp,
+                        const int* __restrict__ s_gid, const double* __restrict__ s_wc,
+                        const int* __restrict__ cell_start, const double* __restrict__ fracw,
+                        const unsigned char* __restrict__ owner, int rank, double r2, double rb2, double tol,
+                        int* __restrict__ cnt_e, int* __restrict__ cnt_b, unsigned* __restrict__ to_mask) {
   int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n_own) return;
+  if (t >= ncent) return;
+  count_row(t, cent_sidx[t], gp, s_gid, s_wc, cell_start, fracw, owner, rank, r2, rb2, tol, cnt_e, cnt_b, to_mask);
+}
+
+// batch: the centre's structure s = sid[gid] gives the grid and the first cell (cell ids of the traversal are local)
+__global__ void k_count_batch(int ncent, const int* __restrict__ cent_sidx, const GridParams* __restrict__ gps,
+                              const int* __restrict__ cell_off, const int* __restrict__ sid,
+                              const int* __restrict__ s_gid, const double* __restrict__ s_wc,
+                              const int* __restrict__ cell_start, const double* __restrict__ fracw,
+                              const unsigned char* __restrict__ owner, double r2, double rb2, double tol,
+                              int* __restrict__ cnt_e, int* __restrict__ cnt_b) {
+  int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= ncent) return;
+  const int ci = cent_sidx[t], s = sid[s_gid[ci]];
+  count_row(t, ci, gps[s], s_gid, s_wc, cell_start + cell_off[s], fracw, owner, 0, r2, rb2, tol, cnt_e, cnt_b,
+            (unsigned*)nullptr);
+}
+
+// fill the owned row t (centre at sorted index ci)
+__device__ __forceinline__ void fill_row(int t, int ci, const GridParams& gp, const int* __restrict__ s_gid,
+                                         const double* __restrict__ s_wc, const int* __restrict__ cell_start,
+                                         const double* __restrict__ fracw, const unsigned char* __restrict__ owner,
+                                         int rank, double r2, double rb2, double tol, const int* __restrict__ row_ptr,
+                                         const int* __restrict__ brow_ptr, int* __restrict__ e_src_gid,
+                                         int* __restrict__ e_dst, int* __restrict__ e_img, int* __restrict__ e_bond,
+                                         float4* __restrict__ e_vec, int* __restrict__ b_src_gid,
+                                         int* __restrict__ b_dst, int* __restrict__ b_img, int* __restrict__ b_edge,
+                                         float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
   int e = row_ptr[t], b = brow_ptr[t];
-  traverse(cent_sidx[t], gp, s_gid, s_wc, cell_start, fracw, r2, tol,
+  traverse(ci, gp, s_gid, s_wc, cell_start, fracw, r2, tol,
            [&](int, int gj, double dx, double dy, double dz, double d2, int ix, int iy, int iz) {
              // (dx,dy,dz) = x_src_image - x_dst ; reference bond_vec = x_dst + off.L - x_src = -(dx,dy,dz)
              float4 v = make_float4((float)(-dx), (float)(-dy), (float)(-dz), (float)sqrt(d2));
@@ -372,6 +456,46 @@ __global__ void k_fill_owned(int n_own, const int* __restrict__ cent_sidx, GridP
              }
              e++;
            });
+}
+
+// fill owned rows
+__global__ void k_fill_owned(int n_own, const int* __restrict__ cent_sidx, GridParams gp,
+                             const int* __restrict__ s_gid, const double* __restrict__ s_wc,
+                             const int* __restrict__ cell_start, const double* __restrict__ fracw,
+                             const unsigned char* __restrict__ owner, int rank, double r2, double rb2, double tol,
+                             const int* __restrict__ row_ptr, const int* __restrict__ brow_ptr,
+                             int* __restrict__ e_src_gid, int* __restrict__ e_dst, int* __restrict__ e_img,
+                             int* __restrict__ e_bond, float4* __restrict__ e_vec, int* __restrict__ b_src_gid,
+                             int* __restrict__ b_dst, int* __restrict__ b_img, int* __restrict__ b_edge,
+                             float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
+  int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_own) return;
+  fill_row(t, cent_sidx[t], gp, s_gid, s_wc, cell_start, fracw, owner, rank, r2, rb2, tol, row_ptr, brow_ptr, e_src_gid,
+           e_dst, e_img, e_bond, e_vec, b_src_gid, b_dst, b_img, b_edge, b_vec, halo_flag);
+}
+
+// batch: as k_count_batch
+__global__ void k_fill_owned_batch(int n_own, const int* __restrict__ cent_sidx, const GridParams* __restrict__ gps,
+                                   const int* __restrict__ cell_off, const int* __restrict__ sid,
+                                   const int* __restrict__ s_gid, const double* __restrict__ s_wc,
+                                   const int* __restrict__ cell_start, const double* __restrict__ fracw,
+                                   const unsigned char* __restrict__ owner, double r2, double rb2, double tol,
+                                   const int* __restrict__ row_ptr, const int* __restrict__ brow_ptr,
+                                   int* __restrict__ e_src_gid, int* __restrict__ e_dst, int* __restrict__ e_img,
+                                   int* __restrict__ e_bond, float4* __restrict__ e_vec, int* __restrict__ b_src_gid,
+                                   int* __restrict__ b_dst, int* __restrict__ b_img, int* __restrict__ b_edge,
+                                   float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
+  int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n_own) return;
+  const int ci = cent_sidx[t], s = sid[s_gid[ci]];
+  fill_row(t, ci, gps[s], s_gid, s_wc, cell_start + cell_off[s], fracw, owner, 0, r2, rb2, tol, row_ptr, brow_ptr,
+           e_src_gid, e_dst, e_img, e_bond, e_vec, b_src_gid, b_dst, b_img, b_edge, b_vec, halo_flag);
+}
+
+// batch: out[s] = ptr[off[s]] (edges before the first row of each structure)
+__global__ void k_gather_at(int n, const int64_t* __restrict__ off, const int* __restrict__ ptr, int* __restrict__ out) {
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = ptr[off[i]];
 }
 
 // fill halo bond rows (every bond whose dst is a halo atom)
@@ -628,12 +752,94 @@ static int read_int(const int* dptr, cudaStream_t st) {
   return v;
 }
 
+// Cell grid of one structure (cell edge >= r_cut where the cell allows it, at most 2^27 cells) from its inverse lattice,
+// periodicity and, for the non-periodic axes, the fractional bounds fmn / fmx [3] of its wrapped atoms.  build() and
+// build_batch() both call it, so a structure gets the same grid alone and in a batch.
+static void cell_grid(const double* inv, const int* pbc, const double* fmn, const double* fmx, double rcut,
+                      GridParams& gp) {
+  // perpendicular height along lattice vector k = 1 / |column k of inv|
+  for (int k = 0; k < 3; k++) {
+    double cn = sqrt(inv[k] * inv[k] + inv[3 + k] * inv[3 + k] + inv[6 + k] * inv[6 + k]);
+    double height = 1.0 / cn;
+    double reff = rcut + 1e-6;
+    if (pbc[k]) {
+      int n = (int)floor(height / reff);
+      if (n < 1) n = 1;
+      if (n > 1024) n = 1024;
+      gp.nc[k] = n;
+      double width = height / n;
+      gp.reach[k] = (int)ceil(reff / width);
+      if (gp.reach[k] < 1) gp.reach[k] = 1;
+      B2M_REQUIRE(gp.reach[k] < 120, B2M_ERR_INVALID, "cell far too small for the cutoff");
+    } else {
+      double ext = (fmx[k] - fmn[k]);
+      double extc = ext * height;
+      int n = (int)floor(extc / reff);
+      if (n < 1) n = 1;
+      if (n > 1024) n = 1024;
+      gp.nc[k] = n;
+      gp.fmin[k] = fmn[k];
+      gp.fscale[k] = ext > 0 ? n / ext : 0.0;
+      gp.reach[k] = 1;
+    }
+  }
+  while ((int64_t)gp.nc[0] * gp.nc[1] * gp.nc[2] > (1LL << 27)) {
+    int kmax = 0;
+    for (int k = 1; k < 3; k++)
+      if (gp.nc[k] > gp.nc[kmax]) kmax = k;
+    gp.nc[kmax] = (gp.nc[kmax] + 1) / 2;
+    gp.reach[kmax] = 2 * gp.reach[kmax];  // conservative
+  }
+}
+
+// per-atom arrays for N atoms, positions and species uploaded (host staging, or the device arrays of an Unfold)
+void Graph::upload(cudaStream_t st, const double* h_cart, const int32_t* h_species) {
+  cart.ensure(3 * N);
+  fracw.ensure(3 * N);
+  wc.ensure(3 * N);
+  corr.ensure(3 * N);
+  species.ensure(N);
+  owner.ensure(N);
+  g2l.ensure(N);
+  cell_of.ensure(N);
+  s_gid.ensure(N);
+  s_wc.ensure(3 * N);
+  sidx_of_gid.ensure(N);
+  tmp_i0.ensure(N + 1);
+  tmp_i1.ensure(N + 1);
+  tmp_i2.ensure(N + 1);
+  tmp_i3.ensure(N + 1);
+  tmp_flag.ensure(2 * N + 16);
+  B2M_CK(cudaMemcpyAsync(cart.p, h_cart, 3 * N * sizeof(double), cudaMemcpyDefault, st));
+  B2M_CK(cudaMemcpyAsync(species.p, h_species, N * sizeof(int), cudaMemcpyDefault, st));
+}
+
+// atoms sorted by cell (s_gid), cell_start; cell_of and the iota in tmp_i0 from k_owner_cell
+void Graph::sort_by_cell(cudaStream_t st, int ncell) {
+  cell_start.ensure(ncell + 2);
+  tmp_i2.ensure(std::max<int64_t>(N + 1, ncell + 2));
+  size_t bytes = 0;
+  int bits = 1;
+  while ((1 << bits) < ncell + 1) bits++;
+  cub::DeviceRadixSort::SortPairs(nullptr, bytes, cell_of.p, tmp_i1.p, tmp_i0.p, s_gid.p, (int)N, 0, bits, st);
+  cub_tmp.ensure(bytes + 16);
+  B2M_CK(cub::DeviceRadixSort::SortPairs(cub_tmp.p, bytes, cell_of.p, tmp_i1.p, tmp_i0.p, s_gid.p, (int)N, 0,
+                                         bits, st));
+  // tmp_i1 = sorted cell ids
+  B2M_CK(cudaMemsetAsync(tmp_i2.p, 0, (ncell + 1) * sizeof(int), st));
+  launch(k_cell_hist, cdiv(N, 256), 256, 0, st, N, tmp_i1.p, tmp_i2.p);
+  excl_scan(cub_tmp, tmp_i2.p, cell_start.p, ncell + 1, st);
+}
+
 void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
                   const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,
                   int rank_, int world_) {
   B2M_REQUIRE(natoms > 0 && natoms < (1LL << 31) / 4, B2M_ERR_INVALID, "natoms out of range");
   B2M_REQUIRE(world_ >= 1 && world_ <= MAXP, B2M_ERR_PARTITIONS, "num_partitions must be in [1,16]");
   B2M_REQUIRE(rbond <= rcut, B2M_ERR_INVALID, "bond_r cannot be greater than regular cutoff");
+  S = 0;
+  b_off.clear();
+  b_volume.clear();
   N = natoms;
   rank = rank_;
   world = world_;
@@ -653,25 +859,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   for (int k = 0; k < 3; k++) gp.pbc[k] = pbc[k];
 
   // ---- upload + wrap ----
-  cart.ensure(3 * N);
-  fracw.ensure(3 * N);
-  wc.ensure(3 * N);
-  corr.ensure(3 * N);
-  species.ensure(N);
-  owner.ensure(N);
-  g2l.ensure(N);
-  cell_of.ensure(N);
-  s_gid.ensure(N);
-  s_wc.ensure(3 * N);
-  sidx_of_gid.ensure(N);
-  tmp_i0.ensure(N + 1);
-  tmp_i1.ensure(N + 1);
-  tmp_i2.ensure(N + 1);
-  tmp_i3.ensure(N + 1);
-  tmp_flag.ensure(2 * N + 16);
-  // host staging, or the device arrays of an Unfold
-  B2M_CK(cudaMemcpyAsync(cart.p, h_cart, 3 * N * sizeof(double), cudaMemcpyDefault, st));
-  B2M_CK(cudaMemcpyAsync(species.p, h_species, N * sizeof(int), cudaMemcpyDefault, st));
+  upload(st, h_cart, h_species);
   for (int k = 0; k < 3; k++) {
     gp.nc[k] = 1;
     gp.reach[k] = 1;
@@ -698,65 +886,15 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       mx[k] = std::max(mx[k], hred[b * 12 + 6 + k]);
     }
 
-  // ---- global cell grid (cell edge >= r_cut where the cell allows it); it does not depend on the walls ----
-  {
-    // perpendicular height along lattice vector k = 1 / |column k of inv|
-    for (int k = 0; k < 3; k++) {
-      double cn = sqrt(inv[k] * inv[k] + inv[3 + k] * inv[3 + k] + inv[6 + k] * inv[6 + k]);
-      double height = 1.0 / cn;
-      double reff = rcut + 1e-6;
-      if (pbc[k]) {
-        int n = (int)floor(height / reff);
-        if (n < 1) n = 1;
-        if (n > 1024) n = 1024;
-        gp.nc[k] = n;
-        double width = height / n;
-        gp.reach[k] = (int)ceil(reff / width);
-        if (gp.reach[k] < 1) gp.reach[k] = 1;
-        B2M_REQUIRE(gp.reach[k] < 120, B2M_ERR_INVALID, "cell far too small for the cutoff");
-      } else {
-        double ext = (mx[3 + k] - mn[3 + k]);
-        double extc = ext * height;
-        int n = (int)floor(extc / reff);
-        if (n < 1) n = 1;
-        if (n > 1024) n = 1024;
-        gp.nc[k] = n;
-        gp.fmin[k] = mn[3 + k];
-        gp.fscale[k] = ext > 0 ? n / ext : 0.0;
-        gp.reach[k] = 1;
-      }
-    }
-    while ((int64_t)gp.nc[0] * gp.nc[1] * gp.nc[2] > (1LL << 27)) {
-      int kmax = 0;
-      for (int k = 1; k < 3; k++)
-        if (gp.nc[k] > gp.nc[kmax]) kmax = k;
-      gp.nc[kmax] = (gp.nc[kmax] + 1) / 2;
-      gp.reach[kmax] = 2 * gp.reach[kmax];  // conservative
-    }
-    for (int k = 0; k < 3; k++) {
-      nc[k] = gp.nc[k];
-      reach[k] = gp.reach[k];
-      fmin[k] = gp.fmin[k];
-      fscale[k] = gp.fscale[k];
-    }
+  // ---- global cell grid; it does not depend on the walls ----
+  cell_grid(inv, pbc, mn + 3, mx + 3, rcut, gp);
+  for (int k = 0; k < 3; k++) {
+    nc[k] = gp.nc[k];
+    reach[k] = gp.reach[k];
+    fmin[k] = gp.fmin[k];
+    fscale[k] = gp.fscale[k];
   }
   const int ncell = gp.nc[0] * gp.nc[1] * gp.nc[2];
-  cell_start.ensure(ncell + 2);
-  tmp_i2.ensure(std::max<int64_t>(N + 1, ncell + 2));
-  // atoms sorted by cell (s_gid), cell_start; cell_of and the iota in tmp_i0 from k_owner_cell
-  auto sort_by_cell = [&] {
-    size_t bytes = 0;
-    int bits = 1;
-    while ((1 << bits) < ncell + 1) bits++;
-    cub::DeviceRadixSort::SortPairs(nullptr, bytes, cell_of.p, tmp_i1.p, tmp_i0.p, s_gid.p, (int)N, 0, bits, st);
-    cub_tmp.ensure(bytes + 16);
-    B2M_CK(cub::DeviceRadixSort::SortPairs(cub_tmp.p, bytes, cell_of.p, tmp_i1.p, tmp_i0.p, s_gid.p, (int)N, 0,
-                                           bits, st));
-    // tmp_i1 = sorted cell ids
-    B2M_CK(cudaMemsetAsync(tmp_i2.p, 0, (ncell + 1) * sizeof(int), st));
-    launch(k_cell_hist, cdiv(N, 256), 256, 0, st, N, tmp_i1.p, tmp_i2.p);
-    excl_scan(cub_tmp, tmp_i2.p, cell_start.p, ncell + 1, st);
-  };
   const double r2 = rcut * rcut, rb2 = rbond * rbond;
 
   Walls wl;
@@ -779,7 +917,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       Walls none = wl;
       none.nw = 0;
       launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, none, gp, owner.p, cell_of.p, tmp_i0.p);
-      sort_by_cell();
+      sort_by_cell(st, ncell);
       tmp_i3.ensure(N + 1);
       launch(k_post_sort, cdiv(N, 256), 256, 0, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i3.p);
       // tmp_i0 still holds the iota: every sorted index is a centre
@@ -860,7 +998,14 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
 
   // ---- owner + cell id, sort by cell (a balanced partition sorted the atoms by cell before placing its walls) ----
   launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, gp, owner.p, cell_of.p, tmp_i0.p);
-  if (!(balanced && world > 1)) sort_by_cell();
+  if (!(balanced && world > 1)) sort_by_cell(st, ncell);
+  build_rows(st, gp);
+}
+
+// Local atoms, edges, halo sections, bonds and angles of the atoms sorted by cell (every build ends here).  A batch
+// (S > 0) has one partition and takes each centre's grid from b_gp.
+void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
+  const double r2 = r_cut * r_cut, rb2 = r_bond * r_bond;
   // own flags, scan -> local ids
   launch(k_post_sort, cdiv(N, 256), 256, 0, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i0.p);
   tmp_i3.ensure(N + 1);
@@ -881,17 +1026,31 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   row_ptr.ensure(n_own + 2);
   DBuf<int>& cnt_e = tmp_i0;
   DBuf<int>& cnt_b = tmp_i1;
-  launch(k_count, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p, owner.p,
-         rank, r2, rb2, tol, cnt_e.p, cnt_b.p, to_mask.p);
+  if (S)
+    launch(k_count_batch, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, b_gp.p, b_cell_off.p, b_sid.p, s_gid.p,
+           s_wc.p, cell_start.p, fracw.p, owner.p, r2, rb2, tol, cnt_e.p, cnt_b.p);
+  else
+    launch(k_count, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p,
+           owner.p, rank, r2, rb2, tol, cnt_e.p, cnt_b.p, to_mask.p);
   B2M_CK(cudaMemsetAsync(cnt_e.p + n_own, 0, sizeof(int), st));
   B2M_CK(cudaMemsetAsync(cnt_b.p + n_own, 0, sizeof(int), st));
   excl_scan(cub_tmp, cnt_e.p, row_ptr.p, n_own + 1, st);
   // owned part of brow_ptr (halo part appended later); brow_ptr sized for n_loc+1 <= N+1
   brow_ptr.ensure(N + 2);
   excl_scan(cub_tmp, cnt_b.p, brow_ptr.p, n_own + 1, st);
+  // batch: the rows of structure s are b_off[s] .. b_off[s + 1] - 1 (every atom owned, cell ids grouped by structure)
+  std::vector<int> e_at(S + 1);
+  if (S) {
+    sel_out.ensure(S + 1);
+    launch(k_gather_at, cdiv(S + 1, 256), 256, 0, st, S + 1, b_doff.p, row_ptr.p, sel_out.p);
+    B2M_CK(cudaMemcpyAsync(e_at.data(), sel_out.p, (S + 1) * sizeof(int), cudaMemcpyDeviceToHost, st));
+  }
   E = read_int(row_ptr.p + n_own, st);
   B_own = read_int(brow_ptr.p + n_own, st);
   B2M_REQUIRE(E > 0, B2M_ERR_INVALID, "No neighbors were found!");
+  for (int s = 0; s < S; s++)
+    B2M_REQUIRE(e_at[s + 1] > e_at[s], B2M_ERR_INVALID,
+                "structure " + std::to_string(s) + " has no edges (No neighbors were found!)");
 
   e_src.ensure(E);
   e_dst.ensure(E);
@@ -909,9 +1068,14 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   b_edge.ensure(B_own + 1);
   unsigned char* halo_flag = tmp_flag.p;
   B2M_CK(cudaMemsetAsync(halo_flag, 0, N, st));
-  launch(k_fill_owned, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p,
-         owner.p, rank, r2, rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p, e_bond.p, e_vec.p,
-         b_src_gid.p, b_dst.p, b_img.p, b_edge.p, b_vec.p, halo_flag);
+  if (S)
+    launch(k_fill_owned_batch, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, b_gp.p, b_cell_off.p, b_sid.p, s_gid.p,
+           s_wc.p, cell_start.p, fracw.p, owner.p, r2, rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p,
+           e_bond.p, e_vec.p, b_src_gid.p, b_dst.p, b_img.p, b_edge.p, b_vec.p, halo_flag);
+  else
+    launch(k_fill_owned, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p,
+           owner.p, rank, r2, rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p, e_bond.p, e_vec.p,
+           b_src_gid.p, b_dst.p, b_img.p, b_edge.p, b_vec.p, halo_flag);
 
   // ---- halo atoms: grouped by owner, gid ascending ----
   n_halo = 0;
@@ -1068,6 +1232,88 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
            gid.p, tmp_i3.p, a_in.p, a_out.p, a_ctr.p);
   }
   B2M_CK(cudaStreamSynchronize(st));
+}
+
+// Batch (DESIGN.md §12): the disjoint union of the structures, each wrapped in its own lattice and given its own cell grid
+// by cell_grid(); cell ids are the structure's first cell + its local cell, so the radix sort groups the atoms by
+// structure, then by cell, and inside a structure reproduces the order of its single build.  Launches and host
+// synchronisations do not depend on the number of structures.
+void Graph::build_batch(cudaStream_t st, int nstruct, const int64_t* natoms, const double* h_cart, const double* h_lat,
+                        const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_) {
+  B2M_REQUIRE(nstruct >= 1, B2M_ERR_INVALID, "a batch needs at least one structure");
+  B2M_REQUIRE(rbond <= rcut, B2M_ERR_INVALID, "bond_r cannot be greater than regular cutoff");
+  auto named = [](int s, const std::string& what) { return "structure " + std::to_string(s) + ": " + what; };
+  std::vector<int64_t> off(nstruct + 1, 0);
+  std::vector<GridParams> gps(nstruct);
+  std::vector<double> vol(nstruct);
+  for (int s = 0; s < nstruct; s++) {
+    B2M_REQUIRE(natoms[s] > 0, B2M_ERR_INVALID, named(s, "no atoms"));
+    off[s + 1] = off[s] + natoms[s];
+    B2M_REQUIRE(off[s + 1] < (1LL << 31) / 4, B2M_ERR_INVALID, "batch has too many atoms");
+    GridParams& gp = gps[s];
+    for (int k = 0; k < 3; k++) {
+      const int f = h_pbc[3 * s + k];
+      B2M_REQUIRE(f == 0 || f == 1, B2M_ERR_INVALID, named(s, "pbc flags must be 0 or 1"));
+      gp.pbc[k] = f, gp.nc[k] = 1, gp.reach[k] = 1, gp.fmin[k] = 0, gp.fscale[k] = 0;
+    }
+    memcpy(gp.lat, h_lat + 9 * s, sizeof gp.lat);
+    double det;
+    inv3(gp.lat, gp.inv, det);
+    B2M_REQUIRE(fabs(det) > 1e-12, B2M_ERR_INVALID, named(s, "singular lattice"));
+    vol[s] = fabs(det);
+  }
+  S = 0;
+  N = off[nstruct];
+  rank = 0, world = 1, axis = 0;
+  for (int k = 0; k < MAXP; k++) walls[k] = 0.0;
+  r_cut = rcut, r_bond = rbond, tol = tol_;
+  volume = 0;
+
+  // ---- upload + wrap: the lattices of the table now, the grids after the min/max ----
+  upload(st, h_cart, h_species);
+  std::vector<int> sid(N);
+  for (int s = 0; s < nstruct; s++) std::fill(sid.begin() + off[s], sid.begin() + off[s + 1], s);
+  b_gp.ensure(nstruct);
+  b_cell_off.ensure(nstruct);
+  b_sid.ensure(N);
+  b_doff.ensure(nstruct + 1);
+  B2M_CK(cudaMemcpyAsync(b_sid.p, sid.data(), N * sizeof(int), cudaMemcpyHostToDevice, st));
+  B2M_CK(cudaMemcpyAsync(b_doff.p, off.data(), (nstruct + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  B2M_CK(cudaMemcpyAsync(b_gp.p, gps.data(), nstruct * sizeof(GridParams), cudaMemcpyHostToDevice, st));
+  launch(k_wrap_batch, cdiv(N, 256), 256, 0, st, N, cart.p, b_gp.p, b_sid.p, fracw.p, wc.p, corr.p);
+
+  // ---- per-structure min/max (one block each), cell grids, first cell of each structure ----
+  red_tmp.ensure((size_t)nstruct * 12);
+  launch(k_minmax_batch, nstruct, 256, 0, st, b_doff.p, wc.p, fracw.p, red_tmp.p);
+  std::vector<double> hred((size_t)nstruct * 12);
+  B2M_CK(cudaMemcpyAsync(hred.data(), red_tmp.p, hred.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaStreamSynchronize(st));
+  std::vector<int> coff(nstruct);
+  int64_t ncell = 0;
+  for (int s = 0; s < nstruct; s++) {
+    try {
+      cell_grid(gps[s].inv, gps[s].pbc, &hred[12 * s + 3], &hred[12 * s + 9], rcut, gps[s]);
+    } catch (const Error& ex) {
+      throw Error(ex.code, named(s, ex.what()));
+    }
+    coff[s] = (int)ncell;
+    ncell += (int64_t)gps[s].nc[0] * gps[s].nc[1] * gps[s].nc[2];
+    B2M_REQUIRE(ncell <= (1LL << 27), B2M_ERR_INVALID, "batch needs more than 2^27 cells; split it");
+  }
+  B2M_CK(cudaMemcpyAsync(b_gp.p, gps.data(), nstruct * sizeof(GridParams), cudaMemcpyHostToDevice, st));
+  B2M_CK(cudaMemcpyAsync(b_cell_off.p, coff.data(), nstruct * sizeof(int), cudaMemcpyHostToDevice, st));
+  for (int k = 0; k < 3; k++) {  // the first structure's grid, for the record
+    nc[k] = gps[0].nc[k], reach[k] = gps[0].reach[k], fmin[k] = gps[0].fmin[k], fscale[k] = gps[0].fscale[k];
+  }
+
+  // ---- owner + cell id, sort by (structure, cell), rows ----
+  launch(k_owner_cell_batch, cdiv(N, 256), 256, 0, st, N, fracw.p, b_sid.p, b_gp.p, b_cell_off.p, owner.p, cell_of.p,
+         tmp_i0.p);
+  sort_by_cell(st, (int)ncell);
+  S = nstruct;
+  b_off = off;
+  b_volume = vol;
+  build_rows(st, gps[0]);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -9,6 +9,14 @@
 
 namespace b2m {
 
+// cell grid of one structure, and its lattice (rows), inverse and periodicity
+struct GridParams {
+  double lat[9];
+  double inv[9];
+  int nc[3], reach[3], pbc[3];
+  double fmin[3], fscale[3];
+};
+
 struct Graph {
   // ---- problem ----
   int64_t N = 0;
@@ -83,11 +91,30 @@ struct Graph {
   bool balanced = false;
   DBuf<double> bal_x;     // [2N] coordinates along the axis, then sorted
   DBuf<long long> bal_w;  // [2N] work per atom, then sorted; its inclusive prefix overwrites the first half
+  // ---- batch (build_batch, DESIGN.md §12): the disjoint union of S structures, structure s owning the gids
+  // b_off[s] .. b_off[s + 1] - 1; S = 0 after a single-structure build ----
+  int S = 0;
+  std::vector<int64_t> b_off;    // [S + 1]
+  std::vector<double> b_volume;  // [S]
+  DBuf<GridParams> b_gp;         // [S] each structure's own cell grid
+  DBuf<int> b_cell_off;          // [S] first global cell id of each structure
+  DBuf<int> b_sid;               // [N] structure of each atom
+  DBuf<int64_t> b_doff;          // [S + 1] b_off on the device
 
   void build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
              const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,
              int rank_, int world_);
+  // world = 1 only: nstruct structures, atoms concatenated in structure order (natoms[s] each), lattices [S][9],
+  // pbc flags [S][3].  Same arrays as build() for the union; inside a structure the rows, edges, bonds and angles come
+  // in the order build() gives that structure alone, with every atom index offset by b_off[s].
+  void build_batch(cudaStream_t st, int nstruct, const int64_t* natoms, const double* h_cart, const double* h_lat,
+                   const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_);
   int64_t export_info(cudaStream_t st, int which, int64_t* out, int64_t cap);
+
+ private:
+  void upload(cudaStream_t st, const double* h_cart, const int32_t* h_species);
+  void sort_by_cell(cudaStream_t st, int ncell);
+  void build_rows(cudaStream_t st, const GridParams& gp);
 };
 
 // Unfolded cell of the heat flux (DESIGN.md §10): the n cell atoms at their given positions, followed by every periodic

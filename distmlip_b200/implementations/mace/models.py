@@ -284,6 +284,12 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
         per-atom virials [n, 3, 3] eV or None)."""
         return self._evaluate(atoms, forces, stress, atomic, 0.0, None)
 
+    def evaluate_batch(self, atoms_list, forces=True, stress=True, atomic=False):
+        """`evaluate` for many independent structures in one graph build and one evaluation (DESIGN.md §12): a list of
+        `evaluate` tuples, one per structure in order.  The model must run on one GPU and one partition."""
+        return [(o["energy"], o["forces"], o["stress"], o["atomic_energies"], o["atomic_virials"])
+                for o in self._evaluate_batch(atoms_list, forces, stress, atomic)]
+
     def evaluate_heat_flux(self, atoms, velocities, reach=None, atomic=False):
         """`evaluate` (energy, forces and stress always) plus the heat flux (J_pot [3], J_conv [3]) of velocities
         [n, 3] (DESIGN.md §10), in eV * velocity unit and not divided by the volume: J_conv = sum_i eps_i v_i over the

@@ -123,6 +123,44 @@ class EngineBackedModel:
         eng.finalize()
         self._engine_finalized, self._final_key = True, key
 
+    def _evaluate_batch(self, atoms_list, forces, stress, atomic, site=False, tol=1e-8, before=None):
+        """Many independent structures in one graph build and one evaluation (b2m_set_structures + b2m_compute_batch,
+        DESIGN.md §12).  Checks everything it can before the engine is touched (an empty list, a model on more than one
+        GPU or partition, an element the model lacks), then calls `before()`, concatenates the structures in order and
+        splits the results: one dict per structure with energy (float, eV), forces [n, 3], stress [3, 3] (GPa), the
+        per-atom energies [n] and virials [n, 3, 3] (eV; with `atomic`), the site-wise readout [n] (with `site`) and the
+        cell; what is not asked for is None."""
+        atoms_list = list(atoms_list)
+        if not atoms_list:
+            raise ValueError("empty batch: pass at least one structure")
+        if not self.__dict__.get("dist_enabled"):
+            raise RuntimeError("call enable_distributed_mode(gpus) first")
+        eng = self._engine
+        if eng.group or eng.world > 1:
+            raise NotImplementedError("a batch runs on one GPU and one partition: enable_distributed_mode([gpu]) in "
+                                      f"a single process, not {len(self.gpus)} GPUs / {eng.world} partitions")
+        species = [self._species_of(a) for a in atoms_list]
+        n = [len(sp) for sp in species]
+        cells = np.array([np.array(a.get_cell(), dtype=np.float64).reshape(3, 3) for a in atoms_list])
+        cart = np.concatenate([np.asarray(a.get_positions(wrap=False), dtype=np.float64).reshape(-1, 3)
+                               for a in atoms_list])
+        pbc = np.array([np.asarray(a.get_pbc(), dtype=np.int32).reshape(3) for a in atoms_list])
+        if before is not None:
+            before()
+        self._set_heat_flux(0.0, None)
+        eng.set_structures(n, cart, cells, np.concatenate(species), pbc, tol)
+        e, f, s = eng.compute_batch(forces=forces, stress=stress)
+        ae, av = eng.atomic(virials=bool(forces or stress)) if atomic else (None, None)
+        sw = eng.sitewise() if site else None
+        cut = np.cumsum(n)[:-1]
+
+        def split(a):
+            return np.split(a, cut) if a is not None else [None] * len(n)
+
+        return [dict(energy=float(e[k]), forces=fk, stress=None if s is None else s[k], atomic_energies=aek,
+                     atomic_virials=avk, site_wise=swk, cell=cells[k])
+                for k, (fk, aek, avk, swk) in enumerate(zip(split(f), split(ae), split(av), split(sw)))]
+
     def heat_flux_reach(self):
         """Receptive-field radius (Angstrom) of an atom's energy: the unfolded cell of the heat flux must hold every
         periodic image within this distance of the cell (DESIGN.md §10)."""

@@ -119,3 +119,34 @@ class Potential_Dist:
         if self.calc_site_wise:
             return total_energies, forces, stresses, hessian, site_wise
         return total_energies, forces, stresses, hessian
+
+    def forward_batch(self, atoms_list, state_attr=None, tol=1.0e-8):
+        """Many independent structures in one graph build and one evaluation (DESIGN.md §12): a list with, for each
+        structure in order, the tuple `forward(atoms)` returns.  With `calc_atomic`, `atomic_energies` and
+        `atomic_stresses` become lists with one entry per structure.  The model must run on one GPU and one partition;
+        the heat flux of a batch is not supported."""
+        if self.calc_heat_flux:
+            raise NotImplementedError("the heat flux of a batch is not supported: evaluate the structures one by one")
+        model = self.model
+        want_backward = bool(self.calc_forces or self.calc_stresses)
+        outs = model._evaluate_batch(
+            atoms_list, self.calc_forces, self.calc_stresses, self.calc_atomic,
+            site=bool(self.calc_site_wise and model._has_site), tol=tol,
+            before=lambda: model._finalize(self.data_mean, self.data_std, self.element_refs))
+        self.last_dist_info = None
+        self.heat_flux = None
+        if self.calc_atomic:
+            self.atomic_energies = [torch.from_numpy(o["atomic_energies"]) for o in outs]
+            # w_i / V, in the unit and sign of `stresses` (pes.py:140-145)
+            self.atomic_stresses = [torch.from_numpy((o["atomic_virials"].astype(np.float64) * (
+                160.21766208 / abs(np.linalg.det(o["cell"])))).astype(np.float32)) if want_backward else None
+                for o in outs]
+        results = []
+        for o in outs:
+            r = (torch.tensor([o["energy"]], dtype=torch.float64),
+                 torch.as_tensor(o["forces"]) if self.calc_forces else None,
+                 torch.as_tensor(o["stress"]) if self.calc_stresses else None, None)
+            if self.calc_site_wise:
+                r += (torch.as_tensor(o["site_wise"]).reshape(-1, 1) if o["site_wise"] is not None else None,)
+            results.append(r)
+        return results

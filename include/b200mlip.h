@@ -184,6 +184,31 @@ int b2m_compute_resident(b2m_handle h, int want_forces, int want_stress, int rep
  * forces [natoms][3] and stress [3][3] (GPa), as b2m_compute returns them; any pointer may be NULL. */
 int b2m_get_results(b2m_handle h, double* energy, float* forces, float* stress9);
 
+/* Batched evaluation (DESIGN.md §12): many independent structures in one graph build and one model pass, for relaxing
+ * or screening many small cells, phonon displacements, strain sets, NEB images or a dataset.  nstruct structures, atoms
+ * concatenated in structure order (structure s owns the atoms off_s .. off_s + natoms[s] - 1, off_s the sum of the
+ * natoms before it): cart [sum natoms][3], lattice9 [nstruct][9] row vectors, species [sum natoms], pbc3 [nstruct][3],
+ * tol as in b2m_set_structure.  The graph is the disjoint union of the structures' graphs: no edge crosses from one
+ * structure to another, each has its own lattice, periodicity and cell grid, and the graph build costs the same number
+ * of launches and host synchronisations whatever nstruct is.
+ * Refused with B2M_ERR_INVALID and a message (nothing of the handle changes but the resident structure, which is gone):
+ * a single-process group (ndev > 1) or a rank of a multi-process job (a batch runs on one partition), nstruct < 1, and,
+ * naming the structure's index, a structure with no atoms, pbc flags other than 0 / 1, a singular lattice, a cell far too
+ * small for the cutoff, or no edge at all (isolated atoms are not supported).  B2M_ERR_STATE while a heat-flux reach is
+ * set.
+ * While a batch is resident, b2m_compute, b2m_compute_resident, b2m_get_results and b2m_compute_heat_flux return
+ * B2M_ERR_STATE (their one energy and one stress do not describe a batch); b2m_get_atomic, b2m_get_sitewise,
+ * b2m_get_counts, b2m_get_partition_info, b2m_last_timings and b2m_release_workspace work, with the atoms numbered in
+ * batch order.  The next b2m_set_structure drops the batch. */
+int b2m_set_structures(b2m_handle h, int32_t nstruct, const int64_t* natoms, const double* cart,
+                       const double* lattice9, const int32_t* species, const int* pbc3, double tol);
+/* Evaluates the resident batch: energies [nstruct] (eV), forces [sum natoms][3] (eV/A), stress9 [nstruct][9] (GPa), each
+ * what b2m_compute returns for that structure alone (the stress from the sum of the structure's per-atom virials over
+ * its own volume).  forces / stress9 may be NULL.  Per-atom energies and virials are always computed for a batch, so
+ * b2m_get_atomic returns them afterwards whatever b2m_set_atomic says (energies[i] with data_mean / natoms[s] of its
+ * structure s). */
+int b2m_compute_batch(b2m_handle h, int want_forces, int want_stress, double* energies, float* forces, float* stress9);
+
 /* Per-atom energies and virials (DESIGN.md "Per-atom energies and virials"), off by default.  With on != 0 the
  * following evaluations (b2m_compute, b2m_compute_resident) also produce, for every atom i,
  *   energies[i] = data_std * e_i + element_ref[Z_i] + data_mean / natoms   (eV; sums to the energy)
