@@ -19,7 +19,7 @@ SYMBOLS = [
     "b2m_compute_resident", "b2m_get_results", "b2m_get_sitewise", "b2m_get_counts", "b2m_get_partition_info",
     "b2m_debug_tensor", "b2m_last_timings", "b2m_release_workspace", "b2m_set_view", "b2m_create_tensornet",
     "b2m_set_atomic", "b2m_get_atomic", "b2m_set_heat_flux", "b2m_compute_heat_flux", "b2m_create_mace",
-    "b2m_set_partition_policy", "b2m_set_structures", "b2m_compute_batch",
+    "b2m_set_partition_policy", "b2m_set_structures", "b2m_compute_batch", "b2m_relax_batch",
 ]
 
 PARTITION_EQUAL, PARTITION_BALANCED = 0, 1
@@ -50,6 +50,17 @@ class MaceDesc(C.Structure):
         ("r_max", C.c_double), ("c_act", C.c_double), ("avg_num_neighbors", C.c_double * 8),
         ("hidden_mul", C.c_int32 * 4),
     ]
+
+
+# the nine constants of ase.optimize.FIRE, in b2m_relax_params order, with ASE's defaults
+FIRE_DEFAULTS = dict(dt=0.1, maxstep=0.2, dtmax=1.0, Nmin=5, finc=1.1, fdec=0.5, astart=0.1, fa=0.99, a=0.1)
+
+
+class RelaxParams(C.Structure):
+    _fields_ = [
+        ("fmax", C.c_double), ("steps", C.c_int32), ("relax_cell", C.c_int32), ("scalar_pressure", C.c_double),
+        ("stress_weight", C.c_double),
+    ] + [(k, C.c_double) for k in FIRE_DEFAULTS]
 
 
 class B2MError(RuntimeError):
@@ -89,6 +100,9 @@ def load_library():
     lib.b2m_set_partition_policy.argtypes = [vp, i32]
     lib.b2m_set_structure.argtypes = [vp, i64, P(dbl), P(dbl), P(C.c_int32), P(C.c_int), dbl]
     lib.b2m_set_structures.argtypes = [vp, i32, P(i64), P(dbl), P(dbl), P(C.c_int32), P(C.c_int), dbl]
+    lib.b2m_relax_batch.argtypes = [vp, i32, P(i64), P(dbl), P(dbl), P(C.c_int32), P(C.c_int), dbl,
+                                    P(RelaxParams), P(dbl), P(C.c_float), P(C.c_float), P(C.c_int32), P(C.c_int32),
+                                    P(dbl)]
     lib.b2m_compute.argtypes = [vp, i32, i32, P(dbl), P(C.c_float), P(C.c_float)]
     lib.b2m_compute_batch.argtypes = [vp, i32, i32, P(dbl), P(C.c_float), P(C.c_float)]
     lib.b2m_compute_resident.argtypes = [vp, i32, i32, i32, P(dbl), P(C.c_float)]
@@ -251,6 +265,48 @@ class Engine:
             f.ctypes.data_as(C.POINTER(C.c_float)) if f is not None else None,
             s.ctypes.data_as(C.POINTER(C.c_float)) if s is not None else None))
         return e, f, (s.reshape(S, 3, 3) if s is not None else None)
+
+    def relax_batch(self, natoms, cart, lattices, species, pbc, fmax=0.1, steps=500, relax_cell=True,
+                    scalar_pressure=0.0, stress_weight=1 / 160.21766208, tol=1e-8, trace=True, **fire):
+        """FIRE (+ Frechet cell filter) on every structure of a batch, the loop on the device (b2m_relax_batch): inputs
+        as set_structures, `fire` any of FIRE_DEFAULTS' keys.  Returns a dict of arrays in input order: cart
+        [sum, 3] and lattices [S, 3, 3] (final geometries), energies [S] (eV), forces [sum, 3] f32, stress [S, 3, 3]
+        f32 GPa, steps [S], converged [S] bool, and (trace; None without) energies per evaluation [S, steps + 1],
+        NaN after a structure stopped.  The batch of the last step stays resident."""
+        unknown = set(fire) - set(FIRE_DEFAULTS)
+        if unknown:
+            raise TypeError(f"unknown FIRE parameters {sorted(unknown)}; FIRE takes {list(FIRE_DEFAULTS)}")
+        natoms = np.ascontiguousarray(natoms, dtype=np.int64).reshape(-1)
+        S = len(natoms)
+        cart = np.array(cart, dtype=np.float64, order="C").reshape(-1, 3)  # copies: the library writes into them
+        lattices = np.array(lattices, dtype=np.float64, order="C").reshape(S, 9)
+        species = np.ascontiguousarray(species, dtype=np.int32)
+        pbc = np.ascontiguousarray(pbc, dtype=np.int32).reshape(S, 3)
+        if len(cart) != int(natoms.sum()) or len(species) != len(cart):
+            raise ValueError(f"positions [{len(cart)}] and species [{len(species)}] must hold sum(natoms) = "
+                             f"{int(natoms.sum())} atoms")
+        prm = RelaxParams(fmax=float(fmax), steps=int(steps), relax_cell=int(bool(relax_cell)),
+                          scalar_pressure=float(scalar_pressure), stress_weight=float(stress_weight),
+                          **{k: float(fire.get(k, d)) for k, d in FIRE_DEFAULTS.items()})
+        e = np.empty(S, dtype=np.float64)
+        f = np.empty((len(cart), 3), dtype=np.float32)
+        s = np.empty((S, 9), dtype=np.float32)
+        nst = np.empty(S, dtype=np.int32)
+        conv = np.empty(S, dtype=np.int32)
+        tr = np.empty((S, max(int(steps), 0) + 1), dtype=np.float64) if trace else None
+        dp = C.POINTER(C.c_double)
+        self.natoms, self.batch_natoms = 0, np.zeros(0, dtype=np.int64)  # no batch is resident if the call fails
+        self._ck(self.lib.b2m_relax_batch(
+            self.h, S, natoms.ctypes.data_as(C.POINTER(C.c_int64)), cart.ctypes.data_as(dp), lattices.ctypes.data_as(dp),
+            species.ctypes.data_as(C.POINTER(C.c_int32)), pbc.ctypes.data_as(C.POINTER(C.c_int)), float(tol),
+            C.byref(prm), e.ctypes.data_as(dp), f.ctypes.data_as(C.POINTER(C.c_float)),
+            s.ctypes.data_as(C.POINTER(C.c_float)), nst.ctypes.data_as(C.POINTER(C.c_int32)),
+            conv.ctypes.data_as(C.POINTER(C.c_int32)), tr.ctypes.data_as(dp) if tr is not None else None))
+        # the batch of the last step stays resident: the structures that ran longest, in input order
+        self.batch_natoms = natoms[nst == nst.max()]
+        self.natoms = int(self.batch_natoms.sum())
+        return dict(cart=cart, lattices=lattices.reshape(S, 3, 3), energies=e, forces=f, stress=s.reshape(S, 3, 3),
+                    steps=nst, converged=conv.astype(bool), trace=tr)
 
     def compute(self, forces=True, stress=True, out_forces=None, out_stress=None):
         e = C.c_double()

@@ -12,8 +12,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200mlip.so")
-SOURCES = ["graph.cu", "kernels.cu", "kernels_wg.cu", "kernels_tn.cu", "kernels_mace.cu", "engine.cu"]
-HEADERS = ["common.cuh", "final_tail.cuh", "graph.cuh", "kernels.cuh", "wgmma.cuh", "engine_chgnet.inl", "tn_state.cuh", "engine_tn.inl", "mace_state.cuh", "mace_cg.cuh", "mace_cg_l2.cuh", "engine_mace.inl", os.path.join("..", "..", "include", "b200mlip.h")]
+SOURCES = ["graph.cu", "kernels.cu", "kernels_wg.cu", "kernels_tn.cu", "kernels_mace.cu", "relax.cu", "engine.cu"]
+HEADERS = ["common.cuh", "final_tail.cuh", "graph.cuh", "kernels.cuh", "wgmma.cuh", "engine_chgnet.inl", "tn_state.cuh", "engine_tn.inl", "mace_state.cuh", "mace_cg.cuh", "mace_cg_l2.cuh", "engine_mace.inl", "relax.cuh", os.path.join("..", "..", "include", "b200mlip.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--extended-lambda",
     "-Xcompiler", "-fPIC", "-Wno-deprecated-declarations",

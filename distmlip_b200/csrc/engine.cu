@@ -25,6 +25,7 @@
 #include "graph.cuh"
 #include "kernels.cuh"
 #include "mace_state.cuh"
+#include "relax.cuh"
 #include "tn_state.cuh"
 
 namespace b2m {
@@ -858,13 +859,19 @@ __global__ void __launch_bounds__(256) k_batch_sums(const int64_t* __restrict__ 
   block_sum_add(acc, out + 10 * blockIdx.x);
 }
 
-// energies [S], forces [N][3] and stress9 [S][9] of the batch just evaluated (any may be null); one launch for any S
-static void fetch_batch(b2m_engine* e, bool grads, double* energies, float* forces, float* stress9) {
+// per-structure energy and virial sums of the batch just evaluated into buf.bsum [S][10], on the stream
+static void batch_sums(b2m_engine* e, bool grads) {
   const Graph& g = e->g;
   e->buf.bsum.ensure((size_t)g.S * 10 + 64);
   e->buf.bsum.zero((size_t)g.S * 10, e->st);
   launch(k_batch_sums, g.S, 256, 0, e->st, g.b_doff.p, e->desc.data_mean, e->buf.atom_e.p,
          grads ? (const float*)e->buf.atom_vir.p : nullptr, e->buf.bsum.p);
+}
+
+// energies [S], forces [N][3] and stress9 [S][9] of the batch just evaluated (any may be null); one launch for any S
+static void fetch_batch(b2m_engine* e, bool grads, double* energies, float* forces, float* stress9) {
+  const Graph& g = e->g;
+  batch_sums(e, grads);
   std::vector<double> hs((size_t)g.S * 10);
   B2M_CK(cudaMemcpyAsync(hs.data(), e->buf.bsum.p, hs.size() * sizeof(double), cudaMemcpyDeviceToHost, e->st));
   fetch(e, nullptr, forces, nullptr);  // forces, and the stream synchronised
@@ -873,6 +880,127 @@ static void fetch_batch(b2m_engine* e, bool grads, double* energies, float* forc
     if (stress9)
       for (int k = 0; k < 9; k++) stress9[9 * s + k] = (float)(hs[10 * s + 1 + k] / g.b_volume[s] * 160.21766208);
   }
+}
+
+// Batched relaxation (b2m_relax_batch, DESIGN.md §13).  Device state in input order; each step builds the graph of the
+// active structures act[] from the emitted positions, evaluates it, runs the relax kernels and copies the [S] status
+// block back, so the launches and host synchronisations of a step do not depend on S or on how many are active.
+struct RelaxOut {
+  double* energies;
+  float* forces;
+  float* stress9;
+  int32_t* steps_taken;
+  int32_t* converged;
+  double* trace;
+};
+
+static void relax_loop(b2m_engine* h, int S, const int64_t* natoms, double* cart, double* lat9, const int32_t* species,
+                       const int* pbc3, double tol, const b2m_relax_params& p, const RelaxOut& out) {
+  std::vector<int64_t> in_off(S + 1, 0);
+  for (int s = 0; s < S; s++) in_off[s + 1] = in_off[s] + natoms[s];
+  const int64_t N = in_off[S];
+  RelaxConst c{p.fmax * p.fmax, p.maxstep, p.dtmax, p.Nmin, p.finc, p.fdec, p.astart, p.fa,
+               p.stress_weight * 160.21766208, p.scalar_pressure, p.relax_cell, p.steps};
+  const int64_t pitch = out.trace ? (int64_t)p.steps + 1 : 0;  // energy trace [S][pitch], only when asked for
+  cudaStream_t st = h->st;
+  DBuf<double> r0, v, stat, res_e, res_s, trace, ecart, dlat;
+  DBuf<float> res_f;
+  DBuf<int> sp_in, sp_out;
+  DBuf<RelaxStruct> rs;
+  DBuf<int64_t> d_in_off, d_sel;
+  r0.ensure(3 * N), v.ensure(3 * N), ecart.ensure(3 * N), res_f.ensure(3 * N), sp_in.ensure(N), sp_out.ensure(N);
+  stat.ensure((size_t)kRelaxStat * S), res_e.ensure(S), res_s.ensure(9 * (size_t)S), rs.ensure(S), dlat.ensure(9 * S);
+  if (pitch) trace.ensure((size_t)pitch * S);
+  d_in_off.ensure(S + 1), d_sel.ensure(2 * (size_t)S + 1);
+  B2M_CK(cudaMemcpyAsync(r0.p, cart, 3 * N * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2M_CK(cudaMemcpyAsync(sp_in.p, species, N * sizeof(int), cudaMemcpyHostToDevice, st));
+  B2M_CK(cudaMemcpyAsync(dlat.p, lat9, 9 * S * sizeof(double), cudaMemcpyHostToDevice, st));
+  B2M_CK(cudaMemcpyAsync(d_in_off.p, in_off.data(), (S + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  v.zero(3 * N, st);
+  if (pitch)  // all-ones bytes are a NaN double
+    B2M_CK(cudaMemsetAsync(trace.p, 0xFF, (size_t)pitch * S * sizeof(double), st));
+  launch_relax_init(st, S, dlat.p, p.dt, p.a, rs.p, stat.p);
+  std::vector<double> hstat((size_t)kRelaxStat * S);
+  B2M_CK(cudaMemcpyAsync(hstat.data(), stat.p, hstat.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaStreamSynchronize(st));
+
+  std::vector<int64_t> act(S), sel, counts;
+  for (int s = 0; s < S; s++) act[s] = s;
+  std::vector<double> lats;
+  std::vector<int> pbcs;
+  for (int it = 0; !act.empty(); it++) {
+    const long long l0 = g_launch_count;
+    const int Sa = (int)act.size();
+    // [act | out_off] in one upload, and the build's host inputs
+    sel.assign(act.begin(), act.end());
+    sel.push_back(0);
+    counts.resize(Sa), lats.resize(9 * (size_t)Sa), pbcs.resize(3 * (size_t)Sa);
+    for (int k = 0; k < Sa; k++) {
+      const int64_t s = act[k];
+      counts[k] = natoms[s];
+      sel.push_back(sel.back() + natoms[s]);
+      for (int q = 0; q < 9; q++) lats[9 * k + q] = hstat[kRelaxStat * s + 3 + q];
+      for (int q = 0; q < 3; q++) pbcs[3 * k + q] = pbc3[3 * s + q];
+    }
+    B2M_CK(cudaMemcpyAsync(d_sel.p, sel.data(), sel.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    const int64_t* d_act = d_sel.p;
+    launch_relax_emit(st, Sa, d_act, d_in_off.p, d_act + Sa, rs.p, r0.p, sp_in.p, ecart.p, sp_out.p);
+    h->have_graph = false;
+    h->atomic_last = 0;
+    h->hf_n = 0, h->hf_seed = -1;
+    h->g.balanced = h->partition_policy == B2M_PARTITION_BALANCED;
+    h->g.walls_from_min = false;
+    h->g.b_name = act;  // errors name the structures by their input index
+    try {
+      h->g.build_batch(st, Sa, counts.data(), ecart.p, lats.data(), sp_out.p, pbcs.data(), h->desc.cutoff,
+                       h->desc.three_body_cutoff, tol);
+      alloc_workspace(h);
+      h->have_graph = true;
+      run(h, true);
+    } catch (const Error& ex) {
+      h->g.b_name.clear();
+      throw Error(ex.code, "relaxation step " + std::to_string(it) + ": " + ex.what());
+    }
+    h->g.b_name.clear();
+    batch_sums(h, true);
+    launch_relax_struct(st, Sa, it, c, d_act, d_in_off.p, h->g.b_doff.p, h->buf.forces.p, h->buf.bsum.p,
+                        h->desc.data_mean, v.p, rs.p, stat.p, res_f.p, res_e.p, res_s.p, trace.p, pitch);
+    launch_relax_rows(st, h->g.N, c, d_act, d_in_off.p, h->g.b_doff.p, h->g.b_sid.p, h->buf.forces.p, rs.p, v.p,
+                      r0.p);
+    B2M_CK(cudaMemcpyAsync(hstat.data(), stat.p, hstat.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    B2M_CK(cudaStreamSynchronize(st));
+    h->launches_last = g_launch_count - l0;
+    size_t keep = 0;
+    for (int k = 0; k < Sa; k++) {
+      const int64_t s = act[k];
+      const int flag = (int)hstat[kRelaxStat * s];
+      if (flag == 0) {
+        act[keep++] = s;
+      } else {
+        out.steps_taken[s] = it;
+        out.converged[s] = flag == 1;
+      }
+    }
+    act.resize(keep);
+  }
+
+  // final geometries (input order) and the results of each structure's last evaluation
+  sel.resize(2 * (size_t)S + 1);
+  for (int s = 0; s < S; s++) sel[s] = s;
+  for (int s = 0; s <= S; s++) sel[S + s] = in_off[s];
+  B2M_CK(cudaMemcpyAsync(d_sel.p, sel.data(), sel.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  launch_relax_emit(st, S, d_sel.p, d_in_off.p, d_sel.p + S, rs.p, r0.p, sp_in.p, ecart.p, sp_out.p);
+  std::vector<double> hs(9 * (size_t)S);
+  B2M_CK(cudaMemcpyAsync(cart, ecart.p, 3 * N * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaMemcpyAsync(out.energies, res_e.p, S * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaMemcpyAsync(out.forces, res_f.p, 3 * N * sizeof(float), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaMemcpyAsync(hs.data(), res_s.p, hs.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  if (out.trace)
+    B2M_CK(cudaMemcpyAsync(out.trace, trace.p, (size_t)pitch * S * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaStreamSynchronize(st));
+  for (size_t k = 0; k < hs.size(); k++) out.stress9[k] = (float)hs[k];
+  for (int s = 0; s < S; s++)
+    for (int q = 0; q < 9; q++) lat9[9 * s + q] = hstat[kRelaxStat * s + 3 + q];
 }
 
 // One forward + backward per readout weight: the three seeds (r_j - c)_alpha, then the cell mask, so that the handle is
@@ -1268,6 +1396,38 @@ int b2m_compute_batch(b2m_handle h, int want_forces, int want_stress, double* en
   const bool grads = want_forces || want_stress;
   run(h, grads);
   fetch_batch(h, grads, energies, want_forces ? forces : nullptr, want_stress ? stress9 : nullptr);
+  API_END
+}
+
+int b2m_relax_batch(b2m_handle h, int32_t nstruct, const int64_t* natoms, double* cart_inout, double* lattice9_inout,
+                    const int32_t* species, const int* pbc3, double tol, const b2m_relax_params* params,
+                    double* energies, float* forces, float* stress9, int32_t* steps_taken, int32_t* converged,
+                    double* energy_trace) {
+  API_BEGIN
+  B2M_REQUIRE(h->parts.empty() && h->world == 1, B2M_ERR_INVALID,
+              "a batch runs on one partition: not on a single-process group (ndev > 1) or a rank of a multi-process job");
+  B2M_REQUIRE(h->hf_reach == 0, B2M_ERR_STATE, "a batch has no heat flux (b2m_set_heat_flux(h, 0) first)");
+  B2M_REQUIRE(h->finalized, B2M_ERR_STATE, "weights not finalized");
+  B2M_REQUIRE(nstruct >= 1, B2M_ERR_INVALID, "a batch needs at least one structure");
+  B2M_REQUIRE(natoms && cart_inout && lattice9_inout && species && pbc3 && params, B2M_ERR_INVALID,
+              "null structure argument");
+  B2M_REQUIRE(energies && forces && stress9 && steps_taken && converged, B2M_ERR_INVALID, "null result argument");
+  const b2m_relax_params& p = *params;
+  B2M_REQUIRE(p.steps >= 0, B2M_ERR_INVALID, "steps must be >= 0");
+  for (double x : {p.fmax, p.scalar_pressure, p.stress_weight, p.dt, p.maxstep, p.dtmax, p.Nmin, p.finc, p.fdec,
+                   p.astart, p.fa, p.a})
+    B2M_REQUIRE(std::isfinite(x), B2M_ERR_INVALID, "relaxation parameters must be finite");
+  B2M_REQUIRE(p.dt > 0 && p.maxstep > 0 && p.dtmax > 0, B2M_ERR_INVALID, "FIRE dt, maxstep and dtmax must be > 0");
+  B2M_REQUIRE(p.fmax >= 0, B2M_ERR_INVALID, "fmax must be >= 0");
+  for (int s = 0; s < nstruct; s++) {
+    B2M_REQUIRE(natoms[s] > 0, B2M_ERR_INVALID, "structure " + std::to_string(s) + ": no atoms");
+    if (p.relax_cell)
+      for (int k = 0; k < 3; k++)
+        B2M_REQUIRE(pbc3[3 * s + k] == 1, B2M_ERR_INVALID,
+                    "structure " + std::to_string(s) + ": relax_cell needs a periodic cell on every axis");
+  }
+  relax_loop(h, nstruct, natoms, cart_inout, lattice9_inout, species, pbc3, tol, p,
+             RelaxOut{energies, forces, stress9, steps_taken, converged, energy_trace});
   API_END
 }
 

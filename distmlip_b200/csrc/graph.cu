@@ -1050,7 +1050,7 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
   B2M_REQUIRE(E > 0, B2M_ERR_INVALID, "No neighbors were found!");
   for (int s = 0; s < S; s++)
     B2M_REQUIRE(e_at[s + 1] > e_at[s], B2M_ERR_INVALID,
-                "structure " + std::to_string(s) + " has no edges (No neighbors were found!)");
+                structure_name(s) + " has no edges (No neighbors were found!)");
 
   e_src.ensure(E);
   e_dst.ensure(E);
@@ -1242,7 +1242,7 @@ void Graph::build_batch(cudaStream_t st, int nstruct, const int64_t* natoms, con
                         const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_) {
   B2M_REQUIRE(nstruct >= 1, B2M_ERR_INVALID, "a batch needs at least one structure");
   B2M_REQUIRE(rbond <= rcut, B2M_ERR_INVALID, "bond_r cannot be greater than regular cutoff");
-  auto named = [](int s, const std::string& what) { return "structure " + std::to_string(s) + ": " + what; };
+  auto named = [this](int s, const std::string& what) { return structure_name(s) + ": " + what; };
   std::vector<int64_t> off(nstruct + 1, 0);
   std::vector<GridParams> gps(nstruct);
   std::vector<double> vol(nstruct);

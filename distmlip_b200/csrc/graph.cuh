@@ -100,6 +100,7 @@ struct Graph {
   DBuf<int> b_cell_off;          // [S] first global cell id of each structure
   DBuf<int> b_sid;               // [N] structure of each atom
   DBuf<int64_t> b_doff;          // [S + 1] b_off on the device
+  std::vector<int64_t> b_name;   // the caller's index of each structure, for error messages; empty: the batch index
 
   void build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
              const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,
@@ -110,6 +111,9 @@ struct Graph {
   void build_batch(cudaStream_t st, int nstruct, const int64_t* natoms, const double* h_cart, const double* h_lat,
                    const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_);
   int64_t export_info(cudaStream_t st, int which, int64_t* out, int64_t cap);
+  std::string structure_name(int s) const {  // "structure <caller's index>"
+    return "structure " + std::to_string(s < (int)b_name.size() ? b_name[s] : (int64_t)s);
+  }
 
  private:
   void upload(cudaStream_t st, const double* h_cart, const int32_t* h_species);

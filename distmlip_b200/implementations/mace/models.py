@@ -290,6 +290,16 @@ class ScaleShiftMACE_Dist(EngineBackedModel):
         return [(o["energy"], o["forces"], o["stress"], o["atomic_energies"], o["atomic_virials"])
                 for o in self._evaluate_batch(atoms_list, forces, stress, atomic)]
 
+    def relax_batch(self, atoms_list, fmax=0.1, steps=500, relax_cell=True, scalar_pressure=0.0, trace=True,
+                    **fire_kwargs):
+        """ASE's FIRE (fire_kwargs: its nine constants dt, maxstep, dtmax, Nmin, finc, fdec, astart, fa, a) with, when
+        relax_cell, the Frechet cell filter at scalar_pressure (eV/A^3), run independently on every structure, the
+        whole loop on the GPU (DESIGN.md §13).  One dict per structure: final_structure (a copy), energy (eV), forces
+        [n, 3] (eV/A), stress [3, 3] (eV/A^3), steps, converged and energies (one per evaluation; None with
+        trace=False).  The model must run on one GPU and one partition."""
+        return self._relax_batch(atoms_list, fmax, steps, relax_cell, float(scalar_pressure), 1 / 160.21766208,
+                                 fire_kwargs, trace=trace)
+
     def evaluate_heat_flux(self, atoms, velocities, reach=None, atomic=False):
         """`evaluate` (energy, forces and stress always) plus the heat flux (J_pot [3], J_conv [3]) of velocities
         [n, 3] (DESIGN.md §10), in eV * velocity unit and not divided by the volume: J_conv = sum_i eps_i v_i over the

@@ -158,7 +158,11 @@ class Relaxer:
             if not hasattr(opt, name):
                 raise KeyError(optimizer)
             optimizer = getattr(opt, name)
+        else:
+            name = getattr(optimizer, "__name__", str(optimizer))
         self.optimizer = optimizer
+        self.optimizer_name = name
+        self.stress_weight = stress_weight
         # ase.py:153-157: the reference passes ONLY stress_weight (GPa -> eV/A^3); stress_unit stays "GPa" (factor 1)
         self.calculator = PESCalculator_Dist(potential=potential, state_attr=state_attr, stress_weight=stress_weight)
         self.relax_cell = relax_cell
@@ -202,6 +206,47 @@ class Relaxer:
         if self.relax_cell:
             atoms = atoms.atoms
         return {"final_structure": adaptor.get_structure(atoms) if adaptor is not None else atoms, "trajectory": obs}
+
+    def relax_batch(self, atoms_list, fmax=0.1, steps=500, ase_cellfilter="Frechet", params_asecellfilter=None,
+                    trace=True, **kwargs):
+        """`relax` for many independent structures at once, the whole loop on the GPU (DESIGN.md §13): FIRE (kwargs:
+        its nine constants dt, maxstep, dtmax, Nmin, finc, fdec, astart, fa, a) and, with relax_cell, the Frechet cell
+        filter (params_asecellfilter: scalar_pressure only, eV/A^3), each structure on its own.  Returns one dict per
+        structure: final_structure (a copy; pymatgen in, pymatgen out), energy (eV), forces [n, 3] (eV/A), stress
+        [3, 3] (eV/A^3), steps, converged and energies (one per evaluation; None with trace=False, which saves an
+        [S, steps + 1] buffer).  The model must run on one GPU and one partition, without heat flux."""
+        if self.optimizer_name != "FIRE":
+            raise NotImplementedError(f"batched relaxation runs FIRE only, not {self.optimizer_name}")
+        if ase_cellfilter != "Frechet":
+            raise NotImplementedError(f"batched relaxation has the Frechet cell filter only, not {ase_cellfilter}")
+        params_asecellfilter = dict(params_asecellfilter or {})
+        unknown = set(params_asecellfilter) - {"scalar_pressure"}
+        if unknown:
+            raise NotImplementedError(f"batched relaxation takes only scalar_pressure as filter parameter, not "
+                                      f"{sorted(unknown)}")
+        pot = self.calculator.potential
+        if pot.calc_heat_flux:
+            raise NotImplementedError("batched relaxation has no heat flux: use a potential with calc_heat_flux=False")
+        atoms_list = list(atoms_list)
+        adaptor, pmg = None, [False] * len(atoms_list)
+        try:
+            from pymatgen.core import Molecule, Structure
+            from pymatgen.io.ase import AseAtomsAdaptor
+
+            adaptor = AseAtomsAdaptor()
+            pmg = [isinstance(a, (Structure, Molecule)) for a in atoms_list]
+            atoms_list = [adaptor.get_atoms(a) if p else a for a, p in zip(atoms_list, pmg)]
+        except ImportError:
+            pass
+        model = pot.model
+        outs = model._relax_batch(
+            atoms_list, fmax, steps, self.relax_cell, float(params_asecellfilter.get("scalar_pressure", 0.0)),
+            self.stress_weight, kwargs, before=lambda: model._finalize(pot.data_mean, pot.data_std, pot.element_refs),
+            trace=trace)
+        for o, p in zip(outs, pmg):
+            if p:
+                o["final_structure"] = adaptor.get_structure(o["final_structure"])
+        return outs
 
 
 class MolecularDynamics:

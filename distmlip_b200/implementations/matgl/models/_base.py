@@ -3,11 +3,16 @@
 `enable_distributed_mode(gpus, balance=False)`, species lookup, weight finalisation and the `potential_forward_dist` seam."""
 from __future__ import annotations
 
+import copy
+
 import numpy as np
 import torch
 
 import distmlip_b200
 from distmlip_b200 import _lib
+
+
+GPA_PER_EVA3 = 160.21766208
 
 
 class EngineBackedModel:
@@ -123,13 +128,10 @@ class EngineBackedModel:
         eng.finalize()
         self._engine_finalized, self._final_key = True, key
 
-    def _evaluate_batch(self, atoms_list, forces, stress, atomic, site=False, tol=1e-8, before=None):
-        """Many independent structures in one graph build and one evaluation (b2m_set_structures + b2m_compute_batch,
-        DESIGN.md §12).  Checks everything it can before the engine is touched (an empty list, a model on more than one
-        GPU or partition, an element the model lacks), then calls `before()`, concatenates the structures in order and
-        splits the results: one dict per structure with energy (float, eV), forces [n, 3], stress [3, 3] (GPa), the
-        per-atom energies [n] and virials [n, 3, 3] (eV; with `atomic`), the site-wise readout [n] (with `site`) and the
-        cell; what is not asked for is None."""
+    def _batch_inputs(self, atoms_list, before):
+        """The prologue of a batch call: refuses an empty list, a model on more than one GPU or partition and an
+        element the model lacks before the engine is touched, then calls `before()` and turns the heat flux off.
+        Returns (engine, natoms [S], positions [sum, 3], cells [S, 3, 3], species [sum], pbc [S, 3])."""
         atoms_list = list(atoms_list)
         if not atoms_list:
             raise ValueError("empty batch: pass at least one structure")
@@ -148,7 +150,48 @@ class EngineBackedModel:
         if before is not None:
             before()
         self._set_heat_flux(0.0, None)
-        eng.set_structures(n, cart, cells, np.concatenate(species), pbc, tol)
+        return eng, n, cart, cells, np.concatenate(species), pbc
+
+    def _relax_batch(self, atoms_list, fmax, steps, relax_cell, scalar_pressure, stress_weight, fire, tol=1e-8,
+                     before=None, trace=True):
+        """FIRE, with the Frechet cell filter when `relax_cell`, on every structure of a batch, the whole loop on the
+        device (b2m_relax_batch, DESIGN.md §13).  `fire`: ase.optimize.FIRE's constants (dt, maxstep, dtmax, Nmin,
+        finc, fdec, astart, fa, a); anything else is refused.  One dict per structure: final_structure (a copy of the
+        input at the final geometry), energy (eV), forces [n, 3] (eV/A), stress [3, 3] (eV/A^3), steps, converged,
+        energies (one per evaluation; None without `trace`, which then costs no [S, steps + 1] buffer)."""
+        unknown = set(fire) - set(_lib.FIRE_DEFAULTS)
+        if unknown:
+            raise TypeError(f"batched FIRE takes only {list(_lib.FIRE_DEFAULTS)}, not {sorted(unknown)}")
+        atoms_list = list(atoms_list)
+        if relax_cell:
+            for k, a in enumerate(atoms_list):
+                if not np.all(a.get_pbc()):
+                    raise ValueError(f"structure {k}: relax_cell needs a cell periodic along every axis")
+        eng, n, cart, cells, species, pbc = self._batch_inputs(atoms_list, before)
+        r = eng.relax_batch(n, cart, cells, species, pbc, fmax=fmax, steps=steps, relax_cell=relax_cell,
+                            scalar_pressure=scalar_pressure, stress_weight=stress_weight, tol=tol, trace=trace,
+                            **fire)
+        cut = np.cumsum(n)[:-1]
+        out = []
+        for k, (a, xk, fk) in enumerate(zip(atoms_list, np.split(r["cart"], cut), np.split(r["forces"], cut))):
+            final = a.copy() if hasattr(a, "copy") else copy.deepcopy(a)
+            final.set_cell(r["lattices"][k], scale_atoms=False)
+            final.set_positions(xk)
+            out.append(dict(final_structure=final, energy=float(r["energies"][k]), forces=fk,
+                            stress=r["stress"][k].astype(np.float64) / GPA_PER_EVA3, steps=int(r["steps"][k]),
+                            converged=bool(r["converged"][k]),
+                            energies=None if r["trace"] is None else r["trace"][k, :r["steps"][k] + 1].copy()))
+        return out
+
+    def _evaluate_batch(self, atoms_list, forces, stress, atomic, site=False, tol=1e-8, before=None):
+        """Many independent structures in one graph build and one evaluation (b2m_set_structures + b2m_compute_batch,
+        DESIGN.md §12).  Checks everything it can before the engine is touched (an empty list, a model on more than one
+        GPU or partition, an element the model lacks), then calls `before()`, concatenates the structures in order and
+        splits the results: one dict per structure with energy (float, eV), forces [n, 3], stress [3, 3] (GPa), the
+        per-atom energies [n] and virials [n, 3, 3] (eV; with `atomic`), the site-wise readout [n] (with `site`) and the
+        cell; what is not asked for is None."""
+        eng, n, cart, cells, species, pbc = self._batch_inputs(atoms_list, before)
+        eng.set_structures(n, cart, cells, species, pbc, tol)
         e, f, s = eng.compute_batch(forces=forces, stress=stress)
         ae, av = eng.atomic(virials=bool(forces or stress)) if atomic else (None, None)
         sw = eng.sitewise() if site else None

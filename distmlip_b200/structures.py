@@ -55,6 +55,12 @@ class SimpleAtoms:
     def set_positions(self, pos):
         self._positions = np.ascontiguousarray(pos, dtype=np.float64)
 
+    def set_cell(self, cell, scale_atoms=False):
+        cell = np.ascontiguousarray(cell, dtype=np.float64).reshape(3, 3)
+        if scale_atoms:
+            self._positions = np.linalg.solve(self._cell.T, self._positions.T).T @ cell
+        self._cell = cell
+
     def get_scaled_positions(self, wrap=True):
         frac = np.linalg.solve(self._cell.T, self._positions.T).T
         if wrap:

@@ -209,6 +209,41 @@ int b2m_set_structures(b2m_handle h, int32_t nstruct, const int64_t* natoms, con
  * structure s). */
 int b2m_compute_batch(b2m_handle h, int want_forces, int want_stress, double* energies, float* forces, float* stress9);
 
+/* Batched relaxation (DESIGN.md §13): ASE's FIRE, optionally with its FrechetCellFilter, run independently on each
+ * structure of a batch, with the whole loop on the device.  fmax (eV/A; 0 never converges), steps (optimizer steps at
+ * most: a structure is evaluated at most steps + 1 times), relax_cell (the Frechet cell filter, exp_cell_factor = natoms,
+ * with scalar_pressure in eV/A^3; the cell force weighs the strain derivative by stress_weight * 160.21766208), and the
+ * nine constants of ase.optimize.FIRE (ASE's defaults: dt 0.1, maxstep 0.2, dtmax 1.0, Nmin 5, finc 1.1, fdec 0.5,
+ * astart 0.1, fa 0.99, a 0.1). */
+typedef struct {
+  double fmax;
+  int32_t steps;
+  int32_t relax_cell;
+  double scalar_pressure;
+  double stress_weight;
+  double dt, maxstep, dtmax, Nmin, finc, fdec, astart, fa, a;
+} b2m_relax_params;
+/* Relaxes nstruct structures, laid out as in b2m_set_structures.  Each step builds the graph of the structures still
+ * running, evaluates it, takes one FIRE step per structure on the device and copies one small status block to the
+ * host; a structure leaves the batch when max_row |f_row| < fmax (cell rows included) or after `steps` steps.  On
+ * return cart_inout [sum natoms][3] and lattice9_inout [nstruct][9] hold the final geometries, and, each at that
+ * geometry (its last evaluation): energies [nstruct] (eV), forces [sum natoms][3] (eV/A), stress9 [nstruct][9] (GPa),
+ * steps_taken [nstruct], converged [nstruct] (1 / 0).  energy_trace [nstruct][steps + 1], if not NULL, gets the energy
+ * of every evaluation, NaN after the structure stopped.  Every output but energy_trace is required.
+ * Refused before anything runs, with B2M_ERR_INVALID: a single-process group or a rank of a multi-process job,
+ * nstruct < 1, a structure with no atoms, relax_cell with a non-periodic axis, steps < 0, non-finite FIRE constants,
+ * fmax or pressure, fmax < 0, dt, maxstep or dtmax <= 0, a NULL output other than energy_trace (whose [nstruct][steps + 1]
+ * buffer is only allocated when it is given); B2M_ERR_STATE while a heat-flux reach is set or before
+ * b2m_finalize_weights.  What b2m_set_structures
+ * refuses in the graph build (a singular lattice, a structure without edges, ...) fails the step it happens in, with
+ * the same code and a message naming the step and the structure by its input index, for example a structure whose
+ * atoms lose every edge; the handle stays usable.  Afterwards the batch of the
+ * last step is resident, as after b2m_compute_batch, and b2m_get_counts' launch count is that of the last step. */
+int b2m_relax_batch(b2m_handle h, int32_t nstruct, const int64_t* natoms, double* cart_inout, double* lattice9_inout,
+                    const int32_t* species, const int* pbc3, double tol, const b2m_relax_params* params,
+                    double* energies, float* forces, float* stress9, int32_t* steps_taken, int32_t* converged,
+                    double* energy_trace);
+
 /* Per-atom energies and virials (DESIGN.md "Per-atom energies and virials"), off by default.  With on != 0 the
  * following evaluations (b2m_compute, b2m_compute_resident) also produce, for every atom i,
  *   energies[i] = data_std * e_i + element_ref[Z_i] + data_mean / natoms   (eV; sums to the energy)
