@@ -63,6 +63,23 @@ class RelaxParams(C.Structure):
     ] + [(k, C.c_double) for k in FIRE_DEFAULTS]
 
 
+def _batch_arrays(natoms, cart, lattices, species, pbc, copy=False):
+    """natoms [S] i64, positions [sum, 3] f64, lattices [S, 9] f64, species [sum] i32 and pbc [S, 3] i32 of a batch, as
+    the library reads them; with `copy` the positions and lattices are new arrays the library may write into"""
+    natoms = np.ascontiguousarray(natoms, dtype=np.int64).reshape(-1)
+    S = len(natoms)
+    f64 = (lambda x: np.array(x, dtype=np.float64, order="C")) if copy else (
+        lambda x: np.ascontiguousarray(x, dtype=np.float64))
+    cart = f64(cart).reshape(-1, 3)
+    lattices = f64(lattices).reshape(S, 9)
+    species = np.ascontiguousarray(species, dtype=np.int32)
+    pbc = np.ascontiguousarray(pbc, dtype=np.int32).reshape(S, 3)
+    if S and (len(cart) != int(natoms.sum()) or len(species) != len(cart)):
+        raise ValueError(f"positions [{len(cart)}] and species [{len(species)}] must hold sum(natoms) = "
+                         f"{int(natoms.sum())} atoms")
+    return natoms, cart, lattices, species, pbc
+
+
 class B2MError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f"libb200mlip error {code}: {msg}")
@@ -238,14 +255,7 @@ class Engine:
     def set_structures(self, natoms, cart, lattices, species, pbc, tol=1e-8):
         """a batch of independent structures (b2m_set_structures): natoms [S] atoms per structure, positions [sum, 3]
         and species [sum] concatenated in structure order, lattices [S, 3, 3] (row vectors), pbc [S, 3]"""
-        natoms = np.ascontiguousarray(natoms, dtype=np.int64).reshape(-1)
-        cart = np.ascontiguousarray(cart, dtype=np.float64)
-        species = np.ascontiguousarray(species, dtype=np.int32)
-        lattices = np.ascontiguousarray(lattices, dtype=np.float64).reshape(len(natoms), 9)
-        pbc = np.ascontiguousarray(pbc, dtype=np.int32).reshape(len(natoms), 3)
-        if len(natoms) and (len(cart) != int(natoms.sum()) or len(species) != len(cart)):
-            raise ValueError(f"positions [{len(cart)}] and species [{len(species)}] must hold sum(natoms) = "
-                             f"{int(natoms.sum())} atoms")
+        natoms, cart, lattices, species, pbc = _batch_arrays(natoms, cart, lattices, species, pbc)
         self.natoms = len(cart)
         self.batch_natoms = natoms
         self._ck(self.lib.b2m_set_structures(
@@ -276,15 +286,9 @@ class Engine:
         unknown = set(fire) - set(FIRE_DEFAULTS)
         if unknown:
             raise TypeError(f"unknown FIRE parameters {sorted(unknown)}; FIRE takes {list(FIRE_DEFAULTS)}")
-        natoms = np.ascontiguousarray(natoms, dtype=np.int64).reshape(-1)
+        # copies: the library writes the final geometries into them
+        natoms, cart, lattices, species, pbc = _batch_arrays(natoms, cart, lattices, species, pbc, copy=True)
         S = len(natoms)
-        cart = np.array(cart, dtype=np.float64, order="C").reshape(-1, 3)  # copies: the library writes into them
-        lattices = np.array(lattices, dtype=np.float64, order="C").reshape(S, 9)
-        species = np.ascontiguousarray(species, dtype=np.int32)
-        pbc = np.ascontiguousarray(pbc, dtype=np.int32).reshape(S, 3)
-        if len(cart) != int(natoms.sum()) or len(species) != len(cart):
-            raise ValueError(f"positions [{len(cart)}] and species [{len(species)}] must hold sum(natoms) = "
-                             f"{int(natoms.sum())} atoms")
         prm = RelaxParams(fmax=float(fmax), steps=int(steps), relax_cell=int(bool(relax_cell)),
                           scalar_pressure=float(scalar_pressure), stress_weight=float(stress_weight),
                           **{k: float(fire.get(k, d)) for k, d in FIRE_DEFAULTS.items()})

@@ -233,7 +233,7 @@ namespace b2m {
 static int64_t cell_atoms(const b2m_engine* e) { return e->hf_n ? e->hf_n : e->g.N; }
 
 // a batch of structures is resident (b2m_set_structures, DESIGN.md §12)
-static bool batched(const b2m_engine* e) { return e->have_graph && e->g.S > 0; }
+static bool batched(const b2m_engine* e) { return e->have_graph && e->g.batch; }
 
 // optional outputs of an evaluation and the readout weights, null where they are off: per-atom energies and virials
 // (b2m_set_atomic; always on for a batch, whose per-structure sums are taken from them), and each atom's energy weight
@@ -812,7 +812,7 @@ static void fetch(b2m_engine* e, double* energy, float* forces, float* stress9) 
   e->last_energy = hs[0] + e->desc.data_mean;
   if (energy) *energy = e->last_energy;
   if (stress9)
-    for (int k = 0; k < 9; k++) stress9[k] = (float)(hs[1 + k] / e->g.volume * 160.21766208);  // pes.py:140-145
+    for (int k = 0; k < 9; k++) stress9[k] = (float)(hs[1 + k] / e->g.volume[0] * 160.21766208);  // pes.py:140-145
 }
 
 // per-atom energies [N] and virials [N][9] of the last evaluation; a group sums its partitions' arrays on the leader's
@@ -878,8 +878,23 @@ static void fetch_batch(b2m_engine* e, bool grads, double* energies, float* forc
   for (int s = 0; s < g.S; s++) {
     if (energies) energies[s] = hs[10 * s] + e->desc.data_mean;
     if (stress9)
-      for (int k = 0; k < 9; k++) stress9[9 * s + k] = (float)(hs[10 * s + 1 + k] / g.b_volume[s] * 160.21766208);
+      for (int k = 0; k < 9; k++) stress9[9 * s + k] = (float)(hs[10 * s + 1 + k] / g.volume[s] * 160.21766208);
   }
+}
+
+// The handle's graph state reset, then the graph of nstruct structures built (Graph::build; as_batch: a batch, DESIGN.md
+// §12) and its workspace allocated.  walls_from_min: the unfolded heat-flux cell (DESIGN.md §10)
+static void build_graph(b2m_engine* h, int nstruct, const int64_t* natoms, const double* cart, const double* lattice9,
+                        const int32_t* species, const int* pbc3, double tol, bool as_batch, bool walls_from_min = false) {
+  h->have_graph = false;
+  h->atomic_last = 0;  // per-atom results of an earlier structure are gone
+  h->hf_n = 0, h->hf_seed = -1;
+  h->g.balanced = h->partition_policy == B2M_PARTITION_BALANCED;
+  h->g.walls_from_min = walls_from_min;
+  h->g.build(h->st, nstruct, natoms, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff, tol,
+             h->rank, h->world, as_batch);
+  alloc_workspace(h);
+  h->have_graph = true;
 }
 
 // Batched relaxation (b2m_relax_batch, DESIGN.md §13).  Device state in input order; each step builds the graph of the
@@ -945,17 +960,9 @@ static void relax_loop(b2m_engine* h, int S, const int64_t* natoms, double* cart
     B2M_CK(cudaMemcpyAsync(d_sel.p, sel.data(), sel.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
     const int64_t* d_act = d_sel.p;
     launch_relax_emit(st, Sa, d_act, d_in_off.p, d_act + Sa, rs.p, r0.p, sp_in.p, ecart.p, sp_out.p);
-    h->have_graph = false;
-    h->atomic_last = 0;
-    h->hf_n = 0, h->hf_seed = -1;
-    h->g.balanced = h->partition_policy == B2M_PARTITION_BALANCED;
-    h->g.walls_from_min = false;
     h->g.b_name = act;  // errors name the structures by their input index
     try {
-      h->g.build_batch(st, Sa, counts.data(), ecart.p, lats.data(), sp_out.p, pbcs.data(), h->desc.cutoff,
-                       h->desc.three_body_cutoff, tol);
-      alloc_workspace(h);
-      h->have_graph = true;
+      build_graph(h, Sa, counts.data(), ecart.p, lats.data(), sp_out.p, pbcs.data(), tol, true);
       run(h, true);
     } catch (const Error& ex) {
       h->g.b_name.clear();
@@ -1329,35 +1336,24 @@ static void set_structure_one(b2m_engine* h, int64_t natoms, const double* cart,
     species = reinterpret_cast<const int32_t*>((const char*)h->pin_in + cb);
   }
   B2M_CK(cudaEventRecord(h->ev[3], h->st));
-  h->atomic_last = 0;  // per-atom results of an earlier structure are gone
-  h->hf_n = 0, h->hf_seed = -1;
-  h->g.balanced = h->partition_policy == B2M_PARTITION_BALANCED;
   if (nstruct > 0) {
-    h->g.walls_from_min = false;
-    h->g.build_batch(h->st, nstruct, counts, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff,
-                     tol);
+    build_graph(h, nstruct, counts, cart, lattice9, species, pbc3, tol, true);
   } else if (h->hf_reach > 0) {
     // heat flux: the unfolded cell, built on the device, is the graph's input; no periodicity
     h->uf.build(h->st, natoms, cart, species, lattice9, pbc3, h->hf_reach);
     const int no_pbc[3] = {0, 0, 0};
-    h->g.walls_from_min = true;
-    h->g.build(h->st, h->uf.N, h->uf.cart.p, lattice9, h->uf.species.p, no_pbc, h->desc.cutoff,
-               h->desc.three_body_cutoff, tol, h->rank, h->world);
+    build_graph(h, 1, &h->uf.N, h->uf.cart.p, lattice9, h->uf.species.p, no_pbc, tol, false, true);
     h->hf_n = natoms;
     h->buf.hf_w.ensure((size_t)h->uf.N + 64);
     for (int m = 0; m < 3; m++) h->hf_c[m] = 0.5 * (lattice9[m] + lattice9[3 + m] + lattice9[6 + m]);
   } else {
-    h->g.walls_from_min = false;
-    h->g.build(h->st, natoms, cart, lattice9, species, pbc3, h->desc.cutoff, h->desc.three_body_cutoff, tol, h->rank,
-               h->world);
+    build_graph(h, 1, &natoms, cart, lattice9, species, pbc3, tol, false);
   }
-  alloc_workspace(h);
   B2M_CK(cudaEventRecord(h->ev[4], h->st));
   B2M_CK(cudaStreamSynchronize(h->st));
   float ms;
   B2M_CK(cudaEventElapsedTime(&ms, h->ev[3], h->ev[4]));
   h->t_graph = ms;
-  h->have_graph = true;
 }
 
 int b2m_set_structure(b2m_handle h, int64_t natoms, const double* cart, const double* lattice9,
@@ -1373,19 +1369,26 @@ int b2m_set_structure(b2m_handle h, int64_t natoms, const double* cart, const do
   API_END
 }
 
-int b2m_set_structures(b2m_handle h, int32_t nstruct, const int64_t* natoms, const double* cart,
-                       const double* lattice9, const int32_t* species, const int* pbc3, double tol) {
-  API_BEGIN
+// what a batch needs of the handle and of its structures (b2m_set_structures, b2m_relax_batch); `args`: the structure
+// arguments are all present.  Returns the number of atoms of the batch
+static int64_t check_batch(b2m_engine* h, int32_t nstruct, const int64_t* natoms, bool args) {
   B2M_REQUIRE(h->parts.empty() && h->world == 1, B2M_ERR_INVALID,
               "a batch runs on one partition: not on a single-process group (ndev > 1) or a rank of a multi-process job");
   B2M_REQUIRE(h->hf_reach == 0, B2M_ERR_STATE, "a batch has no heat flux (b2m_set_heat_flux(h, 0) first)");
   B2M_REQUIRE(nstruct >= 1, B2M_ERR_INVALID, "a batch needs at least one structure");
-  B2M_REQUIRE(natoms && cart && lattice9 && species && pbc3, B2M_ERR_INVALID, "null structure argument");
+  B2M_REQUIRE(args, B2M_ERR_INVALID, "null structure argument");
   int64_t total = 0;
   for (int s = 0; s < nstruct; s++) {
     B2M_REQUIRE(natoms[s] > 0, B2M_ERR_INVALID, "structure " + std::to_string(s) + ": no atoms");
     total += natoms[s];
   }
+  return total;
+}
+
+int b2m_set_structures(b2m_handle h, int32_t nstruct, const int64_t* natoms, const double* cart,
+                       const double* lattice9, const int32_t* species, const int* pbc3, double tol) {
+  API_BEGIN
+  const int64_t total = check_batch(h, nstruct, natoms, natoms && cart && lattice9 && species && pbc3);
   set_structure_one(h, total, cart, lattice9, species, pbc3, tol, nstruct, natoms);
   API_END
 }
@@ -1404,13 +1407,8 @@ int b2m_relax_batch(b2m_handle h, int32_t nstruct, const int64_t* natoms, double
                     double* energies, float* forces, float* stress9, int32_t* steps_taken, int32_t* converged,
                     double* energy_trace) {
   API_BEGIN
-  B2M_REQUIRE(h->parts.empty() && h->world == 1, B2M_ERR_INVALID,
-              "a batch runs on one partition: not on a single-process group (ndev > 1) or a rank of a multi-process job");
-  B2M_REQUIRE(h->hf_reach == 0, B2M_ERR_STATE, "a batch has no heat flux (b2m_set_heat_flux(h, 0) first)");
+  check_batch(h, nstruct, natoms, natoms && cart_inout && lattice9_inout && species && pbc3 && params);
   B2M_REQUIRE(h->finalized, B2M_ERR_STATE, "weights not finalized");
-  B2M_REQUIRE(nstruct >= 1, B2M_ERR_INVALID, "a batch needs at least one structure");
-  B2M_REQUIRE(natoms && cart_inout && lattice9_inout && species && pbc3 && params, B2M_ERR_INVALID,
-              "null structure argument");
   B2M_REQUIRE(energies && forces && stress9 && steps_taken && converged, B2M_ERR_INVALID, "null result argument");
   const b2m_relax_params& p = *params;
   B2M_REQUIRE(p.steps >= 0, B2M_ERR_INVALID, "steps must be >= 0");
@@ -1419,13 +1417,10 @@ int b2m_relax_batch(b2m_handle h, int32_t nstruct, const int64_t* natoms, double
     B2M_REQUIRE(std::isfinite(x), B2M_ERR_INVALID, "relaxation parameters must be finite");
   B2M_REQUIRE(p.dt > 0 && p.maxstep > 0 && p.dtmax > 0, B2M_ERR_INVALID, "FIRE dt, maxstep and dtmax must be > 0");
   B2M_REQUIRE(p.fmax >= 0, B2M_ERR_INVALID, "fmax must be >= 0");
-  for (int s = 0; s < nstruct; s++) {
-    B2M_REQUIRE(natoms[s] > 0, B2M_ERR_INVALID, "structure " + std::to_string(s) + ": no atoms");
-    if (p.relax_cell)
-      for (int k = 0; k < 3; k++)
-        B2M_REQUIRE(pbc3[3 * s + k] == 1, B2M_ERR_INVALID,
-                    "structure " + std::to_string(s) + ": relax_cell needs a periodic cell on every axis");
-  }
+  for (int s = 0; s < nstruct && p.relax_cell; s++)
+    for (int k = 0; k < 3; k++)
+      B2M_REQUIRE(pbc3[3 * s + k] == 1, B2M_ERR_INVALID,
+                  "structure " + std::to_string(s) + ": relax_cell needs a periodic cell on every axis");
   relax_loop(h, nstruct, natoms, cart_inout, lattice9_inout, species, pbc3, tol, p,
              RelaxOut{energies, forces, stress9, steps_taken, converged, energy_trace});
   API_END

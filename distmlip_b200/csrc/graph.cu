@@ -64,32 +64,26 @@ __device__ __forceinline__ void wrap_atom(int64_t i, const double* __restrict__ 
   }
 }
 
-__global__ void k_wrap(int64_t n, const double* __restrict__ cart, GridParams gp,
-                       double* __restrict__ fracw, double* __restrict__ wc, int* __restrict__ corr) {
+template <class G>
+__global__ void k_wrap(int64_t n, const double* __restrict__ cart, G grid, double* __restrict__ fracw,
+                       double* __restrict__ wc, int* __restrict__ corr) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  wrap_atom(i, cart, gp, fracw, wc, corr);
+  wrap_atom(i, cart, grid.grid(grid.structure(i)), fracw, wc, corr);
 }
 
-// batch: atom i in the lattice of its structure sid[i]
-__global__ void k_wrap_batch(int64_t n, const double* __restrict__ cart, const GridParams* __restrict__ gps,
-                             const int* __restrict__ sid, double* __restrict__ fracw, double* __restrict__ wc,
-                             int* __restrict__ corr) {
-  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  wrap_atom(i, cart, gps[sid[i]], fracw, wc, corr);
-}
-
-// per-block min/max of wc[.,0..2] and fracw[.,0..2]; out[block][12]
-__global__ void k_minmax(int64_t n, const double* __restrict__ wc, const double* __restrict__ fracw,
-                         double* __restrict__ out) {
+// min/max of wc[.,0..2] and fracw[.,0..2] over the atoms off[s] .. off[s + 1] - 1 of structure s = blockIdx.x, split
+// over gridDim.y blocks; out[s][blockIdx.y][12]
+__global__ void k_minmax(const int64_t* __restrict__ off, const double* __restrict__ wc,
+                         const double* __restrict__ fracw, double* __restrict__ out) {
   __shared__ double smin[6][256], smax[6][256];
   double mn[6], mx[6];
   for (int k = 0; k < 6; k++) {
     mn[k] = 1e300;
     mx[k] = -1e300;
   }
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+  for (int64_t i = off[blockIdx.x] + blockIdx.y * (int64_t)blockDim.x + threadIdx.x; i < off[blockIdx.x + 1];
+       i += (int64_t)gridDim.y * blockDim.x) {
     for (int k = 0; k < 3; k++) {
       double a = wc[3 * i + k], b = fracw[3 * i + k];
       mn[k] = fmin(mn[k], a);
@@ -112,52 +106,14 @@ __global__ void k_minmax(int64_t n, const double* __restrict__ wc, const double*
     }
     __syncthreads();
   }
-  if (threadIdx.x == 0)
+  if (threadIdx.x == 0) {
+    double* o = out + ((int64_t)blockIdx.x * gridDim.y + blockIdx.y) * 12;
     for (int k = 0; k < 6; k++) {
-      out[blockIdx.x * 12 + k] = smin[k][0];
-      out[blockIdx.x * 12 + 6 + k] = smax[k][0];
+      o[k] = smin[k][0];
+      o[6 + k] = smax[k][0];
     }
+  }
 }
-
-// batch: k_minmax with block s over the atoms off[s] .. off[s + 1] - 1 of structure s; out[s][12]
-__global__ void k_minmax_batch(const int64_t* __restrict__ off, const double* __restrict__ wc,
-                               const double* __restrict__ fracw, double* __restrict__ out) {
-  __shared__ double smin[6][256], smax[6][256];
-  double mn[6], mx[6];
-  for (int k = 0; k < 6; k++) {
-    mn[k] = 1e300;
-    mx[k] = -1e300;
-  }
-  for (int64_t i = off[blockIdx.x] + threadIdx.x; i < off[blockIdx.x + 1]; i += blockDim.x) {
-    for (int k = 0; k < 3; k++) {
-      double a = wc[3 * i + k], b = fracw[3 * i + k];
-      mn[k] = fmin(mn[k], a);
-      mx[k] = fmax(mx[k], a);
-      mn[3 + k] = fmin(mn[3 + k], b);
-      mx[3 + k] = fmax(mx[3 + k], b);
-    }
-  }
-  for (int k = 0; k < 6; k++) {
-    smin[k][threadIdx.x] = mn[k];
-    smax[k][threadIdx.x] = mx[k];
-  }
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) {
-      for (int k = 0; k < 6; k++) {
-        smin[k][threadIdx.x] = fmin(smin[k][threadIdx.x], smin[k][threadIdx.x + s]);
-        smax[k][threadIdx.x] = fmax(smax[k][threadIdx.x], smax[k][threadIdx.x + s]);
-      }
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0)
-    for (int k = 0; k < 6; k++) {
-      out[blockIdx.x * 12 + k] = smin[k][0];
-      out[blockIdx.x * 12 + 6 + k] = smax[k][0];
-    }
-}
-
 
 struct Walls {
   double w[MAXP];
@@ -186,37 +142,27 @@ __device__ __forceinline__ int cell_coord(double f, int k, const GridParams& gp)
   return c;
 }
 
-__global__ void k_owner_cell(int64_t n, const double* __restrict__ fracw, Walls wl, GridParams gp,
-                             unsigned char* __restrict__ owner, int* __restrict__ cell_of,
-                             int* __restrict__ iota) {
+// owner = number of walls <= the coordinate along the axis (0 without walls or partitions); cell id = the structure's first cell + its
+// cell in the structure's grid
+template <class G>
+__global__ void k_owner_cell(int64_t n, const double* __restrict__ fracw, Walls wl, G grid,
+                             unsigned char* __restrict__ owner, int* __restrict__ cell_of, int* __restrict__ iota) {
   int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i >= n) return;
-  double f = fracw[3 * i + wl.axis];
   int o = 0;
-  for (int k = 0; k < wl.nw; k++)
-    if (!(f < wl.w[k])) o = k + 1;  // first wall strictly greater wins (:1312-1322)
+  if (G::kPartitioned) {
+    double f = fracw[3 * i + wl.axis];
+    for (int k = 0; k < wl.nw; k++)
+      if (!(f < wl.w[k])) o = k + 1;  // first wall strictly greater wins (:1312-1322)
+  }
   // walls ascending: o = number of walls <= f
   owner[i] = (unsigned char)o;
+  const int s = grid.structure(i);
+  const GridParams& gp = grid.grid(s);
   int cx = cell_coord(fracw[3 * i + 0], 0, gp);
   int cy = cell_coord(fracw[3 * i + 1], 1, gp);
   int cz = cell_coord(fracw[3 * i + 2], 2, gp);
-  cell_of[i] = (cx * gp.nc[1] + cy) * gp.nc[2] + cz;
-  iota[i] = (int)i;
-}
-
-// batch (one partition): owner 0, cell id = the structure's first cell + its cell in the structure's grid
-__global__ void k_owner_cell_batch(int64_t n, const double* __restrict__ fracw, const int* __restrict__ sid,
-                                   const GridParams* __restrict__ gps, const int* __restrict__ cell_off,
-                                   unsigned char* __restrict__ owner, int* __restrict__ cell_of, int* __restrict__ iota) {
-  int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int s = sid[i];
-  const GridParams& gp = gps[s];
-  owner[i] = 0;
-  int cx = cell_coord(fracw[3 * i + 0], 0, gp);
-  int cy = cell_coord(fracw[3 * i + 1], 1, gp);
-  int cz = cell_coord(fracw[3 * i + 2], 2, gp);
-  cell_of[i] = cell_off[s] + (cx * gp.nc[1] + cy) * gp.nc[2] + cz;
+  cell_of[i] = grid.first_cell(s) + (cx * gp.nc[1] + cy) * gp.nc[2] + cz;
   iota[i] = (int)i;
 }
 
@@ -377,63 +323,48 @@ __device__ __forceinline__ void traverse(int ci, const GridParams& gp, const int
   }
 }
 
-// count edges / bonds of the centre t at sorted index ci
-__device__ __forceinline__ void count_row(int t, int ci, const GridParams& gp, const int* __restrict__ s_gid,
-                                          const double* __restrict__ s_wc, const int* __restrict__ cell_start,
-                                          const double* __restrict__ fracw, const unsigned char* __restrict__ owner,
-                                          int rank, double r2, double rb2, double tol, int* __restrict__ cnt_e,
-                                          int* __restrict__ cnt_b, unsigned* __restrict__ to_mask) {
+// count edges / bonds per centre; centres given by sorted index list.  The traversal's cell ids are those of the centre's
+// structure, so cell_start is offset by its first cell
+template <class G>
+__global__ void k_count(int ncent, const int* __restrict__ cent_sidx, G grid, const int* __restrict__ s_gid,
+                        const double* __restrict__ s_wc, const int* __restrict__ cell_start,
+                        const double* __restrict__ fracw, const unsigned char* __restrict__ owner, int rank, double r2,
+                        double rb2, double tol, int* __restrict__ cnt_e, int* __restrict__ cnt_b,
+                        unsigned* __restrict__ to_mask) {
+  int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= ncent) return;
+  const int ci = cent_sidx[t], s = grid.structure(s_gid[ci]);
   int ne = 0, nb = 0;
   unsigned mask = 0;
-  traverse(ci, gp, s_gid, s_wc, cell_start, fracw, r2, tol,
+  traverse(ci, grid.grid(s), s_gid, s_wc, cell_start + grid.first_cell(s), fracw, r2, tol,
            [&](int, int gj, double, double, double, double d2, int, int, int) {
              ne++;
              if (d2 < rb2 + tol) nb++;
-             int o = owner[gj];
-             if (o != rank) mask |= 1u << o;
+             if (G::kPartitioned) {
+               int o = owner[gj];
+               if (o != rank) mask |= 1u << o;
+             }
            });
   if (cnt_e) cnt_e[t] = ne;
   cnt_b[t] = nb;
-  if (to_mask) to_mask[t] = mask;
+  if (G::kPartitioned && to_mask) to_mask[t] = mask;
 }
 
-// count edges / bonds per centre; centres given by sorted index list
-__global__ void k_count(int ncent, const int* __restrict__ cent_sidx, GridParams gp,
-                        const int* __restrict__ s_gid, const double* __restrict__ s_wc,
-                        const int* __restrict__ cell_start, const double* __restrict__ fracw,
-                        const unsigned char* __restrict__ owner, int rank, double r2, double rb2, double tol,
-                        int* __restrict__ cnt_e, int* __restrict__ cnt_b, unsigned* __restrict__ to_mask) {
+// fill owned rows
+template <class G>
+__global__ void k_fill_owned(int n_own, const int* __restrict__ cent_sidx, G grid, const int* __restrict__ s_gid,
+                             const double* __restrict__ s_wc, const int* __restrict__ cell_start,
+                             const double* __restrict__ fracw, const unsigned char* __restrict__ owner, int rank,
+                             double r2, double rb2, double tol, const int* __restrict__ row_ptr,
+                             const int* __restrict__ brow_ptr, int* __restrict__ e_src_gid, int* __restrict__ e_dst,
+                             int* __restrict__ e_img, int* __restrict__ e_bond, float4* __restrict__ e_vec,
+                             int* __restrict__ b_src_gid, int* __restrict__ b_dst, int* __restrict__ b_img,
+                             int* __restrict__ b_edge, float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
   int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= ncent) return;
-  count_row(t, cent_sidx[t], gp, s_gid, s_wc, cell_start, fracw, owner, rank, r2, rb2, tol, cnt_e, cnt_b, to_mask);
-}
-
-// batch: the centre's structure s = sid[gid] gives the grid and the first cell (cell ids of the traversal are local)
-__global__ void k_count_batch(int ncent, const int* __restrict__ cent_sidx, const GridParams* __restrict__ gps,
-                              const int* __restrict__ cell_off, const int* __restrict__ sid,
-                              const int* __restrict__ s_gid, const double* __restrict__ s_wc,
-                              const int* __restrict__ cell_start, const double* __restrict__ fracw,
-                              const unsigned char* __restrict__ owner, double r2, double rb2, double tol,
-                              int* __restrict__ cnt_e, int* __restrict__ cnt_b) {
-  int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= ncent) return;
-  const int ci = cent_sidx[t], s = sid[s_gid[ci]];
-  count_row(t, ci, gps[s], s_gid, s_wc, cell_start + cell_off[s], fracw, owner, 0, r2, rb2, tol, cnt_e, cnt_b,
-            (unsigned*)nullptr);
-}
-
-// fill the owned row t (centre at sorted index ci)
-__device__ __forceinline__ void fill_row(int t, int ci, const GridParams& gp, const int* __restrict__ s_gid,
-                                         const double* __restrict__ s_wc, const int* __restrict__ cell_start,
-                                         const double* __restrict__ fracw, const unsigned char* __restrict__ owner,
-                                         int rank, double r2, double rb2, double tol, const int* __restrict__ row_ptr,
-                                         const int* __restrict__ brow_ptr, int* __restrict__ e_src_gid,
-                                         int* __restrict__ e_dst, int* __restrict__ e_img, int* __restrict__ e_bond,
-                                         float4* __restrict__ e_vec, int* __restrict__ b_src_gid,
-                                         int* __restrict__ b_dst, int* __restrict__ b_img, int* __restrict__ b_edge,
-                                         float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
+  if (t >= n_own) return;
+  const int ci = cent_sidx[t], s = grid.structure(s_gid[ci]);
   int e = row_ptr[t], b = brow_ptr[t];
-  traverse(ci, gp, s_gid, s_wc, cell_start, fracw, r2, tol,
+  traverse(ci, grid.grid(s), s_gid, s_wc, cell_start + grid.first_cell(s), fracw, r2, tol,
            [&](int, int gj, double dx, double dy, double dz, double d2, int ix, int iy, int iz) {
              // (dx,dy,dz) = x_src_image - x_dst ; reference bond_vec = x_dst + off.L - x_src = -(dx,dy,dz)
              float4 v = make_float4((float)(-dx), (float)(-dy), (float)(-dz), (float)sqrt(d2));
@@ -456,40 +387,6 @@ __device__ __forceinline__ void fill_row(int t, int ci, const GridParams& gp, co
              }
              e++;
            });
-}
-
-// fill owned rows
-__global__ void k_fill_owned(int n_own, const int* __restrict__ cent_sidx, GridParams gp,
-                             const int* __restrict__ s_gid, const double* __restrict__ s_wc,
-                             const int* __restrict__ cell_start, const double* __restrict__ fracw,
-                             const unsigned char* __restrict__ owner, int rank, double r2, double rb2, double tol,
-                             const int* __restrict__ row_ptr, const int* __restrict__ brow_ptr,
-                             int* __restrict__ e_src_gid, int* __restrict__ e_dst, int* __restrict__ e_img,
-                             int* __restrict__ e_bond, float4* __restrict__ e_vec, int* __restrict__ b_src_gid,
-                             int* __restrict__ b_dst, int* __restrict__ b_img, int* __restrict__ b_edge,
-                             float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
-  int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n_own) return;
-  fill_row(t, cent_sidx[t], gp, s_gid, s_wc, cell_start, fracw, owner, rank, r2, rb2, tol, row_ptr, brow_ptr, e_src_gid,
-           e_dst, e_img, e_bond, e_vec, b_src_gid, b_dst, b_img, b_edge, b_vec, halo_flag);
-}
-
-// batch: as k_count_batch
-__global__ void k_fill_owned_batch(int n_own, const int* __restrict__ cent_sidx, const GridParams* __restrict__ gps,
-                                   const int* __restrict__ cell_off, const int* __restrict__ sid,
-                                   const int* __restrict__ s_gid, const double* __restrict__ s_wc,
-                                   const int* __restrict__ cell_start, const double* __restrict__ fracw,
-                                   const unsigned char* __restrict__ owner, double r2, double rb2, double tol,
-                                   const int* __restrict__ row_ptr, const int* __restrict__ brow_ptr,
-                                   int* __restrict__ e_src_gid, int* __restrict__ e_dst, int* __restrict__ e_img,
-                                   int* __restrict__ e_bond, float4* __restrict__ e_vec, int* __restrict__ b_src_gid,
-                                   int* __restrict__ b_dst, int* __restrict__ b_img, int* __restrict__ b_edge,
-                                   float4* __restrict__ b_vec, unsigned char* __restrict__ halo_flag) {
-  int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n_own) return;
-  const int ci = cent_sidx[t], s = sid[s_gid[ci]];
-  fill_row(t, ci, gps[s], s_gid, s_wc, cell_start + cell_off[s], fracw, owner, 0, r2, rb2, tol, row_ptr, brow_ptr,
-           e_src_gid, e_dst, e_img, e_bond, e_vec, b_src_gid, b_dst, b_img, b_edge, b_vec, halo_flag);
 }
 
 // batch: out[s] = ptr[off[s]] (edges before the first row of each structure)
@@ -753,8 +650,8 @@ static int read_int(const int* dptr, cudaStream_t st) {
 }
 
 // Cell grid of one structure (cell edge >= r_cut where the cell allows it, at most 2^27 cells) from its inverse lattice,
-// periodicity and, for the non-periodic axes, the fractional bounds fmn / fmx [3] of its wrapped atoms.  build() and
-// build_batch() both call it, so a structure gets the same grid alone and in a batch.
+// periodicity and, for the non-periodic axes, the fractional bounds fmn / fmx [3] of its wrapped atoms.  A structure gets
+// the same grid alone and in a batch.
 static void cell_grid(const double* inv, const int* pbc, const double* fmn, const double* fmx, double rcut,
                       GridParams& gp) {
   // perpendicular height along lattice vector k = 1 / |column k of inv|
@@ -790,6 +687,25 @@ static void cell_grid(const double* inv, const int* pbc, const double* fmn, cons
     gp.nc[kmax] = (gp.nc[kmax] + 1) / 2;
     gp.reach[kmax] = 2 * gp.reach[kmax];  // conservative
   }
+}
+
+// Bounds of each structure s of the device offsets doff [S + 1]: lo / hi [S][6], the min / max of wc (k = 0..2) and of
+// fracw (k = 3..5), from k_minmax over nb blocks per structure
+static void bounds(cudaStream_t st, int S, int nb, const int64_t* doff, const double* wc, const double* fracw,
+                   DBuf<double>& tmp, std::vector<double>& lo, std::vector<double>& hi) {
+  tmp.ensure((size_t)S * nb * 12);
+  launch(k_minmax, dim3(S, nb), 256, 0, st, doff, wc, fracw, tmp.p);
+  std::vector<double> h((size_t)S * nb * 12);
+  B2M_CK(cudaMemcpyAsync(h.data(), tmp.p, h.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2M_CK(cudaStreamSynchronize(st));
+  lo.assign(6 * (size_t)S, 1e300);
+  hi.assign(6 * (size_t)S, -1e300);
+  for (size_t s = 0; s < (size_t)S; s++)
+    for (size_t b = 0; b < (size_t)nb; b++)
+      for (int k = 0; k < 6; k++) {
+        lo[6 * s + k] = std::min(lo[6 * s + k], h[(s * nb + b) * 12 + k]);
+        hi[6 * s + k] = std::max(hi[6 * s + k], h[(s * nb + b) * 12 + 6 + k]);
+      }
 }
 
 // per-atom arrays for N atoms, positions and species uploaded (host staging, or the device arrays of an Unfold)
@@ -831,76 +747,96 @@ void Graph::sort_by_cell(cudaStream_t st, int ncell) {
   excl_scan(cub_tmp, tmp_i2.p, cell_start.p, ncell + 1, st);
 }
 
-void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
-                  const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,
-                  int rank_, int world_) {
-  B2M_REQUIRE(natoms > 0 && natoms < (1LL << 31) / 4, B2M_ERR_INVALID, "natoms out of range");
+// Every build (DESIGN.md §12): each structure wrapped in its own lattice and given its own cell grid by cell_grid(); cell
+// ids are the structure's first cell + its local cell, so the radix sort groups the atoms by structure, then by cell,
+// and inside a structure reproduces the order of its build alone.  Launches and host synchronisations do not depend on
+// the number of structures.
+void Graph::build(cudaStream_t st, int nstruct, const int64_t* natoms, const double* h_cart, const double* h_lat,
+                  const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_, int rank_,
+                  int world_, bool as_batch) {
+  B2M_REQUIRE(nstruct >= 1 && (as_batch || nstruct == 1), B2M_ERR_INVALID, "a batch needs at least one structure");
   B2M_REQUIRE(world_ >= 1 && world_ <= MAXP, B2M_ERR_PARTITIONS, "num_partitions must be in [1,16]");
+  B2M_REQUIRE(!as_batch || world_ == 1, B2M_ERR_PARTITIONS, "a batch runs on one partition");
   B2M_REQUIRE(rbond <= rcut, B2M_ERR_INVALID, "bond_r cannot be greater than regular cutoff");
-  S = 0;
-  b_off.clear();
-  b_volume.clear();
-  N = natoms;
+  auto named = [&](int s, const std::string& what) { return as_batch ? structure_name(s) + ": " + what : what; };
+  std::vector<int64_t> off(nstruct + 1, 0);
+  std::vector<GridParams> gps(nstruct);
+  std::vector<double> vol(nstruct);
+  for (int s = 0; s < nstruct; s++) {
+    B2M_REQUIRE(natoms[s] > 0, B2M_ERR_INVALID, as_batch ? named(s, "no atoms") : "natoms out of range");
+    off[s + 1] = off[s] + natoms[s];
+    B2M_REQUIRE(off[s + 1] < (1LL << 31) / 4, B2M_ERR_INVALID,
+                as_batch ? "batch has too many atoms" : "natoms out of range");
+    GridParams& gp = gps[s];
+    for (int k = 0; k < 3; k++) {
+      const int f = h_pbc[3 * s + k];
+      B2M_REQUIRE(!as_batch || f == 0 || f == 1, B2M_ERR_INVALID, named(s, "pbc flags must be 0 or 1"));
+      gp.pbc[k] = f ? 1 : 0, gp.nc[k] = 1, gp.reach[k] = 1, gp.fmin[k] = 0, gp.fscale[k] = 0;
+    }
+    memcpy(gp.lat, h_lat + 9 * s, sizeof gp.lat);
+    double det;
+    inv3(gp.lat, gp.inv, det);
+    B2M_REQUIRE(fabs(det) > 1e-12, B2M_ERR_INVALID, named(s, "singular lattice"));
+    vol[s] = fabs(det);
+  }
+  S = nstruct;
+  batch = as_batch;
+  N = off[S];
   rank = rank_;
   world = world_;
   r_cut = rcut;
   r_bond = rbond;
   tol = tol_;
-  for (int i = 0; i < 9; i++) lat[i] = h_lat[i];
-  for (int i = 0; i < 3; i++) pbc[i] = h_pbc[i] ? 1 : 0;
-  double det;
-  inv3(lat, inv, det);
-  B2M_REQUIRE(fabs(det) > 1e-12, B2M_ERR_INVALID, "singular lattice");
-  volume = fabs(det);
+  b_off = off;
+  volume = vol;
+  grids = gps;
 
-  GridParams gp;
-  memcpy(gp.lat, lat, sizeof lat);
-  memcpy(gp.inv, inv, sizeof inv);
-  for (int k = 0; k < 3; k++) gp.pbc[k] = pbc[k];
-
-  // ---- upload + wrap ----
+  // ---- upload + wrap: the lattices of the grids now, the cell grids after the bounds ----
+  b_doff.ensure(S + 1);
+  B2M_CK(cudaMemcpyAsync(b_doff.p, off.data(), (S + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
   upload(st, h_cart, h_species);
-  for (int k = 0; k < 3; k++) {
-    gp.nc[k] = 1;
-    gp.reach[k] = 1;
-    gp.fmin[k] = 0;
-    gp.fscale[k] = 0;
+  if (batch) {
+    std::vector<int> sid(N);
+    for (int s = 0; s < S; s++) std::fill(sid.begin() + off[s], sid.begin() + off[s + 1], s);
+    b_gp.ensure(S);
+    b_cell_off.ensure(S);
+    b_sid.ensure(N);
+    B2M_CK(cudaMemcpyAsync(b_sid.p, sid.data(), N * sizeof(int), cudaMemcpyHostToDevice, st));
+    B2M_CK(cudaMemcpyAsync(b_gp.p, grids.data(), S * sizeof(GridParams), cudaMemcpyHostToDevice, st));
   }
-  launch(k_wrap, cdiv(N, 256), 256, 0, st, N, cart.p, gp, fracw.p, wc.p, corr.p);
+  with_grid([&](auto grid) {
+    launch(k_wrap<decltype(grid)>, cdiv(N, 256), 256, 0, st, N, cart.p, grid, fracw.p, wc.p, corr.p);
+  });
 
-  // ---- min/max (partition axis, walls, non-periodic cell grid) ----
-  const int RB = 256;
-  red_tmp.ensure(RB * 12);
-  launch(k_minmax, RB, 256, 0, st, N, wc.p, fracw.p, red_tmp.p);
-  std::vector<double> hred(RB * 12);
-  B2M_CK(cudaMemcpyAsync(hred.data(), red_tmp.p, RB * 12 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  B2M_CK(cudaStreamSynchronize(st));
-  double mn[6], mx[6];
-  for (int k = 0; k < 6; k++) {
-    mn[k] = 1e300;
-    mx[k] = -1e300;
-  }
-  for (int b = 0; b < RB; b++)
-    for (int k = 0; k < 6; k++) {
-      mn[k] = std::min(mn[k], hred[b * 12 + k]);
-      mx[k] = std::max(mx[k], hred[b * 12 + 6 + k]);
+  // ---- bounds of every structure (partition axis, walls, non-periodic cell grid): 256 blocks for one structure, one
+  // block each in a batch ----
+  std::vector<double> mn, mx;
+  bounds(st, S, batch ? 1 : 256, b_doff.p, wc.p, fracw.p, red_tmp, mn, mx);
+
+  // ---- cell grids and the first cell of every structure; they do not depend on the walls ----
+  std::vector<int> coff(S);
+  int64_t ncell = 0;
+  for (int s = 0; s < S; s++) {
+    try {
+      cell_grid(grids[s].inv, grids[s].pbc, &mn[6 * s + 3], &mx[6 * s + 3], rcut, grids[s]);
+    } catch (const Error& ex) {
+      throw Error(ex.code, named(s, ex.what()));
     }
-
-  // ---- global cell grid; it does not depend on the walls ----
-  cell_grid(inv, pbc, mn + 3, mx + 3, rcut, gp);
-  for (int k = 0; k < 3; k++) {
-    nc[k] = gp.nc[k];
-    reach[k] = gp.reach[k];
-    fmin[k] = gp.fmin[k];
-    fscale[k] = gp.fscale[k];
+    coff[s] = (int)ncell;
+    ncell += (int64_t)grids[s].nc[0] * grids[s].nc[1] * grids[s].nc[2];
+    B2M_REQUIRE(ncell <= (1LL << 27), B2M_ERR_INVALID, "batch needs more than 2^27 cells; split it");
   }
-  const int ncell = gp.nc[0] * gp.nc[1] * gp.nc[2];
+  if (batch) {
+    B2M_CK(cudaMemcpyAsync(b_gp.p, grids.data(), S * sizeof(GridParams), cudaMemcpyHostToDevice, st));
+    B2M_CK(cudaMemcpyAsync(b_cell_off.p, coff.data(), S * sizeof(int), cudaMemcpyHostToDevice, st));
+  }
   const double r2 = rcut * rcut, rb2 = rbond * rbond;
 
   Walls wl;
   wl.nw = world - 1;
   wl.axis = 0;
-  if (world > 1) {
+  if (world > 1) {  // one structure
+    const GridParams& gp = grids[0];
     // create_partition (:1370-1456)
     double diffs[3] = {mx[0] - mn[0], mx[1] - mn[1], mx[2] - mn[2]};
     int longest = 0;
@@ -916,13 +852,14 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       // on the walls, so the cell list is built first), then walls at the work quantiles
       Walls none = wl;
       none.nw = 0;
-      launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, none, gp, owner.p, cell_of.p, tmp_i0.p);
-      sort_by_cell(st, ncell);
+      launch(k_owner_cell<OneGrid>, cdiv(N, 256), 256, 0, st, N, fracw.p, none, OneGrid{gp}, owner.p, cell_of.p,
+             tmp_i0.p);
+      sort_by_cell(st, (int)ncell);
       tmp_i3.ensure(N + 1);
       launch(k_post_sort, cdiv(N, 256), 256, 0, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i3.p);
       // tmp_i0 still holds the iota: every sorted index is a centre
-      launch(k_count, cdiv(N, 256), 256, 0, st, (int)N, tmp_i0.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p, owner.p,
-             rank, r2, rb2, tol, tmp_i1.p, tmp_i2.p, (unsigned*)nullptr);
+      launch(k_count<OneGrid>, cdiv(N, 256), 256, 0, st, (int)N, tmp_i0.p, OneGrid{gp}, s_gid.p, s_wc.p, cell_start.p,
+             fracw.p, owner.p, rank, r2, rb2, tol, tmp_i1.p, tmp_i2.p, (unsigned*)nullptr);
       bal_x.ensure(2 * N);
       bal_w.ensure(2 * N);
       double *x_in = bal_x.p, *x_s = bal_x.p + N;
@@ -944,10 +881,10 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
       // minimum slab width delta = need / h, h the cell's height across the partition axis (stricter than the lattice
       // column for a tilted cell); forward then backward pass against the end bounds
       const double need = 2 * (rcut + rbond);
-      const double h = 1.0 / sqrt(inv[longest] * inv[longest] + inv[3 + longest] * inv[3 + longest] +
-                                  inv[6 + longest] * inv[6 + longest]);
+      const double h = 1.0 / sqrt(gp.inv[longest] * gp.inv[longest] + gp.inv[3 + longest] * gp.inv[3 + longest] +
+                                  gp.inv[6 + longest] * gp.inv[6 + longest]);
       const double delta = need / h;
-      const bool from_min = walls_from_min || !pbc[longest];
+      const bool from_min = walls_from_min || !gp.pbc[longest];
       const double lo = from_min ? fmn : 0.0, hi = from_min ? fmx : 1.0;
       for (int k = 0; k < wl.nw; k++) wl.w[k] = std::max(wl.w[k], (k ? wl.w[k - 1] : lo) + delta);
       for (int k = wl.nw - 1; k >= 0; k--) wl.w[k] = std::min(wl.w[k], (k + 1 < wl.nw ? wl.w[k + 1] : hi) - delta);
@@ -980,7 +917,7 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
     }
     if (!balanced) {
       // check_partition_size (:1512-1529): lattice *column* of the axis, width = walls[0] * |col|
-      double col[3] = {lat[longest], lat[longest + 3], lat[longest + 6]};
+      double col[3] = {gp.lat[longest], gp.lat[longest + 3], gp.lat[longest + 6]};
       double width = (wl.w[0] - (walls_from_min ? fmn : 0.0)) * sqrt(col[0] * col[0] + col[1] * col[1] + col[2] * col[2]);
       double need = 2 * (rcut + rbond);
       if (width <= need) {
@@ -997,14 +934,15 @@ void Graph::build(cudaStream_t st, int64_t natoms, const double* h_cart, const d
   for (int k = 0; k < MAXP; k++) walls[k] = k < wl.nw ? wl.w[k] : 0.0;
 
   // ---- owner + cell id, sort by cell (a balanced partition sorted the atoms by cell before placing its walls) ----
-  launch(k_owner_cell, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, gp, owner.p, cell_of.p, tmp_i0.p);
-  if (!(balanced && world > 1)) sort_by_cell(st, ncell);
-  build_rows(st, gp);
+  with_grid([&](auto grid) {
+    launch(k_owner_cell<decltype(grid)>, cdiv(N, 256), 256, 0, st, N, fracw.p, wl, grid, owner.p, cell_of.p, tmp_i0.p);
+  });
+  if (!(balanced && world > 1)) sort_by_cell(st, (int)ncell);
+  build_rows(st);
 }
 
-// Local atoms, edges, halo sections, bonds and angles of the atoms sorted by cell (every build ends here).  A batch
-// (S > 0) has one partition and takes each centre's grid from b_gp.
-void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
+// Local atoms, edges, halo sections, bonds and angles of the atoms sorted by cell (every build ends here)
+void Graph::build_rows(cudaStream_t st) {
   const double r2 = r_cut * r_cut, rb2 = r_bond * r_bond;
   // own flags, scan -> local ids
   launch(k_post_sort, cdiv(N, 256), 256, 0, st, N, s_gid.p, wc.p, owner.p, rank, s_wc.p, sidx_of_gid.p, tmp_i0.p);
@@ -1026,12 +964,10 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
   row_ptr.ensure(n_own + 2);
   DBuf<int>& cnt_e = tmp_i0;
   DBuf<int>& cnt_b = tmp_i1;
-  if (S)
-    launch(k_count_batch, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, b_gp.p, b_cell_off.p, b_sid.p, s_gid.p,
-           s_wc.p, cell_start.p, fracw.p, owner.p, r2, rb2, tol, cnt_e.p, cnt_b.p);
-  else
-    launch(k_count, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p,
-           owner.p, rank, r2, rb2, tol, cnt_e.p, cnt_b.p, to_mask.p);
+  with_grid([&](auto grid) {
+    launch(k_count<decltype(grid)>, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, grid, s_gid.p, s_wc.p,
+           cell_start.p, fracw.p, owner.p, rank, r2, rb2, tol, cnt_e.p, cnt_b.p, to_mask.p);
+  });
   B2M_CK(cudaMemsetAsync(cnt_e.p + n_own, 0, sizeof(int), st));
   B2M_CK(cudaMemsetAsync(cnt_b.p + n_own, 0, sizeof(int), st));
   excl_scan(cub_tmp, cnt_e.p, row_ptr.p, n_own + 1, st);
@@ -1040,7 +976,7 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
   excl_scan(cub_tmp, cnt_b.p, brow_ptr.p, n_own + 1, st);
   // batch: the rows of structure s are b_off[s] .. b_off[s + 1] - 1 (every atom owned, cell ids grouped by structure)
   std::vector<int> e_at(S + 1);
-  if (S) {
+  if (batch) {
     sel_out.ensure(S + 1);
     launch(k_gather_at, cdiv(S + 1, 256), 256, 0, st, S + 1, b_doff.p, row_ptr.p, sel_out.p);
     B2M_CK(cudaMemcpyAsync(e_at.data(), sel_out.p, (S + 1) * sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1048,7 +984,7 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
   E = read_int(row_ptr.p + n_own, st);
   B_own = read_int(brow_ptr.p + n_own, st);
   B2M_REQUIRE(E > 0, B2M_ERR_INVALID, "No neighbors were found!");
-  for (int s = 0; s < S; s++)
+  for (int s = 0; batch && s < S; s++)
     B2M_REQUIRE(e_at[s + 1] > e_at[s], B2M_ERR_INVALID,
                 structure_name(s) + " has no edges (No neighbors were found!)");
 
@@ -1068,14 +1004,11 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
   b_edge.ensure(B_own + 1);
   unsigned char* halo_flag = tmp_flag.p;
   B2M_CK(cudaMemsetAsync(halo_flag, 0, N, st));
-  if (S)
-    launch(k_fill_owned_batch, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, b_gp.p, b_cell_off.p, b_sid.p, s_gid.p,
-           s_wc.p, cell_start.p, fracw.p, owner.p, r2, rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p,
+  with_grid([&](auto grid) {
+    launch(k_fill_owned<decltype(grid)>, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, grid, s_gid.p, s_wc.p,
+           cell_start.p, fracw.p, owner.p, rank, r2, rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p,
            e_bond.p, e_vec.p, b_src_gid.p, b_dst.p, b_img.p, b_edge.p, b_vec.p, halo_flag);
-  else
-    launch(k_fill_owned, cdiv(n_own, 256), 256, 0, st, n_own, loc_sidx.p, gp, s_gid.p, s_wc.p, cell_start.p, fracw.p,
-           owner.p, rank, r2, rb2, tol, row_ptr.p, brow_ptr.p, e_src_gid.p, e_dst.p, e_img.p, e_bond.p, e_vec.p,
-           b_src_gid.p, b_dst.p, b_img.p, b_edge.p, b_vec.p, halo_flag);
+  });
 
   // ---- halo atoms: grouped by owner, gid ascending ----
   n_halo = 0;
@@ -1114,8 +1047,8 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
   B_halo = 0;
   if (n_halo > 0) {
     DBuf<int>& hb_cnt = tmp_i0;
-    launch(k_count, cdiv(n_halo, 256), 256, 0, st, n_halo, loc_sidx.p + n_own, gp, s_gid.p, s_wc.p, cell_start.p,
-           fracw.p, owner.p, rank, rb2, rb2, tol, (int*)nullptr, hb_cnt.p, (unsigned*)nullptr);
+    launch(k_count<OneGrid>, cdiv(n_halo, 256), 256, 0, st, n_halo, loc_sidx.p + n_own, OneGrid{grids[0]}, s_gid.p,
+           s_wc.p, cell_start.p, fracw.p, owner.p, rank, rb2, rb2, tol, (int*)nullptr, hb_cnt.p, (unsigned*)nullptr);
     B2M_CK(cudaMemsetAsync(hb_cnt.p + n_halo, 0, sizeof(int), st));
     excl_scan(cub_tmp, hb_cnt.p, tmp_i1.p, n_halo + 1, st);
     B_halo = read_int(tmp_i1.p + n_halo, st);
@@ -1145,8 +1078,8 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
     std::swap(nv.cap, b_vec.cap);
   }
   if (n_halo > 0)
-    launch(k_fill_halo_bonds, cdiv(n_halo, 256), 256, 0, st, n_halo, n_own, loc_sidx.p + n_own, gp, s_gid.p, s_wc.p,
-           cell_start.p, fracw.p, rb2, tol, brow_ptr.p, b_src_gid.p, b_dst.p, b_img.p, b_vec.p);
+    launch(k_fill_halo_bonds, cdiv(n_halo, 256), 256, 0, st, n_halo, n_own, loc_sidx.p + n_own, grids[0], s_gid.p,
+           s_wc.p, cell_start.p, fracw.p, rb2, tol, brow_ptr.p, b_src_gid.p, b_dst.p, b_img.p, b_vec.p);
   launch(k_relabel, cdiv(B_loc, 256), 256, 0, st, (int64_t)B_loc, b_src_gid.p, g2l.p, b_src.p);
   for (int q = 0; q <= MAXP; q++) bfrom_off[q] = 0;
   if (n_halo > 0) {
@@ -1232,88 +1165,6 @@ void Graph::build_rows(cudaStream_t st, const GridParams& gp) {
            gid.p, tmp_i3.p, a_in.p, a_out.p, a_ctr.p);
   }
   B2M_CK(cudaStreamSynchronize(st));
-}
-
-// Batch (DESIGN.md §12): the disjoint union of the structures, each wrapped in its own lattice and given its own cell grid
-// by cell_grid(); cell ids are the structure's first cell + its local cell, so the radix sort groups the atoms by
-// structure, then by cell, and inside a structure reproduces the order of its single build.  Launches and host
-// synchronisations do not depend on the number of structures.
-void Graph::build_batch(cudaStream_t st, int nstruct, const int64_t* natoms, const double* h_cart, const double* h_lat,
-                        const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_) {
-  B2M_REQUIRE(nstruct >= 1, B2M_ERR_INVALID, "a batch needs at least one structure");
-  B2M_REQUIRE(rbond <= rcut, B2M_ERR_INVALID, "bond_r cannot be greater than regular cutoff");
-  auto named = [this](int s, const std::string& what) { return structure_name(s) + ": " + what; };
-  std::vector<int64_t> off(nstruct + 1, 0);
-  std::vector<GridParams> gps(nstruct);
-  std::vector<double> vol(nstruct);
-  for (int s = 0; s < nstruct; s++) {
-    B2M_REQUIRE(natoms[s] > 0, B2M_ERR_INVALID, named(s, "no atoms"));
-    off[s + 1] = off[s] + natoms[s];
-    B2M_REQUIRE(off[s + 1] < (1LL << 31) / 4, B2M_ERR_INVALID, "batch has too many atoms");
-    GridParams& gp = gps[s];
-    for (int k = 0; k < 3; k++) {
-      const int f = h_pbc[3 * s + k];
-      B2M_REQUIRE(f == 0 || f == 1, B2M_ERR_INVALID, named(s, "pbc flags must be 0 or 1"));
-      gp.pbc[k] = f, gp.nc[k] = 1, gp.reach[k] = 1, gp.fmin[k] = 0, gp.fscale[k] = 0;
-    }
-    memcpy(gp.lat, h_lat + 9 * s, sizeof gp.lat);
-    double det;
-    inv3(gp.lat, gp.inv, det);
-    B2M_REQUIRE(fabs(det) > 1e-12, B2M_ERR_INVALID, named(s, "singular lattice"));
-    vol[s] = fabs(det);
-  }
-  S = 0;
-  N = off[nstruct];
-  rank = 0, world = 1, axis = 0;
-  for (int k = 0; k < MAXP; k++) walls[k] = 0.0;
-  r_cut = rcut, r_bond = rbond, tol = tol_;
-  volume = 0;
-
-  // ---- upload + wrap: the lattices of the table now, the grids after the min/max ----
-  upload(st, h_cart, h_species);
-  std::vector<int> sid(N);
-  for (int s = 0; s < nstruct; s++) std::fill(sid.begin() + off[s], sid.begin() + off[s + 1], s);
-  b_gp.ensure(nstruct);
-  b_cell_off.ensure(nstruct);
-  b_sid.ensure(N);
-  b_doff.ensure(nstruct + 1);
-  B2M_CK(cudaMemcpyAsync(b_sid.p, sid.data(), N * sizeof(int), cudaMemcpyHostToDevice, st));
-  B2M_CK(cudaMemcpyAsync(b_doff.p, off.data(), (nstruct + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
-  B2M_CK(cudaMemcpyAsync(b_gp.p, gps.data(), nstruct * sizeof(GridParams), cudaMemcpyHostToDevice, st));
-  launch(k_wrap_batch, cdiv(N, 256), 256, 0, st, N, cart.p, b_gp.p, b_sid.p, fracw.p, wc.p, corr.p);
-
-  // ---- per-structure min/max (one block each), cell grids, first cell of each structure ----
-  red_tmp.ensure((size_t)nstruct * 12);
-  launch(k_minmax_batch, nstruct, 256, 0, st, b_doff.p, wc.p, fracw.p, red_tmp.p);
-  std::vector<double> hred((size_t)nstruct * 12);
-  B2M_CK(cudaMemcpyAsync(hred.data(), red_tmp.p, hred.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
-  B2M_CK(cudaStreamSynchronize(st));
-  std::vector<int> coff(nstruct);
-  int64_t ncell = 0;
-  for (int s = 0; s < nstruct; s++) {
-    try {
-      cell_grid(gps[s].inv, gps[s].pbc, &hred[12 * s + 3], &hred[12 * s + 9], rcut, gps[s]);
-    } catch (const Error& ex) {
-      throw Error(ex.code, named(s, ex.what()));
-    }
-    coff[s] = (int)ncell;
-    ncell += (int64_t)gps[s].nc[0] * gps[s].nc[1] * gps[s].nc[2];
-    B2M_REQUIRE(ncell <= (1LL << 27), B2M_ERR_INVALID, "batch needs more than 2^27 cells; split it");
-  }
-  B2M_CK(cudaMemcpyAsync(b_gp.p, gps.data(), nstruct * sizeof(GridParams), cudaMemcpyHostToDevice, st));
-  B2M_CK(cudaMemcpyAsync(b_cell_off.p, coff.data(), nstruct * sizeof(int), cudaMemcpyHostToDevice, st));
-  for (int k = 0; k < 3; k++) {  // the first structure's grid, for the record
-    nc[k] = gps[0].nc[k], reach[k] = gps[0].reach[k], fmin[k] = gps[0].fmin[k], fscale[k] = gps[0].fscale[k];
-  }
-
-  // ---- owner + cell id, sort by (structure, cell), rows ----
-  launch(k_owner_cell_batch, cdiv(N, 256), 256, 0, st, N, fracw.p, b_sid.p, b_gp.p, b_cell_off.p, owner.p, cell_of.p,
-         tmp_i0.p);
-  sort_by_cell(st, (int)ncell);
-  S = nstruct;
-  b_off = off;
-  b_volume = vol;
-  build_rows(st, gps[0]);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1430,22 +1281,17 @@ void Unfold::build(cudaStream_t st, int64_t natoms, const double* h_cart, const 
   species0.ensure(n);
   cnt.ensure(n + 1);
   off.ensure(n + 1);
+  dseg.ensure(2);
   B2M_CK(cudaMemcpyAsync(cart0.p, h_cart, 3 * n * sizeof(double), cudaMemcpyDefault, st));
   B2M_CK(cudaMemcpyAsync(species0.p, h_species, n * sizeof(int), cudaMemcpyDefault, st));
   launch(k_unfold_frac, cdiv(n, 256), 256, 0, st, n, cart0.p, b, frac0.p);
-  // fractional bounding box of the cell atoms (k_minmax's Cartesian half reads the positions and is not used)
-  const int RB = 256;
-  red_tmp.ensure(RB * 12);
-  launch(k_minmax, RB, 256, 0, st, n, cart0.p, frac0.p, red_tmp.p);
-  std::vector<double> hred(RB * 12);
-  B2M_CK(cudaMemcpyAsync(hred.data(), red_tmp.p, RB * 12 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  B2M_CK(cudaStreamSynchronize(st));
+  // fractional bounding box of the cell atoms (the Cartesian half of the bounds reads the positions and is not used)
+  const int64_t seg[2] = {0, n};
+  B2M_CK(cudaMemcpyAsync(dseg.p, seg, sizeof seg, cudaMemcpyHostToDevice, st));
+  std::vector<double> mn, mx;
+  bounds(st, 1, 256, dseg.p, cart0.p, frac0.p, red_tmp, mn, mx);
   for (int k = 0; k < 3; k++) {
-    double fmn = 1e300, fmx = -1e300;
-    for (int r = 0; r < RB; r++) {
-      fmn = std::min(fmn, hred[r * 12 + 3 + k]);
-      fmx = std::max(fmx, hred[r * 12 + 9 + k]);
-    }
+    const double fmn = mn[3 + k], fmx = mx[3 + k];
     b.smin[k] = b.smax[k] = 0;
     b.lo[k] = fmn, b.hi[k] = fmx;
     if (h_pbc[k]) {

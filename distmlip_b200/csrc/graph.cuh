@@ -17,14 +17,33 @@ struct GridParams {
   double fmin[3], fscale[3];
 };
 
+// How a build kernel finds the grid of an atom's structure (DESIGN.md §12).  Each build kernel is one template over
+// these two; a single-structure build runs the OneGrid instantiations, a batch the GridTable ones.
+// OneGrid: one structure, its grid in the kernel parameters, cell ids from 0.
+struct OneGrid {
+  GridParams gp;
+  static constexpr bool kPartitioned = true;  // atoms may be owned by other partitions: owners and halo masks
+  __device__ __forceinline__ int structure(int64_t) const { return 0; }
+  __device__ __forceinline__ const GridParams& grid(int) const { return gp; }
+  __device__ __forceinline__ int first_cell(int) const { return 0; }
+};
+// GridTable: structure s = sid[gid] of a batch, its grid gp[s] and its first global cell id cell_off[s]; one partition.
+struct GridTable {
+  const GridParams* gp;  // [S]
+  const int* cell_off;   // [S]
+  const int* sid;        // [N]
+  static constexpr bool kPartitioned = false;  // every atom owned by partition 0
+  __device__ __forceinline__ int structure(int64_t g) const { return sid[g]; }
+  __device__ __forceinline__ const GridParams& grid(int s) const { return gp[s]; }
+  __device__ __forceinline__ int first_cell(int s) const { return cell_off[s]; }
+};
+
 struct Graph {
   // ---- problem ----
   int64_t N = 0;
   int rank = 0, world = 1;
   int axis = 0;              // partition axis (longest Cartesian extent of wrapped coords)
   double walls[MAXP] = {0};  // world-1 walls in wrapped fractional coordinate
-  double lat[9], inv[9], volume = 0;
-  int pbc[3] = {1, 1, 1};
   double r_cut = 0, r_bond = 0, tol = 1e-8;
   // ---- sizes ----
   int n_own = 0, n_halo = 0, n_loc = 0;
@@ -44,8 +63,6 @@ struct Graph {
   DBuf<double> s_wc;      // [N,3] wrapped Cartesian in sorted order
   DBuf<int> sidx_of_gid;  // [N]
   DBuf<int> cell_start;   // [ncell+1]
-  int nc[3] = {1, 1, 1}, reach[3] = {1, 1, 1};
-  double fmin[3] = {0, 0, 0}, fscale[3] = {0, 0, 0};
   // ---- local atoms: [owned (cell order) | halo (owner, gid order)] ----
   DBuf<int> gid;       // [n_loc]
   DBuf<int> type;      // [n_loc]
@@ -91,25 +108,26 @@ struct Graph {
   bool balanced = false;
   DBuf<double> bal_x;     // [2N] coordinates along the axis, then sorted
   DBuf<long long> bal_w;  // [2N] work per atom, then sorted; its inclusive prefix overwrites the first half
-  // ---- batch (build_batch, DESIGN.md §12): the disjoint union of S structures, structure s owning the gids
-  // b_off[s] .. b_off[s + 1] - 1; S = 0 after a single-structure build ----
+  // ---- structures: the graph is the disjoint union of S structures (S = 1 unless a batch), structure s owning the
+  // gids b_off[s] .. b_off[s + 1] - 1 ----
   int S = 0;
+  bool batch = false;            // built as a batch (DESIGN.md §12): one partition, the GridTable kernels, b_sid filled
   std::vector<int64_t> b_off;    // [S + 1]
-  std::vector<double> b_volume;  // [S]
-  DBuf<GridParams> b_gp;         // [S] each structure's own cell grid
-  DBuf<int> b_cell_off;          // [S] first global cell id of each structure
-  DBuf<int> b_sid;               // [N] structure of each atom
+  std::vector<double> volume;    // [S]
+  std::vector<GridParams> grids; // [S] each structure's own cell grid
+  DBuf<GridParams> b_gp;         // [S] grids on the device (batch)
+  DBuf<int> b_cell_off;          // [S] first global cell id of each structure (batch)
+  DBuf<int> b_sid;               // [N] structure of each atom (batch)
   DBuf<int64_t> b_doff;          // [S + 1] b_off on the device
   std::vector<int64_t> b_name;   // the caller's index of each structure, for error messages; empty: the batch index
 
-  void build(cudaStream_t st, int64_t natoms, const double* h_cart, const double* h_lat,
-             const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_,
-             int rank_, int world_);
-  // world = 1 only: nstruct structures, atoms concatenated in structure order (natoms[s] each), lattices [S][9],
-  // pbc flags [S][3].  Same arrays as build() for the union; inside a structure the rows, edges, bonds and angles come
-  // in the order build() gives that structure alone, with every atom index offset by b_off[s].
-  void build_batch(cudaStream_t st, int nstruct, const int64_t* natoms, const double* h_cart, const double* h_lat,
-                   const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_);
+  // nstruct structures, atoms concatenated in structure order (natoms[s] each), lattices [S][9] (rows), pbc flags
+  // [S][3].  Inside a structure the rows, edges, bonds and angles come in the order a build of that structure alone
+  // gives, with every atom index offset by b_off[s].  A batch (as_batch) needs world = 1 and names the structure in
+  // its errors; otherwise nstruct = 1 and the atoms are split into world slabs, this rank holding slab `rank`.
+  void build(cudaStream_t st, int nstruct, const int64_t* natoms, const double* h_cart, const double* h_lat,
+             const int32_t* h_species, const int* h_pbc, double rcut, double rbond, double tol_, int rank_, int world_,
+             bool as_batch);
   int64_t export_info(cudaStream_t st, int which, int64_t* out, int64_t cap);
   std::string structure_name(int s) const {  // "structure <caller's index>"
     return "structure " + std::to_string(s < (int)b_name.size() ? b_name[s] : (int64_t)s);
@@ -118,7 +136,13 @@ struct Graph {
  private:
   void upload(cudaStream_t st, const double* h_cart, const int32_t* h_species);
   void sort_by_cell(cudaStream_t st, int ncell);
-  void build_rows(cudaStream_t st, const GridParams& gp);
+  void build_rows(cudaStream_t st);
+  // f(grid) with the grid object of this build: GridTable for a batch, else OneGrid of the one structure
+  template <class F>
+  void with_grid(F&& f) const {
+    if (batch) f(GridTable{b_gp.p, b_cell_off.p, b_sid.p});
+    else f(OneGrid{grids[0]});
+  }
 };
 
 // Unfolded cell of the heat flux (DESIGN.md §10): the n cell atoms at their given positions, followed by every periodic
@@ -132,6 +156,7 @@ struct Unfold {
   DBuf<int> species;      // [N]
   DBuf<int> image_of;     // [N] cell atom of every unfolded atom (image_of[i] = i for i < n)
   DBuf<double> cart0, frac0, red_tmp;
+  DBuf<int64_t> dseg;  // [2] the atoms 0 .. n - 1 as one segment of the bounds reduction
   DBuf<int> species0, cnt, off;
   DBuf<char> cub_tmp;
   void build(cudaStream_t st, int64_t natoms, const double* h_cart, const int32_t* h_species, const double* h_lat,
